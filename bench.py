@@ -11,6 +11,7 @@ graph launch (b200rl_onpolicy_iterate).
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...  # the reference-shaped CPU arm (oracle port, all host cores)
     python bench.py --config c3|c5                           # BASELINE configs[2] (Pendulum A2C) / configs[4] (DQN 1M replay), 1 GPU
+    python bench.py ... --dump-outputs DIR                   # also write what the last timed step computed as DIR/*.npy
 
 Prints ONE JSON line (see DESIGN.md "Measurement").  Timing: one CUDA event pair per step on the
 launching stream (L2 flushed between steps, outside the timed region), NO host synchronisation
@@ -46,8 +47,8 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as f:
             d = json.load(f)
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), "measured"
-    return 6650.0, 1590.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), "measured"
+    return 3350.0, 989.0, "fallback"   # H100 SXM data sheet: HBM3 bandwidth, dense BF16
 
 
 def _physical_indices(n):
@@ -330,6 +331,34 @@ def timed_steps(job, step_fn, steps, sampler=None):
     return job.max_over_ranks(total_ms)
 
 
+def dump_onpolicy_outputs(out_dir, agent, net, n, sample=4096, seed=0):
+    """What the last timed iteration computed, as a caller of agent.iterate() would read it back: the network parameters after its
+    updates, and the rollout it trained on (states, actions, log-probs, rewards, terminals, values, advantages, returns) for a
+    fixed, seeded sample of `sample` envs of this rank.  float32 .npy files, a few MB in all."""
+    from b200rl import learners as R
+    os.makedirs(out_dir, exist_ok=True)
+    idx = np.sort(np.random.default_rng(seed).choice(n, min(n, sample), replace=False))
+    out = {"params": net.get(), "env_index": idx}
+    for name, field in (("states", R.ROLL_STATE), ("actions", R.ROLL_ACTION), ("logp", R.ROLL_LOGP), ("rewards", R.ROLL_REWARD),
+                        ("terminals", R.ROLL_TERMINAL), ("values", R.ROLL_VALUE), ("advantages", R.ROLL_ADV), ("returns", R.ROLL_RET)):
+        a = agent.rollout(field)
+        out[name] = a[:, idx] if field == R.ROLL_STATE else a[idx]
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
+def dump_dqn_outputs(out_dir, learner, net, traj):
+    """What the last timed optimise! call computed: the Q-network parameters after it, the prioritised batch it sampled (states,
+    actions, rewards, terminals, next states, replay keys, priorities, importance weights) and its TD errors.  float32 .npy files
+    (replay keys as float64), a few hundred KB."""
+    os.makedirs(out_dir, exist_ok=True)
+    out = {"params": net.get(), "td": learner.last_td()}
+    for name, a in traj.batch().items():
+        out["batch_" + name] = a
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64 if name == "batch_key" else np.float32))
+
+
 def phase_breakdown(job, agent, T, rows, reps=3):
     """Per-phase device times of one iteration on THIS rank (eager launches with events between the phases; measurement aid,
     outside the timed region): rollout | bootstrap + GAE + normalisation + record packing | sum of the loss+backward launches |
@@ -390,6 +419,8 @@ def run_c2(args):
     launches0 = ctx.launch_count()
     total_ms = timed_steps(job, lambda: agent.iterate(1), args.steps, sampler)
     launches = ctx.launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_onpolicy_outputs(args.dump_outputs, agent, net, n)
     clk = sampler.stop() if sampler else None
     graph = agent.graph_active()
     value = n_total * T * args.steps / (total_ms / 1000.0)
@@ -446,27 +477,19 @@ def run_c2(args):
     k_adam = agent.time_kernel(4, 20)
     k_env = agent.time_kernel(2, 20)
     ach_tf = B_local * FLOP_FWD_BWD / (k_loss * 1e-3) / 1e12
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        try:
-            tj = json.load(open(tpath))
-            traffic = tj.get("ac_loss_grad_tc_kernel" if tc_on else "ac_loss_grad_kernel", tj.get("ac_loss_grad_kernel"))
-        except Exception:
-            traffic = None
     ms_step = total_ms / args.steps
     share = (N_EPOCHS * N_MICRO * k_loss) / ms_step
-    kname = ("ac_loss_grad_tc_kernel (PPO loss + backward, one minibatch; 64x64 GEMMs on tcgen05 kind::f16 as a 3-term fp16 split "
-             "hi*hi + hi*lo + lo*hi, FP32 accumulate in TMEM; the optimiser step runs in the tail of the same launch)"
+    kname = ("ac_loss_grad_tc_kernel (PPO loss + backward, one minibatch; 64x64 GEMMs on wgmma f16 as a 3-term fp16 split "
+             "hi*hi + hi*lo + lo*hi, FP32 accumulate; the optimiser step runs in the tail of the same launch)"
              if tc_on else "ac_loss_grad_kernel<64> (PPO loss + backward, one minibatch; FP32 FFMA)")
     roofline = {"kernel": kname, "bound": "tensor", "achieved": ach_tf, "peak": tf_peak,
-                "unit": "TFLOP/s", "frac": ach_tf / tf_peak, "traffic": traffic, "peak_kind": f"bf16 dense GEMM burst, {peak_kind}",
+                "unit": "TFLOP/s", "frac": ach_tf / tf_peak, "peak_kind": f"bf16 dense GEMM, {peak_kind}",
                 "executed_tensor": {"tflops": 3.0 * ach_tf, "peak": tf_peak, "frac": 3.0 * ach_tf / tf_peak,
-                                    "note": "the 1e-5 parity bar needs ~22 mantissa bits: every algorithmic product is three kind::f16 tensor-core products "
-                                            "(fp16 hi/lo split, K = 16 per instruction); executed tensor work / the measured 16-bit dense peak"},
+                                    "note": "the 1e-5 parity bar needs ~22 mantissa bits: every algorithmic product is three f16 tensor-core products "
+                                            "(fp16 hi/lo split, K = 16 per instruction); executed tensor work / the 16-bit dense peak"},
                 "algorithmic_bytes_per_launch": B_local * BYTES_K7_SAMPLE,
-                "note": "achieved = algorithmic FP32 FLOPs (53,376 per sample) / event time; as a fraction of the FP32 CUDA-core peak (~72 TFLOP/s @1.9 GHz) = %.3f"
-                        % (ach_tf / 72.0),
+                "note": "achieved = algorithmic FP32 FLOPs (53,376 per sample) / event time; as a fraction of the H100 SXM data-sheet FP32 peak (67 TFLOP/s) = %.3f"
+                        % (ach_tf / 67.0),
                 "ms_per_launch": k_loss, "ms_per_launch_fp32_ffma_variant": k_loss_ffma, "share_of_step": share,
                 "ms_per_launch_note": "loss + backward alone (the timed iteration additionally runs reduce + clip + Adam in the tail of each launch)",
                 "whole_loop_hbm": {"gbs": value * BYTES_LOOP_ENV_STEP / 1e9, "peak": hbm_peak * world, "frac": value * BYTES_LOOP_ENV_STEP / 1e9 / (hbm_peak * world),
@@ -476,8 +499,8 @@ def run_c2(args):
                     "policy_act_ms": k_act, "policy_act_ms_fp32_ffma_variant": k_act_ffma, "policy_act_tflops": n * FLOP_FWD / (k_act * 1e-3) / 1e12,
                     "env_step_ms": k_env, "env_step_gbs": n * BYTES_ENV_STEP / (k_env * 1e-3) / 1e9, "env_step_frac_hbm": n * BYTES_ENV_STEP / (k_env * 1e-3) / 1e9 / hbm_peak,
                     "gae_ms": k_gae, "gae_gbs_l2_resident": n * T * BYTES_GAE / (k_gae * 1e-3) / 1e9,
-                    "gae_note": "at this size the 52 MB working set of the GAE kernel is L2-resident when timed back to back (ncu: 19 MB DRAM read, 0 written): "
-                                "an L2 figure, not an HBM fraction; the HBM-bound sweep (4 M series) reaches 0.60 of the measured copy bandwidth (profiles/)",
+                    "gae_note": "the GAE kernel's working set at this size (about 52 MB) is close to the 50 MB L2 and largely cached when timed "
+                                "back to back: an L2-assisted figure, not an HBM fraction",
                     "reduce_clip_adam_ms": k_adam,
                     "reduce_clip_adam_note": "the stand-alone optimiser-step kernel (FFMA path, ranks sharing a device, B200RL_FUSED_STEP=0); "
                                              "the tensor-core K7 runs the step in its own tail"}}
@@ -547,6 +570,8 @@ def run_c3(args):
     l0 = ctx.launch_count()
     total_ms = timed_steps(job, lambda: agent.iterate(1), args.steps, sampler)
     launches = ctx.launch_count() - l0
+    if args.dump_outputs:
+        dump_onpolicy_outputs(args.dump_outputs, agent, net, n)
     clk = sampler.stop()
     value = n * T * args.steps / (total_ms / 1000.0)
     ph = phase_breakdown(job, agent, T, 1)
@@ -575,8 +600,8 @@ def run_c3(args):
                        "n_envs": n, "parallelism": "dp1", "l2": "flushed between timed steps, outside the timed region",
                        "launch": "one CUDA graph launch per iteration" if agent.graph_active() else "eager launches"},
             "clocks": clk, "e2e": e2e, "gpu_launches": int(launches), "phases_per_rank": [ph],
-            "roofline": {"kernel": "ac_loss_grad_tc_kernel (A2C loss + backward over the whole rollout, Gaussian head, tanh; 3-term fp16 split on tcgen05 kind::f16)", "bound": "tensor",
-                         "achieved": ach, "peak": tf_peak, "unit": "TFLOP/s", "frac": ach / tf_peak, "traffic": None, "peak_kind": f"bf16 dense GEMM burst, {peak_kind}",
+            "roofline": {"kernel": "ac_loss_grad_tc_kernel (A2C loss + backward over the whole rollout, Gaussian head, tanh; 3-term fp16 split on wgmma f16)", "bound": "tensor",
+                         "achieved": ach, "peak": tf_peak, "unit": "TFLOP/s", "frac": ach / tf_peak, "traffic": None, "peak_kind": f"bf16 dense GEMM, {peak_kind}",
                          "ms_per_launch": k_loss, "share_of_step": k_loss / (total_ms / args.steps)},
             "cpu_baseline": None}
     print(json.dumps(line), flush=True)
@@ -615,6 +640,8 @@ def run_c5(args):
             learner.update()
     total_ms = timed_steps(job, step, args.steps, sampler)
     launches = ctx.launch_count() - l0
+    if args.dump_outputs:
+        dump_dqn_outputs(args.dump_outputs, learner, qnet, tr)
     clk = sampler.stop()
     ups = per_step * args.steps / (total_ms / 1000.0)
     # e2e: the user-facing call with the per-update statistics read back to the host (loss, grad norm, mean |td|: a D2H copy + sync per update)
@@ -647,7 +674,7 @@ def run_c5(args):
             "e2e": {"value": k / sec, "unit": "updates/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": int(16 + 4 + B * 4), "steps": k,
                     "note": "learner.update(want_stats=True): loss, grad norm and the batch's TD errors read back to the host after every update"},
             "roofline": {"kernel": "whole optimise! call (sample+gather, target forward, TD loss+backward, reduce, clip+Adam, priority write-back)", "bound": "tensor",
-                         "achieved": ach, "peak": tf_peak, "unit": "TFLOP/s", "frac": ach / tf_peak, "traffic": None, "peak_kind": f"bf16 dense GEMM burst, {peak_kind}",
+                         "achieved": ach, "peak": tf_peak, "unit": "TFLOP/s", "frac": ach / tf_peak, "traffic": None, "peak_kind": f"bf16 dense GEMM, {peak_kind}",
                          "ms_per_update": ms_update, "sample_gather_ms": ms_sample, "sample_gather_gbs_at_326B": B * 326 / ms_sample / 1e6,
                          "sample_gather_frac_hbm": B * 326 / ms_sample / 1e6 / hbm_peak,
                          "note": "latency-bound at batch 4096: 5 dependent launches of a few microseconds each; the gather moves 1.3 MB"},
@@ -669,7 +696,11 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-weak", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (float32, replay keys float64)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "own":
+        ap.error("--dump-outputs applies to this repo's CUDA path (--impl own)")
     if args.impl == "reference":
         run_reference(args)
     elif args.config == "c3":

@@ -7,7 +7,7 @@
  *   gcc -O2 -Iinclude examples/ppo_cartpole.c -Lreinforcementlearning.jl_b200 -lb200rl \
  *       -Wl,-rpath,$PWD/reinforcementlearning.jl_b200 -lm -o /tmp/ppo_cartpole && /tmp/ppo_cartpole [n_envs] [iterations]
  *
- * Needs a B200 to run (there is no CPU fallback: b200rl_init fails loudly otherwise); building needs none.
+ * Needs an H100 to run (there is no CPU fallback: b200rl_init fails loudly otherwise); building needs none.
  */
 #include <math.h>
 #include <stdint.h>

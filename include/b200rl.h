@@ -1,4 +1,4 @@
-/* b200rl.h — C ABI of libb200rl.so: the Blackwell (sm_100a) vectorised RL inner loop that
+/* b200rl.h — C ABI of libb200rl.so: the H100 (sm_90a) vectorised RL inner loop that
  * sits behind ReinforcementLearning.jl's `Base.run(policy, env, stop, hook)` surface.
  *
  * The reference has no FFI: its extension mechanism is Julia multiple dispatch on
@@ -17,7 +17,7 @@
  *    stream; calls are asynchronous on it except *_get / *_sync and calls taking host arrays.
  *  - handles are not thread-safe (one driver task per ctx, like the reference's
  *    single-threaded _run, RLCore/src/core/run.jl:36-78).
- *  - there is NO CPU fallback: every entry point fails with B200RL_ERR_CUDA when no sm_100
+ *  - there is NO CPU fallback: every entry point fails with B200RL_ERR_CUDA when no sm_90
  *    device is usable.
  */
 #ifndef B200RL_H
@@ -359,7 +359,7 @@ typedef struct {
 int b200rl_dqn_update(b200rl_net* net, b200rl_traj* traj, const b200rl_dqn_config* cfg, float* stats_host);
 int b200rl_dqn_last_td(b200rl_net* net, b200rl_traj* traj, float* host_dst, int64_t count);
 
-/* select the tcgen05 tensor-core kernels (default, H = 64) or the FP32 CUDA-core kernels for the dense layers */
+/* select the wgmma tensor-core kernels (default, H = 64) or the FP32 CUDA-core kernels for the dense layers */
 int b200rl_set_tensor_cores(int enable);
 /* 1 (default; B200RL_FUSED_STEP=0 in the environment starts with 0): the on-policy update runs reduce + [peer exchange] + clip +
  * Adam in the tail of the tensor-core loss + backward launch (one launch per optimiser step); 0: a second kernel does it.

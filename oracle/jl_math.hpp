@@ -10,7 +10,7 @@
 //     float kernels, rounded once; tiny-argument short cuts; Cody–Waite reduction.
 //   * sin/cos(::Float64): msun double kernels for |x| < pi/4, 3-stage Cody–Waite beyond.
 //   * `@horner` expands to `muladd`, which LLVM fuses on every FMA-capable x86-64
-//     (Haswell+, i.e. every B200 host) -> restated as an explicit fma().  Everything
+//     (Haswell+, i.e. every x86-64 GPU host) -> restated as an explicit fma().  Everything
 //     else is NOT contracted (compile with -ffp-contract=off).
 //   * mod(::Float64, ::Float64), clamp.
 // Call sites in the reference: CartPoleEnv.jl:122-123 (cos/sin theta),

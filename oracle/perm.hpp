@@ -2,7 +2,7 @@
 // Minibatch permutation used when the host does not supply `shuffle!(rng, 1:N*T)` itself
 // (SURVEY Appendix B, PPO _update!): a keyed 4-round alternating Feistel bijection on the
 // smallest power-of-two domain 2^bits >= n (bits >= 2; left half floor(bits/2) bits, the halves
-// swap widths every round) with cycle walking.  A B200-side definition (the reference's shuffle!
+// swap widths every round) with cycle walking.  A definition of this project (the reference's shuffle!
 // is a sequential Fisher-Yates on one stream); DESIGN.md §K7.
 #pragma once
 #include <cstdint>

@@ -14,7 +14,7 @@
 //                               is a frame of its own; the entry straddling two episodes exists but is not sampleable)
 // Layout: `lanes` independent rings of cap+1 slots (lanes = 1 is exactly the reference's single-stream CircularArraySARTSTraces wrapped
 // in an EpisodesBuffer).  Entry p of a lane is the transition state[p] -> state[p+1] (MultiplexTraces).  Samplers draw WITH
-// replacement (BatchSampler) from one Xoshiro stream per batch slot (a B200-side definition: the reference draws the whole batch from
+// replacement (BatchSampler) from one Xoshiro stream per batch slot (a definition of this project: the reference draws the whole batch from
 // a single stream).  A terminal bit 1 in push() means "next_obs already is the next episode's first state" (the batched env's in-kernel
 // auto-reset): it is stored twice, as the masked :next_state and as the episode-start frame.
 #pragma once

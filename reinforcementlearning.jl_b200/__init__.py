@@ -1,4 +1,4 @@
-"""b200rl — Blackwell-native vectorised RL inner loop behind ReinforcementLearning.jl's
+"""b200rl — H100-native (sm_90a) vectorised RL inner loop behind ReinforcementLearning.jl's
 run(policy, env, stop, hook) surface.  Python host mirror of the Julia glue
 (julia/B200RL.jl): thin ctypes calls into libb200rl.so; no compute happens in Python and
 there is no CPU fallback."""

@@ -1,7 +1,7 @@
 """ctypes binding of libb200rl.so (include/b200rl.h).  No torch types cross this boundary.
 
-The library is built in-tree by ``build.py`` (nvcc, sm_100a).  There is no CPU fallback: if
-the shared object is missing, or no sm_100 device is usable, calls fail loudly."""
+The library is built in-tree by ``build.py`` (nvcc, sm_90a).  There is no CPU fallback: if
+the shared object is missing, or no sm_90 (H100) device is usable, calls fail loudly."""
 import ctypes as C
 import os
 

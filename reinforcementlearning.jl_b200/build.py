@@ -1,4 +1,4 @@
-"""Build libb200rl.so in-tree with nvcc for sm_100a (no torch, no JIT cache).
+"""Build libb200rl.so in-tree with nvcc for sm_90a (H100; no torch, no JIT cache).
 
     python reinforcementlearning.jl_b200/build.py [--force] [--verbose]
 
@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb200rl.so")
 BUILD = os.path.join(HERE, "build")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-diag-suppress", "177"]
 # (source, extra flags)
 SOURCES = [
@@ -24,8 +24,6 @@ SOURCES = [
 ]
 ENV_FLAGS = ["-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false"]
 OPTIONAL = [("traj.cu", []), ("nn.cu", []), ("algo.cu", []), ("nn_tc.cu", []), ("fwd_tc.cu", ENV_FLAGS)]
-# diagnostic probe of the tcgen05 operand layouts (profiles/umma_probe*.py): its own library, NOT part of the product .so
-SELFTEST_OUT = os.path.join(BUILD, "libb200rl_selftest.so")
 
 
 def _nvcc():
@@ -82,22 +80,8 @@ def build(force=False, verbose=False, variant=None, defs=()):
     return out_so
 
 
-def build_selftest():
-    """build/libb200rl_selftest.so: csrc/umma_selftest.cu linked against the product library (it borrows the ctx / scratch helpers)."""
-    so = build()
-    nvcc = _nvcc()
-    host_cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-    obj = os.path.join(BUILD, "umma_selftest.o")
-    subprocess.check_call([nvcc, "-ccbin", host_cxx] + ARCH + COMMON + ["-c", os.path.join(CSRC, "umma_selftest.cu"), "-o", obj])
-    subprocess.check_call([nvcc, "-ccbin", host_cxx] + ARCH + ["-shared", "-Xcompiler", "-fPIC", "-o", SELFTEST_OUT, obj, "-L" + HERE, "-lb200rl",
-                           "-Xlinker", "-rpath=" + HERE])
-    return SELFTEST_OUT
-
-
 if __name__ == "__main__":
-    if "--selftest" in sys.argv:
-        print(build_selftest())
-    elif "--variant" in sys.argv:      # python build.py --variant NAME -DFOO=1 -DBAR
+    if "--variant" in sys.argv:      # python build.py --variant NAME -DFOO=1 -DBAR
         name = sys.argv[sys.argv.index("--variant") + 1]
         print(build(variant=name, defs=[a for a in sys.argv if a.startswith("-D")], verbose="--verbose" in sys.argv))
     else:

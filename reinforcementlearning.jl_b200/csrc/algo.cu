@@ -55,7 +55,7 @@ __global__ void stats_row_kernel(float* __restrict__ row, const float* __restric
 }
 // After GAE: one 32-byte record per rollout sample {state (zero padded to 4), action bits, logp_old, advantage, return}, so the
 // randomly permuted minibatch gather of K7 touches ONE DRAM sector per sample instead of one per array (5 arrays: ~4x the
-// algorithmic bytes, profiles/r01_ncu_summary.md).  Streaming: 32 B read + 32 B written per sample, fully coalesced.
+// algorithmic bytes).  Streaming: 32 B read + 32 B written per sample, fully coalesced.
 template <int NS>
 __global__ void __launch_bounds__(256) pack_records_kernel(float4* __restrict__ rec, const float* __restrict__ states, const uint32_t* __restrict__ actions,
                                                           const float* __restrict__ logp, const float* __restrict__ adv, const float* __restrict__ ret,

@@ -1,7 +1,7 @@
 // comm.cu — multi-GPU exchange: env-index data parallelism needs exactly one sum all-reduce of
 // the flat gradient (np fp32, ~36 KB) per optimiser step plus two doubles for the global
 // advantage normalisation (SURVEY §8e).  One process per GPU; the communicator is NCCL over
-// NVLink 5 / NVSwitch, resolved at run time with dlopen("libnccl.so.2") so the library has no
+// NVLink / NVSwitch, resolved at run time with dlopen("libnccl.so.2") so the library has no
 // link-time dependency and shares the NCCL already loaded by the host process (e.g. torch's).
 #include <dlfcn.h>
 

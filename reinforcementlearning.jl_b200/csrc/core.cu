@@ -53,14 +53,14 @@ int b200rl_init(int device, b200rl_ctx** out) {
     REQUIRE(device >= 0 && device < count, B200RL_ERR_INVALID, "device index out of range");
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        b200rl_set_error("b200rl_init: device %d is sm_%d%d; libb200rl.so contains sm_100a code only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        b200rl_set_error("b200rl_init: device %d is sm_%d%d; libb200rl.so contains sm_90a code only", device, prop.major, prop.minor);
         return B200RL_ERR_UNSUPPORTED;
     }
     CUDA_TRY(cudaSetDevice(device));
     {   // L2 fetch granularity 32 B: the minibatch gathers of the update read one 32-byte record per sample at random; with the
-        // default (128 B) granularity every such read drags 3 neighbouring sectors out of HBM (ncu: 46.0 MB per K7 launch vs
-        // 16.9 MB at 32 B = 1.01x the algorithmic bytes; streaming kernels request whole lines either way).  A hint, per context;
+        // default (128 B) granularity every such read drags 3 neighbouring sectors out of HBM (streaming kernels request whole
+        // lines either way).  A hint, per context;
         // B200RL_L2_FETCH=64|128 restores a larger one, 0 leaves the driver default.
         size_t gran = 32;
         if (const char* g = getenv("B200RL_L2_FETCH")) gran = (size_t)atoi(g);

@@ -21,11 +21,10 @@ void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n);
 namespace {
 
 struct SmemFwd {
+    alignas(128) uint8_t T[TILE_BYTES];   // A operand / accumulator image of the tile (tc_fwd.cuh)
     NetSm net;
     float X[kInMax * TM];                 // [i][s]
     float Zp[2 * kOutMax * TM];           // head partials [half][o][s]
-    alignas(8) uint64_t bar;
-    uint32_t tmem;
 };
 
 __device__ __forceinline__ void load_rng32(const unsigned long long* rng, int64_t i, unsigned long long (&s)[4]) {
@@ -56,16 +55,9 @@ forward_tc_kernel(MlpDesc actor, MlpDesc critic, const float* __restrict__ param
     const int q = warp & 3, c = warp >> 2;
     const int s = 32 * q + lane;
     load_net(sm.net, d, params + poff, (ACT >= 0 ? ACT : d.act) == B200RL_ACT_RELU && ACT >= 0 ? kScale : 1.0f);
-    if (warp == 0) umma::tmem_alloc(&sm.tmem, TMEM_COLS);
-    if (tid == 32) umma::mbar_init(&sm.bar, 1);
-    umma::fence_proxy_async();
-    umma::fence_before_sync();
+    wg::fence_proxy_async();
     __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem = sm.tmem;
-    const uint32_t tmem_lane = tmem + ((uint32_t)(32 * q) << 16);
     const int64_t ntiles = (N + TM - 1) / TM;
-    uint32_t phase = 0;
     for (int64_t tile = cta; tile < ntiles; tile += nctas) {
         if (tid < TM) {
             int64_t i = tile * TM + tid;
@@ -93,27 +85,19 @@ forward_tc_kernel(MlpDesc actor, MlpDesc critic, const float* __restrict__ param
             float x[kInMax];
 #pragma unroll
             for (int k = 0; k < kInMax; ++k) x[k] = sm.X[k * TM + s];
-            layer1_to_tmem<ACT>(sm.net, d.act, x, c, tmem_lane);
+            layer1_to_smem<ACT>(sm.net, d.act, x, c, s, sm.T);
         }
-        umma::fence_before_sync();
+        wg::fence_proxy_async();
         __syncthreads();
-        if (tid == 0) {   // (elect.sync measured 3 % slower here, profiles/umma_pacing.py notes)
-            umma::fence_after_sync();
-            issue_gemm(tmem, sm.net);
-            umma::commit(&sm.bar);
-        }
-        __syncwarp();
-        umma::mbar_wait(&sm.bar, phase);
-        phase ^= 1u;
-        umma::fence_after_sync();
+        gemm_block(sm.T + c * BLK, sm.net, c);   // warpgroup c: samples 64c .. 64c+63
+        __syncthreads();
         {
             float zp[kOutMax];
-            head_partials<ACT>(sm.net, d.act, c, tmem_lane, zp);
+            head_partials<ACT>(sm.net, d.act, c, s, sm.T, zp);
 #pragma unroll
             for (int o = 0; o < kOutMax; ++o) sm.Zp[(c * kOutMax + o) * TM + s] = zp[o];
         }
-        umma::fence_before_sync();     // TMEM reads done before the next tile's layer 1 / MMA overwrite A and D
-        __syncthreads();
+        __syncthreads();               // accumulator reads done before the next tile's layer 1 overwrites the image
         if (tid < TM) {
             int64_t i = tile * TM + tid;
             if (i < N) {
@@ -137,16 +121,13 @@ forward_tc_kernel(MlpDesc actor, MlpDesc critic, const float* __restrict__ param
         }
         __syncthreads();
     }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem, TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // fused rollout
 constexpr int kSlots = 2;   // tiles of 128 envs a CTA keeps resident
 
-template <class Env> struct SlotState {   // env state of one tile, one entry per env (owner thread = TMEM lane)
+template <class Env> struct SlotState {   // env state of one tile, one entry per env (owner thread = sample s)
     typename Env::S st[TM];
     int t[TM];
     int flags[TM];
@@ -157,14 +138,13 @@ template <class Env> struct SlotState {   // env state of one tile, one entry pe
     unsigned long long prng[4 * TM];   // policy stream
 };
 template <class Env> struct SmemRoll {
+    alignas(128) uint8_t T[TILE_BYTES];    // A operand / accumulator image of the tile being evaluated (tc_fwd.cuh)
     NetSm net[2];                          // actor, critic
     float X[kInMax * TM];
     float Zp[2][2 * kOutMax * TM];         // [net][half][o][s]
     SlotState<Env> slot[kSlots];
     float red_f[8];
     int red_i[8], red_l[8];
-    alignas(8) uint64_t bar;
-    uint32_t tmem;
 };
 
 struct RollArgs {
@@ -198,8 +178,6 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
     const int64_t ntiles = (N + TM - 1) / TM;
     load_net(sm.net[0], g.actor, g.params, ACT == B200RL_ACT_RELU ? kScale : 1.0f);
     load_net(sm.net[1], g.critic, g.params + g.actor.nparams(), ACT == B200RL_ACT_RELU ? kScale : 1.0f);
-    if (warp == 0) umma::tmem_alloc(&sm.tmem, TMEM_COLS);
-    if (tid == 32) umma::mbar_init(&sm.bar, 1);
     // resident env state
     int nslots = 0;
     for (int k = 0; k < kSlots; ++k)
@@ -221,13 +199,8 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
             }
         }
     }
-    umma::fence_proxy_async();
-    umma::fence_before_sync();
+    wg::fence_proxy_async();
     __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem = sm.tmem;
-    const uint32_t tmem_lane = tmem + ((uint32_t)(32 * q) << 16);
-    uint32_t phase = 0;
     // episode statistics of this thread's envs (device-side TotalRewardPerEpisode / BatchStepsPerEpisode, hooks.jl:146-231)
     int fin_cnt = 0, fin_len = 0;
     float fin_ret = 0.f;
@@ -264,37 +237,27 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
             uint32_t a_bits = 0;
             if (!boot) {
                 // ---- actor ---------------------------------------------------------------------------------------
-                layer1_to_tmem<ACT>(sm.net[0], g.actor.act, x, c, tmem_lane);
-                umma::fence_before_sync();
+                layer1_to_smem<ACT>(sm.net[0], g.actor.act, x, c, s, sm.T);
+                wg::fence_proxy_async();
                 __syncthreads();
-                if (tid == 0) {   // (elect.sync measured 3 % slower here, profiles/umma_pacing.py notes)
-                    umma::fence_after_sync();
-                    issue_gemm(tmem, sm.net[0]);
-                    umma::commit(&sm.bar);
-                }
-                __syncwarp();
-                umma::mbar_wait(&sm.bar, phase);
-                phase ^= 1u;
-                umma::fence_after_sync();
+                gemm_block(sm.T + c * BLK, sm.net[0], c);   // warpgroup c: samples 64c .. 64c+63
+                __syncthreads();
                 {
                     float zp[kOutMax];
-                    head_partials<ACT>(sm.net[0], g.actor.act, c, tmem_lane, zp);
+                    head_partials<ACT>(sm.net[0], g.actor.act, c, s, sm.T, zp);
 #pragma unroll
                     for (int o = 0; o < kOutMax; ++o) sm.Zp[0][(c * kOutMax + o) * TM + s] = zp[o];
                 }
-                umma::fence_before_sync();
                 __syncthreads();
             }
-            // ---- critic GEMM in flight while the owner threads sample the action and step the env -----------------------
-            layer1_to_tmem<ACT>(sm.net[1], g.critic.act, x, c, tmem_lane);
-            umma::fence_before_sync();
+            // ---- critic GEMM (warpgroup 1, both blocks) while the owner threads (warpgroup 0) sample the action and step the env
+            layer1_to_smem<ACT>(sm.net[1], g.critic.act, x, c, s, sm.T);
+            wg::fence_proxy_async();
             __syncthreads();
-            if (tid == 0) {   // (elect.sync measured 3 % slower here, profiles/umma_pacing.py notes)
-                umma::fence_after_sync();
-                issue_gemm(tmem, sm.net[1]);
-                umma::commit(&sm.bar);
+            if (!owner) {
+                gemm_block(sm.T, sm.net[1], 1);
+                gemm_block(sm.T + BLK, sm.net[1], 1);
             }
-            __syncwarp();
             if (owner && live && !boot) {
                 float z[kOutMax];
 #pragma unroll
@@ -333,15 +296,12 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
                 sl.last_rew[s] = rew;
                 { act_t tmp = act; uint32_t bits; memcpy(&bits, &tmp, 4); sl.last_act[s] = bits; }
             }
-            umma::mbar_wait(&sm.bar, phase);
-            phase ^= 1u;
-            umma::fence_after_sync();
+            __syncthreads();
             {
                 float zp[kOutMax];
-                head_partials<ACT>(sm.net[1], g.critic.act, c, tmem_lane, zp);
+                head_partials<ACT>(sm.net[1], g.critic.act, c, s, sm.T, zp);
                 sm.Zp[1][(c * kOutMax) * TM + s] = zp[0];
             }
-            umma::fence_before_sync();
             __syncthreads();
             if (owner && live) g.values[(size_t)N * t + i] = sm.net[1].b3[0] + sm.Zp[1][s] + sm.Zp[1][kOutMax * TM + s];
             // (the next pass's X / Zp writes are ordered behind this read by its first __syncthreads)
@@ -385,9 +345,6 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
             if (cc > 0) { atomicAdd(&ea.stats[0], cc); atomicAdd(&ea.stats[1], rr); atomicAdd(&ea.stats[2], ll); }
         }
     }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem, TMEM_COLS);
 }
 
 template <class Env> int launch_rollout(b200rl_ctx* ctx, const RollArgs& g, const typename Env::P& p, const EnvArrays& ea) {

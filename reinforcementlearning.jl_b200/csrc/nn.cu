@@ -732,7 +732,7 @@ __global__ void __launch_bounds__(1024) clip_adam_kernel(float* __restrict__ p, 
 }
 
 // Fused K8: partial reduce -> [peer exchange over NVLink] -> global norm -> clip -> Adam in ONE launch.  The CTAs meet at a
-// device-wide counter (all ceil(np/256) <= 148 CTAs are co-resident), every CTA then sums the per-CTA sum-of-squares in
+// device-wide counter (all ceil(np/256) <= sm_count CTAs are co-resident), every CTA then sums the per-CTA sum-of-squares in
 // CTA order, so the result is bit-identical to the two-kernel path and run-to-run deterministic.
 // XCHG (sharded run, SURVEY §8e): every thread pushes its element of the local gradient into the peers' inboxes as a
 // self-validating {value, sequence} packet (remote NVLink store), then reads the peers' packets from the own inbox and sums

@@ -42,12 +42,12 @@ struct AcBatch {
 };
 
 // Optimiser step fused into the tail of the tensor-core K7 (nn_ac_loss_grad_step): reduce the per-CTA partials -> [NVLink peer
-// exchange] -> global norm -> clip_by_global_norm! -> Adam, behind two grid barriers inside the SAME launch (the 148 persistent
-// CTAs are co-resident), instead of a second kernel (~14-20 us of launch, L2 round trips and barrier per optimiser step).
+// exchange] -> global norm -> clip_by_global_norm! -> Adam, behind two grid barriers inside the SAME launch (the persistent
+// CTAs, one per SM, are co-resident), instead of a second kernel (a launch, L2 round trips and a barrier per optimiser step).
 struct AcStep {
     float* params; float* grad; float* m; float* v; float* beta_t;
     float* loss_out4; float* stats_row; float* gnorm_out;     // each may be null
-    double* cta_sumsq;            // >= 148 doubles
+    double* cta_sumsq;            // >= grid doubles (<= 256)
     unsigned int* counter;        // 4 zero-initialised uints (self-resetting grid barriers)
     unsigned int* tick;           // may be null: device update counter incremented once by the launch
     unsigned int* seq_ptr;        // gradient-exchange sequence number (sharded run)
@@ -82,7 +82,7 @@ int nn_reduce_partials(b200rl_ctx* ctx, const float* partial, int n_partials, in
 int nn_clip_adam(b200rl_ctx* ctx, float* params, float* grad, float* m, float* v, float* beta_t /* device [2] */, int64_t np,
                  float max_grad_norm, float lr, float b1, float b2, float eps, float grad_scale, float* gnorm_out /* device */);
 // fused single-launch variant (single GPU, or a sharded run with the NVLink peer exchange attached; stats_row (may be null)
-// receives {4 loss sums, grad norm}): cta_sumsq >= 148 doubles, counter2 = 2 zero-initialised uints (self-resetting grid barrier),
+// receives {4 loss sums, grad norm}): cta_sumsq >= grid doubles, counter2 = 2 zero-initialised uints (self-resetting grid barrier),
 // tick (may be null) = device counter incremented once by the launch (the agent's update counter that keys the permutation)
 int nn_reduce_clip_adam(b200rl_ctx* ctx, const float* partial, int n_partials, int64_t np, float* params, float* grad, float* m, float* v,
                         float* beta_t, const float* loss_partial, int n_loss, float* loss_out4, float max_grad_norm, float lr, float b1, float b2,
@@ -97,7 +97,7 @@ int nn_q_act(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float
 int nn_q_explore(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float* obs, int64_t N, unsigned long long* rng,
                  const b200rl_explorer& ex, int32_t* action_out, float* q_out);
 
-// tensor-core (tcgen05) variants, nn_tc.cu.  Used for H = 64 unless disabled (B200RL_TC=0 or b200rl_set_tensor_cores(0)).
+// tensor-core (wgmma) variants, nn_tc.cu.  Used for H = 64 unless disabled (B200RL_TC=0 or b200rl_set_tensor_cores(0)).
 bool nn_tc_enabled();
 bool nn_tc_supported(const MlpDesc& d);
 int nn_tc_forward(b200rl_ctx* ctx, int grid, const MlpDesc& actor, const MlpDesc& critic, const float* params, const AcHyper& hp, int mode,

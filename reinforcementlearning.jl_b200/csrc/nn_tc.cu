@@ -1,26 +1,24 @@
-// nn_tc.cu — K7 on tensor cores (tcgen05 / TMEM): PPO / A2C loss + backward for H = 64.
+// nn_tc.cu — K7 on tensor cores (Hopper wgmma): PPO / A2C loss + backward for H = 64.
 //
-// The 64 x 64 layers are [128 samples x 64] x [64 x 64] GEMMs per tile: one warp issues tcgen05.mma (SWIZZLE_NONE canonical
-// layout, see umma.cuh) with the FP32 accumulators in TMEM; the worker warps pull them back with tcgen05.ld.  Parity needs
-// ~FP32 accuracy (1e-5 relative on losses), which no single tensor-core input format gives, so every product is a 3-term split
+// The 64 x 64 layers are [128 samples x 64] x [64 x 64] GEMMs per tile, run by one MMA warpgroup with wgmma (both operands in
+// shared memory, SWIZZLE_NONE canonical layout, see wgmma.cuh) into FP32 registers; it hands the results to the worker warps
+// through shared memory.  Parity needs ~FP32 accuracy (1e-5 relative on losses), which no single tensor-core input format
+// gives, so every product is a 3-term split
 //     A*B ~= A_hi*B_hi + A_hi*B_lo + A_lo*B_hi,   x_hi = fp16(x * S), x_lo = fp16(x * S - x_hi)      (22 mantissa bits)
-// with a power-of-two scale S per operand (exact; undone on the FP32 accumulator), accumulated in FP32.  Round 1 used the same
-// split on kind::tf32 (K = 8 per instruction); kind::f16 covers K = 16 per instruction at the same 2^-22 product accuracy.
-// A tcgen05.mma (M = 128, K = 16) occupies the pipe for 10 + N/2 cycles with A in TMEM and 43 + N/2 with A in shared memory
-// (profiles/umma_pacing.py) PROVIDED it is issued under an elect.sync predicate (umma::elect_one): under `lane == 0` ptxas wraps
-// every MMA in an ELECT / BRA.U.ANY loop that costs ~100 cycles of issue time.  fp16 has 5 exponent bits: activations
+// with a power-of-two scale S per operand (exact; undone on the FP32 accumulator), accumulated in FP32.  fp16 covers K = 16 per
+// instruction at the same 2^-22 product accuracy as a tf32 split at K = 8.  fp16 has 5 exponent bits: activations
 // must stay below 65504 in magnitude (scale 1), weights below 1023 (scale 64); gradients are scaled by ~1/(4 inv_B) at launch.
 // Below 6e-5 the lo part is subnormal: absolute error <= 2^-25 per element, far inside the 1e-5 bar.  Layer 1 (K <= 4) and the
 // heads (N <= 2) stay on FFMA.  The forward-only kernels (policy inference, fused rollout) live in fwd_tc.cu (same split).
 #include "nn.cuh"
 #include "perm.cuh"
 #include "tc_split.h"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int NT = 256;
-constexpr int TM = 128;              // samples per tile = UMMA M
+constexpr int TM = 128;              // samples per tile = two wgmma M = 64 blocks
 constexpr int H = 64;
 constexpr int G_F = 128;             // weight image (fp16, K-major): byte stride between 8-element K chunks = one 8 x 16 B core matrix
 constexpr int GW_S = 8 * G_F;        // stride between 8-row groups (64 K elements = 8 chunks)
@@ -53,47 +51,43 @@ __device__ __forceinline__ int64_t head_b(const MlpDesc& d, int o) {
 __device__ __forceinline__ uint32_t wimg_off(int n, int k) { return (uint32_t)((n >> 3) * GW_S + (k >> 3) * G_F + (n & 7) * 16 + (k & 7) * 2); }
 
 // =====================================================================================================
-// K7 on tensor cores: PPO / A2C loss + backward for one minibatch, all three 64x64 GEMMs on tcgen05.
-//   GEMM1  H2pre[s][o] = sum_i H1[s][i]  W2[o][i]     A = H1 (TMEM, written by tcgen05.st), B = W2 image (smem)
-//   GEMM2  dH1[s][i]   = sum_j dP2[s][j] W2[j][i]     A = dP2 (TMEM),                        B = W2^T image (smem)
-//   GEMM3  dW2[j][i]  += sum_s dP2[s][j] H1[s][i]     A = dP2^T, B = H1^T: feature-major K-major images (smem),
-//                                                     accumulated in TMEM across ALL tiles of the CTA, read once.
-// every product the 3-term fp16 split (hi*hi + hi*lo + lo*hi), FP32 accumulate.
-// One CTA per SM (512 threads, role = blockIdx & 1), persistent, software-pipelined across tiles (see the loop).
-// Thread <-> data: warp w: TMEM lane quadrant q = w % 4, feature block c = w / 4; thread = sample s = 32q + lane.
+// K7 on tensor cores: PPO / A2C loss + backward for one minibatch, all four tile GEMMs on wgmma.
+//   GEMM1  H2pre[s][o] = sum_i H1[s][i]  W2[o][i]     A = H1 image (K-major), B = W2 image (K-major)
+//   GEMM2  dH1[s][i]   = sum_j dP2[s][j] W2[j][i]     A = dP2 image (K-major view of dP2^T), B = the W2 image read MN-major
+//   GEMM3  dW2[j][i]  += sum_s dP2[s][j] H1[s][i]     A = dP2^T, B = [H1^T | ones]: feature-major images (MN-major)
+//   GEMM4  dW1 | db1  += sum_s dP1[s][f] [x | 1][s]   A = dP1^T, B = [x | 1]^T (MN-major)
+// every product the 3-term fp16 split (hi*hi + hi*lo + lo*hi), FP32 accumulate.  GEMM3 / GEMM4 reduce over the tile's samples;
+// the MMA warpgroup adds their results into FP32 shared-memory accumulators (round-to-nearest adds, fixed owner per entry).
+// One CTA per SM (640 threads, actor or critic), persistent, software-pipelined across tiles (see the loop).
+// Thread <-> data (workers): warp w: sample quadrant q = w % 4, feature block c = w / 4; thread = sample s = 32q + lane.
 constexpr int NT7 = 512;
-// Operands of the two GEMMs that reduce over the SAMPLES (GEMM3, GEMM4: K = sample) are MN-major (SWIZZLE_NONE) images: a core
-// matrix is 8 k-rows (samples) x 16 B (8 consecutive features), element (feature f, sample s) at
-//     (f / 8) * GS_T + (s / 8) * GF_T + (s % 8) * 16 + (f % 8) * 2        (descriptor: LBO = GF_T, SBO = GS_T; profiles/umma_probe_mn.py)
-// With GF_T = 128 that is simply [feature block of 8][sample][8 features]: thread = sample writes 8 features as ONE 16-byte
-// vector, and the 32 lanes of a warp cover 512 contiguous bytes (no bank conflicts).  Until round 2 these images were K-major
-// (8 samples x one feature per 16 B): 32 two-byte transposed stores per thread and image, 4.5 M bank conflicts per launch.
-constexpr int GF_T = 128;                 // stride between 8-sample k-blocks
+// The activation images: element (feature f, sample s) at
+//     (f / 8) * GS_T + (s / 8) * GF_T + (s % 8) * 16 + (f % 8) * 2
+// i.e. [feature block of 8][sample][8 features]: thread = sample writes 8 features as ONE 16-byte vector, and the 32 lanes of a
+// warp cover 512 contiguous bytes (no bank conflicts).  Read MN-major (MN = feature, K = sample: LBO = GF_T, SBO = GS_T) they
+// are the operands of GEMM3 / GEMM4; read K-major (M = sample, K = feature: LBO = GS_T, SBO = GF_T) those of GEMM1 / GEMM2.
+constexpr int GF_T = 128;                 // stride between 8-sample groups
 constexpr int GS_T = 16 * GF_T;           // stride between 8-feature blocks (128 samples)
 constexpr int FIMG = 8 * GS_T;            // [64 features x 128 samples] fp16 = 16 KB
-// TMEM columns: R1 = D1 of GEMM1 (64 columns: hi*hi + hi*lo + lo*hi accumulated in place), then (after P3 consumed it) the dP2 A
-// operand of GEMM2 in the same 64 columns (hi: 32 columns of fp16 pairs | lo: 32); D2 = GEMM2 accumulator (64 columns); D3 = GEMM3
-// accumulator (all tiles; hi|lo operands stacked along M and N, one MMA per K step); AH = H1 A operand of GEMM1 (hi 32 | lo 32).
-// D3 has 144 columns: the B operand of GEMM3 carries a constant "ones" row behind H1^T, so column 128 is sum_s dP2 = db2.
-// D4 = GEMM4 accumulator (16 columns): dW1 | db1 = dP1^T x [x | 1], accumulated over all tiles like D3.
-constexpr uint32_t COL_R1 = 0, COL_D2 = 128, COL_D3 = 256, COL_D4 = 400, COL_AH = 448;
 constexpr float kScaleH = 64.0f, kScaleX = 64.0f;   // power-of-two scales of the H1 / observation operands (weights: kScaleW)
 constexpr int kNo = 2;   // head outputs this kernel handles (nn_tc_bwd_supported: actor n_out <= 2, critic n_out = 1)
 
 struct SmemBwd {
-    static_assert(FIMG % 128 == 0 && WIMG_BYTES % 128 == 0 && (2 * GS_T) % 16 == 0, "hi/lo(/ones) images must be adjacent to form one operand");
+    static_assert(FIMG % 128 == 0 && WIMG_BYTES % 128 == 0 && (2 * GS_T) % 16 == 0, "operand images must stay 128-byte aligned");
     alignas(128) uint8_t FP_full[FIMG];    // dP2^T hi (rows = feature j, K = sample), fp16
-    alignas(128) uint8_t FP_lo[FIMG];      // ... lo: directly behind, so [hi; lo] is one 128-row operand
+    alignas(128) uint8_t FP_lo[FIMG];
+    alignas(128) uint8_t FH_lo[FIMG];      // H1^T lo
     alignas(128) uint8_t FH_full[FIMG];    // H1^T hi
-    alignas(128) uint8_t FH_lo[FIMG];
-    alignas(16) uint8_t FH_ones[2 * GS_T]; // 16 more B rows (features 128..143) of GEMM3: feature 128 = 1.0 for every sample (-> db2), the rest 0; written once
+    alignas(16) uint8_t FH_ones[2 * GS_T]; // B operand of the db2 GEMM: feature 0 = 1.0 for every sample, the rest 0; written once
     alignas(128) uint8_t FQ_full[FIMG];    // dP1^T hi | lo: A operand of GEMM4
     alignas(128) uint8_t FQ_lo[FIMG];
     alignas(128) uint8_t B1[WIMG_BYTES];   // rows 0..63: hi, 64..127: lo of (n = out o, k = in i)  = 64 W2[o + 64 i]
-    alignas(128) uint8_t B2[WIMG_BYTES];   // (n = in i,  k = out j) = 64 W2[j + 64 i]
     // B operand of GEMM4, double-buffered by tile parity (written at publish time, read by the GEMM4 of the same tile one
-    // phase later): rows 0..3 = x_i hi, row 4 = 1.0 (-> db1), rows 8..11 = x_i lo, the rest 0;  K = sample
+    // phase later): features 0..3 = x_i hi, 4 = 1.0 (-> db1), 8..11 = x_i lo, the rest 0;  K = sample
     alignas(128) uint8_t XT[2][2 * GS_T];
+    alignas(128) uint8_t AH_full[FIMG];    // H1 hi | lo of the tile GEMM1 runs on (same layout as FH)
+    alignas(128) uint8_t AH_lo[FIMG];
+    alignas(16) float D[TM * H];           // FP32 result of GEMM1 or GEMM2 for the workers (d_off layout)
     float W1[kInMax * H];
     float b1[H], b2[H];
     float W3[H * kNo];                     // [feature][head output]
@@ -106,10 +100,36 @@ struct SmemBwd {
     alignas(8) uint64_t bar2;
     alignas(8) uint64_t bar3;
     alignas(8) uint64_t bar4;
-    float AccW2[64 * 65 + 64];             // FP32 accumulators the flushes add D3 into: dW2[j][i] at j * 65 + i, then db2[j] (all still operand-scaled)
-    float AccD4[64 * 9];                   // ... D4: dW1[f][i] at f * 9 + i, db1[f] at f * 9 + 4
-    uint32_t tmem;
+    float AccW2[64 * 65 + 64];             // FP32 accumulators of GEMM3: dW2[j][i] at j * 65 + i, then db2[j] (all still operand-scaled)
+    float AccD4[64 * 9];                   // ... of GEMM4: dW1[f][i] at f * 9 + i, db1[f] at f * 9 + 4
 };
+// D[s][col] (floats): 16-byte units XOR-swizzled by the sample, so that 8 consecutive samples read at the same column hit 8
+// different bank groups
+__device__ __forceinline__ int d_off(int s, int col) { return s * H + ((((col >> 2) ^ (s & 15))) << 2) + (col & 3); }
+__device__ __forceinline__ void d_ld16(const float* D, int s, int f0, float (&v)[16]) {
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+        const float4 q4 = *reinterpret_cast<const float4*>(D + d_off(s, f0 + 4 * u));
+        v[4 * u] = q4.x; v[4 * u + 1] = q4.y; v[4 * u + 2] = q4.z; v[4 * u + 3] = q4.w;
+    }
+}
+// MMA warpgroup: samples 64h .. 64h+63 of a [128 samples x 64] A image pair (hi, lo; K-major view of an F image) times the W2
+// image (TB = 0: K-major, GEMM1; TB = 1: MN-major, GEMM2; b_step = bytes its descriptor advances per K = 16 step), the three
+// split terms accumulated into the same registers
+template <int TB>
+__device__ __forceinline__ void gemm_ts3(float (&d)[32], const uint8_t* a_hi, const uint8_t* a_lo, int h, uint64_t dB, uint32_t b_step) {
+    const uint64_t dA = wg::make_desc(wg::smem_u32(a_hi) + 8 * h * GF_T, GS_T, GF_T), dAl = wg::make_desc(wg::smem_u32(a_lo) + 8 * h * GF_T, GS_T, GF_T);
+    wg::fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint32_t aa = k * 2 * GS_T, bb = k * b_step;
+        wg::mma_m64n64k16<0, TB>(d, wg::desc_add(dA, aa), wg::desc_add(dB, bb), k ? 1u : 0u);
+        wg::mma_m64n64k16<0, TB>(d, wg::desc_add(dA, aa), wg::desc_add(dB, 8 * GW_S + bb), 1u);   // W2 lo: rows 64..127 of the image
+        wg::mma_m64n64k16<0, TB>(d, wg::desc_add(dAl, aa), wg::desc_add(dB, bb), 1u);
+    }
+    wg::commit();
+    wg::wait_all();
+}
 __device__ __forceinline__ uint32_t fimg_off(int f, int s) { return (uint32_t)((f >> 3) * GS_T + (s >> 3) * GF_T + (s & 7) * 16 + (f & 7) * 2); }
 // 16 features (8 packed fp16 pairs) of sample s, starting at feature f0 (a multiple of 16): two 16-byte vectors
 __device__ __forceinline__ void store16_feat(uint8_t* img, int f0, int s, const uint32_t (&v)[8]) {
@@ -155,16 +175,16 @@ __device__ __forceinline__ float lane_transpose_reduce32(float (&v)[32], int lan
     return v[0];   // value index = lane
 }
 
-// worker-only barrier (the MMA warp never joins it)
+// worker-only barrier (the MMA warpgroup never joins it)
 __device__ __forceinline__ void worker_sync() { asm volatile("bar.sync 1, 512;" ::: "memory"); }
-// barrier of the four warps that share one TMEM lane quadrant q (= one 32-sample slice of the tile, feature blocks c = 0..3).
-// Everything the workers exchange per tile (X, Aux, Zp, the TMEM columns of a lane) is exchanged between the four threads of ONE
+// barrier of the four warps that share one sample quadrant q (= one 32-sample slice of the tile, feature blocks c = 0..3).
+// Everything the workers exchange per tile (X, Aux, Zp, the D entries of a sample) is exchanged between the four threads of ONE
 // sample, i.e. inside such a group, so the per-tile barriers are group-local (ids 5..8, 128 threads) and the four groups — one
 // per warp scheduler — drift freely within a tile; the tensor-core hand-overs (bar.arrive) and the mbarrier waits bound the drift.
 __device__ __forceinline__ void group_sync(int q) { asm volatile("bar.sync %0, 128;" ::"r"(5 + q) : "memory"); }
-// operand hand-over to the issuer warp: 512 worker threads arrive without waiting, the 32 issuer threads wait
-__device__ __forceinline__ void ready_arrive(int id) { asm volatile("bar.arrive %0, 544;" ::"r"(id) : "memory"); }
-__device__ __forceinline__ void ready_wait(int id) { asm volatile("bar.sync %0, 544;" ::"r"(id) : "memory"); }
+// operand hand-over to the MMA warpgroup: 512 worker threads arrive without waiting, its 128 threads wait
+__device__ __forceinline__ void ready_arrive(int id) { asm volatile("bar.arrive %0, 640;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void ready_wait(int id) { asm volatile("bar.sync %0, 640;" ::"r"(id) : "memory"); }
 // per-sample loss and d(loss)/d(head outputs); identical arithmetic on every thread that evaluates a sample
 struct LossOut { float dz[kNo]; float l0, l1; };
 __device__ __forceinline__ LossOut sample_loss(const MlpDesc& actor, int role, const AcHyper& hp, float inv_B, const float (&z)[kNo],
@@ -248,27 +268,21 @@ __device__ __forceinline__ LossOut sample_loss(const MlpDesc& actor, int role, c
     return r;
 }
 
-#ifdef B200RL_K7_TIMING   // debug build only (profiles/k7_phase_timing.py): per-phase cycle sums seen by CTA 0 / one watched thread
+#ifdef B200RL_K7_TIMING   // debug build only: per-phase cycle sums seen by one watched worker thread
 __device__ unsigned long long g_k7_phase[40];
-__device__ int g_k7_watch = 0;   // watched worker thread (low 16 bits) of CTA (high bits; even = actor, odd = critic) whose timeline is recorded
+__device__ int g_k7_watch = 0;   // watched worker thread (low 16 bits) of CTA (high bits; CTAs below n_actor = actor) whose timeline is recorded
 #define K7_T(i) do { if (tid == (g_k7_watch & 0xFFFF) && (int)blockIdx.x == (g_k7_watch >> 16)) { long long now_ = clock64(); g_k7_phase[i] += (unsigned long long)(now_ - tprev_); tprev_ = now_; } } while (0)
-// issuer warp of CTA 0 (lane 0): phases 18..23 = wait RdyA | issue G2 | wait RdyB | issue G1 + G3 | wait RdyC | issue G4
-#define K7_TI(i) do { if (lane == 0 && (int)blockIdx.x == (g_k7_watch >> 16)) { long long now_ = clock64(); g_k7_phase[i] += (unsigned long long)(now_ - tprevi_); tprevi_ = now_; } } while (0)
 #else
 #define K7_T(i) do { } while (0)
-#define K7_TI(i) do { } while (0)
 #endif
-// 16 worker warps + one warpgroup (warps 16..19) whose first warp feeds the tensor core.  The issuing thread blocks once the MMA
-// queue is full (the issue side of a GEMM takes as long as its execution), which used to stall a worker warp — and with it
-// everybody at the next barrier.  The register file is per scheduler (16 K registers, 5 warps
-// each now), so the issuer warpgroup gives its registers back (setmaxnreg.dec 24) and the workers take 120 (setmaxnreg.inc).
+// 16 worker warps + one MMA warpgroup (warps 16..19) that runs every wgmma: wgmma accumulators are registers of the warpgroup that
+// issues it, so the GEMMs sit on their own warpgroup and the workers never wait for the tensor core except where they need a result.
+// 640 threads leave 96 registers a thread; the MMA warpgroup holds at most one 64 x 64 accumulator (32 registers) at a time and
+// gives registers back (setmaxnreg.dec 64) so that the workers can take 104 (setmaxnreg.inc): 128 x 64 + 512 x 104 = 640 x 96.
 constexpr int NT7_ALL = NT7 + 128;
-// The tensor core adds into an FP32 accumulator with truncation: a chain of n accumulating MMAs biases a same-signed sum by
-// ~n * 2^-25 relative (measured: 1e-4 on b1 / W2 gradients after 1 770 adds, profiles/k7_grad_error.py).  The accumulators that live
-// across tiles (D3, D4) are therefore flushed into FP32 shared-memory accumulators (round-to-nearest adds) every kFlushTiles
-// tiles and restarted: chains of 64 adds, bias ~2e-6.
-constexpr int kFlushTiles = 8;
-constexpr int kBarRdyA = 2, kBarRdyB = 3, kBarRdyC = 4;   // named barriers: workers arrive (bar.arrive), the issuer warp waits (bar.sync)
+constexpr int kRegsMma = 64, kRegsWorker = 104;
+static_assert(128 * kRegsMma + NT7 * kRegsWorker <= NT7_ALL * 96, "setmaxnreg split must fit the CTA's register allocation");
+constexpr int kBarRdyA = 2, kBarRdyB = 3, kBarRdyC = 4;   // named barriers: workers arrive (bar.arrive), the MMA warpgroup waits (bar.sync)
 
 // ACT: the trunks' activation as a compile-time constant (B200RL_ACT_RELU / B200RL_ACT_TANH; -1 = read it from the descriptors, for
 // an actor and a critic with different activations).  With the activation known the relu build carries no tanhf expansions at
@@ -281,8 +295,8 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
                        int n_actor /* CTAs [0, n_actor) work on the actor, the rest on the critic */) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     SmemBwd& sm = *reinterpret_cast<SmemBwd*>(smem_raw);
-    // The actor's loss (softmax / Gaussian log-density, entropy, PPO ratio) makes its tiles ~4 % longer than the critic's, so the CTAs
-    // are split unevenly (76 : 72 of 148 for the categorical PPO loss) and both roles finish together.  Gradient partials: row
+    // The actor's loss (softmax / Gaussian log-density, entropy, PPO ratio) makes its tiles longer than the critic's, so the CTAs
+    // are split unevenly (tc_split.h) and both roles finish together.  Gradient partials: row
     // `cta` holds the actor half written by actor CTA `cta` and the critic half written by critic CTA `cta`; the role with more
     // CTAs zero-fills the other half of its surplus rows.
     const int role = (int)blockIdx.x < n_actor ? 0 : 1;
@@ -320,118 +334,127 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             const __half wh = __float2half_rn(w), wl = __float2half_rn(w - __half2float(wh));
             *reinterpret_cast<__half*>(sm.B1 + wimg_off(o, i)) = wh;
             *reinterpret_cast<__half*>(sm.B1 + wimg_off(H + o, i)) = wl;
-            *reinterpret_cast<__half*>(sm.B2 + wimg_off(i, o)) = wh;
-            *reinterpret_cast<__half*>(sm.B2 + wimg_off(H + i, o)) = wl;
         }
     }
-    // constant operand rows of GEMM3's B: feature 128 = 1.0 (fp16 0x3C00) for every sample, 129..143 = 0 (the XT buffers are written whole by publish())
+    // constant B operand of the db2 GEMM: feature 0 = 1.0 (fp16 0x3C00) for every sample, the rest 0 (the XT buffers are written whole by publish())
     for (int k = tid; k < 2 * TM; k += NT7_ALL)
         *reinterpret_cast<uint4*>(sm.FH_ones + 16 * k) = make_uint4(k < TM ? 0x3C00u : 0u, 0u, 0u, 0u);
-    if (warp == 0) umma::tmem_alloc(&sm.tmem, 512);
-    if (tid == 32) {
-        umma::mbar_init(&sm.bar1, 1); umma::mbar_init(&sm.bar2, 1); umma::mbar_init(&sm.bar3, 1); umma::mbar_init(&sm.bar4, 1);
+    if (tid == 32) {   // every thread of the MMA warpgroup arrives once per phase
+        wg::mbar_init(&sm.bar1, 128); wg::mbar_init(&sm.bar2, 128); wg::mbar_init(&sm.bar3, 128); wg::mbar_init(&sm.bar4, 128);
     }
-    umma::fence_proxy_async();
-    umma::fence_before_sync();
+    wg::fence_proxy_async();
     __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem = sm.tmem;
-    const uint32_t idesc = umma::make_idesc_f16(128, 64, 0, 0), idesc128 = umma::make_idesc_f16(128, 128, 0, 0);
-    const uint32_t idesc144 = umma::make_idesc_f16(128, 144, 1, 1), idesc16 = umma::make_idesc_f16(128, 16, 1, 1);   // GEMM3 / GEMM4: MN-major A and B
     // undo the operand scales (exact powers of two): D1 = H1 W2, D2 = dP2 W2, D3 = dP2^T [H1 | 1], D4 = dP1^T [x | 1]
-    const float inv_s1 = 1.0f / (kScaleH * kScaleW), inv_s2 = 1.0f / (scale_p * kScaleW), inv_s3 = 1.0f / (scale_p * kScaleH), inv_sp = 1.0f / scale_p,
-                inv_s4 = 1.0f / (scale_p * kScaleX);
+    const float inv_s1 = 1.0f / (kScaleH * kScaleW), inv_s3 = 1.0f / (scale_p * kScaleH), inv_sp = 1.0f / scale_p, inv_s4 = 1.0f / (scale_p * kScaleX);
     const int64_t ntiles = (b.B + TM - 1) / TM;
 
-    const uint64_t dB1f = umma::make_desc(umma::smem_u32(sm.B1), G_F, GW_S);
-    const uint64_t dB2f = umma::make_desc(umma::smem_u32(sm.B2), G_F, GW_S);
-    const uint64_t dFPf = umma::make_desc(umma::smem_u32(sm.FP_full), GF_T, GS_T);
-    const uint64_t dFHf = umma::make_desc(umma::smem_u32(sm.FH_full), GF_T, GS_T);
-    const uint64_t dFQf = umma::make_desc(umma::smem_u32(sm.FQ_full), GF_T, GS_T);
     if (warp >= NT7 / 32) {
-        // ================= issuer warpgroup: warp 16 feeds the tensor core, warps 17..19 only return their registers ====
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
-        if (warp == NT7 / 32) {
-            // 3-term product of a TMEM A operand (hi fp16 pairs at a_col, lo at a_col + 32; 8 columns per K = 16 step) with a
-            // [B_hi ; B_lo] weight image, all three terms accumulated into the SAME 64 columns: hi*hi, hi*lo, lo*hi (three N = 64
-            // MMAs per K step, ~42 cycles each, instead of one N = 128 + one N = 64: the same pipe time, but the workers read back
-            // 64 accumulator columns instead of 128 and add nothing)
-            auto issue_ts3 = [&](uint32_t d_col, uint32_t a_col, uint64_t dB) {
-                const uint64_t dBlo = dB + (uint64_t)((8 * GW_S) >> 4);   // rows 64..127 of the image
+        // ================= MMA warpgroup ================================================================================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsMma));
+        const int t = tid - NT7, row0 = 16 * (t >> 5) + ((t & 31) >> 2), col0 = 2 * (t & 3);   // accumulator fragment (wgmma.cuh)
+        const uint64_t dB1k = wg::make_desc(wg::smem_u32(sm.B1), G_F, GW_S);   // W2 image K-major (n = o, k = i): GEMM1
+        const uint64_t dB1t = wg::make_desc(wg::smem_u32(sm.B1), GW_S, G_F);   // the same bytes MN-major (n = i, k = o): GEMM2
+        float dacc[32];
+        auto store_d = [&](int h) {   // GEMM1 / GEMM2 result of samples 64h .. 64h+63 -> D
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const uint64_t adv = (uint64_t)(k * (2 * G_F / 16));
-                    umma::mma_f16_ts(tmem + d_col, tmem + a_col + 8 * k, dB + adv, idesc, k ? 1u : 0u);
-                    umma::mma_f16_ts(tmem + d_col, tmem + a_col + 8 * k, dBlo + adv, idesc, 1u);
-                    umma::mma_f16_ts(tmem + d_col, tmem + a_col + 32 + 8 * k, dB + adv, idesc, 1u);
-                }
-            };
-            // GEMM3 (dW2 += dP2^T x H1, K = 128 samples), ONE M = 128 x N = 128 MMA per K = 16 step: FP_full|FP_lo are adjacent row
-            // groups (A rows 0..63 = hi, 64..127 = lo) and FH_full|FH_lo adjacent column groups, so D3[0:64][0:64] = hi*hi,
-            // D3[0:64][64:128] = hi*lo, D3[64:128][0:64] = lo*hi (and lo*lo, unused).
-            uint32_t d3_acc = 0u;
-            auto issue_g3 = [&]() {
+            for (int j = 0; j < 8; ++j)
 #pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                    const uint64_t adt = (uint64_t)(k * (2 * GF_T / 16));
-                    umma::mma_f16(tmem + COL_D3, dFPf + adt, dFHf + adt, idesc144, k ? 1u : d3_acc);   // N = 144: [H1^T hi | H1^T lo | ones]
-                }
-            };
-            // GEMM4 (dW1 | db1 += dP1^T x [x | 1], K = 128 samples): A rows 0..63 = hi, 64..127 = lo; B columns 0..7 = [x hi, 1], 8..15 = x lo
-            uint32_t d4_acc = 0u;
-            auto issue_g4 = [&](int buf) {
-                const uint64_t dXT = umma::make_desc(umma::smem_u32(sm.XT[buf]), GF_T, GS_T);
+                for (int hh = 0; hh < 2; ++hh)
+                    *reinterpret_cast<float2*>(sm.D + d_off(64 * h + row0 + 8 * hh, 8 * j + col0)) = make_float2(dacc[4 * j + 2 * hh], dacc[4 * j + 2 * hh + 1]);
+        };
+        auto gemm1 = [&](int h) { gemm_ts3<0>(dacc, sm.AH_full, sm.AH_lo, h, dB1k, 2 * G_F); };
+        auto gemm2 = [&](int h) { gemm_ts3<1>(dacc, sm.FP_full, sm.FP_lo, h, dB1t, 2 * GW_S); };   // dH1 = dP2 x W2
+        // GEMM3 (K = 128 samples, M = 64 features j): dP2^T hi x H1^T hi, lo x hi and hi x lo into one accumulator, then
+        // [dP2^T hi | lo] x ones = sum_s dP2 = db2 (column 0 of an N = 8 accumulator).  Added into AccW2 by the fragment's owner thread.
+        auto gemm3 = [&]() {
+            const uint64_t dPh = wg::make_desc(wg::smem_u32(sm.FP_full), GF_T, GS_T), dPl = wg::make_desc(wg::smem_u32(sm.FP_lo), GF_T, GS_T);
+            const uint64_t dHh = wg::make_desc(wg::smem_u32(sm.FH_full), GF_T, GS_T), dHl = wg::make_desc(wg::smem_u32(sm.FH_lo), GF_T, GS_T);
+            wg::fence();
 #pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                    const uint64_t adt = (uint64_t)(k * (2 * GF_T / 16));
-                    umma::mma_f16(tmem + COL_D4, dFQf + adt, dXT + adt, idesc16, k ? 1u : d4_acc);
-                }
-            };
-            // One warp issues every MMA (its elected lane: umma::elect_one), so the tensor pipe executes them in program order: G2(t)
-            // reads R1 before G1(t+1) overwrites it without any cross-thread fence.  Per tile: G2(t) | G1(t+1) | G3(t) | G4(t).
-            // d3_acc / d4_acc are warp-uniform (every lane tracks them).
-            if (cta < ntiles) {
-                ready_wait(kBarRdyB);                      // H1 operand of the first tile is in TMEM
-                umma::fence_after_sync();
-                if (umma::elect_one()) { issue_ts3(COL_R1, COL_AH, dB1f); umma::commit(&sm.bar1); }
-                __syncwarp();
+            for (int k = 0; k < 8; ++k) {
+                const uint32_t a = k * 2 * GF_T;
+                wg::mma_m64n64k16<1, 1>(dacc, wg::desc_add(dPh, a), wg::desc_add(dHh, a), k ? 1u : 0u);
+                wg::mma_m64n64k16<1, 1>(dacc, wg::desc_add(dPl, a), wg::desc_add(dHh, a), 1u);
+                wg::mma_m64n64k16<1, 1>(dacc, wg::desc_add(dPh, a), wg::desc_add(dHl, a), 1u);
             }
-            int buf = 0, ord = 0;     // ord = ordinal of the tile within this CTA (the workers count the same way)
-#ifdef B200RL_K7_TIMING
-            long long tprevi_ = clock64();
-#endif
-            for (int64_t tile = cta; tile < ntiles; tile += nctas, buf ^= 1, ++ord) {
-                if (ord % kFlushTiles == 0) { d3_acc = 0u; d4_acc = 0u; }   // the workers have flushed D3 / D4 before handing this tile's operands over
-                ready_wait(kBarRdyA);                      // dP2 operand (TMEM) and the dP2^T / H1^T images (smem) of this tile
-                umma::fence_after_sync();
-                K7_TI(18);
-                if (umma::elect_one()) { issue_ts3(COL_D2, COL_R1, dB2f); umma::commit(&sm.bar2); }      // GEMM2: dH1 = dP2 x W2
-                __syncwarp();
-                K7_TI(19);
-                if (tile + nctas < ntiles) {
-                    ready_wait(kBarRdyB);                  // H1 operand of the next tile
-                    umma::fence_after_sync();
-                    K7_TI(20);
-                    if (umma::elect_one()) { issue_ts3(COL_R1, COL_AH, dB1f); umma::commit(&sm.bar1); }  // GEMM1 of the next tile
-                    __syncwarp();
-                }
-                if (umma::elect_one()) { issue_g3(); umma::commit(&sm.bar3); }                   // GEMM3 of this tile
-                d3_acc = 1u;
-                __syncwarp();
-                K7_TI(21);
-                ready_wait(kBarRdyC);                      // dP1^T image of this tile (its x^T | 1 operand was written at publish time)
-                umma::fence_after_sync();
-                K7_TI(22);
-                if (umma::elect_one()) { issue_g4(buf); umma::commit(&sm.bar4); }                // GEMM4 of this tile
-                d4_acc = 1u;
-                __syncwarp();
-                K7_TI(23);
+            wg::commit();
+            wg::wait_all();
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) sm.AccW2[(row0 + 8 * hh) * 65 + 8 * j + col0 + e] += dacc[4 * j + 2 * hh + e];
+            const uint64_t dOnes = wg::make_desc(wg::smem_u32(sm.FH_ones), GF_T, GS_T);
+            float d8[4] = {0.f, 0.f, 0.f, 0.f};
+            wg::fence();
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const uint32_t a = k * 2 * GF_T;
+                wg::mma_m64n8k16<1, 1>(d8, wg::desc_add(dPh, a), wg::desc_add(dOnes, a), k ? 1u : 0u);
+                wg::mma_m64n8k16<1, 1>(d8, wg::desc_add(dPl, a), wg::desc_add(dOnes, a), 1u);
             }
+            wg::commit();
+            wg::wait_all();
+            if (col0 == 0) {
+                sm.AccW2[64 * 65 + row0] += d8[0];
+                sm.AccW2[64 * 65 + row0 + 8] += d8[2];
+            }
+        };
+        // GEMM4 (K = 128 samples, M = 64 features f): dP1^T hi x [x hi, 1], hi x x lo, lo x [x hi, 1]; columns 0..3 = dW1, 4 = db1
+        auto gemm4 = [&](int buf) {
+            const uint64_t dQh = wg::make_desc(wg::smem_u32(sm.FQ_full), GF_T, GS_T), dQl = wg::make_desc(wg::smem_u32(sm.FQ_lo), GF_T, GS_T);
+            const uint64_t dX = wg::make_desc(wg::smem_u32(sm.XT[buf]), GF_T, GS_T);
+            float d4[4] = {0.f, 0.f, 0.f, 0.f};
+            wg::fence();
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const uint32_t a = k * 2 * GF_T;
+                wg::mma_m64n8k16<1, 1>(d4, wg::desc_add(dQh, a), wg::desc_add(dX, a), k ? 1u : 0u);
+                wg::mma_m64n8k16<1, 1>(d4, wg::desc_add(dQh, a), wg::desc_add(dX, GS_T + a), 1u);
+                wg::mma_m64n8k16<1, 1>(d4, wg::desc_add(dQl, a), wg::desc_add(dX, a), 1u);
+            }
+            wg::commit();
+            wg::wait_all();
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+                for (int e = 0; e < 2; ++e)
+                    if (col0 + e < 5) sm.AccD4[(row0 + 8 * hh) * 9 + col0 + e] += d4[2 * hh + e];
+        };
+        // Per tile: G2(t) | G3(t) | G1(t+1), samples 0..63 (held in registers) | G1(t+1), samples 64..127 | G4(t).  D holds one
+        // result at a time: D2(t) is read by the workers' P7(t), so D1(t+1) is stored once they have handed over RdyC(t), which
+        // they do after P7(t).
+        if (cta < ntiles) {
+            ready_wait(kBarRdyB);                      // H1 operand of the first tile
+            for (int h = 0; h < 2; ++h) { gemm1(h); store_d(h); }
+            wg::mbar_arrive(&sm.bar1);
+        }
+        int buf = 0;
+        for (int64_t tile = cta; tile < ntiles; tile += nctas, buf ^= 1) {
+            const bool has_next = tile + nctas < ntiles;
+            ready_wait(kBarRdyA);                      // dP2 / H1^T images of this tile; the workers have read D1(t)
+            for (int h = 0; h < 2; ++h) { gemm2(h); store_d(h); }
+            wg::mbar_arrive(&sm.bar2);
+            gemm3();
+            wg::mbar_arrive(&sm.bar3);
+            if (has_next) {
+                ready_wait(kBarRdyB);                  // H1 operand of the next tile
+                gemm1(0);                              // GEMM1 of the next tile, first half
+            }
+            ready_wait(kBarRdyC);                      // dP1^T image of this tile (its x^T | 1 operand was written at publish time); D2 read
+            if (has_next) {
+                store_d(0);
+                gemm1(1);
+                store_d(1);
+                wg::mbar_arrive(&sm.bar1);
+            }
+            gemm4(buf);
+            wg::mbar_arrive(&sm.bar4);
         }
     } else {
     // ================= 16 worker warps =======================================================================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 112;");
-    const uint32_t lane_base = (uint32_t)(32 * q) << 16;
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsWorker));
     // persistent per-thread gradient partials (over this thread's sample slot), reduced once at the end
     float g3[2][16];                  // dW3[o][16c + k]   (db2, dW1, db1 and dW2 are reduced over the samples by the tensor core)
     float gb3a0 = 0.f, gb3a1 = 0.f;   // (c == 0 threads) sum_s dz[o]
@@ -487,56 +510,11 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
     float* const gb2 = gW2 + (int64_t)H * H;
     for (int k = tid; k < 64 * 65 + 64; k += NT7) sm.AccW2[k] = 0.f;
     for (int k = tid; k < 64 * 9; k += NT7) sm.AccD4[k] = 0.f;
-    // flush D3 (dW2 | db2) / D4 (dW1 | db1) into the shared-memory accumulators and let the issuer restart them (see kFlushTiles).
-    // Rows 0..63 of an accumulator (hi rows of the A operand) go first, rows 64..127 (lo rows) after a barrier: two threads per
-    // entry, in a fixed order => deterministic.  (Stride 65 / 9: the 32 lanes of a warp hit 32 different banks.)
-    auto flush_d3 = [&]() {
-        if (q < 2) {
-            float v[16], v2[16];
-            umma::tmem_ld16x2(tmem + lane_base + COL_D3 + 16 * c, tmem + lane_base + COL_D3 + 64 + 16 * c, v, v2);
-#pragma unroll
-            for (int k = 0; k < 16; ++k) sm.AccW2[s * 65 + 16 * c + k] += v[k] + v2[k];
-            if (c == 0) {
-                umma::tmem_ld16(tmem + lane_base + COL_D3 + 128, v);
-                sm.AccW2[64 * 65 + s] += v[0];
-            }
-        }
-        worker_sync();
-        if (q >= 2) {
-            float v[16];
-            umma::tmem_ld16(tmem + lane_base + COL_D3 + 16 * c, v);
-#pragma unroll
-            for (int k = 0; k < 16; ++k) sm.AccW2[(s - 64) * 65 + 16 * c + k] += v[k];
-            if (c == 0) {
-                umma::tmem_ld16(tmem + lane_base + COL_D3 + 128, v);
-                sm.AccW2[64 * 65 + (s - 64)] += v[0];
-            }
-        }
-        umma::fence_before_sync();
-    };
-    auto flush_d4 = [&]() {
-        if (c == 0 && q < 2) {
-            float d4[16];
-            umma::tmem_ld16(tmem + lane_base + COL_D4, d4);
-#pragma unroll
-            for (int i = 0; i < kInMax; ++i) sm.AccD4[s * 9 + i] += d4[i] + d4[8 + i];
-            sm.AccD4[s * 9 + 4] += d4[4];
-        }
-        worker_sync();
-        if (c == 0 && q >= 2) {
-            float d4[16];
-            umma::tmem_ld16(tmem + lane_base + COL_D4, d4);
-#pragma unroll
-            for (int i = 0; i < 5; ++i) sm.AccD4[(s - 64) * 9 + i] += d4[i];
-        }
-        umma::fence_before_sync();
-    };
-    int ord = 0;   // ordinal of the current tile within this CTA
     // ---- software pipeline (one tile = 128 samples; tensor core and CUDA cores work on different tiles / phases) ----
-    //   CUDA cores : ... P3(t) P45(t) | P0(t+1) P1(t+1) | P7(t) | P3(t+1) ...
-    //   tensor core:              G2(t) ......... G1(t+1) .... G3(t) .....
-    // G2(t) runs under P0/P1(t+1), G1(t+1) under P7(t), G3(t) under P3/P45(t+1); the issuer warp queues each GEMM as soon
-    // as the workers have handed its operands over (ready_arrive), so no worker ever blocks on the MMA queue.
+    //   workers        : ... P3(t) P45(t) | P0(t+1) P1(t+1) | P7(t) | P3(t+1) ...
+    //   MMA warpgroup  :              G2(t) G3(t) ..... G1(t+1) ........ G4(t) ...
+    // G2(t) / G3(t) run under P0/P1(t+1), G1(t+1) under P7(t), G4(t) under P3(t+1); the MMA warpgroup starts each GEMM as soon
+    // as the workers have handed its operands over (ready_arrive), so no worker waits for a GEMM whose result it does not need.
     // P0: the next tile's records leave the prefetch registers (x -> layer 1 and the x^T operand of GEMM4, scalars -> aux),
     // the records of the tile after it are requested, the index of the one after that computed / requested
     float xo[kInMax];
@@ -562,7 +540,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         K7_T(17);
     };
     uint32_t h1pos = 0, h1pos_tile = 0;   // relu: bit k = (H1[16c + k] > 0) of the tile layer1() ran on last / of the tile P7 works on
-    auto layer1 = [&]() {   // P1: H1 = act(W1 x + b1) -> TMEM A operand (hi | lo fp16 pairs)
+    auto layer1 = [&]() {   // P1: H1 = act(W1 x + b1) -> A operand of GEMM1 (hi | lo fp16 images)
         uint32_t pos = 0;
         uint32_t hi8[8], lo8[8];
 #pragma unroll
@@ -586,16 +564,15 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             split2(h[2], h[3], hi8[2 * ch + 1], lo8[2 * ch + 1]);
         }
         h1pos = pos;
-        umma::tmem_st8(tmem + lane_base + COL_AH + 8 * c, hi8);
-        umma::tmem_st8(tmem + lane_base + COL_AH + 32 + 8 * c, lo8);
-        umma::tmem_st_wait();
+        store16_feat(sm.AH_full, 16 * c, s, hi8);
+        store16_feat(sm.AH_lo, 16 * c, s, lo8);
     };
-    if (cta < ntiles) {   // prologue: P0 / P1 of the first tile (the issuer queues its G1)
+    if (cta < ntiles) {   // prologue: P0 / P1 of the first tile (the MMA warpgroup runs its G1)
         request(index_of(cta), pfx, pfa);
         gi_next = index_of(cta + nctas);
         publish(cta);
         layer1();
-        umma::fence_before_sync();
+        wg::fence_proxy_async();
         ready_arrive(kBarRdyB);
     }
 #ifdef B200RL_K7_TIMING
@@ -604,14 +581,13 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
     for (int64_t tile = cta; tile < ntiles; tile += nctas) {
         const bool has_next = tile + nctas < ntiles;
         // ---- P3: H2 = act(D1 + b2) (registers) + head partials ---------------------------------------
-        umma::mbar_wait(&sm.bar1, ph1);
+        wg::mbar_wait(&sm.bar1, ph1);
         ph1 ^= 1u;
-        umma::fence_after_sync();
         K7_T(0);
         float h2[16];
         {
             float v[16];
-            umma::tmem_ld16(tmem + lane_base + COL_R1 + 16 * c, v);
+            d_ld16(sm.D, s, 16 * c, v);
             float zp[kNo] = {0.f, 0.f};
 #pragma unroll
             for (int k = 0; k < 16; ++k) {
@@ -627,8 +603,8 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         group_sync(q);
         K7_T(2);
         // ---- P4+P5: loss (evaluated by all four feature-block threads of a sample: no exchange, no idle warps),
-        //            dW3 / db2 partials, dP2 = (W3^T dz) .* act'(H2) -> TMEM A operand (over D1, which this thread
-        //            has just consumed) + dP2^T / H1^T images for GEMM3 ----------------------------------------------
+        //            dW3 / db2 partials, dP2 = (W3^T dz) .* act'(H2) -> dP2^T image (A operand of GEMM2 and GEMM3) and
+        //            the H1^T image for GEMM3 -------------------------------------------------------------------------
         {
             float z[kNo];
 #pragma unroll
@@ -655,28 +631,26 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             uint32_t hi8[8], lo8[8];
 #pragma unroll
             for (int m = 0; m < 8; ++m) split2(dp[2 * m], dp[2 * m + 1], hi8[m], lo8[m]);
-            umma::tmem_st8(tmem + lane_base + COL_R1 + 8 * c, hi8);
-            umma::tmem_st8(tmem + lane_base + COL_R1 + 32 + 8 * c, lo8);
             K7_T(3);
-            if (gemm3_pending) {   // the previous tile's GEMM3 must have consumed the images before they are overwritten
-                umma::mbar_wait(&sm.bar3, ph3);
+            if (gemm3_pending) {   // the previous tile's GEMM2 / GEMM3 must have consumed the images before they are overwritten
+                wg::mbar_wait(&sm.bar3, ph3);
                 ph3 ^= 1u;
-                umma::fence_after_sync();
                 gemm3_pending = false;
             }
-            if (ord > 0 && ord % kFlushTiles == 0) flush_d3();   // every GEMM3 so far has completed; the next one restarts the accumulator
             K7_T(4);
             store16_feat(sm.FP_full, 16 * c, s, hi8);
             store16_feat(sm.FP_lo, 16 * c, s, lo8);
-            // H1 of this tile (hi | lo fp16 pairs) back from its TMEM operand -> H1^T image
-            umma::tmem_ld8x2(tmem + lane_base + COL_AH + 8 * c, tmem + lane_base + COL_AH + 32 + 8 * c, hi8, lo8);
-            store16_feat(sm.FH_full, 16 * c, s, hi8);
-            store16_feat(sm.FH_lo, 16 * c, s, lo8);
-            umma::tmem_st_wait();
+            // H1 of this tile (this thread's own entries of the GEMM1 operand, which layer1() of the next tile overwrites) -> H1^T image
+            {
+                const uint32_t off = fimg_off(16 * c, s);
+                const uint4 h0 = *reinterpret_cast<const uint4*>(sm.AH_full + off), h1 = *reinterpret_cast<const uint4*>(sm.AH_full + off + GS_T);
+                const uint4 l0 = *reinterpret_cast<const uint4*>(sm.AH_lo + off), l1 = *reinterpret_cast<const uint4*>(sm.AH_lo + off + GS_T);
+                *reinterpret_cast<uint4*>(sm.FH_full + off) = h0; *reinterpret_cast<uint4*>(sm.FH_full + off + GS_T) = h1;
+                *reinterpret_cast<uint4*>(sm.FH_lo + off) = l0; *reinterpret_cast<uint4*>(sm.FH_lo + off + GS_T) = l1;
+            }
         }
         K7_T(5);
-        umma::fence_proxy_async();
-        umma::fence_before_sync();
+        wg::fence_proxy_async();
         ready_arrive(kBarRdyA);     // this thread's share of the GEMM2 / GEMM3 operands is in place
         gemm3_pending = true;       // (Zp is rewritten in P3 of the next tile, behind its wait for GEMM1, i.e. after every thread has passed
                                     //  this point: no barrier needed here)
@@ -685,29 +659,27 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         h1pos_tile = h1pos;         // this tile's H1 signs, before layer1() of the next tile replaces them
         if (has_next) {
             if (gemm4_pending) {   // the previous tile's GEMM4 must have consumed its XT buffer (same parity as the next tile's) and the
-                umma::mbar_wait(&sm.bar4, ph4);   // dP1^T image before either is overwritten
+                wg::mbar_wait(&sm.bar4, ph4);     // dP1^T image before either is overwritten
                 ph4 ^= 1u;
-                umma::fence_after_sync();
                 gemm4_pending = false;
             }
             publish(tile + nctas);
             K7_T(8);
             K7_T(9);
             layer1();
-            umma::fence_before_sync();
+            wg::fence_proxy_async();
             K7_T(10);
             ready_arrive(kBarRdyB);
             K7_T(11);
         }
         K7_T(12);
         // ---- P7: dP1 = D2 .* act'(H1) -> dP1^T image (GEMM4 reduces it against [x | 1] into dW1 | db1) ----------
-        umma::mbar_wait(&sm.bar2, ph2);
+        wg::mbar_wait(&sm.bar2, ph2);
         ph2 ^= 1u;
-        umma::fence_after_sync();
         K7_T(13);
         {
             float v[16];
-            umma::tmem_ld16(tmem + lane_base + COL_D2 + 16 * c, v);
+            d_ld16(sm.D, s, 16 * c, v);
 #pragma unroll
             // D2 carries scale_p * kScaleW; the dP1 operand wants scale_p: one exact power-of-two factor (bit-identical to unscaling
             // to dH1 and rescaling)
@@ -731,12 +703,10 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
                 }
             }
             if (gemm4_pending) {   // (last tile: no publish() waited for it)
-                umma::mbar_wait(&sm.bar4, ph4);
+                wg::mbar_wait(&sm.bar4, ph4);
                 ph4 ^= 1u;
-                umma::fence_after_sync();
                 gemm4_pending = false;
             }
-            if (ord > 0 && ord % kFlushTiles == 0) flush_d4();
             {
                 uint32_t hi8[8], lo8[8];
 #pragma unroll
@@ -750,18 +720,13 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
 #ifdef B200RL_K7_TIMING
         if (tid == (g_k7_watch & 0xFFFF) && (int)blockIdx.x == (g_k7_watch >> 16)) g_k7_phase[15] += 1;
 #endif
-        umma::fence_proxy_async();
-        umma::fence_before_sync();
+        wg::fence_proxy_async();
         ready_arrive(kBarRdyC);
-        ++ord;
     }
-    // ---- drain: last GEMM3 / GEMM4, final flush, then the head gradients (fixed-order reductions) ---------------
-    if (gemm3_pending) umma::mbar_wait(&sm.bar3, ph3);
-    if (gemm4_pending) umma::mbar_wait(&sm.bar4, ph4);
-    umma::fence_after_sync();
-    worker_sync();
-    if (cta < ntiles) { flush_d3(); flush_d4(); }        // (a CTA without tiles writes the zeros the accumulators were initialised with)
-    worker_sync();
+    // ---- drain: last GEMM3 / GEMM4 (their sums are in AccW2 / AccD4), then the head gradients (fixed-order reductions) -------
+    if (gemm3_pending) wg::mbar_wait(&sm.bar3, ph3);
+    if (gemm4_pending) wg::mbar_wait(&sm.bar4, ph4);
+    worker_sync();                                       // (a CTA without tiles writes the zeros the accumulators were initialised with)
     for (int k = tid; k < H * H; k += NT7) gW2[k] = sm.AccW2[(k & 63) * 65 + (k >> 6)] * inv_s3;     // gW2[j + 64 i]
     if (tid < H) {
         gb2[tid] = sm.AccW2[64 * 65 + tid] * inv_sp;
@@ -981,9 +946,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         K7_T(31);
     }
     }  // worker warps
-    umma::fence_before_sync();
     __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem, 512);
 }
 
 }  // namespace

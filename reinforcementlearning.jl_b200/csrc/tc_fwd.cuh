@@ -1,20 +1,20 @@
 // tc_fwd.cuh — device building blocks of the tensor-core forward pass of one 2 x 64 MLP (K6), shared by the policy
-// inference kernel and the fused rollout kernel (fwd_tc.cu).  One tile = 128 samples = UMMA M.
+// inference kernel and the fused rollout kernel (fwd_tc.cu).  One tile = 128 samples = two 64-sample wgmma blocks.
 //
-//   layer 1 (K <= 4)  : FP32 FFMA, thread = (sample, 32 features), written straight into TMEM as the A operand (hi | lo fp16 pairs)
-//   layer 2 (64 x 64) : tcgen05.mma kind::f16 (K = 16), TS form (A from TMEM, B = W2 image in shared memory), the 3-term fp16 split
+//   layer 1 (K <= 4)  : FP32 FFMA, thread = (sample, 32 features), written into shared memory as the A operand (hi | lo fp16)
+//   layer 2 (64 x 64) : wgmma m64n64k16 f16 -> FP32, both operands in shared memory, the 3-term fp16 split
 //                       x_hi = fp16(64 x), x_lo = fp16(64 x - x_hi) (22 mantissa bits, like 3xTF32, at half the instruction count;
-//                       see nn_tc.cu for the pacing measurement and the range limits):
-//                         MMA 1 (N = 128): D[0:64) = hi*hi, D[64:128) = hi*lo     (rows 0..63 | 64..127 of the B image)
-//                         MMA 2 (N =  64): D[0:64) += lo*hi
-//   heads             : FP32 FFMA on the epilogue registers, partial sums of the two 32-feature halves meet in shared memory
+//                       see nn_tc.cu for the range limits): per K = 16 step hi*hi, hi*lo and lo*hi into the same accumulator
+//   heads             : FP32 FFMA on the layer-2 outputs, partial sums of the two 32-feature halves meet in shared memory
 //
-// Thread <-> data: warp w: TMEM lane quadrant q = w % 4 (samples 32q .. 32q+31), column half c = w / 4; thread = sample
-// s = 32q + lane, features 32c .. 32c+31.  Every multiply-add is an explicit fmaf / separate op: the arithmetic does not
-// depend on the contraction flags of the including translation unit.
+// Thread <-> data: warp w: sample quadrant q = w % 4 (samples 32q .. 32q+31), column half c = w / 4; thread = sample
+// s = 32q + lane, features 32c .. 32c+31.  The tile image holds, per 64-sample block, the A operand [hi 8 KB | lo 8 KB]; once
+// the block's wgmmas have completed, the warpgroup that ran them overwrites it with the FP32 accumulator (64 x 64).  Every
+// multiply-add is an explicit fmaf / separate op: the arithmetic does not depend on the contraction flags of the including
+// translation unit.
 #pragma once
 #include "nn.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace tcfwd {
 
@@ -24,9 +24,9 @@ constexpr int H = 64;
 constexpr int G_F = 128;              // byte stride between 8-element (16-byte) chunks along K: one 8 x 16 B core matrix
 constexpr int GW_S = 8 * G_F;         // weight image: stride between 8-row groups (K = 64 = 8 chunks)
 constexpr int WIMG_BYTES = 16 * GW_S; // [hi (64 rows) ; lo (64 rows)] x [K = 64] fp16 weight image (SWIZZLE_NONE, K-major core matrices)
-constexpr uint32_t COL_D = 0, COL_A = 128;   // TMEM columns: accumulator [hh+lh | hl], A operand [hi: 32 columns of fp16 pairs | lo: 32]
+constexpr int BLK = 8 * GW_S * 2;     // one 64-sample block of the tile image: A operand [hi | lo], later its FP32 accumulator
+constexpr int TILE_BYTES = 2 * BLK;
 constexpr float kScale = 64.0f;       // power-of-two scale of both operands (exact; undone on the accumulator)
-constexpr uint32_t TMEM_COLS = 256;
 constexpr float kLog2Pi = 1.8378770664093453f;
 
 struct NetSm {   // one network's weights in shared memory
@@ -59,6 +59,9 @@ __device__ __forceinline__ int64_t head_b(const MlpDesc& d, int o) {
     return head_base(d) + (d.heads2 ? (int64_t)o * (d.H + 1) + d.H : (int64_t)d.nout * d.H + o);
 }
 __device__ __forceinline__ uint32_t wimg_off(int n, int k) { return (uint32_t)((n >> 3) * GW_S + (k >> 3) * G_F + (n & 7) * 16 + (k & 7) * 2); }
+// FP32 accumulator of one block, row r, column col: 16-byte units XOR-swizzled by the row, so that 8 consecutive rows read
+// at the same column hit 8 different bank groups
+__device__ __forceinline__ uint32_t dacc_off(int r, int col) { return (uint32_t)(r * 256 + (((col >> 2) ^ (r & 15)) << 4) + (col & 3) * 4); }
 
 // s1: scale folded into W1 / b1 (kScale for relu trunks: relu(S z) = S relu(z) exactly for a power of two S, so layer 1 then
 // produces the scaled H1 operand without a multiply per feature; 1 otherwise)
@@ -95,13 +98,16 @@ __device__ __forceinline__ unsigned long long xo_next(unsigned long long (&s)[4]
 __device__ __forceinline__ double xo_f64(unsigned long long (&s)[4]) { return (double)(xo_next(s) >> 11) * 0x1p-53; }
 __device__ __forceinline__ float xo_f32(unsigned long long (&s)[4]) { return (float)((unsigned)(xo_next(s) >> 32) >> 8) * 0x1p-24f; }
 
-// layer 1 of this thread's sample: H1[32c .. 32c+32) = act(W1 x + b1) -> TMEM A operand (hi pairs at COL_A, lo pairs at COL_A + 32)
+// layer 1 of this thread's sample: H1[32c .. 32c+32) = act(W1 x + b1) -> A operand of its block (hi at +0, lo at +8 KB; the
+// image layout of the weights, row = sample)
 // (the loops over 16-feature halves here and 8-feature groups in head_partials are deliberately NOT unrolled: tanhf is ~40
 // instructions, and with every instance inlined the rollout kernel was 290 KB of SASS whose dominant stall was instruction fetch)
 // ACT: the activation as a compile-time constant (-1: read `act`); relu trunks expect load_net(.., s1 = kScale)
 template <int ACT>
-__device__ __forceinline__ void layer1_to_tmem(const NetSm& w, int act_rt, const float (&x)[kInMax], int c, uint32_t tmem_lane) {
+__device__ __forceinline__ void layer1_to_smem(const NetSm& w, int act_rt, const float (&x)[kInMax], int c, int s, uint8_t* tile) {
     const int act = ACT >= 0 ? ACT : act_rt;
+    uint8_t* blk = tile + (s >> 6) * BLK;
+    const int r = s & 63;
 #pragma unroll(ACT == B200RL_ACT_RELU ? 2 : 1)
     for (int half = 0; half < 2; ++half) {
         uint32_t hi8[8], lo8[8];
@@ -125,37 +131,58 @@ __device__ __forceinline__ void layer1_to_tmem(const NetSm& w, int act_rt, const
             split2(h[0], h[1], hi8[2 * ch], lo8[2 * ch]);
             split2(h[2], h[3], hi8[2 * ch + 1], lo8[2 * ch + 1]);
         }
-        umma::tmem_st8(tmem_lane + COL_A + 16 * c + 8 * half, hi8);
-        umma::tmem_st8(tmem_lane + COL_A + 32 + 16 * c + 8 * half, lo8);
+        const int f0 = 32 * c + 16 * half;
+        *reinterpret_cast<uint4*>(blk + wimg_off(r, f0)) = make_uint4(hi8[0], hi8[1], hi8[2], hi8[3]);
+        *reinterpret_cast<uint4*>(blk + wimg_off(r, f0 + 8)) = make_uint4(hi8[4], hi8[5], hi8[6], hi8[7]);
+        *reinterpret_cast<uint4*>(blk + 8 * GW_S + wimg_off(r, f0)) = make_uint4(lo8[0], lo8[1], lo8[2], lo8[3]);
+        *reinterpret_cast<uint4*>(blk + 8 * GW_S + wimg_off(r, f0 + 8)) = make_uint4(lo8[4], lo8[5], lo8[6], lo8[7]);
     }
-    umma::tmem_st_wait();
 }
 
-// one elected thread: D = A x W2^T as the 3-term fp16 split, all three terms accumulated into the same 64 columns
-// (12 MMAs of N = 64, K = 16 each: hi*hi, hi*lo, lo*hi)
-__device__ __forceinline__ void issue_gemm(uint32_t tmem, const NetSm& w) {
-    const uint32_t idesc64 = umma::make_idesc_f16(128, 64, 0, 0);
-    const uint64_t dB = umma::make_desc(umma::smem_u32(w.B), G_F, GW_S);
-    const uint64_t dBlo = dB + (uint64_t)((8 * GW_S) >> 4);   // rows 64..127 of the image
+// one warpgroup (wgid = its index in the CTA, 128 threads): D = A x W2^T of one 64-sample block as the 3-term fp16 split, all three
+// terms accumulated into the same registers (12 wgmma m64n64k16: hi*hi, hi*lo, lo*hi per K step), then D over the block's A image.
+// The caller has made the A image visible to the async proxy (fence + barrier).
+__device__ __forceinline__ void gemm_block(uint8_t* blk, const NetSm& w, int wgid) {
+    const uint64_t dA = wg::make_desc(wg::smem_u32(blk), G_F, GW_S), dAlo = wg::desc_add(dA, 8 * GW_S);
+    const uint64_t dB = wg::make_desc(wg::smem_u32(w.B), G_F, GW_S), dBlo = wg::desc_add(dB, 8 * GW_S);
+    float d[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) d[i] = 0.f;
+    wg::fence();
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-        const uint64_t adv = (uint64_t)(k * (2 * G_F / 16));
-        umma::mma_f16_ts(tmem + COL_D, tmem + COL_A + 8 * k, dB + adv, idesc64, k ? 1u : 0u);
-        umma::mma_f16_ts(tmem + COL_D, tmem + COL_A + 8 * k, dBlo + adv, idesc64, 1u);
-        umma::mma_f16_ts(tmem + COL_D, tmem + COL_A + 32 + 8 * k, dB + adv, idesc64, 1u);
+        const uint32_t adv = (uint32_t)(k * 2 * G_F);
+        wg::mma_m64n64k16<0, 0>(d, wg::desc_add(dA, adv), wg::desc_add(dB, adv), k ? 1u : 0u);
+        wg::mma_m64n64k16<0, 0>(d, wg::desc_add(dA, adv), wg::desc_add(dBlo, adv), 1u);
+        wg::mma_m64n64k16<0, 0>(d, wg::desc_add(dAlo, adv), wg::desc_add(dB, adv), 1u);
     }
+    wg::commit();
+    wg::wait_all();
+    asm volatile("bar.sync %0, 128;" ::"r"(9 + wgid) : "memory");   // every warp's operand reads are done before D overwrites A
+    const int t = threadIdx.x & 127, row0 = 16 * (t >> 5) + ((t & 31) >> 2), col0 = 2 * (t & 3);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+            *reinterpret_cast<float2*>(blk + dacc_off(row0 + 8 * h, 8 * j + col0)) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
 }
 
 // epilogue of this thread's sample: H2[32c .. 32c+32) = act(D + b2), partial head sums over these 32 features
 template <int ACT>
-__device__ __forceinline__ void head_partials(const NetSm& w, int act_rt, int c, uint32_t tmem_lane, float (&zp)[kOutMax]) {
+__device__ __forceinline__ void head_partials(const NetSm& w, int act_rt, int c, int s, const uint8_t* tile, float (&zp)[kOutMax]) {
     const int act = ACT >= 0 ? ACT : act_rt;
+    const uint8_t* blk = tile + (s >> 6) * BLK;
+    const int r = s & 63;
 #pragma unroll
     for (int o = 0; o < kOutMax; ++o) zp[o] = 0.f;
 #pragma unroll(ACT == B200RL_ACT_RELU ? 2 : 1)
     for (int grp = 0; grp < 2; ++grp) {
         float v[16];
-        umma::tmem_ld16(tmem_lane + COL_D + 32 * c + 16 * grp, v);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const float4 q4 = *reinterpret_cast<const float4*>(blk + dacc_off(r, 32 * c + 16 * grp + 4 * u));
+            v[4 * u] = q4.x; v[4 * u + 1] = q4.y; v[4 * u + 2] = q4.z; v[4 * u + 3] = q4.w;
+        }
 #pragma unroll
         for (int k = 0; k < 16; ++k) {
             const int f = 32 * c + 16 * grp + k;

@@ -3,10 +3,11 @@
 #pragma once
 #include <cstdint>
 
-// CTAs given to the actor out of `grid` (the rest work on the critic).  A critic tile costs ~0.87 of an actor tile with the
-// categorical PPO / A2C loss and ~0.85 with the Gaussian head (B200 sweeps, profiles/na_sweep.sh: 79 : 69 is the optimum for the
-// 4 096-tile BASELINE minibatch, 80 : 68 for the 8 192-tile Pendulum batch); the split minimises the longer of the two roles'
-// whole-tile counts.  At most grid / 2 + 8 (the fused optimiser step stages <= 82 partial rows), at least grid / 2.
+// CTAs given to the actor out of `grid` (the rest work on the critic).  Cost model: a critic tile costs ~0.87 of an actor tile
+// with the categorical PPO / A2C loss and ~0.85 with the Gaussian head (the critic skips the softmax / log-density, entropy and
+// PPO ratio); the split minimises the longer of the two roles' whole-tile counts.  The two ratios were swept on an earlier
+// version of this kernel for another GPU and are inherited unmeasured for the H100 (wgmma) kernel; a sweep there could change
+// them.  At most grid / 2 + 8 (the fused optimiser step stages <= 82 partial rows), at least grid / 2.
 static inline int b200rl_tc_actor_ctas(int grid, bool gaussian_head, int64_t ntiles) {
     const double r = gaussian_head ? 0.85 : 0.87;
     int best = grid / 2;

@@ -49,7 +49,7 @@ def acrobot_params(link_length_a=1.0, link_length_b=1.0, link_mass_a=1.0, link_m
 
 
 class B200VecEnv:
-    """N classic-control envs stepped by one sm_100a kernel launch.
+    """N classic-control envs stepped by one sm_90a kernel launch.
 
     ``rng_state``: (N, 4) uint64 raw Xoshiro256++ states (what Julia's ``Xoshiro(seed_i)`` holds).
     ``auto_reset``: fuse MultiThreadEnv's soft reset of finished sub-envs into ``act_``."""

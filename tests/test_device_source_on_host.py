@@ -187,9 +187,10 @@ def test_env_with_non_default_parameters_bitwise(hd, hkind, okind, dtype, n_act,
 
 
 def test_actor_critic_cta_split_rule(hd):
-    """tc_split.h: the split of the 148 persistent CTAs of the loss + backward kernel.  Pinned: the two measured optima (79 : 69 for the
-    4 096-tile BASELINE minibatch, 80 : 68 for the 8 192-tile Pendulum batch), the bounds the fused optimiser step relies on, and
-    optimality of the returned split under the cost model for arbitrary tile counts."""
+    """tc_split.h: the split of the persistent CTAs of the loss + backward kernel between actor and critic.  Pinned: the rule's
+    splits of 148 CTAs (79 : 69 for the 4 096-tile BASELINE minibatch, 80 : 68 for the 8 192-tile Pendulum batch), the bounds the
+    fused optimiser step relies on, and optimality of the returned split under the cost model for arbitrary tile counts and grids
+    (132 = one CTA per SM of an H100)."""
     assert hd.hd_tc_actor_ctas(148, 0, 4096) == 79 and hd.hd_tc_actor_ctas(148, 1, 8192) == 80
     import math
     for grid in (148, 132, 2, 8):

@@ -279,7 +279,7 @@ def test_run_loop_with_host_actions_matches_fused_path(pkg, ctx):
 
 
 def test_tensor_core_and_cuda_core_paths_agree(pkg, ctx):
-    """K6/K7 exist as tcgen05 (3xTF32, H = 64) and FP32-FFMA kernels; both must meet the oracle
+    """K6/K7 exist as wgmma (3-term fp16 split, H = 64) and FP32-FFMA kernels; both must meet the oracle
     and each other well inside the 1e-5 bar."""
     net, desc, params = make_net(pkg, ctx, 4, 64, 2, 0, 0, 17)
     rng = np.random.default_rng(3)
