@@ -294,6 +294,24 @@ typedef struct {
 } b200rl_explorer;
 int b200rl_net_q_explore(b200rl_net* net, const float* obs_dev, int64_t n, uint64_t* rng_dev, const b200rl_explorer* explorer,
                          int32_t* action_out_dev);
+/* plan!(greedy policy, obs): findmax of the logits / Q-values (kinds 0, 2; int32 1-based, first maximum wins, NaN ranks
+ * highest, -0.0 below 0.0), mu (kind 1; float, unclamped); no RNG.  on_device applies to obs and action_out. */
+int b200rl_net_act_greedy(b200rl_net* net, const float* obs, int64_t n, void* action_out, int on_device);
+
+/* ---------------------------------------------------------------- evaluation ------- */
+/* run(policy, env, StopAfterNSteps(n_steps)) (RLCore/src/core/run.jl:36-78) with the network's greedy (mode 0, see
+ * b200rl_net_act_greedy; a continuous env receives clamp(mu, lo, hi)) or sampling (mode 1, b200rl_net_act's sampler on the
+ * (4, N) DEVICE streams policy_rng_dev, advanced; kinds 0 / 1) policy: reset!(env; is_force = true) for every env, then n_steps
+ * x {plan!, act!} with the env's in-kernel auto-reset (MaxTimeoutEnv honoured).  Outputs (each may be NULL):
+ *   returns (K, N) f32, lengths (K, N) i32 : the first K = max_episodes episodes of each env that end inside the window, the
+ *       Float32 sum of their rewards in step order and env.t at termination; slots no episode reaches are left untouched
+ *   counts (N) i32                         : episodes each env finished in the window (may exceed K)
+ * The env ends where the stage protocol leaves it (every field, its streams and episode statistics); the network and every
+ * other handle are only read.  Float32 envs with <= 4 observations.  on_device = 0: host outputs (synchronises), 1: device
+ * outputs (asynchronous on the ctx stream). */
+typedef struct { int32_t mode, n_steps, max_episodes; } b200rl_eval_config;   /* mode 0 greedy, 1 sample */
+int b200rl_evaluate(b200rl_net* net, b200rl_env* env, const b200rl_eval_config* cfg, uint64_t* policy_rng_dev,
+                    float* returns_out, int32_t* lengths_out, int32_t* counts_out, int on_device);
 
 /* ---------------------------------------------------------------- on-policy agent -- */
 /* PPO (clipped surrogate) / A2C hyper-parameters; defaults of the in-tree example

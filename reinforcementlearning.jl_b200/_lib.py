@@ -56,6 +56,11 @@ class Explorer(C.Structure):
                 ("step", C.c_int64), ("kind", C.c_int32), ("is_break_tie", C.c_int32)]
 
 
+class EvalConfig(C.Structure):
+    """b200rl_eval_config: mode 0 greedy | 1 sample, window length, records kept per env."""
+    _fields_ = [(n, C.c_int32) for n in ("mode", "n_steps", "max_episodes")]
+
+
 class MountainCarParams(C.Structure):
     _fields_ = [(n, C.c_double) for n in ("min_pos", "max_pos", "max_speed", "goal_pos", "goal_velocity", "power", "gravity")] + [
         ("max_steps", C.c_int64)]
@@ -141,6 +146,8 @@ SIGNATURES = {
     "b200rl_net_values": (_i32, [_vp, _vp, _i64, _vp, _i32, _i32]),
     "b200rl_net_q_act": (_i32, [_vp, _vp, _i64, _vp, _f32, _vp]),
     "b200rl_net_q_explore": (_i32, [_vp, _vp, _i64, _vp, _vp, _vp]),
+    "b200rl_net_act_greedy": (_i32, [_vp, _vp, _i64, _vp, _i32]),
+    "b200rl_evaluate": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32]),
     "b200rl_net_ac_step": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _f32, _f32, _i32, _vp]),
     "b200rl_onpolicy_create": (_i32, [_vp, _vp, _vp, _vp, _vp, _pp]),
     "b200rl_onpolicy_destroy": (_i32, [_vp]),

@@ -8,6 +8,7 @@
 // FluxApproximator/optimise! policies/learners/flux_approximator.jl:11-46; TargetNetwork
 // target_network.jl:27-88; PPO/A2C/DQN update rules: ReinforcementLearningZoo (absent from the
 // snapshot; SURVEY Appendix B), hyper-parameters docs/homepage/blog/a_practical_introduction_to_RL.jl/index.html:15238-15286.
+#include "greedy.cuh"
 #include "nn.cuh"
 
 // other translation units
@@ -32,6 +33,8 @@ int b200rl_env_internal_kind(const b200rl_env* e);
 int b200rl_env_internal_max_timeout(const b200rl_env* e);
 int b200rl_env_internal_dtype(const b200rl_env* e);
 void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n);
+int b200rl_env_internal_n_actions(const b200rl_env* e);
+static void* env_field(b200rl_env* e, int f);
 static bool fused_rollout_enabled() {   // B200RL_FUSED_ROLLOUT=0: step through plan!/act! launches instead (same results)
     static int v = -1;
     if (v < 0) { const char* e = getenv("B200RL_FUSED_ROLLOUT"); v = (e && e[0] == '0') ? 0 : 1; }
@@ -42,6 +45,42 @@ namespace {
 __global__ void clamp_copy_kernel(float* __restrict__ dst, const float* __restrict__ src, int64_t n, float lo, float hi) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) dst[i] = fminf(fmaxf(src[i], lo), hi);
+}
+// plan!(greedy policy) on the (nout, N) head outputs: raw action bits (greedy.cuh); clamp != 0: a continuous action is
+// handed to the env as clamp(mu, lo, hi)
+__global__ void greedy_select_kernel(const float* __restrict__ heads, MlpDesc d, int64_t n, int clamp, float lo, float hi,
+                                     uint32_t* __restrict__ out) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float z[kOutMax];
+#pragma unroll
+    for (int o = 0; o < kOutMax; ++o) z[o] = o < d.nout ? heads[(int64_t)d.nout * i + o] : 0.f;
+    uint32_t a = greedy::greedy_action(d, z);
+    if (clamp) a = __float_as_uint(fminf(fmaxf(__uint_as_float(a), lo), hi));
+    out[i] = a;
+}
+// staged b200rl_evaluate, after each act!: per-env Float32 return (rewards added in step order, like the env's EPISODE_RETURN)
+// and length; an episode that ended is recorded in slot cnt (< K) of its env
+__global__ void eval_record_kernel(const float* __restrict__ reward, const uint8_t* __restrict__ flags, int64_t n, int K,
+                                   float* __restrict__ acc_ret, int32_t* __restrict__ acc_len, int32_t* __restrict__ cnt,
+                                   float* __restrict__ returns, int32_t* __restrict__ lengths) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float ret = __fadd_rn(acc_ret[i], reward[i]);
+    const int32_t len = acc_len[i] + 1;
+    if (flags[i] & 1) {
+        const int e = cnt[i];
+        if (e < K) {
+            if (returns) returns[(size_t)K * i + e] = ret;
+            if (lengths) lengths[(size_t)K * i + e] = len;
+        }
+        cnt[i] = e + 1;
+        acc_ret[i] = 0.f;
+        acc_len[i] = 0;
+    } else {
+        acc_ret[i] = ret;
+        acc_len[i] = len;
+    }
 }
 __global__ void copy_f32_kernel(float* __restrict__ dst, const float* __restrict__ src, int64_t n) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -325,6 +364,115 @@ int b200rl_net_q_explore(b200rl_net* n, const float* obs_dev, int64_t N, uint64_
     void* s;
     TRY(ctx_scratch(n->ctx, (size_t)N * n->actor.nout * 4 + 256, &s));
     return nn_q_explore(n->ctx, n->actor, n->params, obs_dev, N, (unsigned long long*)rng_dev, *ex, action_out_dev, (float*)s);
+}
+
+/* plan!(greedy policy, obs): findmax of the logits / Q-values (kinds 0, 2), mu (kind 1); no RNG.  Same forward pass as
+ * b200rl_net_values / the head outputs of b200rl_net_act. */
+int b200rl_net_act_greedy(b200rl_net* n, const float* obs, int64_t N, void* action_out, int on_device) {
+    REQUIRE(n && obs && action_out, B200RL_ERR_INVALID, "null argument");
+    REQUIRE(N > 0, B200RL_ERR_INVALID, "empty batch");
+    TRY(ctx_bind(n->ctx));
+    const size_t hb = ((size_t)N * n->actor.nout * 4 + 255) / 256 * 256;
+    const float* dobs;
+    void* ex = nullptr;
+    TRY(stage_obs(n, obs, N, on_device, &dobs, hb + (size_t)N * 4 + 256, &ex));
+    float* heads = (float*)ex;
+    uint32_t* da = on_device ? (uint32_t*)action_out : (uint32_t*)((char*)ex + hb);
+    TRY(nn_mlp_forward(n->ctx, n->actor, n->params, dobs, N, heads));
+    greedy_select_kernel<<<grid_for(N, 256), 256, 0, n->ctx->stream>>>(heads, n->actor, N, 0, 0.f, 0.f, da);
+    LAUNCH_CHECK(n->ctx);
+    if (!on_device) {
+        CUDA_TRY(cudaMemcpyAsync(action_out, da, (size_t)N * 4, cudaMemcpyDeviceToHost, n->ctx->stream));
+        CUDA_TRY(cudaStreamSynchronize(n->ctx->stream));
+    }
+    return B200RL_OK;
+}
+
+/* run(policy, env, StopAfterNSteps(n_steps)) with the network's greedy (mode 0) or sampling (mode 1) policy; see b200rl.h.
+ * Fused into one launch (fwd_tc.cu) for H = 64 on the tensor-core path, otherwise staged launches with the same arithmetic. */
+int b200rl_evaluate(b200rl_net* n, b200rl_env* env, const b200rl_eval_config* cfg, uint64_t* policy_rng_dev, float* returns_out,
+                    int32_t* lengths_out, int32_t* counts_out, int on_device) {
+    REQUIRE(n && env && cfg, B200RL_ERR_INVALID, "null argument");
+    REQUIRE(b200rl_env_internal_ctx(env) == n->ctx, B200RL_ERR_INVALID, "net/env belong to another ctx");
+    REQUIRE(b200rl_env_internal_dtype(env) == B200RL_F32, B200RL_ERR_UNSUPPORTED, "the networks read Float32 observations: construct the env with T = Float32");
+    REQUIRE(b200rl_env_internal_kind(env) != B200RL_ENV_ACROBOT, B200RL_ERR_UNSUPPORTED, "AcrobotEnv has 6 observations (networks take at most 4)");
+    REQUIRE(cfg->mode == 0 || cfg->mode == 1, B200RL_ERR_INVALID, "mode must be 0 (greedy) or 1 (sample)");
+    REQUIRE(!(cfg->mode == 1 && n->kind == 2), B200RL_ERR_UNSUPPORTED, "mode 1 samples a policy head: evaluate a Q-network with mode 0 or QBasedPolicy");
+    REQUIRE(b200rl_env_internal_nobs(env) == n->actor.in, B200RL_ERR_INVALID, "network input width != observation width");
+    const bool cont = b200rl_env_internal_continuous(env);
+    REQUIRE(cont == (n->kind == 1), B200RL_ERR_INVALID, "head kind != action-space kind (Gaussian head <-> continuous actions)");
+    REQUIRE(cont || n->actor.nout == b200rl_env_internal_n_actions(env), B200RL_ERR_INVALID, "head width != number of discrete actions");
+    REQUIRE(cfg->n_steps >= 1, B200RL_ERR_INVALID, "n_steps must be >= 1");
+    REQUIRE(cfg->max_episodes >= 0, B200RL_ERR_INVALID, "max_episodes must be >= 0");
+    REQUIRE(cfg->mode == 0 || policy_rng_dev, B200RL_ERR_INVALID, "mode 1 needs the (4, N) device policy streams");
+    TRY(ctx_bind(n->ctx));
+    b200rl_ctx* ctx = n->ctx;
+    const int64_t N = b200rl_env_internal_n(env);
+    const int K = cfg->max_episodes, mode = cfg->mode, nsteps = cfg->n_steps;
+    const size_t rec_bytes = (size_t)N * K * 4;
+    auto round256 = [](size_t b) { return (b + 255) / 256 * 256; };
+    // device buffers: the caller's (on_device) or scratch; the staged path also keeps per-env accumulators and its actions
+    size_t off = 0;
+    const size_t o_ret = off; off += on_device ? 0 : round256(rec_bytes);
+    const size_t o_len = off; off += on_device ? 0 : round256(rec_bytes);
+    const size_t o_cnt = off; off += round256((size_t)N * 4);
+    const size_t o_acc = off; off += round256((size_t)N * 4) * 2;
+    const size_t o_act = off; off += round256((size_t)N * 4) * 2;
+    const size_t o_heads = off; off += round256((size_t)N * n->actor.nout * 4);
+    void* sc;
+    TRY(ctx_scratch(ctx, off, &sc));
+    char* base = (char*)sc;
+    float* dret = returns_out ? (on_device ? returns_out : (float*)(base + o_ret)) : nullptr;
+    int32_t* dlen = lengths_out ? (on_device ? lengths_out : (int32_t*)(base + o_len)) : nullptr;
+    int32_t* dcnt = (on_device && counts_out) ? counts_out : (int32_t*)(base + o_cnt);
+    if (!on_device) {   // record slots the window does not fill keep the caller's values
+        if (dret && rec_bytes) CUDA_TRY(cudaMemcpyAsync(dret, returns_out, rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
+        if (dlen && rec_bytes) CUDA_TRY(cudaMemcpyAsync(dlen, lengths_out, rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    AcHyper hp{0.1f, 1.f, 0.5f, 0.001f, 0.f, __builtin_inff(), 0, 0};   // b200rl_net_act's sampler
+    unsigned long long* prng = (unsigned long long*)policy_rng_dev;
+    TRY(b200rl_env_reset(env, 1));   // reset!(env; is_force = true), run.jl:46
+    int st = nn_tc_enabled() ? nn_tc_evaluate(ctx, env, n->actor, n->params, hp, mode, nsteps, K, prng, dret, dlen, dcnt) : B200RL_ERR_UNSUPPORTED;
+    if (st == B200RL_ERR_UNSUPPORTED) {   // staged: plan! -> act! (auto-reset) -> record, n_steps times, no host sync
+        float* acc_ret = (float*)(base + o_acc);
+        int32_t* acc_len = (int32_t*)(base + o_acc + round256((size_t)N * 4));
+        uint32_t* act = (uint32_t*)(base + o_act);
+        float* act_clamped = (float*)(base + o_act + round256((size_t)N * 4));
+        float* heads = (float*)(base + o_heads);
+        CUDA_TRY(cudaMemsetAsync(dcnt, 0, (size_t)N * 4, ctx->stream));
+        CUDA_TRY(cudaMemsetAsync(acc_ret, 0, round256((size_t)N * 4) * 2, ctx->stream));
+        const float* obs = (const float*)env_field(env, B200RL_FIELD_OBS);
+        const float* rew = (const float*)env_field(env, B200RL_FIELD_REWARD);
+        const uint8_t* flags = (const uint8_t*)env_field(env, B200RL_FIELD_FLAGS);
+        const float bound = b200rl_env_internal_kind(env) == B200RL_ENV_PENDULUM ? 2.0f : 1.0f;   // action_space -2.0..2.0 | -1.0..1.0
+        for (int k = 0; k < nsteps; ++k) {
+            const void* a_env = act;
+            if (mode == 0) {
+                TRY(nn_mlp_forward(ctx, n->actor, n->params, obs, N, heads));
+                greedy_select_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(heads, n->actor, N, cont ? 1 : 0, -bound, bound, act);
+                LAUNCH_CHECK(ctx);
+            } else {
+                TRY(nn_policy_act(ctx, n->actor, n->critic, n->params, hp, obs, N, prng, act, nullptr, nullptr, nullptr, nullptr));
+                if (cont) {
+                    clamp_copy_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(act_clamped, (const float*)act, N, -bound, bound);
+                    LAUNCH_CHECK(ctx);
+                    a_env = act_clamped;
+                }
+            }
+            TRY(b200rl_env_step(env, a_env, 1, 1));
+            eval_record_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(rew, flags, N, K, acc_ret, acc_len, dcnt, dret, dlen);
+            LAUNCH_CHECK(ctx);
+        }
+    } else if (st != B200RL_OK) {
+        return st;
+    }
+    if (!on_device) {
+        if (returns_out && rec_bytes) CUDA_TRY(cudaMemcpyAsync(returns_out, dret, rec_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        if (lengths_out && rec_bytes) CUDA_TRY(cudaMemcpyAsync(lengths_out, dlen, rec_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        if (counts_out) CUDA_TRY(cudaMemcpyAsync(counts_out, dcnt, (size_t)N * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    }
+    return B200RL_OK;
 }
 
 /* One optimiser step from explicit on-policy minibatch arrays (all HOST; test / generic entry):

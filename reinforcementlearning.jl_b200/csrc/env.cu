@@ -539,5 +539,10 @@ int b200rl_env_internal_dtype(const b200rl_env* e) { return e->dtype; }
 int64_t b200rl_env_internal_n(const b200rl_env* e) { return e->N; }
 int b200rl_env_internal_kind(const b200rl_env* e) { return e->kind; }
 int b200rl_env_internal_nobs(const b200rl_env* e) { return e->nobs; }
+int b200rl_env_internal_n_actions(const b200rl_env* e) {   // size of a discrete action space (0: continuous)
+    if (e->continuous) return 0;
+    if (e->kind == B200RL_ENV_PENDULUM) return e->dtype == B200RL_F64 ? e->p.pend64.n_actions : e->p.pend.n_actions;
+    return e->kind == B200RL_ENV_CARTPOLE ? 2 : 3;
+}
 b200rl_ctx* b200rl_env_internal_ctx(const b200rl_env* e) { return e->ctx; }
 bool b200rl_env_internal_continuous(const b200rl_env* e) { return e->continuous; }

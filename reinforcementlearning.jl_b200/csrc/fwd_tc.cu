@@ -5,11 +5,14 @@
 //                        write the transition into column t of the rollout tensors }.  A CTA owns up to two tiles of 128
 //                        envs for the whole launch; their env state and both RNG streams stay in shared memory, the weights of
 //                        both networks too.  Replaces 2 launches per env step (agent_base.jl:45-66 stage loop, run.jl:52-68).
+//   evaluate_tc_kernel : n_steps x { obs -> actor -> greedy | sampled action -> env step (+ fused auto-reset) -> per-env episode
+//                        records }: the actor alone, no rollout tensors (b200rl_evaluate).
 //
 // Both kernels are built from the same device functions (tc_fwd.cuh, env_device.cuh) and compiled with the env flags
 // (-fmad=false): stepping through plan!/act! one launch at a time or through the fused rollout gives bit-identical results.
 #include "common.cuh"
 #include "env_device.cuh"
+#include "greedy.cuh"
 #include "tc_fwd.cuh"
 
 using namespace tcfwd;
@@ -364,6 +367,237 @@ template <class Env> int launch_rollout(b200rl_ctx* ctx, const RollArgs& g, cons
     return B200RL_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// fused evaluation (b200rl_evaluate): n_steps x { obs -> actor -> greedy | sampled action -> env step (+ fused auto-reset) ->
+// record of the episodes that end }.  The weights are fixed, so nothing couples the tiles: a CTA runs the whole window on one
+// group of up to kSlots resident tiles, writes the group back and takes the next one (no limit on N).  The head outputs come
+// from the device functions, template activation and operand scale of forward_tc_kernel's mode 1, so the staged greedy
+// policy (b200rl_net_act_greedy -> nn_mlp_forward) and this kernel pick the same actions bit for bit.
+template <class Env> struct EvalSlot {     // env state of one tile, one entry per env (owner thread = sample s)
+    typename Env::S st[TM];
+    int t[TM];
+    int flags[TM];
+    float ep_ret[TM];
+    float last_rew[TM];
+    uint32_t last_act[TM];
+    int cnt[TM];                           // episodes finished in the window
+    unsigned long long erng[4 * TM];       // env stream  [word][env]
+    unsigned long long prng[4 * TM];       // policy stream (MODE 1)
+};
+template <class Env> struct SmemEval {
+    alignas(128) uint8_t T[TILE_BYTES];
+    NetSm net;                             // actor (or Q-network)
+    float X[kInMax * TM];
+    float Zp[2 * kOutMax * TM];            // [half][o][s]
+    EvalSlot<Env> slot[kSlots];
+    int fin_cnt[TM], fin_len[TM];          // episode statistics of owner thread s (shared memory: no registers held across the window)
+    float fin_ret[TM];
+    float red_f[8];
+    int red_i[8], red_l[8];
+};
+
+struct EvalArgs {
+    MlpDesc actor;
+    const float* params;
+    AcHyper hp;
+    int64_t N;
+    int nsteps, K;
+    float act_lo, act_hi;               // continuous actions: the env receives clamp(a, lo, hi)
+    unsigned long long* policy_rng;     // (4, N), MODE 1
+    float* returns;                     // (K, N), may be null
+    int32_t* lengths;                   // (K, N), may be null
+    int32_t* counts;                    // (N), may be null
+};
+
+// MODE 0: greedy (greedy.cuh, no draw), 1: sample_head on the policy streams
+// (layer 1 and the head epilogue not unrolled: the relu variants would exceed 128 registers and spill)
+template <class Env, int ACT, int MODE>
+__global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename Env::P p, EnvArrays ea) {
+    using act_t = typename Env::act_t;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    SmemEval<Env>& sm = *reinterpret_cast<SmemEval<Env>*>(smem_raw);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int q = warp & 3, c = warp >> 2;
+    const int s = 32 * q + lane;
+    const bool owner = c == 0;              // warps 0..3: thread s also owns env s of each resident tile
+    const int64_t N = g.N;
+    const int nctas = gridDim.x;
+    const int64_t ntiles = (N + TM - 1) / TM;
+    load_net(sm.net, g.actor, g.params, ACT == B200RL_ACT_RELU ? kScale : 1.0f);
+    if (owner) { sm.fin_cnt[s] = 0; sm.fin_len[s] = 0; sm.fin_ret[s] = 0.f; }
+#pragma unroll 1
+    for (int64_t base = blockIdx.x; base < ntiles; base += (int64_t)nctas * kSlots) {   // tiles base + k * nctas, k < kSlots
+        int nslots = 0;
+        for (int k = 0; k < kSlots; ++k)
+            if (base + (int64_t)k * nctas < ntiles) nslots = k + 1;
+        if (owner) {
+            for (int k = 0; k < nslots; ++k) {
+                const int64_t i = (base + (int64_t)k * nctas) * TM + s;
+                EvalSlot<Env>& sl = sm.slot[k];
+                if (i < N) {
+                    sl.st[s] = Env::load(ea.state, i);
+                    sl.t[s] = ea.t[i];
+                    sl.flags[s] = ea.flags[i];
+                    sl.ep_ret[s] = ea.ep_ret[i];
+                    sl.cnt[s] = 0;
+                    Xo e = load_rng(ea.rng, i);
+                    sl.erng[s] = e.s0; sl.erng[TM + s] = e.s1; sl.erng[2 * TM + s] = e.s2; sl.erng[3 * TM + s] = e.s3;
+                    if (MODE == 1) {
+                        unsigned long long pr[4];
+                        load_rng32(g.policy_rng, i, pr);
+                        sl.prng[s] = pr[0]; sl.prng[TM + s] = pr[1]; sl.prng[2 * TM + s] = pr[2]; sl.prng[3 * TM + s] = pr[3];
+                    }
+                }
+            }
+        }
+        wg::fence_proxy_async();            // (the first pass: the weight image written by load_net, read by wgmma)
+        __syncthreads();
+#pragma unroll 1
+        for (int step = 0; step < g.nsteps; ++step) {
+#pragma unroll 1
+            for (int k = 0; k < nslots; ++k) {
+                // (env index and slot are recomputed after the GEMM rather than held in registers across it)
+                if (owner) {
+                    float o[kInMax] = {0.f, 0.f, 0.f, 0.f};
+                    if ((base + (int64_t)k * nctas) * TM + s < N) Env::observe(sm.slot[k].st[s], o);
+#pragma unroll
+                    for (int j = 0; j < kInMax; ++j) sm.X[j * TM + s] = o[j];
+                }
+                __syncthreads();
+                {
+                    float x[kInMax];
+#pragma unroll
+                    for (int j = 0; j < kInMax; ++j) x[j] = sm.X[j * TM + s];
+                    layer1_to_smem<ACT, 1>(sm.net, g.actor.act, x, c, s, sm.T);
+                }
+                wg::fence_proxy_async();
+                __syncthreads();
+                gemm_block(sm.T + c * BLK, sm.net, c);   // warpgroup c: samples 64c .. 64c+63
+                __syncthreads();
+                {
+                    float zp[kOutMax];
+                    head_partials<ACT, 1>(sm.net, g.actor.act, c, s, sm.T, zp);
+#pragma unroll
+                    for (int o = 0; o < kOutMax; ++o) sm.Zp[(c * kOutMax + o) * TM + s] = zp[o];
+                }
+                __syncthreads();   // (the next pass's X / tile image writes are ordered behind these reads by its first barrier)
+                const int64_t i = (base + (int64_t)k * nctas) * TM + s;
+                if (owner && i < N) {
+                    EvalSlot<Env>& sl = sm.slot[k];
+                    float z[kOutMax];
+#pragma unroll
+                    for (int o = 0; o < kOutMax; ++o) z[o] = sm.net.b3[o] + sm.Zp[o * TM + s] + sm.Zp[(kOutMax + o) * TM + s];
+                    uint32_t a_bits;
+                    if (MODE == 0) {
+                        a_bits = greedy::greedy_action(g.actor, z);
+                    } else {
+                        unsigned long long pr[4] = {sl.prng[s], sl.prng[TM + s], sl.prng[2 * TM + s], sl.prng[3 * TM + s]};
+                        float lp;
+                        a_bits = sample_head(g.actor, g.hp, z, pr, lp);
+                        sl.prng[s] = pr[0]; sl.prng[TM + s] = pr[1]; sl.prng[2 * TM + s] = pr[2]; sl.prng[3 * TM + s] = pr[3];
+                    }
+                    // act!(env, a) + fused soft reset: the sequence of env_step_kernel<Env, false, true> (and rollout_tc_kernel)
+                    act_t act;
+                    if (std::is_same<act_t, float>::value) act = (act_t)fminf(fmaxf(__uint_as_float(a_bits), g.act_lo), g.act_hi);
+                    else act = (act_t)(int32_t)a_bits;
+                    typename Env::S st = sl.st[s];
+                    int tt = sl.t[s];
+                    const int prev = sl.flags[s];
+                    bool done;
+                    float rew;
+                    Env::step(p, st, tt, act, done, rew);
+                    if (ea.max_timeout > 0 && tt + 1 > ea.max_timeout) done = true;
+                    float ret = sl.ep_ret[s] + rew;
+                    int f = done ? 1 : 0;
+                    if (done && !((prev & 1) && !(prev & 2))) { sm.fin_cnt[s] += 1; sm.fin_ret[s] += ret; sm.fin_len[s] += tt; }
+                    if (done) {
+                        const int e = sl.cnt[s];   // record of the episode that ends: its return and env.t
+                        if (e < g.K) {
+                            if (g.returns) g.returns[(size_t)g.K * i + e] = ret;
+                            if (g.lengths) g.lengths[(size_t)g.K * i + e] = tt;
+                        }
+                        sl.cnt[s] = e + 1;
+                        ret = 0.f;
+                        Xo ex{sl.erng[s], sl.erng[TM + s], sl.erng[2 * TM + s], sl.erng[3 * TM + s]};
+                        Env::reset(p, st, ex, act);
+                        sl.erng[s] = ex.s0; sl.erng[TM + s] = ex.s1; sl.erng[2 * TM + s] = ex.s2; sl.erng[3 * TM + s] = ex.s3;
+                        tt = 0;
+                        f = 3;
+                    }
+                    sl.st[s] = st; sl.t[s] = tt; sl.flags[s] = f; sl.ep_ret[s] = ret;
+                    sl.last_rew[s] = rew;
+                    { act_t tmp = act; uint32_t bits; memcpy(&bits, &tmp, 4); sl.last_act[s] = bits; }
+                }
+            }
+        }
+        // ---- write the group back (each owner thread touches only its own entries: no barrier before the next group's loads)
+        if (owner) {
+            for (int k = 0; k < nslots; ++k) {
+                const int64_t i = (base + (int64_t)k * nctas) * TM + s;
+                EvalSlot<Env>& sl = sm.slot[k];
+                if (i < N) {
+                    Env::store(ea.state, i, sl.st[s]);
+                    if (!Env::kObsIsState) Env::write_obs(ea.obs, i, N, sl.st[s]);
+                    ea.t[i] = sl.t[s];
+                    ea.flags[i] = (uint8_t)sl.flags[s];
+                    ea.ep_ret[i] = sl.ep_ret[s];
+                    store_rng(ea.rng, i, Xo{sl.erng[s], sl.erng[TM + s], sl.erng[2 * TM + s], sl.erng[3 * TM + s]});
+                    if (MODE == 1) {
+                        unsigned long long pr[4] = {sl.prng[s], sl.prng[TM + s], sl.prng[2 * TM + s], sl.prng[3 * TM + s]};
+                        store_rng32(g.policy_rng, i, pr);
+                    }
+                    reinterpret_cast<float*>(ea.reward)[i] = sl.last_rew[s];
+                    reinterpret_cast<uint32_t*>(ea.action)[i] = sl.last_act[s];
+                    if (g.counts) g.counts[i] = sl.cnt[s];
+                }
+            }
+        }
+    }
+    // episode statistics: one atomicAdd triple per CTA
+    {
+        int fin_cnt = owner ? sm.fin_cnt[s] : 0, fin_len = owner ? sm.fin_len[s] : 0;
+        float fin_ret = owner ? sm.fin_ret[s] : 0.f;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            fin_cnt += __shfl_xor_sync(0xffffffffu, fin_cnt, o);
+            fin_len += __shfl_xor_sync(0xffffffffu, fin_len, o);
+            fin_ret += __shfl_xor_sync(0xffffffffu, fin_ret, o);
+        }
+        __syncthreads();
+        if (lane == 0) { sm.red_i[warp] = fin_cnt; sm.red_f[warp] = fin_ret; sm.red_l[warp] = fin_len; }
+        __syncthreads();
+        if (tid == 0) {
+            double cc = 0, rr = 0, ll = 0;
+            for (int w = 0; w < NT / 32; ++w) { cc += sm.red_i[w]; rr += sm.red_f[w]; ll += sm.red_l[w]; }
+            if (cc > 0) { atomicAdd(&ea.stats[0], cc); atomicAdd(&ea.stats[1], rr); atomicAdd(&ea.stats[2], ll); }
+        }
+    }
+}
+
+template <class Env> int launch_evaluate(b200rl_ctx* ctx, const EvalArgs& g, const typename Env::P& p, const EnvArrays& ea, int mode) {
+    const size_t smem = sizeof(SmemEval<Env>) + 128;
+    static unsigned long long attr_devices = 0;   // once per device
+    if (first_use_on_device(attr_devices, ctx->device)) {
+        CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_RELU, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_TANH, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_RELU, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_TANH, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
+    const int64_t groups = ((g.N + TM - 1) / TM + kSlots - 1) / kSlots;
+    int grid = 2 * ctx->sm_count;
+    if ((int64_t)grid > groups) grid = (int)groups;
+    const bool relu = g.actor.act == B200RL_ACT_RELU;
+    if (mode == 0) {
+        if (relu) evaluate_tc_kernel<Env, B200RL_ACT_RELU, 0><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
+        else evaluate_tc_kernel<Env, B200RL_ACT_TANH, 0><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
+    } else {
+        if (relu) evaluate_tc_kernel<Env, B200RL_ACT_RELU, 1><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
+        else evaluate_tc_kernel<Env, B200RL_ACT_TANH, 1><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
+    }
+    LAUNCH_CHECK(ctx);
+    return B200RL_OK;
+}
+
 }  // namespace
 
 bool nn_tc_supported(const MlpDesc& d) { return d.H == 64 && d.in <= kInMax && d.nout <= kOutMax; }
@@ -432,6 +666,47 @@ int nn_tc_rollout(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const 
             } else {
                 if (actor.nout != 3) return B200RL_ERR_UNSUPPORTED;
                 st = launch_rollout<MountainCarD<false>>(ctx, g, v.p.mc, v.a);
+            }
+            break;
+    }
+    if (st == B200RL_OK) b200rl_env_internal_add_steps(env, (uint64_t)nsteps);
+    return st;
+}
+
+// Fused evaluation window (after the caller's forced reset).  The caller has validated net <-> env; B200RL_ERR_UNSUPPORTED
+// (no side effect, no error message) = outside the fused envelope: the caller steps through staged launches instead.
+int nn_tc_evaluate(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const float* params, const AcHyper& hp, int mode, int nsteps,
+                   int K, unsigned long long* policy_rng, float* returns, int32_t* lengths, int32_t* counts) {
+    EnvView v;
+    TRY(b200rl_env_internal_view(env, &v));
+    if (!nn_tc_supported(actor) || v.dtype != B200RL_F32) return B200RL_ERR_UNSUPPORTED;
+    EvalArgs g{actor, params, hp, v.N, nsteps, K, -1.0f, 1.0f, policy_rng, returns, lengths, counts};
+    int st = B200RL_ERR_UNSUPPORTED;
+    switch (v.kind) {
+        case B200RL_ENV_CARTPOLE:
+            if (v.continuous) {
+                CartPoleD<float, true>::P q;
+                memcpy(&q, &v.p.cp32, sizeof q);
+                st = launch_evaluate<CartPoleD<float, true>>(ctx, g, q, v.a, mode);
+            } else {
+                st = launch_evaluate<CartPoleD<float, false>>(ctx, g, v.p.cp32, v.a, mode);
+            }
+            break;
+        case B200RL_ENV_PENDULUM:
+            if (v.continuous) {
+                g.act_lo = -2.0f; g.act_hi = 2.0f;      // PendulumEnv.jl:73: action_space -2.0..2.0
+                st = launch_evaluate<PendulumD<true>>(ctx, g, v.p.pend, v.a, mode);
+            } else {
+                st = launch_evaluate<PendulumD<false>>(ctx, g, v.p.pend, v.a, mode);
+            }
+            break;
+        case B200RL_ENV_MOUNTAINCAR:
+            if (v.continuous) {
+                MountainCarD<true>::P q;
+                memcpy(&q, &v.p.mc, sizeof q);
+                st = launch_evaluate<MountainCarD<true>>(ctx, g, q, v.a, mode);
+            } else {
+                st = launch_evaluate<MountainCarD<false>>(ctx, g, v.p.mc, v.a, mode);
             }
             break;
     }

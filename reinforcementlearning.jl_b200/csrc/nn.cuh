@@ -109,6 +109,10 @@ struct b200rl_env;
 int nn_tc_rollout(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const MlpDesc& critic, const float* params, const AcHyper& hp,
                   unsigned long long* policy_rng, int t0, int nsteps, int T, int final_bootstrap, float* states, void* actions, float* logp,
                   float* values, float* rewards, uint8_t* terminals);
+// fused evaluation window (fwd_tc.cu): nsteps x {actor -> greedy (mode 0) | sampled (mode 1) action, env step, episode records};
+// B200RL_ERR_UNSUPPORTED = outside the fused envelope, step through staged launches instead
+int nn_tc_evaluate(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const float* params, const AcHyper& hp, int mode, int nsteps,
+                   int K, unsigned long long* policy_rng, float* returns, int32_t* lengths, int32_t* counts);
 bool nn_tc_bwd_supported(const MlpDesc& actor, const MlpDesc& critic);
 int nn_tc_partial_rows(int grid, const MlpDesc& actor, const AcHyper& hp, int64_t B);   // gradient-partial rows the tensor-core K7 writes with `grid` CTAs
 int nn_tc_ac_loss_grad(b200rl_ctx* ctx, int grid, const MlpDesc& actor, const MlpDesc& critic, const float* params, const AcHyper& hp,

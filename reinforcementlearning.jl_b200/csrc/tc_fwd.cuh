@@ -102,13 +102,14 @@ __device__ __forceinline__ float xo_f32(unsigned long long (&s)[4]) { return (fl
 // image layout of the weights, row = sample)
 // (the loops over 16-feature halves here and 8-feature groups in head_partials are deliberately NOT unrolled: tanhf is ~40
 // instructions, and with every instance inlined the rollout kernel was 290 KB of SASS whose dominant stall was instruction fetch)
-// ACT: the activation as a compile-time constant (-1: read `act`); relu trunks expect load_net(.., s1 = kScale)
-template <int ACT>
+// ACT: the activation as a compile-time constant (-1: read `act`); relu trunks expect load_net(.., s1 = kScale).  UNROLL: copies
+// of the half loop (the arithmetic per feature and its order do not depend on it; 1 saves registers)
+template <int ACT, int UNROLL = (ACT == B200RL_ACT_RELU ? 2 : 1)>
 __device__ __forceinline__ void layer1_to_smem(const NetSm& w, int act_rt, const float (&x)[kInMax], int c, int s, uint8_t* tile) {
     const int act = ACT >= 0 ? ACT : act_rt;
     uint8_t* blk = tile + (s >> 6) * BLK;
     const int r = s & 63;
-#pragma unroll(ACT == B200RL_ACT_RELU ? 2 : 1)
+#pragma unroll(UNROLL)
     for (int half = 0; half < 2; ++half) {
         uint32_t hi8[8], lo8[8];
 #pragma unroll
@@ -167,15 +168,15 @@ __device__ __forceinline__ void gemm_block(uint8_t* blk, const NetSm& w, int wgi
             *reinterpret_cast<float2*>(blk + dacc_off(row0 + 8 * h, 8 * j + col0)) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
 }
 
-// epilogue of this thread's sample: H2[32c .. 32c+32) = act(D + b2), partial head sums over these 32 features
-template <int ACT>
+// epilogue of this thread's sample: H2[32c .. 32c+32) = act(D + b2), partial head sums over these 32 features (UNROLL: as above)
+template <int ACT, int UNROLL = (ACT == B200RL_ACT_RELU ? 2 : 1)>
 __device__ __forceinline__ void head_partials(const NetSm& w, int act_rt, int c, int s, const uint8_t* tile, float (&zp)[kOutMax]) {
     const int act = ACT >= 0 ? ACT : act_rt;
     const uint8_t* blk = tile + (s >> 6) * BLK;
     const int r = s & 63;
 #pragma unroll
     for (int o = 0; o < kOutMax; ++o) zp[o] = 0.f;
-#pragma unroll(ACT == B200RL_ACT_RELU ? 2 : 1)
+#pragma unroll(UNROLL)
     for (int grp = 0; grp < 2; ++grp) {
         float v[16];
 #pragma unroll

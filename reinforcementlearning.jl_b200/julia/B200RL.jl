@@ -29,7 +29,7 @@ using ReinforcementLearningCore: AbstractStage, PreExperimentStage, PostExperime
     EpsilonGreedyExplorer, GreedyExplorer, AbstractExplorer
 
 export B200Context, B200VecEnv, B200Network, B200OnPolicyAgent, B200RandomPolicy, B200Trajectory, B200DQNLearner, B200QBasedPolicy,
-    B200Agent, B200EpisodeStats, InsertSampleRatio
+    B200Agent, B200EpisodeStats, InsertSampleRatio, B200GreedyPolicy, evaluate
 
 const LIB = get(ENV, "B200RL_LIB", joinpath(@__DIR__, "..", "libb200rl.so"))
 
@@ -571,6 +571,68 @@ function RLBase.plan!(p::B200QBasedPolicy{GreedyExplorer}, env::B200VecEnv)
     check(ccall((:b200rl_net_q_act, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Ptr{Cvoid}, Cfloat, Ptr{Cvoid}),
                 p.learner.net.h, device_ptr(env, OBS), p.n, C_NULL, 0f0, p.d_action))
     DeviceActions(p.d_action)
+end
+
+# ---- evaluation -------------------------------------------------------------------------------
+"""
+    B200GreedyPolicy(net::B200Network, n)
+
+The network's greedy policy on a batch of `n` envs with a discrete action space: `findmax` of the logits / Q-values
+(`GreedyExplorer`, explorers/epsilon_greedy_explorer.jl:196-204; no RNG).  `plan!` leaves the actions on the device
+(`DeviceActions`), so `run(B200GreedyPolicy(net, n), env, StopAfterNSteps(k), hook)` never copies an action to the host.
+For a Gaussian policy use [`evaluate`](@ref), which hands `clamp(μ, lo, hi)` to the env inside the kernel.
+"""
+mutable struct B200GreedyPolicy <: AbstractPolicy
+    net::B200Network
+    n::Int
+    d_action::Ptr{Cvoid}
+end
+function B200GreedyPolicy(net::B200Network, n::Integer)
+    p = B200GreedyPolicy(net, Int(n), dmalloc(net.ctx, 4n))
+    finalizer(x -> (x.net.ctx.h == C_NULL || ccall((:b200rl_free, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), x.net.ctx.h, x.d_action)), p)
+end
+function RLBase.plan!(p::B200GreedyPolicy, env::B200VecEnv)
+    env.continuous && throw(ArgumentError("B200GreedyPolicy plans discrete actions; evaluate a Gaussian policy with `evaluate`"))
+    check(ccall((:b200rl_net_act_greedy, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Ptr{Cvoid}, Cint),
+                p.net.h, device_ptr(env, OBS), p.n, p.d_action, 1))
+    DeviceActions(p.d_action)
+end
+
+struct EvalConfigC
+    mode::Int32; n_steps::Int32; max_episodes::Int32
+end
+"""
+    evaluate(net, env; n_steps, max_episodes = 1, mode = :greedy, policy_seeds = nothing)
+
+`run(policy, env, StopAfterNSteps(n_steps))` with the network's greedy (`:greedy`) or sampling (`:sample`, one policy stream per
+env from `policy_seeds`) policy, as one fused kernel launch where the network allows it (b200rl_evaluate): every env is reset
+first, finished envs auto-reset.  Returns `(; returns, lengths, counts)`: the first `max_episodes` episodes of each env that
+end inside the window (`max_episodes × n` matrices; NaN / -1 where no episode ended) and the number of episodes per env.
+Average over the envs with `counts .>= max_episodes` to avoid the bias towards short episodes of a fixed window.  The env's
+episode statistics advance as under `run`; the network is only read.
+"""
+function evaluate(net::B200Network, env::B200VecEnv; n_steps::Integer, max_episodes::Integer = 1, mode::Symbol = :greedy,
+                  policy_seeds::Union{Nothing,AbstractVector{Xoshiro}} = nothing)
+    m = mode === :greedy ? 0 : mode === :sample ? 1 : throw(ArgumentError("mode must be :greedy or :sample"))
+    n = env.n
+    returns = fill(NaN32, max_episodes, n)
+    lengths = fill(Int32(-1), max_episodes, n)
+    counts = zeros(Int32, n)
+    d_rng = C_NULL
+    if policy_seeds !== nothing
+        length(policy_seeds) == n || throw(ArgumentError("need one Xoshiro per env"))
+        st = raw_states(policy_seeds)
+        d_rng = dmalloc(net.ctx, 32n)
+        GC.@preserve st check(ccall((:b200rl_memcpy_h2d, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Csize_t, Cint), net.ctx.h, d_rng, st, 32n, 0))
+    end
+    try
+        GC.@preserve returns lengths counts check(ccall((:b200rl_evaluate, LIB), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Ref{EvalConfigC}, Ptr{Cvoid}, Ptr{Float32}, Ptr{Int32}, Ptr{Int32}, Cint),
+            net.h, env.h, Ref(EvalConfigC(m, n_steps, max_episodes)), d_rng, returns, lengths, counts, 0))
+    finally
+        d_rng == C_NULL || ccall((:b200rl_free, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), net.ctx.h, d_rng)
+    end
+    (; returns, lengths, counts)
 end
 
 """

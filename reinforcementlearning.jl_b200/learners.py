@@ -459,6 +459,111 @@ class QBasedPolicy(AbstractPolicy):
                 self.learner.update()
 
 
+EVAL_MODES = {"greedy": 0, "sample": 1}
+
+
+class EvaluationPolicy(AbstractPolicy):
+    """The network's policy without training: ``plan`` runs one forward pass on state(env) and leaves the actions on the
+    device, ``act_fused`` hands them to ``env.act_``.  ``run(EvaluationPolicy(net, n), env, StopAfterNSteps(k), hook)`` is the
+    stage protocol of :func:`evaluate`.
+
+    mode "greedy": findmax of the logits / Q-values, mu of a Gaussian head (b200rl_net_act_greedy; no RNG).
+    mode "sample": b200rl_net_act's sampler on one policy stream per env; ``rng``: (N, 4) uint64 raw Xoshiro states.
+    A continuous action goes to the env as clamp(a, lo, hi) of its action space (through the host, like OnPolicyAgent's
+    host-action path)."""
+
+    def __init__(self, net, n, mode="greedy", rng=None):
+        if mode not in EVAL_MODES:
+            raise ValueError(f"mode must be one of {sorted(EVAL_MODES)}")
+        if mode == "sample" and rng is None:
+            raise ValueError('mode "sample" needs rng: (N, 4) uint64 policy streams')
+        self.net, self.ctx, self.lib, self.n, self.mode = net, net.ctx, net.ctx.lib, int(n), mode
+        self._d_action = self.ctx.malloc(self.n * 4)
+        self._d_rng = None
+        if mode == "sample":
+            rng = np.ascontiguousarray(rng, np.uint64).reshape(self.n, 4)
+            self._d_rng = self.ctx.malloc(rng.nbytes)
+            self.ctx.h2d(self._d_rng, rng)
+        self._host_act = None
+
+    def close(self):
+        for name in ("_d_action", "_d_rng"):
+            p = getattr(self, name, None)
+            if p:
+                self.ctx.free(p)
+                setattr(self, name, None)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def plan_device(self, env):
+        """plan!(policy, env) leaving the raw actions (int32 | float) on the device; returns their device pointer."""
+        obs = C.c_void_p(env.device_ptr(L.FIELD_OBS))
+        if self.mode == "greedy":
+            L.check(self.lib.b200rl_net_act_greedy(self.net.h, obs, self.n, C.c_void_p(self._d_action), 1))
+        else:
+            L.check(self.lib.b200rl_net_act(self.net.h, obs, self.n, C.c_void_p(self._d_rng), C.c_void_p(self._d_action),
+                                            None, None, None, 1))
+        return self._d_action
+
+    def plan(self, env):
+        d = self.plan_device(env)
+        if env.continuous:
+            if self._host_act is None:
+                self._host_act = np.empty(self.n, np.float32)
+            lo, hi = env.action_space()
+            return np.clip(self.ctx.d2h(self._host_act, d), np.float32(lo), np.float32(hi))
+        return FusedAction("policy")
+
+    def act_fused(self, env):
+        env.act_(int(self._d_action))
+
+    def rng_state(self):
+        """the policy streams (N, 4) after the steps so far (mode "sample")"""
+        out = np.empty((self.n, 4), np.uint64)
+        return self.ctx.d2h(out, self._d_rng)
+
+
+def evaluate(net, env, n_steps, max_episodes=1, mode="greedy", rng=None):
+    """b200rl_evaluate: ``run(policy, env, StopAfterNSteps(n_steps))`` with the network's greedy or sampling policy, in one
+    fused launch where the network allows it.  Forces a reset of every env first; the env's episode statistics advance as
+    under ``run``.
+
+    ``rng`` (mode "sample"): (N, 4) uint64 policy streams, advanced in place, or a device pointer (int) to them.
+    Returns ``returns`` (K, N) float32 and ``lengths`` (K, N) int32 (the first K = max_episodes episodes of each env that
+    end inside the window; slots no episode reaches hold NaN / -1) and ``counts`` (N,) int32 (episodes per env, may exceed K).
+    Average over the envs with ``counts >= K`` to avoid the bias towards short episodes of a fixed window."""
+    if mode not in EVAL_MODES:
+        raise ValueError(f"mode must be one of {sorted(EVAL_MODES)}")
+    ctx, lib, n, K = net.ctx, net.ctx.lib, env.n, int(max_episodes)
+    returns = np.full((K, n), np.nan, np.float32, order="F")
+    lengths = np.full((K, n), -1, np.int32, order="F")
+    counts = np.zeros(n, np.int32)
+    d_rng, host_rng = None, None
+    if rng is not None and not isinstance(rng, (int, np.integer)):
+        host_rng = rng
+        arr = np.ascontiguousarray(rng, np.uint64).reshape(n, 4)
+        d_rng = ctx.malloc(arr.nbytes)
+        ctx.h2d(d_rng, arr)
+    elif rng is not None:
+        d_rng = int(rng)
+    cfg = L.EvalConfig(EVAL_MODES[mode], int(n_steps), K)
+    try:
+        L.check(lib.b200rl_evaluate(net.h, env.h, C.byref(cfg), None if d_rng is None else C.c_void_p(d_rng), L.ptr(returns),
+                                    L.ptr(lengths), L.ptr(counts), 0))
+        if host_rng is not None:
+            out = np.empty((n, 4), np.uint64)
+            ctx.d2h(out, d_rng)
+            host_rng[...] = out.reshape(np.shape(host_rng))
+    finally:
+        if host_rng is not None:
+            ctx.free(d_rng)
+    return dict(returns=returns, lengths=lengths, counts=counts)
+
+
 class Agent(AbstractPolicy):
     """Agent(policy, trajectory) (agent_base.jl:18-66) for a device-resident replay trajectory: pushes the env's
     transition frames (state / action / reward / terminal never visit the host) and lets the policy's learner train
