@@ -377,6 +377,35 @@ typedef struct {
 int b200rl_dqn_update(b200rl_net* net, b200rl_traj* traj, const b200rl_dqn_config* cfg, float* stats_host);
 int b200rl_dqn_last_td(b200rl_net* net, b200rl_traj* traj, float* host_dst, int64_t count);
 
+/* ---------------------------------------------------------------- DQN agent loop --- */
+/* InsertSampleRatioController(ratio, threshold) (ReinforcementLearningTrajectories 0.4): one insertion = one pushed frame of
+ * every lane; after it, batches are sampled while n_inserted >= threshold and n_sampled <= (n_inserted - threshold) * ratio
+ * (Float64 product, as the Julia / Python controller computes it). */
+typedef struct { double ratio; int64_t threshold, n_inserted, n_sampled; } b200rl_insert_sample_ratio;
+typedef struct b200rl_replay b200rl_replay;
+/* run(Agent(QBasedPolicy(DQNLearner, explorer), Trajectory), env, StopAfterNSteps(n)) (RLCore/src/core/run.jl:52-68) on the
+ * device, for a hook with nothing to do per step: n_steps x {plan! (BatchExplorer over Q(state(env), .)), act!, push!(trajectory),
+ * optimise! (one DQN update per batch the controller allows)}.  act! ALWAYS uses the in-kernel auto-reset (b200rl_env_step(..., 1))
+ * and honours MaxTimeoutEnv: drive a soft-reset env through the stage protocol instead.  A stretch of steps without an update is
+ * ONE collect launch for H = 64 on the tensor-core path (replay_collect_tc_kernel; the sum tree is rebuilt once per stretch) and
+ * staged launches otherwise; each "1 step + m updates" unit is replayed from a CUDA graph keyed by m (captured on its second use).
+ * Results equal the stage protocol's bit for bit (the FP64 return sum of the episode statistics may differ in its last bits
+ * where rewards are not integers).  The explorer step, the update counter and the controller counters advance on the host by
+ * arithmetic.  The trajectory keeps (min(2k + 1, capacity + 1), N) touched-leaf keys for the longest stretch k (prioritised).
+ * create refuses, before any side effect: a network that is not a Q-network, a Float64 / continuous-action / Acrobot env,
+ * trajectory lanes != N or a state width that does not match, a sharded ctx (world > 1).  The trajectory needs a sampler. */
+int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl_traj* traj, const b200rl_dqn_config* cfg,
+                         b200rl_replay** out);
+/* explorer_rng_dev: (4, N) DEVICE explorer streams (one per env, advanced).  ex: EpsilonGreedyExplorer (its step is advanced
+ * by n_steps * N), NULL = GreedyExplorer (findmax, no draw).  ctl: counters advanced.  stats4 (may be NULL; synchronises):
+ * loss, grad_norm, mean |td|, n_updates of the last update in the window (untouched when the window ran none).  Refuses a bad
+ * explorer schedule or controller values before any side effect.  A CUDA error part-way through returns with the device state
+ * advanced and *ex / *ctl NOT advanced: the run cannot be continued from them. */
+int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explorer* ex, b200rl_insert_sample_ratio* ctl,
+                      int64_t n_steps, float* stats4);
+int b200rl_replay_graph_active(b200rl_replay* r, int* out);   /* 1: a "1 step + m updates" unit has been captured and replayed */
+int b200rl_replay_destroy(b200rl_replay* r);
+
 /* select the wgmma tensor-core kernels (default, H = 64) or the FP32 CUDA-core kernels for the dense layers */
 int b200rl_set_tensor_cores(int enable);
 /* 1 (default; B200RL_FUSED_STEP=0 in the environment starts with 0): the on-policy update runs reduce + [peer exchange] + clip +

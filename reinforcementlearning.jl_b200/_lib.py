@@ -56,6 +56,11 @@ class Explorer(C.Structure):
                 ("step", C.c_int64), ("kind", C.c_int32), ("is_break_tie", C.c_int32)]
 
 
+class InsertSampleRatio(C.Structure):
+    """b200rl_insert_sample_ratio: InsertSampleRatioController's ratio, threshold and counters."""
+    _fields_ = [("ratio", C.c_double), ("threshold", C.c_int64), ("n_inserted", C.c_int64), ("n_sampled", C.c_int64)]
+
+
 class EvalConfig(C.Structure):
     """b200rl_eval_config: mode 0 greedy | 1 sample, window length, records kept per env."""
     _fields_ = [(n, C.c_int32) for n in ("mode", "n_steps", "max_episodes")]
@@ -166,6 +171,10 @@ SIGNATURES = {
     "b200rl_onpolicy_time_kernel": (_i32, [_vp, _i32, _i32, C.POINTER(_f32)]),
     "b200rl_dqn_update": (_i32, [_vp, _vp, _vp, _vp]),
     "b200rl_dqn_last_td": (_i32, [_vp, _vp, _vp, _i64]),
+    "b200rl_replay_create": (_i32, [_vp, _vp, _vp, _vp, _vp, _pp]),
+    "b200rl_replay_run": (_i32, [_vp, _vp, _vp, _vp, _i64, _vp]),
+    "b200rl_replay_graph_active": (_i32, [_vp, C.POINTER(_i32)]),
+    "b200rl_replay_destroy": (_i32, [_vp]),
     "b200rl_set_tensor_cores": (_i32, [_i32]),
     "b200rl_set_fused_step": (_i32, [_i32]),
     "b200rl_comm_unique_id": (_i32, [_vp]),

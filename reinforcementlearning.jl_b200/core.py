@@ -340,19 +340,26 @@ def run(policy, env=None, stop_condition=None, hook=None, reset_condition=None):
     # {plan!, act!, push!}) — the same transitions, parameters and statistics as stepping through the stages.
     if (getattr(policy, "fusable", False) and env.auto_reset and not getattr(hook, "per_step", True)
             and isinstance(stop_condition, StopAfterNSteps) and isinstance(reset_condition, ResetIfEnvTerminated)):
-        while not is_stop:
-            if policy._t == 0 and stop_condition.remaining() >= policy.T and hasattr(policy, "iterate"):
-                # whole iterations (rollout + update) as one CUDA-graph launch each (b200rl_onpolicy_iterate)
-                k = stop_condition.remaining() // policy.T if not policy.fetch_stats else 1
-                policy.iterate(k, want_stats=policy.fetch_stats)
-                is_stop = stop_condition.advance(k * policy.T)
-                continue
-            n = min(policy.T - policy._t, stop_condition.remaining())
-            policy.collect(n)
-            if policy._t == policy.T:
-                policy._t = 0
-                policy.update(want_stats=policy.fetch_stats)
-            is_stop = stop_condition.advance(n)
+        if hasattr(policy, "run_replay"):
+            # replay Agent: the whole stretch as device launches (b200rl_replay_run), updates replayed as CUDA graphs
+            if policy.replay_supported(env):
+                n = stop_condition.remaining()
+                policy.run_replay(env, n)
+                is_stop = stop_condition.advance(n)
+        else:
+            while not is_stop:
+                if policy._t == 0 and stop_condition.remaining() >= policy.T and hasattr(policy, "iterate"):
+                    # whole iterations (rollout + update) as one CUDA-graph launch each (b200rl_onpolicy_iterate)
+                    k = stop_condition.remaining() // policy.T if not policy.fetch_stats else 1
+                    policy.iterate(k, want_stats=policy.fetch_stats)
+                    is_stop = stop_condition.advance(k * policy.T)
+                    continue
+                n = min(policy.T - policy._t, stop_condition.remaining())
+                policy.collect(n)
+                if policy._t == policy.T:
+                    policy._t = 0
+                    policy.update(want_stats=policy.fetch_stats)
+                is_stop = stop_condition.advance(n)
     def act(action):
         if isinstance(action, FusedAction):
             if action.kind == "random":

@@ -1,6 +1,7 @@
 // algo.cu — host-side orchestration behind the C ABI: network handle (FluxApproximator +
 // optimiser state + TargetNetwork), the on-policy agent (PPO / A2C: plan! -> act! -> push! ->
-// optimise!), and the DQN update on a prioritised trajectory.  All arithmetic is in the
+// optimise!), the DQN update on a prioritised trajectory and the DQN agent loop (plan! -> act! ->
+// push! -> optimise! with the updates replayed as CUDA graphs).  All arithmetic is in the
 // kernels of nn.cu / returns.cu / traj.cu / env.cu; this file sequences launches on the ctx
 // stream and owns the rollout tensors.
 //
@@ -8,8 +9,12 @@
 // FluxApproximator/optimise! policies/learners/flux_approximator.jl:11-46; TargetNetwork
 // target_network.jl:27-88; PPO/A2C/DQN update rules: ReinforcementLearningZoo (absent from the
 // snapshot; SURVEY Appendix B), hyper-parameters docs/homepage/blog/a_practical_introduction_to_RL.jl/index.html:15238-15286.
+#include <map>
+
 #include "greedy.cuh"
 #include "nn.cuh"
+#include "replay_schedule.h"
+#include "ring.cuh"
 
 // other translation units
 int b200rl_gae_fused_internal(b200rl_ctx* ctx, float* adv, float* ret, const float* r, const float* v, const uint8_t* term, float gamma,
@@ -26,6 +31,12 @@ TrajBatchView b200rl_traj_internal_batch(b200rl_traj* t);
 bool b200rl_traj_internal_prioritized(b200rl_traj* t);
 b200rl_ctx* b200rl_traj_internal_ctx(b200rl_traj* t);
 int64_t b200rl_traj_internal_lanes(b200rl_traj* t);
+void b200rl_traj_internal_add_pushed(b200rl_traj* t, int64_t n);
+int64_t b200rl_traj_internal_pushed(b200rl_traj* t);
+Ring b200rl_traj_internal_ring(b200rl_traj* t);
+float b200rl_traj_internal_default_priority(b200rl_traj* t);
+int b200rl_traj_internal_tree_rebuild(b200rl_traj* t, const int64_t* keys, const float* vals, int64_t n);
+uint64_t b200rl_env_internal_steps(const b200rl_env* e);
 int b200rl_traj_internal_priority_from_td(b200rl_traj* t, const float* td_dev, float eps, float alpha);
 int b200rl_comm_allreduce_internal(b200rl_ctx* ctx, void* buf, int64_t n, int is_double);
 int b200rl_comm_world(b200rl_ctx* ctx);
@@ -1049,11 +1060,10 @@ int b200rl_traj_push_env(b200rl_traj* t, b200rl_env* env, int first_state_only) 
 
 /* optimise!(DQNLearner / PrioritizedDQNLearner, batch): sample + gather (K4), TD loss + backward
  * (K7), clip + Adam (K8), priority write-back, target sync every target_update_freq updates.
- * stats_host[4] = loss, grad_norm, mean |td|, n_updates (NULL = no sync). */
-int b200rl_dqn_update(b200rl_net* n, b200rl_traj* t, const b200rl_dqn_config* cfg, float* stats_host) {
-    REQUIRE(n && t && cfg && n->kind == 2, B200RL_ERR_INVALID, "bad argument (needs a Q-network)");
-    REQUIRE(n->ctx == b200rl_traj_internal_ctx(t), B200RL_ERR_INVALID, "net/trajectory belong to different ctx");
-    TRY(ctx_bind(n->ctx));
+ * upd_dev (may be null): the sync phase is counted on the device (nn_target_sync_counted) instead of by a host `if`, so the
+ * sequence can be captured and replayed; n->n_updates advances either way.  td_keep (may be null): copy of the TD errors. */
+static int dqn_update_seq(b200rl_net* n, b200rl_traj* t, const b200rl_dqn_config* cfg, unsigned long long* upd_dev, float* td_keep,
+                          float** td_out) {
     b200rl_ctx* ctx = n->ctx;
     TRY(b200rl_traj_sample(t, cfg->per_beta));
     TrajBatchView b = b200rl_traj_internal_batch(t);
@@ -1083,19 +1093,39 @@ int b200rl_dqn_update(b200rl_net* n, b200rl_traj* t, const b200rl_dqn_config* cf
     }
     if (b200rl_traj_internal_prioritized(t)) TRY(b200rl_traj_internal_priority_from_td(t, td, cfg->per_eps, cfg->per_alpha));
     n->n_updates += 1;
-    if (cfg->target_update_freq > 0 && n->n_updates % (uint64_t)cfg->target_update_freq == 0) TRY(nn_target_sync(ctx, n->target, n->params, n->np, cfg->rho));
-    if (stats_host) {
-        float l4[4], gn;
-        std::vector<float> tdh((size_t)b.B);
-        CUDA_TRY(cudaMemcpyAsync(l4, n->loss4, 16, cudaMemcpyDeviceToHost, ctx->stream));
-        CUDA_TRY(cudaMemcpyAsync(&gn, n->gnorm, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CUDA_TRY(cudaMemcpyAsync(tdh.data(), td, (size_t)b.B * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-        double s = 0;
-        for (float x : tdh) s += x < 0 ? -x : x;
-        stats_host[0] = l4[0] / ((float)b.B * (float)world); stats_host[1] = gn; stats_host[2] = (float)(s / (double)b.B);
-        stats_host[3] = (float)n->n_updates;
+    if (upd_dev) TRY(nn_target_sync_counted(ctx, n->target, n->params, n->np, cfg->rho, upd_dev, cfg->target_update_freq));
+    else if (cfg->target_update_freq > 0 && n->n_updates % (uint64_t)cfg->target_update_freq == 0) TRY(nn_target_sync(ctx, n->target, n->params, n->np, cfg->rho));
+    if (td_keep) {
+        copy_f32_kernel<<<grid_for(b.B, 256), 256, 0, ctx->stream>>>(td_keep, td, b.B);
+        LAUNCH_CHECK(ctx);
     }
+    if (td_out) *td_out = td;
+    return B200RL_OK;
+}
+// stats4 = loss, grad_norm, mean |td|, n_updates of the update that wrote loss4 / gnorm / td (synchronises)
+static int dqn_stats(b200rl_net* n, const float* td, int64_t B, float* stats4) {
+    b200rl_ctx* ctx = n->ctx;
+    float l4[4], gn;
+    std::vector<float> tdh((size_t)B);
+    CUDA_TRY(cudaMemcpyAsync(l4, n->loss4, 16, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(&gn, n->gnorm, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(tdh.data(), td, (size_t)B * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    double s = 0;
+    for (float x : tdh) s += x < 0 ? -x : x;
+    const int world = b200rl_comm_world(ctx);
+    stats4[0] = l4[0] / ((float)B * (float)world); stats4[1] = gn; stats4[2] = (float)(s / (double)B);
+    stats4[3] = (float)n->n_updates;
+    return B200RL_OK;
+}
+
+int b200rl_dqn_update(b200rl_net* n, b200rl_traj* t, const b200rl_dqn_config* cfg, float* stats_host) {
+    REQUIRE(n && t && cfg && n->kind == 2, B200RL_ERR_INVALID, "bad argument (needs a Q-network)");
+    REQUIRE(n->ctx == b200rl_traj_internal_ctx(t), B200RL_ERR_INVALID, "net/trajectory belong to different ctx");
+    TRY(ctx_bind(n->ctx));
+    float* td = nullptr;
+    TRY(dqn_update_seq(n, t, cfg, nullptr, nullptr, &td));
+    if (stats_host) TRY(dqn_stats(n, td, b200rl_traj_internal_batch(t).B, stats_host));
     return B200RL_OK;
 }
 /* TD errors (B floats) of the batch used by the last b200rl_dqn_update (for parity tests) */
@@ -1108,6 +1138,267 @@ int b200rl_dqn_last_td(b200rl_net* n, b200rl_traj* t, float* host_dst, int64_t c
     REQUIRE(n->ctx->scratch_bytes >= q_bytes + (size_t)b.B * 4, B200RL_ERR_INVALID, "no update has run yet");
     CUDA_TRY(cudaMemcpyAsync(host_dst, (char*)n->ctx->scratch + q_bytes, (size_t)b.B * 4, cudaMemcpyDeviceToHost, n->ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(n->ctx->stream));
+    return B200RL_OK;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------ DQN agent loop ---------
+namespace {
+__global__ void add_i64_kernel(long long* __restrict__ v, long long d) { *v += d; }
+}  // namespace
+
+struct ReplayGraph {   // one "1 step + m updates" unit
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    uint64_t launches = 0;   // kernels in the graph (ctx->launches advances by this per replay)
+    int uses = 0;
+};
+// what the captured launches bake in besides the handles: a change means re-capture
+struct ReplayKey {
+    int tc, max_timeout, greedy, pad;
+    b200rl_explorer ex;          // step zeroed (it lives in device memory)
+    const void* rng;
+    const void* scratch;
+    const void* keys;
+    bool operator!=(const ReplayKey& o) const { return memcmp(this, &o, sizeof *this) != 0; }
+};
+struct b200rl_replay {
+    b200rl_ctx* ctx;
+    b200rl_net* net;
+    b200rl_env* env;
+    b200rl_traj* traj;
+    b200rl_dqn_config cfg;
+    int64_t N, B;
+    int32_t* action;              // (N) planned actions
+    long long* ex_step_dev;       // explorer step, advanced by N per step on the device
+    unsigned long long* upd_dev;  // optimiser steps of the Q-network (the target-sync phase), advanced per update on the device
+    float* td_keep;               // TD errors of the last update
+    int64_t* keys; float* vals;   // (stride, N) sum-tree leaves a fused collect window touched (prioritised ring)
+    int stride_cap;               // rows of keys / vals allocated
+    long long h_counters[2];
+    std::map<int64_t, ReplayGraph> graphs;
+    ReplayKey key;
+    bool graph_failed;
+};
+
+static void replay_drop_graphs(b200rl_replay* r) {
+    for (auto& kv : r->graphs) {
+        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+        if (kv.second.graph) cudaGraphDestroy(kv.second.graph);
+        kv.second.exec = nullptr; kv.second.graph = nullptr;
+    }
+}
+
+// plan! -> act! -> push!(trajectory): the launches of the stage protocol (QBasedPolicy.plan_device, env.act_, Agent.push)
+static int replay_collect_step(b200rl_replay* r, uint64_t* rng, const b200rl_explorer* ex) {
+    b200rl_ctx* ctx = r->ctx;
+    b200rl_net* n = r->net;
+    const float* obs = (const float*)env_field(r->env, B200RL_FIELD_OBS);
+    void* s;
+    TRY(ctx_scratch(ctx, (size_t)r->N * n->actor.nout * 4 + 256, &s));
+    if (ex) {
+        TRY(nn_q_explore(ctx, n->actor, n->params, obs, r->N, (unsigned long long*)rng, *ex, r->action, (float*)s, r->ex_step_dev));
+        add_i64_kernel<<<1, 1, 0, ctx->stream>>>(r->ex_step_dev, (long long)r->N);
+        LAUNCH_CHECK(ctx);
+    } else {
+        TRY(nn_q_act(ctx, n->actor, n->params, obs, r->N, nullptr, 0.0f, r->action, (float*)s));
+    }
+    TRY(b200rl_env_step(r->env, r->action, 1, 1));
+    return b200rl_traj_push_env(r->traj, r->env, 0);
+}
+static int replay_stride(const b200rl_replay* r, int64_t k) {
+    const int64_t F = b200rl_traj_internal_ring(r->traj).frames();
+    return (int)(2 * k + 1 < F ? 2 * k + 1 : F);
+}
+// k collect steps: one fused launch (H = 64 on the tensor-core path; + one sum-tree rebuild for a prioritised ring), otherwise k x
+// the staged launches
+static int replay_collect(b200rl_replay* r, uint64_t* rng, const b200rl_explorer* ex, int64_t k) {
+    b200rl_ctx* ctx = r->ctx;
+    b200rl_net* n = r->net;
+    const bool prio = b200rl_traj_internal_prioritized(r->traj);
+    const int stride = replay_stride(r, k);
+    if (nn_tc_enabled() && (!prio || stride <= r->stride_cap)) {
+        int st = nn_tc_replay_collect(ctx, r->env, n->actor, n->params, ex, r->ex_step_dev, (unsigned long long*)rng, b200rl_traj_internal_ring(r->traj),
+                                      b200rl_traj_internal_default_priority(r->traj), prio ? 1 : 0, (int)k, r->keys, r->vals, stride);
+        if (st == B200RL_OK) {
+            if (ex) {
+                add_i64_kernel<<<1, 1, 0, ctx->stream>>>(r->ex_step_dev, (long long)r->N * k);
+                LAUNCH_CHECK(ctx);
+            }
+            b200rl_traj_internal_add_pushed(r->traj, k);
+            if (prio) TRY(b200rl_traj_internal_tree_rebuild(r->traj, r->keys, r->vals, (int64_t)stride * r->N));
+            return B200RL_OK;
+        }
+        if (st != B200RL_ERR_UNSUPPORTED) return st;
+    }
+    for (int64_t j = 0; j < k; ++j) TRY(replay_collect_step(r, rng, ex));
+    return B200RL_OK;
+}
+static int replay_unit(b200rl_replay* r, uint64_t* rng, const b200rl_explorer* ex, int64_t m) {
+    TRY(replay_collect(r, rng, ex, 1));
+    for (int64_t k = 0; k < m; ++k) TRY(dqn_update_seq(r->net, r->traj, &r->cfg, r->upd_dev, r->td_keep, nullptr));
+    return B200RL_OK;
+}
+
+extern "C" {
+
+int b200rl_replay_destroy(b200rl_replay* r) {
+    if (!r) return B200RL_OK;
+    cudaSetDevice(r->ctx->device);
+    cudaStreamSynchronize(r->ctx->stream);
+    replay_drop_graphs(r);
+    cudaFree(r->action); cudaFree(r->ex_step_dev); cudaFree(r->upd_dev); cudaFree(r->td_keep); cudaFree(r->keys); cudaFree(r->vals);
+    delete r;
+    return B200RL_OK;
+}
+
+int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl_traj* traj, const b200rl_dqn_config* cfg, b200rl_replay** out) {
+    TRY(ctx_bind(ctx));
+    REQUIRE(q && env && traj && cfg && out, B200RL_ERR_INVALID, "null argument");
+    REQUIRE(q->kind == 2, B200RL_ERR_INVALID, "needs a Q-network (kind 2)");
+    REQUIRE(q->ctx == ctx && b200rl_env_internal_ctx(env) == ctx && b200rl_traj_internal_ctx(traj) == ctx, B200RL_ERR_INVALID,
+            "net/env/trajectory belong to another ctx");
+    REQUIRE(b200rl_env_internal_dtype(env) == B200RL_F32, B200RL_ERR_UNSUPPORTED, "the Q-network reads Float32 observations: construct the env with T = Float32");
+    REQUIRE(b200rl_env_internal_kind(env) != B200RL_ENV_ACROBOT, B200RL_ERR_UNSUPPORTED, "AcrobotEnv has 6 observations (networks take at most 4)");
+    REQUIRE(!b200rl_env_internal_continuous(env), B200RL_ERR_UNSUPPORTED, "QBasedPolicy needs a discrete action space");
+    REQUIRE(b200rl_env_internal_nobs(env) == q->actor.in, B200RL_ERR_INVALID, "network input width != observation width");
+    REQUIRE(q->actor.nout == b200rl_env_internal_n_actions(env), B200RL_ERR_INVALID, "Q head width != number of discrete actions");
+    const int64_t N = b200rl_env_internal_n(env);
+    REQUIRE(b200rl_traj_internal_lanes(traj) == N, B200RL_ERR_INVALID, "trajectory lanes != number of envs");
+    TrajBatchView b = b200rl_traj_internal_batch(traj);
+    REQUIRE(b.B > 0, B200RL_ERR_INVALID, "the trajectory was created without a sampler (batch_size = 0)");
+    REQUIRE(b.ns == q->actor.in, B200RL_ERR_INVALID, "trajectory state width != network input width");
+    REQUIRE(b200rl_comm_world(ctx) == 1, B200RL_ERR_UNSUPPORTED, "the replay agent loop runs on one GPU (communicator world > 1)");
+    b200rl_replay* r = new b200rl_replay();
+    r->ctx = ctx; r->net = q; r->env = env; r->traj = traj; r->cfg = *cfg; r->N = N; r->B = b.B;
+    r->action = nullptr; r->ex_step_dev = nullptr; r->upd_dev = nullptr; r->td_keep = nullptr; r->keys = nullptr; r->vals = nullptr;
+    r->stride_cap = 0;
+    memset(&r->key, 0, sizeof r->key);
+    r->graph_failed = false;
+#define R_TRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { b200rl_set_error("%s -> %s", #x, cudaGetErrorString(_e)); b200rl_replay_destroy(r); return _e == cudaErrorMemoryAllocation ? B200RL_ERR_OOM : B200RL_ERR_CUDA; } } while (0)
+    R_TRY(cudaMalloc(&r->action, (size_t)N * 4));
+    R_TRY(cudaMalloc(&r->ex_step_dev, sizeof(long long)));
+    R_TRY(cudaMalloc(&r->upd_dev, sizeof(unsigned long long)));
+    R_TRY(cudaMalloc(&r->td_keep, (size_t)b.B * 4));
+#undef R_TRY
+    *out = r;
+    return B200RL_OK;
+}
+
+int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explorer* ex, b200rl_insert_sample_ratio* ctl, int64_t n_steps, float* stats4) {
+    REQUIRE(r && ctl, B200RL_ERR_INVALID, "null argument");
+    REQUIRE(n_steps >= 0, B200RL_ERR_INVALID, "n_steps must be >= 0");
+    if (ex) {
+        REQUIRE(explorer_rng_dev, B200RL_ERR_INVALID, "an epsilon-greedy explorer needs the (4, N) device explorer streams");
+        REQUIRE((ex->kind == 0 || ex->kind == 1) && ex->warmup_steps >= 0 && ex->decay_steps >= 0, B200RL_ERR_INVALID, "bad explorer schedule");
+        REQUIRE(ex->eps_stable >= 0.0 && ex->eps_stable <= 1.0 && ex->eps_init >= 0.0 && ex->eps_init <= 1.0, B200RL_ERR_INVALID, "epsilon outside [0, 1]");
+        REQUIRE(n_steps <= ((1ll << 62) - (ex->step > 0 ? ex->step : 0)) / r->N, B200RL_ERR_INVALID, "explorer step would overflow");
+    }
+    REQUIRE(replay::controller_ok(*ctl), B200RL_ERR_INVALID, "bad controller values (ratio finite in [0, 1e6], counters >= 0)");
+    REQUIRE(ctl->n_inserted + n_steps < (1ll << 52), B200RL_ERR_INVALID, "controller counters too large");
+    TRY(ctx_bind(r->ctx));
+    b200rl_ctx* ctx = r->ctx;
+    b200rl_net* n = r->net;
+    if (n_steps == 0) return B200RL_OK;
+    // every scratch user of the loop at its final size now, so that no captured launch sees the buffer move
+    void* sc;
+    const size_t q_bytes = (size_t)r->B * n->actor.nout * 4 * 2 + 256;
+    const size_t need_upd = q_bytes + (size_t)r->B * 4 + 256, need_q = (size_t)r->N * n->actor.nout * 4 + 256;
+    TRY(ctx_scratch(ctx, need_upd > need_q ? need_upd : need_q, &sc));
+    // the schedule of the window: m updates after each step; stretches of steps without an update become one collect launch
+    b200rl_insert_sample_ratio c = *ctl;
+    std::vector<int64_t> ms((size_t)n_steps);
+    int64_t longest = 1, run = 0;
+    for (int64_t j = 0; j < n_steps; ++j) {
+        ms[(size_t)j] = replay::insert_then_sample(c);
+        run = ms[(size_t)j] == 0 ? run + 1 : 0;
+        if (run > longest) longest = run;
+    }
+    if (b200rl_traj_internal_prioritized(r->traj) && replay_stride(r, longest) > r->stride_cap) {   // touched-leaf lists of a window
+        const int stride = replay_stride(r, longest);
+        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+        cudaFree(r->keys); cudaFree(r->vals);
+        r->keys = nullptr; r->vals = nullptr; r->stride_cap = 0;
+        CUDA_TRY(cudaMalloc(&r->keys, (size_t)stride * r->N * 8));
+        CUDA_TRY(cudaMalloc(&r->vals, (size_t)stride * r->N * 4));
+        r->stride_cap = stride;
+    }
+    ReplayKey key;
+    memset(&key, 0, sizeof key);
+    key.tc = nn_tc_enabled() ? 1 : 0;
+    key.max_timeout = b200rl_env_internal_max_timeout(r->env);
+    key.greedy = ex ? 0 : 1;
+    if (ex) { key.ex = *ex; key.ex.step = 0; }
+    key.rng = explorer_rng_dev;
+    key.scratch = ctx->scratch;
+    key.keys = r->keys;
+    if (key != r->key) { replay_drop_graphs(r); r->key = key; }
+    // device copies of the counters the launches read
+    r->h_counters[0] = ex ? (long long)ex->step : 0;
+    r->h_counters[1] = (long long)n->n_updates;
+    CUDA_TRY(cudaMemcpyAsync(r->ex_step_dev, &r->h_counters[0], sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(r->upd_dev, &r->h_counters[1], sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
+    static int graph_env = -1;
+    if (graph_env < 0) { const char* e = getenv("B200RL_GRAPH"); graph_env = (e && e[0] == '0') ? 0 : 1; }
+    const bool capturable = graph_env && !r->graph_failed && ctx->phase_base < 0;
+    bool updated = false;
+    for (int64_t j = 0; j < n_steps;) {
+        const int64_t m = ms[(size_t)j];
+        if (m == 0) {   // a stretch of steps without an update: one collect window
+            int64_t k = 1;
+            while (j + k < n_steps && ms[(size_t)(j + k)] == 0) ++k;
+            TRY(replay_collect(r, explorer_rng_dev, ex, k));
+            j += k;
+            continue;
+        }
+        ++j;
+        updated = true;
+        ReplayGraph& G = r->graphs[m];
+        if (!capturable || G.uses++ == 0) {   // first use eager (lazy loading, function attributes)
+            TRY(replay_unit(r, explorer_rng_dev, ex, m));
+            continue;
+        }
+        if (!G.exec) {
+            // capture does not execute: the host-side bookkeeping of the captured calls is measured, rolled back and redone per replay
+            const uint64_t l0 = ctx->launches, nu0 = n->n_updates, es0 = b200rl_env_internal_steps(r->env);
+            const int64_t p0 = b200rl_traj_internal_pushed(r->traj);
+            CUDA_TRY(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
+            int st = replay_unit(r, explorer_rng_dev, ex, m);
+            cudaGraph_t g = nullptr;
+            cudaError_t ce = cudaStreamEndCapture(ctx->stream, &g);
+            G.launches = ctx->launches - l0;
+            ctx->launches = l0; n->n_updates = nu0;
+            b200rl_env_internal_add_steps(r->env, es0 - b200rl_env_internal_steps(r->env));
+            b200rl_traj_internal_add_pushed(r->traj, p0 - b200rl_traj_internal_pushed(r->traj));
+            cudaError_t ie = cudaErrorUnknown;
+            if (st == B200RL_OK && ce == cudaSuccess && g) ie = cudaGraphInstantiate(&G.exec, g, 0);
+            if (ie != cudaSuccess) {
+                if (g) cudaGraphDestroy(g);
+                cudaGetLastError();
+                G.exec = nullptr;
+                r->graph_failed = true;   // stay on eager launches
+                TRY(replay_unit(r, explorer_rng_dev, ex, m));
+                continue;
+            }
+            G.graph = g;
+        }
+        CUDA_TRY(cudaGraphLaunch(G.exec, ctx->stream));
+        ctx->launches += G.launches;
+        n->n_updates += (uint64_t)m;
+        b200rl_env_internal_add_steps(r->env, 1);
+        b200rl_traj_internal_add_pushed(r->traj, 1);
+    }
+    *ctl = c;
+    if (ex) ex->step += n_steps * r->N;
+    if (stats4 && updated) TRY(dqn_stats(n, r->td_keep, r->B, stats4));
+    return B200RL_OK;
+}
+
+int b200rl_replay_graph_active(b200rl_replay* r, int* out) {
+    REQUIRE(r && out, B200RL_ERR_INVALID, "null argument");
+    *out = 0;
+    for (auto& kv : r->graphs) if (kv.second.exec) *out = 1;
     return B200RL_OK;
 }
 

@@ -534,6 +534,7 @@ int b200rl_env_internal_view(b200rl_env* e, envdev::EnvView* out) {
     return B200RL_OK;
 }
 void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n) { e->steps_launched += n; }
+uint64_t b200rl_env_internal_steps(const b200rl_env* e) { return e->steps_launched; }
 int b200rl_env_internal_max_timeout(const b200rl_env* e) { return e->a.max_timeout; }
 int b200rl_env_internal_dtype(const b200rl_env* e) { return e->dtype; }
 int64_t b200rl_env_internal_n(const b200rl_env* e) { return e->N; }

@@ -12,7 +12,9 @@
 // (-fmad=false): stepping through plan!/act! one launch at a time or through the fused rollout gives bit-identical results.
 #include "common.cuh"
 #include "env_device.cuh"
+#include "explore.cuh"
 #include "greedy.cuh"
+#include "ring.cuh"
 #include "tc_fwd.cuh"
 
 using namespace tcfwd;
@@ -598,6 +600,256 @@ template <class Env> int launch_evaluate(b200rl_ctx* ctx, const EvalArgs& g, con
     return B200RL_OK;
 }
 
+
+// ---------------------------------------------------------------------------------------------------------------------
+// fused DQN collect (b200rl_replay_run): nsteps x { obs -> Q -> BatchExplorer column (explore.cuh) | findmax (GreedyExplorer) ->
+// env step (+ fused auto-reset) -> push!(trajectory) of the lane (ring.cuh) }.  The Q-network is fixed during a window, so a CTA
+// runs the whole window on one group of up to kSlots resident tiles (env state, env stream and explorer stream in shared
+// memory), writes it back and takes the next group (no limit on N).  Sum-tree leaves are written as the pushes happen (a lane
+// owns its leaves, so the last write is the final value); after the window each lane emits the keys of its touched slots — a
+// contiguous run mod cap + 1, at most cap + 1 of them, no duplicates — and the caller rebuilds the tree once from the children,
+// which gives the tree the per-step rebuilds give.  The head outputs are those of nn_mlp_forward's tensor-core path (see
+// evaluate_tc_kernel), so the actions equal the staged q_explore / q_act selection bit for bit.
+template <class Env> struct ReplaySlot {
+    typename Env::S st[TM];
+    int t[TM];
+    int flags[TM];
+    float ep_ret[TM];
+    float last_rew[TM];
+    int32_t last_act[TM];
+    int p0[TM];                            // slot of the first touched leaf of the lane (head - 1 at the start)
+    int adv[TM];                           // frames written in the window
+    unsigned long long erng[4 * TM];       // env stream      [word][env]
+    unsigned long long xrng[4 * TM];       // explorer stream [word][env]
+};
+template <class Env> struct SmemReplay {
+    alignas(128) uint8_t T[TILE_BYTES];
+    NetSm net;
+    float X[kInMax * TM];
+    float Zp[2 * kOutMax * TM];
+    ReplaySlot<Env> slot[kSlots];
+    int fin_cnt[TM], fin_len[TM];
+    float fin_ret[TM];
+    long long dv[TM];                      // change of the sampleable count, per owner thread
+    float red_f[8];
+    int red_i[8], red_l[8];
+    long long red_v[8];
+};
+struct ReplayArgs {
+    MlpDesc q;
+    const float* params;
+    int64_t N;
+    int nsteps;
+    int greedy;                            // 1: GreedyExplorer (findmax with `>`, no draw)
+    b200rl_explorer ex;
+    const long long* step_dev;             // explorer step before the window (device)
+    unsigned long long* xrng;              // (4, N) explorer streams
+    Ring ring;
+    float default_priority;
+    int prioritized;
+    int64_t* keys;                         // (stride, lanes): touched leaves of each lane, -1 padded
+    float* vals;
+    int stride;                            // min(2 nsteps + 1, cap + 1)
+};
+
+template <class Env, int ACT>
+__global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, typename Env::P p, EnvArrays ea) {
+    using act_t = typename Env::act_t;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    SmemReplay<Env>& sm = *reinterpret_cast<SmemReplay<Env>*>(smem_raw);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int q = warp & 3, c = warp >> 2;
+    const int s = 32 * q + lane;
+    const bool owner = c == 0;
+    const int64_t N = g.N;
+    const int nctas = gridDim.x;
+    const int64_t ntiles = (N + TM - 1) / TM;
+    const long long step0 = g.greedy ? 0 : *g.step_dev;
+    const Ring& r = g.ring;
+    const int64_t F = r.frames();
+    load_net(sm.net, g.q, g.params, ACT == B200RL_ACT_RELU ? kScale : 1.0f);
+    if (owner) { sm.fin_cnt[s] = 0; sm.fin_len[s] = 0; sm.fin_ret[s] = 0.f; sm.dv[s] = 0; }
+#pragma unroll 1
+    for (int64_t base = blockIdx.x; base < ntiles; base += (int64_t)nctas * kSlots) {
+        int nslots = 0;
+        for (int k = 0; k < kSlots; ++k)
+            if (base + (int64_t)k * nctas < ntiles) nslots = k + 1;
+        if (owner) {
+            for (int k = 0; k < nslots; ++k) {
+                const int64_t i = (base + (int64_t)k * nctas) * TM + s;
+                ReplaySlot<Env>& sl = sm.slot[k];
+                if (i < N) {
+                    sl.st[s] = Env::load(ea.state, i);
+                    sl.t[s] = ea.t[i];
+                    sl.flags[s] = ea.flags[i];
+                    sl.ep_ret[s] = ea.ep_ret[i];
+                    sl.p0[s] = (int)(((int64_t)r.head[i] + F - 1) % F);
+                    sl.adv[s] = 0;
+                    Xo e = load_rng(ea.rng, i);
+                    sl.erng[s] = e.s0; sl.erng[TM + s] = e.s1; sl.erng[2 * TM + s] = e.s2; sl.erng[3 * TM + s] = e.s3;
+                    if (!g.greedy) {
+                        unsigned long long xr[4];
+                        load_rng32(g.xrng, i, xr);
+                        sl.xrng[s] = xr[0]; sl.xrng[TM + s] = xr[1]; sl.xrng[2 * TM + s] = xr[2]; sl.xrng[3 * TM + s] = xr[3];
+                    }
+                }
+            }
+        }
+        wg::fence_proxy_async();
+        __syncthreads();
+#pragma unroll 1
+        for (int step = 0; step < g.nsteps; ++step) {
+#pragma unroll 1
+            for (int k = 0; k < nslots; ++k) {
+                if (owner) {
+                    float o[kInMax] = {0.f, 0.f, 0.f, 0.f};
+                    if ((base + (int64_t)k * nctas) * TM + s < N) Env::observe(sm.slot[k].st[s], o);
+#pragma unroll
+                    for (int j = 0; j < kInMax; ++j) sm.X[j * TM + s] = o[j];
+                }
+                __syncthreads();
+                {
+                    float x[kInMax];
+#pragma unroll
+                    for (int j = 0; j < kInMax; ++j) x[j] = sm.X[j * TM + s];
+                    layer1_to_smem<ACT, 1>(sm.net, g.q.act, x, c, s, sm.T);
+                }
+                wg::fence_proxy_async();
+                __syncthreads();
+                gemm_block(sm.T + c * BLK, sm.net, c);
+                __syncthreads();
+                {
+                    float zp[kOutMax];
+                    head_partials<ACT, 1>(sm.net, g.q.act, c, s, sm.T, zp);
+#pragma unroll
+                    for (int o = 0; o < kOutMax; ++o) sm.Zp[(c * kOutMax + o) * TM + s] = zp[o];
+                }
+                __syncthreads();
+                const int64_t i = (base + (int64_t)k * nctas) * TM + s;
+                if (owner && i < N) {
+                    ReplaySlot<Env>& sl = sm.slot[k];
+                    float z[kOutMax];
+#pragma unroll
+                    for (int o = 0; o < kOutMax; ++o) z[o] = sm.net.b3[o] + sm.Zp[o * TM + s] + sm.Zp[(kOutMax + o) * TM + s];
+                    int a1;
+                    if (g.greedy) {
+                        int best = 0;      // q_act_kernel with epsilon = 0: the first maximum under `>`
+                        for (int o = 1; o < g.q.nout; ++o) if (z[o] > z[best]) best = o;
+                        a1 = best + 1;
+                    } else {
+                        unsigned long long xr[4] = {sl.xrng[s], sl.xrng[TM + s], sl.xrng[2 * TM + s], sl.xrng[3 * TM + s]};
+                        a1 = explore::select(g.ex, step0 + (long long)step * N + i, z, g.q.nout, xr);
+                        sl.xrng[s] = xr[0]; sl.xrng[TM + s] = xr[1]; sl.xrng[2 * TM + s] = xr[2]; sl.xrng[3 * TM + s] = xr[3];
+                    }
+                    // act!(env, a) + fused auto-reset: the sequence of env_step_kernel<Env, false, true>
+                    act_t act = (act_t)a1;
+                    typename Env::S st = sl.st[s];
+                    int tt = sl.t[s];
+                    const int prev = sl.flags[s];
+                    bool done;
+                    float rew;
+                    Env::step(p, st, tt, act, done, rew);
+                    if (ea.max_timeout > 0 && tt + 1 > ea.max_timeout) done = true;
+                    float ret = sl.ep_ret[s] + rew;
+                    int f = done ? 1 : 0;
+                    if (done && !((prev & 1) && !(prev & 2))) { sm.fin_cnt[s] += 1; sm.fin_ret[s] += ret; sm.fin_len[s] += tt; }
+                    if (done) {
+                        ret = 0.f;
+                        Xo ex{sl.erng[s], sl.erng[TM + s], sl.erng[2 * TM + s], sl.erng[3 * TM + s]};
+                        Env::reset(p, st, ex, act);
+                        sl.erng[s] = ex.s0; sl.erng[TM + s] = ex.s1; sl.erng[2 * TM + s] = ex.s2; sl.erng[3 * TM + s] = ex.s3;
+                        tt = 0;
+                        f = 3;
+                    }
+                    sl.st[s] = st; sl.t[s] = tt; sl.flags[s] = f; sl.ep_ret[s] = ret;
+                    sl.last_rew[s] = rew;
+                    sl.last_act[s] = (int32_t)act;
+                    // push!(trajectory, (state = s', action, reward, terminal)) of lane i
+                    float nobs[kInMax];
+                    Env::observe(st, nobs);
+                    RingLeaves lv;
+                    int adv = 0;
+                    sm.dv[s] += ring::push_sart(r, i, (int32_t)act, rew, (uint8_t)f, nobs, g.default_priority, lv, &adv);
+                    sl.adv[s] += adv;
+                    if (g.prioritized)
+                        for (int j = 0; j < 3; ++j) if (lv.key[j] >= 0) r.tree[r.L + lv.key[j]] = lv.val[j];
+                }
+            }
+        }
+        if (owner) {
+            for (int k = 0; k < nslots; ++k) {
+                const int64_t i = (base + (int64_t)k * nctas) * TM + s;
+                ReplaySlot<Env>& sl = sm.slot[k];
+                if (i < N) {
+                    Env::store(ea.state, i, sl.st[s]);
+                    if (!Env::kObsIsState) Env::write_obs(ea.obs, i, N, sl.st[s]);
+                    ea.t[i] = sl.t[s];
+                    ea.flags[i] = (uint8_t)sl.flags[s];
+                    ea.ep_ret[i] = sl.ep_ret[s];
+                    store_rng(ea.rng, i, Xo{sl.erng[s], sl.erng[TM + s], sl.erng[2 * TM + s], sl.erng[3 * TM + s]});
+                    if (!g.greedy) {
+                        unsigned long long xr[4] = {sl.xrng[s], sl.xrng[TM + s], sl.xrng[2 * TM + s], sl.xrng[3 * TM + s]};
+                        store_rng32(g.xrng, i, xr);
+                    }
+                    if (g.nsteps > 0) {
+                        reinterpret_cast<float*>(ea.reward)[i] = sl.last_rew[s];
+                        reinterpret_cast<int32_t*>(ea.action)[i] = sl.last_act[s];
+                    }
+                    if (g.prioritized) {   // the lane's touched slots p0, p0 + 1, ... (mod cap + 1), one key each
+                        const int n_touched = (int)min((int64_t)sl.adv[s] + 1, F);
+                        for (int j = 0; j < g.stride; ++j) {
+                            int64_t key = -1;
+                            float v = 0.f;
+                            if (j < n_touched) { key = (((int64_t)sl.p0[s] + j) % F) * r.lanes + i; v = r.tree[r.L + key]; }
+                            g.keys[(int64_t)j * N + i] = key;
+                            g.vals[(int64_t)j * N + i] = v;
+                        }
+                    }
+                }
+            }
+        }
+    }
+    // episode statistics and the sampleable count: one atomic each per CTA
+    {
+        int fin_cnt = owner ? sm.fin_cnt[s] : 0, fin_len = owner ? sm.fin_len[s] : 0;
+        float fin_ret = owner ? sm.fin_ret[s] : 0.f;
+        long long dv = owner ? sm.dv[s] : 0;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            fin_cnt += __shfl_xor_sync(0xffffffffu, fin_cnt, o);
+            fin_len += __shfl_xor_sync(0xffffffffu, fin_len, o);
+            fin_ret += __shfl_xor_sync(0xffffffffu, fin_ret, o);
+            dv += __shfl_xor_sync(0xffffffffu, dv, o);
+        }
+        __syncthreads();
+        if (lane == 0) { sm.red_i[warp] = fin_cnt; sm.red_f[warp] = fin_ret; sm.red_l[warp] = fin_len; sm.red_v[warp] = dv; }
+        __syncthreads();
+        if (tid == 0) {
+            double cc = 0, rr = 0, ll = 0;
+            long long vv = 0;
+            for (int w = 0; w < NT / 32; ++w) { cc += sm.red_i[w]; rr += sm.red_f[w]; ll += sm.red_l[w]; vv += sm.red_v[w]; }
+            if (cc > 0) { atomicAdd(&ea.stats[0], cc); atomicAdd(&ea.stats[1], rr); atomicAdd(&ea.stats[2], ll); }
+            if (vv != 0) atomicAdd((unsigned long long*)r.n_valid, (unsigned long long)vv);
+        }
+    }
+}
+
+template <class Env> int launch_replay_collect(b200rl_ctx* ctx, const ReplayArgs& g, const typename Env::P& p, const EnvArrays& ea) {
+    const size_t smem = sizeof(SmemReplay<Env>) + 128;
+    static unsigned long long attr_devices = 0;   // once per device
+    if (first_use_on_device(attr_devices, ctx->device)) {
+        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_TANH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
+    const int64_t groups = ((g.N + TM - 1) / TM + kSlots - 1) / kSlots;
+    int grid = 2 * ctx->sm_count;
+    if ((int64_t)grid > groups) grid = (int)groups;
+    if (g.q.act == B200RL_ACT_RELU) replay_collect_tc_kernel<Env, B200RL_ACT_RELU><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
+    else replay_collect_tc_kernel<Env, B200RL_ACT_TANH><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
+    LAUNCH_CHECK(ctx);
+    return B200RL_OK;
+}
+
 }  // namespace
 
 bool nn_tc_supported(const MlpDesc& d) { return d.H == 64 && d.in <= kInMax && d.nout <= kOutMax; }
@@ -709,6 +961,26 @@ int nn_tc_evaluate(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const
                 st = launch_evaluate<MountainCarD<false>>(ctx, g, v.p.mc, v.a, mode);
             }
             break;
+    }
+    if (st == B200RL_OK) b200rl_env_internal_add_steps(env, (uint64_t)nsteps);
+    return st;
+}
+
+// Fused DQN collect window (see replay_collect_tc_kernel).  The caller has validated net <-> env <-> ring and sized keys / vals to
+// (stride, N); B200RL_ERR_UNSUPPORTED (no side effect) = outside the fused envelope: the caller steps through staged launches.
+int nn_tc_replay_collect(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& q, const float* params, const b200rl_explorer* ex,
+                         const long long* step_dev, unsigned long long* xrng, const Ring& ring, float default_priority, int prioritized,
+                         int nsteps, int64_t* keys, float* vals, int stride) {
+    EnvView v;
+    TRY(b200rl_env_internal_view(env, &v));
+    if (!nn_tc_supported(q) || v.dtype != B200RL_F32 || v.continuous || ring.ns > kInMax) return B200RL_ERR_UNSUPPORTED;
+    ReplayArgs g{q, params, v.N, nsteps, ex ? 0 : 1, ex ? *ex : b200rl_explorer{}, step_dev, xrng, ring, default_priority, prioritized,
+                 keys, vals, stride};
+    int st = B200RL_ERR_UNSUPPORTED;
+    switch (v.kind) {
+        case B200RL_ENV_CARTPOLE: st = launch_replay_collect<CartPoleD<float, false>>(ctx, g, v.p.cp32, v.a); break;
+        case B200RL_ENV_PENDULUM: st = launch_replay_collect<PendulumD<false>>(ctx, g, v.p.pend, v.a); break;
+        case B200RL_ENV_MOUNTAINCAR: st = launch_replay_collect<MountainCarD<false>>(ctx, g, v.p.mc, v.a); break;
     }
     if (st == B200RL_OK) b200rl_env_internal_add_steps(env, (uint64_t)nsteps);
     return st;

@@ -13,6 +13,7 @@
 // (RLCore/src/utils/networks.jl:405-432), Gaussian head + diagnormlogpdf (networks.jl:44-116,
 // distributions.jl:9-34), clip_by_global_norm! (basic.jl:19-29), TargetNetwork sync
 // (policies/learners/target_network.jl:70-88).
+#include "explore.cuh"
 #include "nn.cuh"
 #include "perm.cuh"
 
@@ -840,6 +841,16 @@ __global__ void target_sync_kernel(float* __restrict__ target, const float* __re
     int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (k < np) target[k] = rho * target[k] + (1.0f - rho) * model[k];
 }
+// the same sync behind a device-side update counter (single CTA): *upd += 1, then sync when *upd % freq == 0 — the phase check of
+// b200rl_dqn_update without a host `if`, so the update sequence can be captured once and replayed
+__global__ void __launch_bounds__(1024) target_sync_counted_kernel(float* __restrict__ target, const float* __restrict__ model, int64_t np, float rho,
+                                                                 unsigned long long* __restrict__ upd, int freq) {
+    const unsigned long long u = *upd + 1;
+    __syncthreads();
+    if (threadIdx.x == 0) *upd = u;
+    if (freq <= 0 || u % (unsigned long long)freq != 0) return;
+    for (int64_t k = threadIdx.x; k < np; k += blockDim.x) target[k] = rho * target[k] + (1.0f - rho) * model[k];
+}
 
 // ------------------------------------------------------------- DQN --------------------------
 // phase A (forward_kernel mode 1 on the target / online nets) gives Q(s') tables; this kernel
@@ -939,67 +950,18 @@ __global__ void q_act_kernel(const float* __restrict__ qv, int na, int64_t N, un
     action_out[i] = best + 1;
 }
 
-// rand(rng, Base.OneTo(n)) — Lemire nearly-divisionless on UInt64 (Julia 1.10 SamplerRangeNDL), 1-based
-__device__ __forceinline__ int xo_oneto(unsigned long long (&s)[4], unsigned long long n) {
-    unsigned long long x = xo_next(s);
-    unsigned long long hi = __umul64hi(x, n), lo = x * n;
-    if (lo < n) {
-        unsigned long long t = (0ull - n) % n;
-        while (lo < t) {
-            x = xo_next(s);
-            hi = __umul64hi(x, n);
-            lo = x * n;
-        }
-    }
-    return (int)hi + 1;
-}
-// get_ϵ(s::EpsilonGreedyExplorer{:linear | :exp}, step) (epsilon_greedy_explorer.jl:69-91): Float64, evaluated left to
-// right with explicitly rounded operations (no FMA contraction, like the reference's Julia code)
-__device__ __forceinline__ double explorer_eps(const b200rl_explorer& e, long long step) {
-    if (step <= e.warmup_steps) return e.eps_init;
-    if (e.kind == 0) {
-        if (step >= e.warmup_steps + e.decay_steps) return e.eps_stable;
-        long long steps_left = e.warmup_steps + e.decay_steps - step;
-        return __dadd_rn(e.eps_stable, __dmul_rn(__ddiv_rn((double)steps_left, (double)e.decay_steps), __dsub_rn(e.eps_init, e.eps_stable)));
-    }
-    long long n = step - e.warmup_steps;
-    double scale = __dsub_rn(e.eps_init, e.eps_stable);
-    return __dadd_rn(e.eps_stable, __dmul_rn(scale, exp(__ddiv_rn(__dmul_rn(-1.0, (double)n), (double)e.decay_steps))));
-}
 // BatchExplorer(EpsilonGreedyExplorer) over the columns of a (na, N) Q table (explorers/batch_explorer.jl:15-21,
 // epsilon_greedy_explorer.jl:102-112): column i is planned with get_ϵ(step + i) — the inner explorer's step advances once
-// per column — drawing from its own stream: rand(rng) >= ϵ ? (findmax | rand(rng, find_all_max)) : rand(rng, 1:na).
-// The uniform draw happens even when ϵ = 0, exactly like the reference.
+// per column — drawing from its own stream (explore.cuh).  step_dev (may be null): the step is read from device memory
+// instead of ex.step, so a captured launch can be replayed.
 __global__ void q_explore_kernel(const float* __restrict__ qv, int na, int64_t N, unsigned long long* __restrict__ rng, b200rl_explorer ex,
-                                 int32_t* __restrict__ action_out) {
+                                 const long long* __restrict__ step_dev, int32_t* __restrict__ action_out) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
-    const float* v = qv + (int64_t)na * i;
-    const double eps = explorer_eps(ex, ex.step + i);
+    const long long step = step_dev ? *step_dev : ex.step;
     unsigned long long st[4];
     load_rng32(rng, i, st);
-    const double u = xo_f64(st);
-    int action;
-    if (u >= eps) {
-        int best = 0;
-        for (int o = 1; o < na; ++o) {
-            const float a = v[o], b = v[best];
-            if ((a != a && b == b) || a > b) best = o;     // findmax: first maximum, NaN ranks highest
-        }
-        action = best + 1;
-        if (ex.is_break_tie) {
-            float mx = v[0];
-            for (int o = 1; o < na; ++o) mx = v[o] > mx ? v[o] : mx;
-            int cnt = 0;
-            for (int o = 0; o < na; ++o) cnt += v[o] == mx;
-            int pick = xo_oneto(st, (unsigned long long)(cnt > 0 ? cnt : 1));
-            for (int o = 0; o < na; ++o) {
-                if (v[o] == mx && --pick == 0) { action = o + 1; break; }
-            }
-        }
-    } else {
-        action = xo_oneto(st, (unsigned long long)na);
-    }
+    const int action = explore::select(ex, step + i, qv + (int64_t)na * i, na, st);
     store_rng32(rng, i, st);
     action_out[i] = action;
 }
@@ -1177,6 +1139,11 @@ int nn_target_sync(b200rl_ctx* ctx, float* target, const float* model, int64_t n
     LAUNCH_CHECK(ctx);
     return B200RL_OK;
 }
+int nn_target_sync_counted(b200rl_ctx* ctx, float* target, const float* model, int64_t np, float rho, unsigned long long* upd_dev, int freq) {
+    target_sync_counted_kernel<<<1, 1024, 0, ctx->stream>>>(target, model, np, rho, upd_dev, freq);
+    LAUNCH_CHECK(ctx);
+    return B200RL_OK;
+}
 
 // returns the number of gradient partials written (> 0) or a negative status
 int nn_dqn_loss_grad(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float* target, const float* s, const int32_t* a,
@@ -1201,9 +1168,9 @@ int nn_dqn_loss_grad(b200rl_ctx* ctx, const MlpDesc& q, const float* params, con
 int nn_dqn_max_partials(b200rl_ctx* ctx, int H) { return H == 64 ? 2 * ctx->sm_count : ctx->sm_count; }
 
 int nn_q_explore(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float* obs, int64_t N, unsigned long long* rng,
-                 const b200rl_explorer& ex, int32_t* action_out, float* q_out) {
+                 const b200rl_explorer& ex, int32_t* action_out, float* q_out, const long long* step_dev) {
     TRY(nn_mlp_forward(ctx, q, params, obs, N, q_out));
-    q_explore_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(q_out, q.nout, N, rng, ex, action_out);
+    q_explore_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(q_out, q.nout, N, rng, ex, step_dev, action_out);
     LAUNCH_CHECK(ctx);
     return B200RL_OK;
 }

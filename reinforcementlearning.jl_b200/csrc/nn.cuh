@@ -88,14 +88,17 @@ int nn_reduce_clip_adam(b200rl_ctx* ctx, const float* partial, int n_partials, i
                         float* beta_t, const float* loss_partial, int n_loss, float* loss_out4, float max_grad_norm, float lr, float b1, float b2,
                         float eps, float* gnorm_out, double* cta_sumsq, unsigned int* counter2, float* stats_row, unsigned int* tick);
 int nn_target_sync(b200rl_ctx* ctx, float* target, const float* model, int64_t np, float rho);
+// target sync every `freq` optimiser steps, counted on the device: *upd_dev += 1, sync when it is a multiple of freq
+int nn_target_sync_counted(b200rl_ctx* ctx, float* target, const float* model, int64_t np, float rho, unsigned long long* upd_dev, int freq);
 // DQN: TD loss + backward on a gathered batch (device arrays s (in,B), a, r, t, s2, w)
 int nn_dqn_loss_grad(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float* target, const float* s, const int32_t* a,
                      const float* r, const uint8_t* t, const float* s2, const float* w, int64_t B, float inv_B, float gamma, int huber,
                      int double_dqn, float* partial, float* loss_partial, float* td_out);
 int nn_q_act(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float* obs, int64_t N, unsigned long long* rng, float epsilon,
              int32_t* action_out, float* q_out);
+// step_dev (may be null): explorer step read from device memory instead of ex.step
 int nn_q_explore(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float* obs, int64_t N, unsigned long long* rng,
-                 const b200rl_explorer& ex, int32_t* action_out, float* q_out);
+                 const b200rl_explorer& ex, int32_t* action_out, float* q_out, const long long* step_dev = nullptr);
 
 // tensor-core (wgmma) variants, nn_tc.cu.  Used for H = 64 unless disabled (B200RL_TC=0 or b200rl_set_tensor_cores(0)).
 bool nn_tc_enabled();
@@ -113,6 +116,12 @@ int nn_tc_rollout(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const 
 // B200RL_ERR_UNSUPPORTED = outside the fused envelope, step through staged launches instead
 int nn_tc_evaluate(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const float* params, const AcHyper& hp, int mode, int nsteps,
                    int K, unsigned long long* policy_rng, float* returns, int32_t* lengths, int32_t* counts);
+// fused DQN collect window (fwd_tc.cu): nsteps x {Q -> explorer column | findmax, env step, ring push} for H = 64; the touched
+// sum-tree leaves of each lane go to keys / vals (stride, N) for one tree rebuild.  B200RL_ERR_UNSUPPORTED = outside the envelope
+struct Ring;
+int nn_tc_replay_collect(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& q, const float* params, const b200rl_explorer* ex,
+                         const long long* step_dev, unsigned long long* xrng, const Ring& ring, float default_priority, int prioritized,
+                         int nsteps, int64_t* keys, float* vals, int stride);
 bool nn_tc_bwd_supported(const MlpDesc& actor, const MlpDesc& critic);
 int nn_tc_partial_rows(int grid, const MlpDesc& actor, const AcHyper& hp, int64_t B);   // gradient-partial rows the tensor-core K7 writes with `grid` CTAs
 int nn_tc_ac_loss_grad(b200rl_ctx* ctx, int grid, const MlpDesc& actor, const MlpDesc& critic, const float* params, const AcHyper& hp,

@@ -19,6 +19,7 @@
 // A push is one thread per lane (neighbouring lanes write neighbouring addresses unless their episode counts differ);
 // a sample is one thread per batch slot: Xoshiro draw -> (rejection | sum-tree descent) -> 2 x state gather + scalars.
 #include "common.cuh"
+#include "ring.cuh"
 
 namespace {
 
@@ -53,87 +54,30 @@ __device__ __forceinline__ unsigned long long rand_below(Xo4& g, unsigned long l
     return hi;
 }
 
-struct Ring {
-    int ns;
-    int64_t lanes, cap;
-    float* state; int32_t* action; float* reward; uint8_t* flag;
-    int32_t* head;       // (lanes) next slot to write
-    int32_t* count;      // (lanes) state frames stored, <= cap + 1
-    uint8_t* pending;    // (lanes) the last stored transition was terminal and its episode-start frame has not been pushed yet
-    long long* n_valid;  // (1) sampleable entries over all lanes
-    float* tree; int64_t L;
-    __host__ __device__ int64_t frames() const { return cap + 1; }
-};
-constexpr uint8_t kTerminal = 1, kSampleable = 2;
-
-// ---- push kernels: one thread per lane; `keys`/`vals` (3 per lane) receive the sum-tree leaves to rewrite (key -1 = none) --------
-__device__ __forceinline__ void write_state(const Ring& r, int64_t slot, int64_t e, const float* __restrict__ obs) {
-    float* dst = r.state + (int64_t)r.ns * (slot * r.lanes + e);
-    const float* src = obs + (int64_t)r.ns * e;
-    for (int c = 0; c < r.ns; ++c) dst[c] = src[c];
-}
-// the state frame at `slot` is about to be overwritten: the entry that started there is gone
-__device__ __forceinline__ int destroy_entry(const Ring& r, int64_t slot, int64_t e) {
-    const int64_t k = slot * r.lanes + e;
-    const int was = (r.flag[k] & kSampleable) ? 1 : 0;
-    r.flag[k] = 0;
-    return was;
+// ---- push kernels: one thread per lane (ring.cuh); `keys`/`vals` (3 per lane) receive the sum-tree leaves to rewrite (key -1 = none)
+__device__ __forceinline__ void emit_leaves(int64_t e, const RingLeaves& lv, int64_t* __restrict__ keys, float* __restrict__ vals) {
+    if (!keys) return;
+    for (int j = 0; j < 3; ++j) { keys[3 * e + j] = lv.key[j]; vals[3 * e + j] = lv.val[j]; }
 }
 // push!(trajectory, (state = s0,)): mode 0 every lane, 1 only lanes whose last transition was terminal (soft reset)
 __global__ void push_episode_start_kernel(Ring r, const float* __restrict__ obs, int mode, float default_priority, int64_t* __restrict__ keys,
                                           float* __restrict__ vals) {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= r.lanes) return;
-    if (keys) { keys[3 * e] = -1; keys[3 * e + 1] = -1; keys[3 * e + 2] = -1; }
-    if (mode == 1 && !r.pending[e]) return;
-    const int64_t F = r.frames();
-    const int64_t h = r.head[e];
-    const int lost = destroy_entry(r, h, e);
-    write_state(r, h, e, obs);
-    if (keys) { keys[3 * e] = h * r.lanes + e; vals[3 * e] = 0.f; }
-    r.head[e] = (int32_t)((h + 1) % F);
-    r.count[e] = (int32_t)min((int64_t)r.count[e] + 1, F);
-    r.pending[e] = 0;
-    if (lost) atomicAdd((unsigned long long*)r.n_valid, (unsigned long long)(-1ll));
+    RingLeaves lv{{-1, -1, -1}, {0.f, 0.f, 0.f}};
+    if (mode == 1 && !r.pending[e]) { emit_leaves(e, lv, keys, vals); return; }
+    const long long dv = ring::push_episode_start(r, e, obs + (int64_t)r.ns * e, lv);
+    emit_leaves(e, lv, keys, vals);
+    if (dv != 0) atomicAdd((unsigned long long*)r.n_valid, (unsigned long long)dv);
 }
-// push!(trajectory, (state = s', action, reward, terminal)).  term[e]: bit0 terminal, bit1 "the env has already auto-reset: next_obs
-// is the first state of the next episode" (the env's FLAGS byte) -> the episode-start frame is written in the same launch.
+// push!(trajectory, (state = s', action, reward, terminal)).  term[e]: the env's FLAGS byte (ring::push_sart)
 __global__ void push_sart_kernel(Ring r, const int32_t* __restrict__ a, const float* __restrict__ rew, const uint8_t* __restrict__ term,
                                  const float* __restrict__ next_obs, float default_priority, int64_t* __restrict__ keys, float* __restrict__ vals) {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= r.lanes) return;
-    const int64_t F = r.frames();
-    const int64_t h = r.head[e];
-    const int64_t p = (h + F - 1) % F;                 // slot of the state the action was taken in
-    const uint8_t t = term[e];
-    r.action[p * r.lanes + e] = a[e];
-    r.reward[p * r.lanes + e] = rew[e];
-    r.flag[p * r.lanes + e] = (uint8_t)((t & kTerminal) | kSampleable);
-    long long dv = 1;
-    dv -= destroy_entry(r, h, e);
-    write_state(r, h, e, next_obs);
-    int64_t nh = (h + 1) % F;
-    int cnt = (int)min((int64_t)r.count[e] + 1, F);
-    if (keys) {
-        keys[3 * e] = p * r.lanes + e; vals[3 * e] = default_priority;
-        keys[3 * e + 1] = h * r.lanes + e; vals[3 * e + 1] = 0.f;
-        keys[3 * e + 2] = -1;
-    }
-    uint8_t pend = 0;
-    if (t & kTerminal) {
-        if (t & 2) {                                   // auto-reset: next_obs doubles as the episode-start frame
-            dv -= destroy_entry(r, nh, e);
-            write_state(r, nh, e, next_obs);
-            if (keys) { keys[3 * e + 2] = nh * r.lanes + e; vals[3 * e + 2] = 0.f; }
-            nh = (nh + 1) % F;
-            cnt = (int)min((int64_t)cnt + 1, F);
-        } else {
-            pend = 1;                                  // the caller pushes the episode start once the env has been reset
-        }
-    }
-    r.head[e] = (int32_t)nh;
-    r.count[e] = cnt;
-    r.pending[e] = pend;
+    RingLeaves lv;
+    const long long dv = ring::push_sart(r, e, a[e], rew[e], term[e], next_obs + (int64_t)r.ns * e, default_priority, lv, nullptr);
+    emit_leaves(e, lv, keys, vals);
     if (dv != 0) atomicAdd((unsigned long long*)r.n_valid, (unsigned long long)dv);
 }
 
@@ -227,7 +171,7 @@ __global__ void __launch_bounds__(128) sample_gather_kernel(Ring r, unsigned lon
             const int64_t cnt = r.count[e];
             if (j >= cnt - 1) continue;
             const int64_t slot = ((int64_t)r.head[e] - cnt + j + 2 * F) % F;
-            if (r.flag[slot * r.lanes + e] & kSampleable) { key = slot * r.lanes + e; break; }
+            if (r.flag[slot * r.lanes + e] & kRingSampleable) { key = slot * r.lanes + e; break; }
         }
         if (key < 0) __trap();   // (practically) nothing sampleable
     }
@@ -244,7 +188,7 @@ __global__ void __launch_bounds__(128) sample_gather_kernel(Ring r, unsigned lon
     }
     o.a[k] = r.action[key];
     o.r[k] = r.reward[key];
-    o.t[k] = r.flag[key] & kTerminal;
+    o.t[k] = r.flag[key] & kRingTerminal;
     o.key[k] = key;
     o.prio[k] = p;
     o.w[k] = w;
@@ -552,6 +496,17 @@ TrajBatchView b200rl_traj_internal_batch(b200rl_traj* t) {
 bool b200rl_traj_internal_prioritized(b200rl_traj* t) { return t->prioritized; }
 b200rl_ctx* b200rl_traj_internal_ctx(b200rl_traj* t) { return t->ctx; }
 int64_t b200rl_traj_internal_lanes(b200rl_traj* t) { return t->r.lanes; }
+void b200rl_traj_internal_add_pushed(b200rl_traj* t, int64_t n) { t->pushed += n; }
+int64_t b200rl_traj_internal_pushed(b200rl_traj* t) { return t->pushed; }
+Ring b200rl_traj_internal_ring(b200rl_traj* t) { return t->r; }
+float b200rl_traj_internal_default_priority(b200rl_traj* t) { return t->default_priority; }
+// rebuild the sum-tree paths of n keys (key -1 = none) whose leaves already hold their values: tree[L + key] = vals is rewritten with
+// the same values, then the paths are recomputed from the children (tree_update_keys_kernel)
+int b200rl_traj_internal_tree_rebuild(b200rl_traj* t, const int64_t* keys, const float* vals, int64_t n) {
+    tree_update_keys_kernel<<<1, 1024, 0, t->ctx->stream>>>(t->r.tree, t->r.L, keys, vals, n);
+    LAUNCH_CHECK(t->ctx);
+    return B200RL_OK;
+}
 int b200rl_traj_internal_priority_from_td(b200rl_traj* t, const float* td_dev, float eps, float alpha) {
     td_to_priority_kernel<<<grid_for(t->B, 256), 256, 0, t->ctx->stream>>>(td_dev, t->new_prio, t->B, eps, alpha);
     LAUNCH_CHECK(t->ctx);

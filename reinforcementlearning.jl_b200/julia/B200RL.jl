@@ -29,7 +29,7 @@ using ReinforcementLearningCore: AbstractStage, PreExperimentStage, PostExperime
     EpsilonGreedyExplorer, GreedyExplorer, AbstractExplorer
 
 export B200Context, B200VecEnv, B200Network, B200OnPolicyAgent, B200RandomPolicy, B200Trajectory, B200DQNLearner, B200QBasedPolicy,
-    B200Agent, B200EpisodeStats, InsertSampleRatio, B200GreedyPolicy, evaluate
+    B200Agent, B200EpisodeStats, InsertSampleRatio, B200GreedyPolicy, evaluate, replay!
 
 const LIB = get(ENV, "B200RL_LIB", joinpath(@__DIR__, "..", "libb200rl.so"))
 
@@ -255,6 +255,15 @@ function RLCore._run(policy::AbstractPolicy, env::B200VecEnv, stop_condition::Ab
             stop_condition.progress === nothing || RLCore.ProgressMeter.update!(stop_condition.progress, min(stop_condition.cur, stop_condition.step))
             stop_condition.cur > stop_condition.step && break
         end
+        push!(policy, PostExperimentStage(), env)
+        push!(hook, PostExperimentStage(), policy, env)
+        check(ccall((:b200rl_env_check, LIB), Cint, (Ptr{Cvoid},), env.h))
+        return hook
+    end
+    # the replay agent's device loop (Python: Agent.run_replay): the whole window in one replay! call
+    if policy isa B200Agent && hook isa Union{B200EpisodeStats,RLCore.EmptyHook} && stop_condition isa StopAfterNSteps &&
+       reset_condition isa ResetIfEnvTerminated && replay!(policy, env, max(1, stop_condition.step - stop_condition.cur + 1))
+        stop_condition.cur += max(1, stop_condition.step - stop_condition.cur + 1)
         push!(policy, PostExperimentStage(), env)
         push!(hook, PostExperimentStage(), policy, env)
         check(ccall((:b200rl_env_check, LIB), Cint, (Ptr{Cvoid},), env.h))
@@ -646,6 +655,13 @@ that end inside the loop start their next frame in the push kernel (in-kernel au
 mutable struct B200Agent <: AbstractPolicy
     policy::B200QBasedPolicy
     trajectory::B200Trajectory
+    fused::Bool            # false: `_run` always steps through the stages (the stage protocol)
+    replay::Ptr{Cvoid}     # b200rl_replay handle of the device loop (kept across `run` calls: its CUDA graphs stay captured)
+    replay_env::Ptr{Cvoid} # the env it was created for
+end
+function B200Agent(policy::B200QBasedPolicy, trajectory::B200Trajectory)
+    a = B200Agent(policy, trajectory, true, C_NULL, C_NULL)
+    finalizer(x -> (x.replay == C_NULL || ccall((:b200rl_replay_destroy, LIB), Cint, (Ptr{Cvoid},), x.replay); x.replay = C_NULL), a)
 end
 RLBase.plan!(a::B200Agent, env::B200VecEnv) = RLBase.plan!(a.policy, env)
 Base.push!(a::B200Agent, ::PreEpisodeStage, env::B200VecEnv) = (push_env!(a.trajectory, env; mode = 1); nothing)      # push!(trajectory, (state = s0,)), all lanes
@@ -664,6 +680,45 @@ function RLBase.optimise!(a::B200Agent, ::PostActStage)
     nothing
 end
 RLBase.optimise!(::B200Agent, ::AbstractStage) = nothing
+
+struct InsertSampleRatioC
+    ratio::Cdouble; threshold::Int64; n_inserted::Int64; n_sampled::Int64
+end
+"""
+    replay!(agent::B200Agent, env, n_steps) -> Bool
+
+`n_steps` × {plan!, act!, push!, optimise!} of the stage protocol on the device (b200rl_replay_run): a stretch of steps without an
+update is one collect launch (H = 64 on the tensor cores) and each "1 step + m updates" unit is replayed from a CUDA graph.  The
+same transitions, updates, streams and counters as stepping through the stages; the explorer's `step` and the controller's counters
+advance.  `false` (nothing done) when the agent / env are outside the device loop: the caller steps through the stages instead.
+"""
+function replay!(a::B200Agent, env::B200VecEnv, n_steps::Integer)
+    p, t, c = a.policy, a.trajectory, a.trajectory.controller
+    (a.fused && env isa B200VecEnv{Float32} && env.auto_reset && !env.continuous && t.batch_size > 0 && t.lanes == env.n &&
+     p.explorer isa Union{EpsilonGreedyExplorer,GreedyExplorer}) || return false
+    if a.replay == C_NULL || a.replay_env != env.h
+        a.replay == C_NULL || ccall((:b200rl_replay_destroy, LIB), Cint, (Ptr{Cvoid},), a.replay)
+        a.replay = C_NULL
+        h = Ref{Ptr{Cvoid}}(C_NULL)
+        st = ccall((:b200rl_replay_create, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ref{DQNConfigC}, Ref{Ptr{Cvoid}}),
+                   p.ctx.h, p.learner.net.h, env.h, t.h, Ref(p.learner.cfg), h)
+        st in (-1, -3) && return false              # B200RL_ERR_INVALID / _UNSUPPORTED (e.g. a sharded ctx): the stage loop runs it
+        check(st)
+        a.replay, a.replay_env = h[], env.h
+    end
+    ctl = Ref(InsertSampleRatioC(c.ratio, c.threshold, c.n_inserted, c.n_sampled))
+    if p.explorer isa EpsilonGreedyExplorer
+        ex = Ref(ExplorerC(p.explorer))
+        check(ccall((:b200rl_replay_run, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ref{ExplorerC}, Ref{InsertSampleRatioC}, Int64, Ptr{Cfloat}),
+                    a.replay, p.d_rng, ex, ctl, n_steps, C_NULL))
+        p.explorer.step = ex[].step
+    else                                                           # GreedyExplorer: findmax, no draw
+        check(ccall((:b200rl_replay_run, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ref{InsertSampleRatioC}, Int64, Ptr{Cfloat}),
+                    a.replay, p.d_rng, C_NULL, ctl, n_steps, C_NULL))
+    end
+    c.n_inserted, c.n_sampled = Int(ctl[].n_inserted), Int(ctl[].n_sampled)
+    true
+end
 
 # ---- pure-function drop-ins (utils/basic.jl:138-417) --------------------------------------------
 "`generalized_advantage_estimation(rewards, values, γ, λ; dims, terminal)` on the GPU (Float32 / Float64 matrices)."

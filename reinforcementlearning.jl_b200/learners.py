@@ -9,6 +9,8 @@ import numpy as np
 
 from . import _lib as L
 from .core import AbstractPolicy, FusedAction, PostActStage, PreActStage, PreEpisodeStage, PreExperimentStage
+from .envs import _NOBS
+from .explorers import EpsilonGreedyExplorer, GreedyExplorer
 
 ACT_RELU, ACT_TANH = 0, 1
 KIND_CATEGORICAL, KIND_GAUSSIAN, KIND_Q = 0, 1, 2
@@ -581,6 +583,70 @@ class Agent(AbstractPolicy):
         if not hasattr(trajectory, "controller"):
             trajectory.controller = InsertSampleRatioController()
         self._host_act = None
+        # run() may hand whole stretches of the loop to run_replay (b200rl_replay_run): a DQN learner behind an epsilon-greedy
+        # or greedy explorer whose actions stay on the device.  The env's side is checked per run (replay_supported).
+        self.fusable = (not host_actions and isinstance(policy, QBasedPolicy) and isinstance(policy.learner, DQNLearner)
+                        and type(policy.explorer) in (EpsilonGreedyExplorer, GreedyExplorer))
+        self._replay, self._replay_key = None, None
+
+    def close(self):
+        if getattr(self, "_replay", None):
+            self.policy.lib.b200rl_replay_destroy(self._replay)
+            self._replay = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    # ---- device agent loop ----------------------------------------------------------------------
+    def replay_supported(self, env):
+        """The env side of the device loop: in-kernel auto-reset, Float32, a discrete action space, <= 4 observations, and
+        the trajectory's controller is an InsertSampleRatioController; the ctx must not be sharded (refused by create)."""
+        t, lr = self.trajectory, self.policy.learner
+        return (self.fusable and env.auto_reset and env.T is np.float32 and not env.continuous and env.kind != L.ENV_ACROBOT
+                and type(t.controller) is InsertSampleRatioController and t.batch_size > 0 and t.lanes == env.n and t.ns == lr.net.n_in
+                and lr.net.n_in == _NOBS.get(env.kind) and self._handle(env) is not None)
+
+    def _handle(self, env):
+        pol, lr = self.policy, self.policy.learner
+        key = (env.h.value, lr.net.h.value, self.trajectory.h.value, bytes(lr.cfg))
+        if self._replay is not None and self._replay_key == key:
+            return self._replay
+        self.close()
+        h = C.c_void_p()
+        st = pol.lib.b200rl_replay_create(pol.ctx.h, lr.net.h, env.h, self.trajectory.h, C.byref(lr.cfg), C.byref(h))
+        if st in (L.ERR_UNSUPPORTED, L.ERR_INVALID):
+            return None            # e.g. a sharded ctx: the stage loop keeps running the agent (and raises its own errors)
+        L.check(st)
+        self._replay, self._replay_key = h, key
+        return h
+
+    def run_replay(self, env, n_steps, want_stats=False):
+        """n_steps x {plan!, act!, push!, optimise!} of the stage protocol on the device (b200rl_replay_run): the same
+        transitions, updates, streams and counters.  Returns the last update's {loss, grad_norm, mean_abs_td, n_updates}
+        (want_stats, synchronises) or None."""
+        pol, c = self.policy, self.trajectory.controller
+        h = self._handle(env)
+        ex = pol.explorer.as_struct() if isinstance(pol.explorer, EpsilonGreedyExplorer) else None
+        ctl = L.InsertSampleRatio(c.ratio, c.threshold, c.n_inserted, c.n_sampled)
+        stats = np.full(4, np.nan, np.float32) if want_stats else None
+        L.check(pol.lib.b200rl_replay_run(h, C.c_void_p(pol._d_rng), None if ex is None else C.byref(ex), C.byref(ctl), int(n_steps),
+                                          L.ptr(stats)))
+        if ex is not None:
+            pol.explorer.step = ex.step
+        c.n_inserted, c.n_sampled = ctl.n_inserted, ctl.n_sampled
+        if stats is None or np.isnan(stats[3]):
+            return None
+        return dict(loss=stats[0], grad_norm=stats[1], mean_abs_td=stats[2], n_updates=int(stats[3]))
+
+    def graph_active(self):
+        v = C.c_int()
+        if self._replay is None:
+            return False
+        L.check(self.policy.lib.b200rl_replay_graph_active(self._replay, C.byref(v)))
+        return bool(v.value)
 
     def push(self, stage, env, action=None):
         if stage == PreEpisodeStage:
