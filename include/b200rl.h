@@ -241,8 +241,15 @@ int b200rl_traj_set(b200rl_traj* traj, int field, const void* host_src, size_t b
  * descent that never enters an empty subtree); the batch (state, action, reward, terminal, next_state, key, priority, weight) stays
  * on device.  beta: importance-weight exponent, w = (n p / total)^-beta / max w, n = n_sampleable */
 int b200rl_traj_sample(b200rl_traj* traj, float beta);
+/* NStepBatchSampler(n, gamma) (ReinforcementLearningTrajectories 0.4; DESIGN.md §3): from the next sample on, the drawn entry q
+ * (drawn exactly as by the 1-step sampler) opens a window of m <= n entries of its lane that ends early at a terminal entry or
+ * before an entry that is not sampleable; the batch then holds reward = the Float32 discounted sum of the window (in
+ * discount_rewards' order), terminal = that of entry q+m-1, next_state = state frame q+m, discount = gamma^m, horizon = m.
+ * n = 1 is the BatchSampler (the default, with gamma 0.99).  Refused, before any side effect, unless 1 <= n <= min(32, capacity)
+ * and gamma is finite in [0, 1].  Configuration, not state: b200rl_traj_get / set do not carry it. */
+int b200rl_traj_set_nstep(b200rl_traj* traj, int32_t n, float gamma);
 /* field: 0 state (ns,B) | 1 action (B) i32 | 2 reward | 3 terminal u8 | 4 next_state | 5 key i64 |
- * 6 priority | 7 weight | 8 sampler rng (4,B) u64 */
+ * 6 priority | 7 weight | 8 sampler rng (4,B) u64 | 9 discount (B) f32 | 10 horizon (B) i32 (n = 1: gamma and 1) */
 int b200rl_traj_batch_get(b200rl_traj* traj, int field, void* host_dst, size_t bytes);
 /* priority write-back for the keys of the last sampled batch (trajectory[:priority, keys] = p) */
 int b200rl_traj_update_priority(b200rl_traj* traj, const float* priority, int on_device);
@@ -373,7 +380,9 @@ typedef struct {
     int32_t huber, double_dqn, target_update_freq;
 } b200rl_dqn_config;
 /* optimise!(DQNLearner / PrioritizedDQNLearner): sample, TD loss + backward, clip + Adam,
- * priority write-back, target sync.  stats_host[4] = loss, grad_norm, mean|td|, n_updates (NULL: async) */
+ * priority write-back, target sync.  stats_host[4] = loss, grad_norm, mean|td|, n_updates (NULL: async).
+ * With an n-step sampler (n > 1) the target is R = reward + discount * (1 - terminal) * q'(next_state), and a trajectory whose
+ * n-step gamma differs from cfg->gamma is refused before any side effect. */
 int b200rl_dqn_update(b200rl_net* net, b200rl_traj* traj, const b200rl_dqn_config* cfg, float* stats_host);
 int b200rl_dqn_last_td(b200rl_net* net, b200rl_traj* traj, float* host_dst, int64_t count);
 
@@ -393,7 +402,8 @@ typedef struct b200rl_replay b200rl_replay;
  * where rewards are not integers).  The explorer step, the update counter and the controller counters advance on the host by
  * arithmetic.  The trajectory keeps (min(2k + 1, capacity + 1), N) touched-leaf keys for the longest stretch k (prioritised).
  * create refuses, before any side effect: a network that is not a Q-network, a Float64 / continuous-action / Acrobot env,
- * trajectory lanes != N or a state width that does not match, a sharded ctx (world > 1).  The trajectory needs a sampler. */
+ * trajectory lanes != N or a state width that does not match, a sharded ctx (world > 1), an n-step gamma != cfg->gamma (also
+ * refused by run).  The trajectory needs a sampler; a change of its n-step setting between runs re-captures the graphs. */
 int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl_traj* traj, const b200rl_dqn_config* cfg,
                          b200rl_replay** out);
 /* explorer_rng_dev: (4, N) DEVICE explorer streams (one per env, advanced).  ex: EpsilonGreedyExplorer (its step is advanced

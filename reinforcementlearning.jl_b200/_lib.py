@@ -134,6 +134,7 @@ SIGNATURES = {
     "b200rl_traj_push": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32]),
     "b200rl_traj_push_env": (_i32, [_vp, _vp, _i32]),
     "b200rl_traj_sample": (_i32, [_vp, _f32]),
+    "b200rl_traj_set_nstep": (_i32, [_vp, _i32, _f32]),
     "b200rl_traj_batch_get": (_i32, [_vp, _i32, _vp, _sz]),
     "b200rl_traj_update_priority": (_i32, [_vp, _vp, _i32]),
     "b200rl_traj_total_priority": (_i32, [_vp, C.POINTER(_f32)]),

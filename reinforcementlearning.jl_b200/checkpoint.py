@@ -8,7 +8,9 @@ constructor's business, exactly as `PPOPolicy(...)` is rebuilt before `Flux.load
 
 `checkpoint` / `restore` cover on-policy runs (env + actor-critic net + OnPolicyAgent).  Replay runs (`Agent(QBasedPolicy, Trajectory)`)
 go through `checkpoint_replay` / `restore_replay`, which add the Q-network's update counter (the target-sync phase), the ring with its
-per-lane bookkeeping and sum tree, the sampler / explorer streams, the explorer's step and the controller's counters."""
+per-lane bookkeeping and sum tree, the sampler / explorer streams, the explorer's step and the controller's counters.  The
+trajectory's n-step setting (`Trajectory(..., n_step, gamma)`, the NStepBatchSampler) is configuration, not state: it is not
+saved, and the restored trajectory must be constructed with the same one."""
 import numpy as np
 
 from . import _lib as L

@@ -35,6 +35,8 @@ void b200rl_traj_internal_add_pushed(b200rl_traj* t, int64_t n);
 int64_t b200rl_traj_internal_pushed(b200rl_traj* t);
 Ring b200rl_traj_internal_ring(b200rl_traj* t);
 float b200rl_traj_internal_default_priority(b200rl_traj* t);
+void b200rl_traj_internal_nstep(b200rl_traj* t, int* n, float* gamma);
+const float* b200rl_traj_internal_discount(b200rl_traj* t);
 int b200rl_traj_internal_tree_rebuild(b200rl_traj* t, const int64_t* keys, const float* vals, int64_t n);
 uint64_t b200rl_env_internal_steps(const b200rl_env* e);
 int b200rl_traj_internal_priority_from_td(b200rl_traj* t, const float* td_dev, float eps, float alpha);
@@ -1075,7 +1077,7 @@ static int dqn_update_seq(b200rl_net* n, b200rl_traj* t, const b200rl_dqn_config
     float* td = (float*)((char*)sc + q_bytes);
     int world = b200rl_comm_world(ctx);
     int np_ = nn_dqn_loss_grad(ctx, n->actor, n->params, n->target, b.s, b.a, b.r, b.t, b.s2, b.w, b.B, 1.0f / ((float)b.B * (float)world), cfg->gamma,
-                               cfg->huber, cfg->double_dqn, n->partial, n->loss_partial, td);
+                               cfg->huber, cfg->double_dqn, n->partial, n->loss_partial, td, b200rl_traj_internal_discount(t));
     if (np_ < 0) return np_;
     P2PTable peers;
     const unsigned adam_grid = grid_for(n->np, 256);
@@ -1102,6 +1104,13 @@ static int dqn_update_seq(b200rl_net* n, b200rl_traj* t, const b200rl_dqn_config
     if (td_out) *td_out = td;
     return B200RL_OK;
 }
+// an n-step sampler discounts its windows by its own γ: the learner's must be the same one
+static int check_nstep_gamma(b200rl_traj* t, const b200rl_dqn_config* cfg) {
+    int ns; float g;
+    b200rl_traj_internal_nstep(t, &ns, &g);
+    REQUIRE(ns == 1 || g == cfg->gamma, B200RL_ERR_INVALID, "the trajectory's n-step gamma differs from the learner's gamma");
+    return B200RL_OK;
+}
 // stats4 = loss, grad_norm, mean |td|, n_updates of the update that wrote loss4 / gnorm / td (synchronises)
 static int dqn_stats(b200rl_net* n, const float* td, int64_t B, float* stats4) {
     b200rl_ctx* ctx = n->ctx;
@@ -1122,6 +1131,7 @@ static int dqn_stats(b200rl_net* n, const float* td, int64_t B, float* stats4) {
 int b200rl_dqn_update(b200rl_net* n, b200rl_traj* t, const b200rl_dqn_config* cfg, float* stats_host) {
     REQUIRE(n && t && cfg && n->kind == 2, B200RL_ERR_INVALID, "bad argument (needs a Q-network)");
     REQUIRE(n->ctx == b200rl_traj_internal_ctx(t), B200RL_ERR_INVALID, "net/trajectory belong to different ctx");
+    TRY(check_nstep_gamma(t, cfg));
     TRY(ctx_bind(n->ctx));
     float* td = nullptr;
     TRY(dqn_update_seq(n, t, cfg, nullptr, nullptr, &td));
@@ -1157,6 +1167,7 @@ struct ReplayGraph {   // one "1 step + m updates" unit
 // what the captured launches bake in besides the handles: a change means re-capture
 struct ReplayKey {
     int tc, max_timeout, greedy, pad;
+    int nstep_n; float nstep_gamma;  // the sampler's n-step setting (picks the sample kernel and its window arguments)
     b200rl_explorer ex;          // step zeroed (it lives in device memory)
     const void* rng;
     const void* scratch;
@@ -1270,6 +1281,7 @@ int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl
     REQUIRE(b.B > 0, B200RL_ERR_INVALID, "the trajectory was created without a sampler (batch_size = 0)");
     REQUIRE(b.ns == q->actor.in, B200RL_ERR_INVALID, "trajectory state width != network input width");
     REQUIRE(b200rl_comm_world(ctx) == 1, B200RL_ERR_UNSUPPORTED, "the replay agent loop runs on one GPU (communicator world > 1)");
+    TRY(check_nstep_gamma(traj, cfg));
     b200rl_replay* r = new b200rl_replay();
     r->ctx = ctx; r->net = q; r->env = env; r->traj = traj; r->cfg = *cfg; r->N = N; r->B = b.B;
     r->action = nullptr; r->ex_step_dev = nullptr; r->upd_dev = nullptr; r->td_keep = nullptr; r->keys = nullptr; r->vals = nullptr;
@@ -1297,6 +1309,7 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
     }
     REQUIRE(replay::controller_ok(*ctl), B200RL_ERR_INVALID, "bad controller values (ratio finite in [0, 1e6], counters >= 0)");
     REQUIRE(ctl->n_inserted + n_steps < (1ll << 52), B200RL_ERR_INVALID, "controller counters too large");
+    TRY(check_nstep_gamma(r->traj, &r->cfg));
     TRY(ctx_bind(r->ctx));
     b200rl_ctx* ctx = r->ctx;
     b200rl_net* n = r->net;
@@ -1329,6 +1342,7 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
     key.tc = nn_tc_enabled() ? 1 : 0;
     key.max_timeout = b200rl_env_internal_max_timeout(r->env);
     key.greedy = ex ? 0 : 1;
+    b200rl_traj_internal_nstep(r->traj, &key.nstep_n, &key.nstep_gamma);
     if (ex) { key.ex = *ex; key.ex.step = 0; }
     key.rng = explorer_rng_dev;
     key.scratch = ctx->scratch;

@@ -854,13 +854,15 @@ __global__ void __launch_bounds__(1024) target_sync_counted_kernel(float* __rest
 
 // ------------------------------------------------------------- DQN --------------------------
 // phase A (forward_kernel mode 1 on the target / online nets) gives Q(s') tables; this kernel
-// does the online forward on s, the TD loss and the backward.
-template <int H>
+// does the online forward on s, the TD loss and the backward.  DISC: the target discounts by the per-sample disc[j] (γ^m of an
+// n-step window, nstep.cuh) instead of the scalar gamma.
+template <int H, bool DISC>
 __global__ void __launch_bounds__(NT, (H == 64) ? 2 : 1)
 dqn_loss_grad_kernel(MlpDesc q, const float* __restrict__ params, const float* __restrict__ s, const int32_t* __restrict__ a,
                      const float* __restrict__ r, const uint8_t* __restrict__ t, const float* __restrict__ qnext_t,
                      const float* __restrict__ qnext_o, const float* __restrict__ w, int64_t B, float inv_B, float gamma, int huber,
-                     float* __restrict__ partial, float* __restrict__ loss_partial, float* __restrict__ td_out) {
+                     float* __restrict__ partial, float* __restrict__ loss_partial, float* __restrict__ td_out,
+                     const float* __restrict__ disc) {
     using C = Cfg<H>;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     Smem<H, true>& sm = *reinterpret_cast<Smem<H, true>*>(smem_raw);
@@ -898,7 +900,7 @@ dqn_loss_grad_kernel(MlpDesc q, const float* __restrict__ params, const float* _
                     qn = qnext_t[(int64_t)na * j];
                     for (int o = 1; o < na; ++o) qn = fmaxf(qn, qnext_t[(int64_t)na * j + o]);
                 }
-                float R = r[j] + gamma * (t[j] ? 0.f : 1.f) * qn;
+                float R = r[j] + (DISC ? disc[j] : gamma) * (t[j] ? 0.f : 1.f) * qn;
                 int ai = a[j] - 1;
                 float qv = 0.f;
 #pragma unroll
@@ -1007,13 +1009,13 @@ static int launch_ac(b200rl_ctx* ctx, int grid, const MlpDesc& actor, const MlpD
     LAUNCH_CHECK(ctx);
     return B200RL_OK;
 }
-template <int H>
+template <int H, bool DISC>
 static int launch_dqn(b200rl_ctx* ctx, int grid, const MlpDesc& q, const float* params, const float* s, const int32_t* a, const float* r,
                       const uint8_t* t, const float* qt, const float* qo, const float* w, int64_t B, float inv_B, float gamma, int huber,
-                      float* partial, float* loss_partial, float* td_out) {
-    TRY(set_smem(dqn_loss_grad_kernel<H>, smem_bytes<H, true>()));
-    dqn_loss_grad_kernel<H><<<grid, NT, smem_bytes<H, true>(), ctx->stream>>>(q, params, s, a, r, t, qt, qo, w, B, inv_B, gamma, huber, partial,
-                                                                             loss_partial, td_out);
+                      float* partial, float* loss_partial, float* td_out, const float* disc) {
+    TRY(set_smem(dqn_loss_grad_kernel<H, DISC>, smem_bytes<H, true>()));
+    dqn_loss_grad_kernel<H, DISC><<<grid, NT, smem_bytes<H, true>(), ctx->stream>>>(q, params, s, a, r, t, qt, qo, w, B, inv_B, gamma, huber,
+                                                                                   partial, loss_partial, td_out, disc);
     LAUNCH_CHECK(ctx);
     return B200RL_OK;
 }
@@ -1148,7 +1150,7 @@ int nn_target_sync_counted(b200rl_ctx* ctx, float* target, const float* model, i
 // returns the number of gradient partials written (> 0) or a negative status
 int nn_dqn_loss_grad(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float* target, const float* s, const int32_t* a,
                      const float* r, const uint8_t* t, const float* s2, const float* w, int64_t B, float inv_B, float gamma, int huber,
-                     int double_dqn, float* partial, float* loss_partial, float* td_out) {
+                     int double_dqn, float* partial, float* loss_partial, float* td_out, const float* disc) {
     TRY(check_desc(q));
     // Q(s') tables in ctx scratch: target net always, online net for double DQN
     void* scratch;
@@ -1160,8 +1162,14 @@ int nn_dqn_loss_grad(b200rl_ctx* ctx, const MlpDesc& q, const float* params, con
     int ctas = nn_dqn_max_partials(ctx, q.H);
     int nt = tiles_for(q.H, B);
     if (ctas > nt) ctas = nt;
-    int st = q.H == 64 ? launch_dqn<64>(ctx, ctas, q, params, s, a, r, t, qt, double_dqn ? qo : nullptr, w, B, inv_B, gamma, huber, partial, loss_partial, td_out)
-                       : launch_dqn<128>(ctx, ctas, q, params, s, a, r, t, qt, double_dqn ? qo : nullptr, w, B, inv_B, gamma, huber, partial, loss_partial, td_out);
+    const float* qo_ = double_dqn ? qo : nullptr;
+    int st;
+    if (disc)
+        st = q.H == 64 ? launch_dqn<64, true>(ctx, ctas, q, params, s, a, r, t, qt, qo_, w, B, inv_B, gamma, huber, partial, loss_partial, td_out, disc)
+                       : launch_dqn<128, true>(ctx, ctas, q, params, s, a, r, t, qt, qo_, w, B, inv_B, gamma, huber, partial, loss_partial, td_out, disc);
+    else
+        st = q.H == 64 ? launch_dqn<64, false>(ctx, ctas, q, params, s, a, r, t, qt, qo_, w, B, inv_B, gamma, huber, partial, loss_partial, td_out, nullptr)
+                       : launch_dqn<128, false>(ctx, ctas, q, params, s, a, r, t, qt, qo_, w, B, inv_B, gamma, huber, partial, loss_partial, td_out, nullptr);
     if (st != B200RL_OK) return st;
     return ctas;
 }

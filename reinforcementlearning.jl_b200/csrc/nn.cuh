@@ -90,10 +90,11 @@ int nn_reduce_clip_adam(b200rl_ctx* ctx, const float* partial, int n_partials, i
 int nn_target_sync(b200rl_ctx* ctx, float* target, const float* model, int64_t np, float rho);
 // target sync every `freq` optimiser steps, counted on the device: *upd_dev += 1, sync when it is a multiple of freq
 int nn_target_sync_counted(b200rl_ctx* ctx, float* target, const float* model, int64_t np, float rho, unsigned long long* upd_dev, int freq);
-// DQN: TD loss + backward on a gathered batch (device arrays s (in,B), a, r, t, s2, w)
+// DQN: TD loss + backward on a gathered batch (device arrays s (in,B), a, r, t, s2, w).  disc (may be null): per-sample discount
+// (n-step γ^m) in place of the scalar gamma
 int nn_dqn_loss_grad(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float* target, const float* s, const int32_t* a,
                      const float* r, const uint8_t* t, const float* s2, const float* w, int64_t B, float inv_B, float gamma, int huber,
-                     int double_dqn, float* partial, float* loss_partial, float* td_out);
+                     int double_dqn, float* partial, float* loss_partial, float* td_out, const float* disc);
 int nn_q_act(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float* obs, int64_t N, unsigned long long* rng, float epsilon,
              int32_t* action_out, float* q_out);
 // step_dev (may be null): explorer step read from device memory instead of ex.step

@@ -19,6 +19,7 @@
 // A push is one thread per lane (neighbouring lanes write neighbouring addresses unless their episode counts differ);
 // a sample is one thread per batch slot: Xoshiro draw -> (rejection | sum-tree descent) -> 2 x state gather + scalars.
 #include "common.cuh"
+#include "nstep.cuh"
 #include "ring.cuh"
 
 namespace {
@@ -126,13 +127,20 @@ __global__ void __launch_bounds__(1024) tree_update_keys_kernel(float* __restric
 struct BatchOut {
     float* s; int32_t* a; float* r; uint8_t* t; float* s2; int64_t* key; float* prio; float* w;
 };
+// the n-step setting of a sample (NSTEP instantiations only) and its two extra per-sample outputs
+struct NStepArgs {
+    int n; float gamma;
+    float* discount; int32_t* horizon;
+};
 
 // The descent of the binary sum tree is a chain of dependent reads (20 levels for 1 M leaves): the top kTopLevels levels
 // (nodes 1 .. 2^kTopLevels - 1, 16 KB) are staged in shared memory by the CTA with independent loads, which leaves 8 dependent
 // L2 round trips instead of 20; a node's two children are adjacent and read as one 8-byte word.  Same values, same comparisons.
 constexpr int kTopLevels = 12;
-template <bool PRIO>
-__global__ void __launch_bounds__(128) sample_gather_kernel(Ring r, unsigned long long* __restrict__ slots, int64_t B, float beta, BatchOut o) {
+// NSTEP: reward / terminal / next_state come from the n-step window of the drawn entry (nstep.cuh); the draw itself is unchanged
+template <bool PRIO, bool NSTEP>
+__global__ void __launch_bounds__(128) sample_gather_kernel(Ring r, unsigned long long* __restrict__ slots, int64_t B, float beta, BatchOut o,
+                                                            NStepArgs nsa) {
     __shared__ float top[PRIO ? (1 << kTopLevels) : 1];
     if (PRIO) {
         const int64_t ntop = min((int64_t)(1 << kTopLevels), 2 * r.L);
@@ -177,7 +185,9 @@ __global__ void __launch_bounds__(128) sample_gather_kernel(Ring r, unsigned lon
     }
     store_xo(slots, k, g);
     const int64_t slot = key / r.lanes, e = key % r.lanes;
-    const int64_t nslot = (slot + 1) % F;
+    NStepWindow win;
+    if (NSTEP) win = nstep::window(r, key, nsa.n, nsa.gamma);
+    const int64_t nslot = NSTEP ? win.next_slot : (slot + 1) % F;
     const float* s = r.state + (int64_t)r.ns * (slot * r.lanes + e);
     const float* s2 = r.state + (int64_t)r.ns * (nslot * r.lanes + e);
     if (r.ns == 4) {   // one 16-byte row each way
@@ -187,8 +197,15 @@ __global__ void __launch_bounds__(128) sample_gather_kernel(Ring r, unsigned lon
         for (int c = 0; c < r.ns; ++c) { o.s[(int64_t)r.ns * k + c] = s[c]; o.s2[(int64_t)r.ns * k + c] = s2[c]; }
     }
     o.a[k] = r.action[key];
-    o.r[k] = r.reward[key];
-    o.t[k] = r.flag[key] & kRingTerminal;
+    if (NSTEP) {
+        o.r[k] = win.G;
+        o.t[k] = win.terminal;
+        nsa.discount[k] = win.discount;
+        nsa.horizon[k] = win.m;
+    } else {
+        o.r[k] = r.reward[key];
+        o.t[k] = r.flag[key] & kRingTerminal;
+    }
     o.key[k] = key;
     o.prio[k] = p;
     o.w[k] = w;
@@ -222,6 +239,8 @@ struct b200rl_traj {
     int64_t B;
     unsigned long long* slots;  // (4, B) sampler streams
     BatchOut batch;
+    int nstep_n; float nstep_gamma;   // NStepBatchSampler(n, γ); n = 1 is the BatchSampler (discount / horizon buffers unused)
+    float* discount; int32_t* horizon;
     float* new_prio;            // (B) scratch for priority write-back
     int64_t* keys; float* vals; // (3 * lanes) sum-tree leaves rewritten by a push
     void* stage;                // staging for host-side pushes
@@ -253,6 +272,7 @@ int b200rl_traj_create(b200rl_ctx* ctx, int ns, int64_t lanes, int64_t capacity,
     b200rl_traj* t = new b200rl_traj();
     memset(t, 0, sizeof *t);
     t->ctx = ctx; t->prioritized = prioritized != 0; t->default_priority = default_priority; t->B = batch_size;
+    t->nstep_n = 1; t->nstep_gamma = 0.99f;
     Ring& r = t->r;
     r.ns = ns; r.lanes = lanes; r.cap = capacity;
     size_t slots = (size_t)lanes * (capacity + 1);
@@ -286,6 +306,9 @@ int b200rl_traj_create(b200rl_ctx* ctx, int ns, int64_t lanes, int64_t capacity,
         CUDA_TRY(cudaMalloc(&t->batch.key, B * 8));
         CUDA_TRY(cudaMalloc(&t->batch.prio, B * 4));
         CUDA_TRY(cudaMalloc(&t->batch.w, B * 4));
+        CUDA_TRY(cudaMalloc(&t->discount, B * 4));
+        CUDA_TRY(cudaMalloc(&t->horizon, B * 4));
+        CUDA_TRY(cudaMemsetAsync(t->discount, 0, B * 4, ctx->stream)); CUDA_TRY(cudaMemsetAsync(t->horizon, 0, B * 4, ctx->stream));
         CUDA_TRY(cudaMalloc(&t->new_prio, B * 4));
     }
     t->stage_bytes = (size_t)lanes * (ns * 4 + 4 + 4 + 1) + 64;
@@ -302,7 +325,8 @@ int b200rl_traj_destroy(b200rl_traj* t) {
     cudaFree(t->r.state); cudaFree(t->r.action); cudaFree(t->r.reward); cudaFree(t->r.flag); cudaFree(t->r.tree);
     cudaFree(t->r.head); cudaFree(t->r.count); cudaFree(t->r.pending); cudaFree(t->r.n_valid); cudaFree(t->keys); cudaFree(t->vals);
     cudaFree(t->slots); cudaFree(t->batch.s); cudaFree(t->batch.s2); cudaFree(t->batch.a); cudaFree(t->batch.r); cudaFree(t->batch.t);
-    cudaFree(t->batch.key); cudaFree(t->batch.prio); cudaFree(t->batch.w); cudaFree(t->new_prio); cudaFree(t->stage);
+    cudaFree(t->batch.key); cudaFree(t->batch.prio); cudaFree(t->batch.w); cudaFree(t->new_prio);
+    cudaFree(t->discount); cudaFree(t->horizon); cudaFree(t->stage);
     delete t;
     return B200RL_OK;
 }
@@ -376,18 +400,33 @@ int b200rl_traj_push(b200rl_traj* t, const int32_t* action, const float* reward,
     return B200RL_OK;
 }
 
-/* BatchSampler / prioritised sampler + gather into the trajectory's device batch buffers */
+/* NStepBatchSampler(n, γ): refused before any side effect unless 1 <= n <= min(32, capacity) and γ is finite in [0, 1] */
+int b200rl_traj_set_nstep(b200rl_traj* t, int32_t n, float gamma) {
+    REQUIRE(t, B200RL_ERR_INVALID, "null argument");
+    REQUIRE(n >= 1 && n <= kNStepMax && (int64_t)n <= t->r.cap, B200RL_ERR_INVALID, "n-step horizon must be in 1 .. min(32, capacity)");
+    REQUIRE(gamma >= 0.f && gamma <= 1.f, B200RL_ERR_INVALID, "gamma must be finite and in [0, 1]");   // false for NaN
+    t->nstep_n = n; t->nstep_gamma = gamma;
+    return B200RL_OK;
+}
+
+/* BatchSampler / prioritised sampler (+ the n-step window) + gather into the trajectory's device batch buffers */
 int b200rl_traj_sample(b200rl_traj* t, float beta) {
     REQUIRE(t && t->B > 0, B200RL_ERR_INVALID, "trajectory was created without a sampler");
     REQUIRE(t->pushed >= 1, B200RL_ERR_INVALID, "nothing to sample yet");
     TRY(ctx_bind(t->ctx));
+    const NStepArgs nsa{t->nstep_n, t->nstep_gamma, t->discount, t->horizon};
+    const bool ns = t->nstep_n > 1;
+    const unsigned grid = grid_for(t->B, 128);
+    cudaStream_t st = t->ctx->stream;
     if (t->prioritized) {
-        sample_gather_kernel<true><<<grid_for(t->B, 128), 128, 0, t->ctx->stream>>>(t->r, t->slots, t->B, beta, t->batch);
+        if (ns) sample_gather_kernel<true, true><<<grid, 128, 0, st>>>(t->r, t->slots, t->B, beta, t->batch, nsa);
+        else sample_gather_kernel<true, false><<<grid, 128, 0, st>>>(t->r, t->slots, t->B, beta, t->batch, nsa);
         LAUNCH_CHECK(t->ctx);
         normalize_weights_kernel<<<1, 1024, 0, t->ctx->stream>>>(t->batch.w, t->B);
         LAUNCH_CHECK(t->ctx);
     } else {
-        sample_gather_kernel<false><<<grid_for(t->B, 128), 128, 0, t->ctx->stream>>>(t->r, t->slots, t->B, beta, t->batch);
+        if (ns) sample_gather_kernel<false, true><<<grid, 128, 0, st>>>(t->r, t->slots, t->B, beta, t->batch, nsa);
+        else sample_gather_kernel<false, false><<<grid, 128, 0, st>>>(t->r, t->slots, t->B, beta, t->batch, nsa);
         LAUNCH_CHECK(t->ctx);
     }
     return B200RL_OK;
@@ -438,11 +477,21 @@ int b200rl_traj_set(b200rl_traj* t, int field, const void* host_src, size_t byte
     if (field == 5) t->pushed = 1;   // a restored ring may be sampled
     return B200RL_OK;
 }
-/* field: 0 state (ns,B) 1 action (B) i32 2 reward 3 terminal u8 4 next_state 5 key i64 6 priority 7 weight 8 sampler rng (4,B) */
+/* field: 0 state (ns,B) 1 action (B) i32 2 reward 3 terminal u8 4 next_state 5 key i64 6 priority 7 weight 8 sampler rng (4,B)
+ * 9 discount (B) f32 10 horizon (B) i32 (n = 1: γ and 1) */
 int b200rl_traj_batch_get(b200rl_traj* t, int field, void* host_dst, size_t bytes) {
     REQUIRE(t && host_dst && t->B > 0, B200RL_ERR_INVALID, "bad argument");
     TRY(ctx_bind(t->ctx));
     size_t B = (size_t)t->B;
+    if ((field == 9 || field == 10) && t->nstep_n == 1) {   // the 1-step sampler writes neither: every window has length 1
+        REQUIRE(bytes >= B * 4, B200RL_ERR_INVALID, "destination too small");
+        CUDA_TRY(cudaStreamSynchronize(t->ctx->stream));
+        for (size_t k = 0; k < B; ++k) {
+            if (field == 9) ((float*)host_dst)[k] = t->nstep_gamma;
+            else ((int32_t*)host_dst)[k] = 1;
+        }
+        return B200RL_OK;
+    }
     const void* src = nullptr;
     size_t need = 0;
     switch (field) {
@@ -455,6 +504,8 @@ int b200rl_traj_batch_get(b200rl_traj* t, int field, void* host_dst, size_t byte
         case 6: src = t->batch.prio; need = B * 4; break;
         case 7: src = t->batch.w; need = B * 4; break;
         case 8: src = t->slots; need = B * 32; break;
+        case 9: src = t->discount; need = B * 4; break;
+        case 10: src = t->horizon; need = B * 4; break;
         default: REQUIRE(false, B200RL_ERR_INVALID, "unknown batch field");
     }
     REQUIRE(bytes >= need, B200RL_ERR_INVALID, "destination too small");
@@ -500,6 +551,9 @@ void b200rl_traj_internal_add_pushed(b200rl_traj* t, int64_t n) { t->pushed += n
 int64_t b200rl_traj_internal_pushed(b200rl_traj* t) { return t->pushed; }
 Ring b200rl_traj_internal_ring(b200rl_traj* t) { return t->r; }
 float b200rl_traj_internal_default_priority(b200rl_traj* t) { return t->default_priority; }
+// the n-step setting; discount: the per-sample γ^m of the last batch, or null for the 1-step sampler (the learner's scalar γ)
+void b200rl_traj_internal_nstep(b200rl_traj* t, int* n, float* gamma) { *n = t->nstep_n; *gamma = t->nstep_gamma; }
+const float* b200rl_traj_internal_discount(b200rl_traj* t) { return t->nstep_n > 1 ? t->discount : nullptr; }
 // rebuild the sum-tree paths of n keys (key -1 = none) whose leaves already hold their values: tree[L + key] = vals is rewritten with
 // the same values, then the paths are recomputed from the children (tree_update_keys_kernel)
 int b200rl_traj_internal_tree_rebuild(b200rl_traj* t, const int64_t* keys, const float* vals, int64_t n) {

@@ -29,7 +29,7 @@ using ReinforcementLearningCore: AbstractStage, PreExperimentStage, PostExperime
     EpsilonGreedyExplorer, GreedyExplorer, AbstractExplorer
 
 export B200Context, B200VecEnv, B200Network, B200OnPolicyAgent, B200RandomPolicy, B200Trajectory, B200DQNLearner, B200QBasedPolicy,
-    B200Agent, B200EpisodeStats, InsertSampleRatio, B200GreedyPolicy, evaluate, replay!
+    B200Agent, B200EpisodeStats, InsertSampleRatio, B200GreedyPolicy, evaluate, replay!, set_nstep!
 
 const LIB = get(ENV, "B200RL_LIB", joinpath(@__DIR__, "..", "libb200rl.so"))
 
@@ -472,11 +472,13 @@ function on_sample!(c::InsertSampleRatio)
 end
 """
     B200Trajectory(ctx; state_size, lanes, capacity, batch_size, sampler_seeds, prioritized = false, default_priority = 1f0,
-                   controller = InsertSampleRatio())
+                   controller = InsertSampleRatio(), n_step = 1, γ = 0.99f0)
 
-`Trajectory(container = CircularArraySARTSTraces(capacity) [wrapped in CircularPrioritizedTraces], sampler = BatchSampler(batch_size),
-controller = InsertSampleRatioController(ratio, threshold))` (ReinforcementLearningTrajectories 0.4) resident on the device:
-a ring of `capacity + 1` frames of `lanes` sub-envs; `next_state` of frame j is frame j + 1.
+`Trajectory(container = CircularArraySARTSTraces(capacity) [wrapped in CircularPrioritizedTraces], sampler = BatchSampler(batch_size)
+| NStepBatchSampler(n_step, γ, batch_size), controller = InsertSampleRatioController(ratio, threshold))` (ReinforcementLearningTrajectories
+0.4) resident on the device: a ring of `capacity + 1` frames of `lanes` sub-envs; `next_state` of frame j is frame j + 1.  With
+`n_step > 1` a sampled entry's reward / terminal / next_state come from its n-step window, `discount = γ^m` and `horizon = m` say how
+long it was (DESIGN.md §3), and the learner's γ must be the same.
 """
 mutable struct B200Trajectory
     ctx::B200Context
@@ -484,18 +486,39 @@ mutable struct B200Trajectory
     lanes::Int
     batch_size::Int
     controller::InsertSampleRatio
+    state_size::Int
+    n_step::Int
+    γ::Float32
 end
 function B200Trajectory(ctx::B200Context; state_size::Integer, lanes::Integer, capacity::Integer, batch_size::Integer,
                         sampler_seeds::AbstractVector{Xoshiro}, prioritized::Bool = false, default_priority = 1f0,
-                        controller = InsertSampleRatio())
+                        controller = InsertSampleRatio(), n_step::Integer = 1, γ = 0.99f0)
     length(sampler_seeds) == batch_size || throw(ArgumentError("need one Xoshiro per batch slot"))
     st = raw_states(sampler_seeds)
     out = Ref{Ptr{Cvoid}}(C_NULL)
     GC.@preserve st check(ccall((:b200rl_traj_create, LIB), Cint,
         (Ptr{Cvoid}, Cint, Int64, Int64, Cint, Cfloat, Ptr{UInt64}, Int64, Ref{Ptr{Cvoid}}),
         ctx.h, state_size, lanes, capacity, prioritized, default_priority, st, batch_size, out))
-    t = B200Trajectory(ctx, out[], lanes, batch_size, controller)
+    t = B200Trajectory(ctx, out[], lanes, batch_size, controller, state_size, 1, 0.99f0)
     finalizer(x -> (x.h == C_NULL || ccall((:b200rl_traj_destroy, LIB), Cint, (Ptr{Cvoid},), x.h); x.h = C_NULL), t)
+    n_step == 1 || set_nstep!(t, n_step, γ)
+    t
+end
+"`NStepBatchSampler(n, γ)` from the next sample on (`n = 1`: the BatchSampler); refused unless 1 ≤ n ≤ min(32, capacity), γ ∈ [0, 1]."
+function set_nstep!(t::B200Trajectory, n::Integer, γ)
+    check(ccall((:b200rl_traj_set_nstep, LIB), Cint, (Ptr{Cvoid}, Int32, Cfloat), t.h, n, γ))
+    t.n_step, t.γ = Int(n), Float32(γ)
+    t
+end
+"The last sampled batch: `(state, action, reward, terminal, next_state, key, priority, weight, discount, horizon)`."
+function batch(t::B200Trajectory)
+    B, ns = t.batch_size, t.state_size
+    field!(f, a) = (GC.@preserve a check(ccall((:b200rl_traj_batch_get, LIB), Cint, (Ptr{Cvoid}, Cint, Ptr{Cvoid}, Csize_t),
+                                                t.h, f, a, sizeof(a))); a)
+    (state = field!(0, Matrix{Float32}(undef, ns, B)), action = field!(1, Vector{Int32}(undef, B)), reward = field!(2, Vector{Float32}(undef, B)),
+     terminal = field!(3, Vector{UInt8}(undef, B)) .!= 0, next_state = field!(4, Matrix{Float32}(undef, ns, B)), key = field!(5, Vector{Int64}(undef, B)),
+     priority = field!(6, Vector{Float32}(undef, B)), weight = field!(7, Vector{Float32}(undef, B)), discount = field!(9, Vector{Float32}(undef, B)),
+     horizon = field!(10, Vector{Int32}(undef, B)))
 end
 function Base.length(t::B200Trajectory)
     n = Ref{Int64}(0)

@@ -248,13 +248,19 @@ class OnPolicyAgent(AbstractPolicy):
 
 
 BATCH_STATE, BATCH_ACTION, BATCH_REWARD, BATCH_TERMINAL, BATCH_NEXT_STATE, BATCH_KEY, BATCH_PRIORITY, BATCH_WEIGHT, BATCH_RNG = range(9)
+BATCH_DISCOUNT, BATCH_HORIZON = 9, 10
 
 
 class Trajectory:
     """Trajectory(container = CircularArraySARTSTraces(capacity) [+ CircularPrioritizedTraces],
-    sampler = BatchSampler(batch_size)) resident on the device."""
+    sampler = BatchSampler(batch_size) | NStepBatchSampler(n_step, gamma)) resident on the device.
 
-    def __init__(self, ctx, ns, capacity, lanes=1, batch_size=0, sampler_rng=None, prioritized=False, default_priority=1.0):
+    n_step > 1: a sampled entry's reward / terminal / next_state come from its n-step window (it ends early at a terminal entry,
+    the lane's newest frame or a forced reset), and the batch's ``discount`` (gamma^m) and ``horizon`` (m) say how long the window
+    was; the DQN learner's gamma must equal ``gamma``.  n_step = 1 is the BatchSampler, bit for bit."""
+
+    def __init__(self, ctx, ns, capacity, lanes=1, batch_size=0, sampler_rng=None, prioritized=False, default_priority=1.0, n_step=1,
+                 gamma=0.99):
         self.ctx, self.lib = ctx, ctx.lib
         self.ns, self.lanes, self.capacity, self.batch_size, self.prioritized = ns, lanes, capacity, batch_size, prioritized
         if batch_size:
@@ -262,6 +268,18 @@ class Trajectory:
         h = C.c_void_p()
         L.check(self.lib.b200rl_traj_create(ctx.h, ns, lanes, capacity, int(prioritized), default_priority, L.ptr(sampler_rng), batch_size, C.byref(h)))
         self.h = h
+        self.n_step, self.gamma = 1, 0.99
+        if n_step != 1:
+            try:
+                self.set_nstep(n_step, gamma)
+            except Exception:
+                self.close()
+                raise
+
+    def set_nstep(self, n_step, gamma):
+        """NStepBatchSampler(n_step, gamma) from the next sample on (b200rl_traj_set_nstep); n_step = 1 is the BatchSampler."""
+        L.check(self.lib.b200rl_traj_set_nstep(self.h, int(n_step), float(gamma)))
+        self.n_step, self.gamma = int(n_step), float(np.float32(gamma))
 
     def close(self):
         if getattr(self, "h", None):
@@ -342,7 +360,8 @@ class Trajectory:
         B, ns = self.batch_size, self.ns
         spec = {"state": (BATCH_STATE, (ns, B), np.float32), "action": (BATCH_ACTION, (B,), np.int32), "reward": (BATCH_REWARD, (B,), np.float32),
                 "terminal": (BATCH_TERMINAL, (B,), np.uint8), "next_state": (BATCH_NEXT_STATE, (ns, B), np.float32),
-                "key": (BATCH_KEY, (B,), np.int64), "priority": (BATCH_PRIORITY, (B,), np.float32), "weight": (BATCH_WEIGHT, (B,), np.float32)}
+                "key": (BATCH_KEY, (B,), np.int64), "priority": (BATCH_PRIORITY, (B,), np.float32), "weight": (BATCH_WEIGHT, (B,), np.float32),
+                "discount": (BATCH_DISCOUNT, (B,), np.float32), "horizon": (BATCH_HORIZON, (B,), np.int32)}
         out = {}
         for k, (f, shape, dt) in spec.items():
             a = np.empty(shape, dt, order="F")
