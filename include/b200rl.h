@@ -259,8 +259,14 @@ int b200rl_traj_total_priority(b200rl_traj* traj, float* out);
 /* kind 0: ActorCritic(actor -> n_out logits, critic -> 1)   (RLCore/src/utils/networks.jl:15-20, 405-432)
  * kind 1: ActorCritic(GaussianNetwork mu/sigma heads, 1-d action; sigma = clamp(softplus(raw)))  (networks.jl:44-116)
  * kind 2: Q-network n_in -> hidden -> hidden -> n_out with a TargetNetwork copy (target_network.jl:27-88)
+ * kind 3: dueling Q-network, DuelingNetwork(base = trunk, val = Dense(hidden,1), adv = Dense(hidden,n_out)) (networks.jl:500-522)
+ *         with a TargetNetwork copy: Q = (val + adv) - mean(adv), n_out = number of actions (1..3; 4 -> B200RL_ERR_UNSUPPORTED).
+ *         Flat vector: trunk, Wv (1 x hidden), bv, Wa (n_out x hidden), ba — Flux.destructure(DuelingNetwork(...)) as it is.
  * Trunks are Dense(n_in,hidden,act) -> Dense(hidden,hidden,act); act 0 relu, 1 tanh; hidden 64|128.
- * Parameters are one flat fp32 vector in Flux.destructure order (weights (out,in) column-major). */
+ * Parameters are one flat fp32 vector in Flux.destructure order (weights (out,in) column-major).
+ * Q-network entry points (kinds 2 and 3): net_values, net_q_act, net_q_explore, net_act_greedy, evaluate mode 0, dqn_update,
+ * dqn_last_td, replay_create.  Actor-critic entry points (kinds 0 and 1): net_act, net_ac_step, onpolicy_create, evaluate
+ * mode 1; they refuse kinds 2 and 3 before any side effect. */
 typedef struct { int32_t n_in, hidden, act, n_out, kind; } b200rl_net_desc;
 int b200rl_net_nparams(const b200rl_net_desc* desc, int64_t* out);
 /* FluxApproximator(model, Adam) (RLCore/src/policies/learners/flux_approximator.jl:11-46) */
@@ -282,7 +288,7 @@ int b200rl_net_target_sync(b200rl_net* net, float rho);
  * Outputs may be NULL; on_device applies to obs and outputs. */
 int b200rl_net_act(b200rl_net* net, const float* obs, int64_t n, uint64_t* rng_dev, void* action_out, float* logp_out, float* value_out,
                    float* heads_out, int on_device);
-/* critic V(s) -> (N) for kinds 0/1, Q(s, .) -> (n_out, N) for kind 2 */
+/* critic V(s) -> (N) for kinds 0/1, Q(s, .) -> (n_out, N) for kinds 2/3 (kind 3: the combined Q) */
 int b200rl_net_values(b200rl_net* net, const float* obs, int64_t n, float* out, int use_target, int on_device);
 /* QBasedPolicy + EpsilonGreedyExplorer (q_based_policy.jl:13-49, explorers/epsilon_greedy_explorer.jl:69-131); DEVICE pointers */
 int b200rl_net_q_act(b200rl_net* net, const float* obs_dev, int64_t n, uint64_t* rng_dev, float epsilon, int32_t* action_out_dev);
@@ -301,7 +307,7 @@ typedef struct {
 } b200rl_explorer;
 int b200rl_net_q_explore(b200rl_net* net, const float* obs_dev, int64_t n, uint64_t* rng_dev, const b200rl_explorer* explorer,
                          int32_t* action_out_dev);
-/* plan!(greedy policy, obs): findmax of the logits / Q-values (kinds 0, 2; int32 1-based, first maximum wins, NaN ranks
+/* plan!(greedy policy, obs): findmax of the logits / Q-values (kinds 0, 2, 3; int32 1-based, first maximum wins, NaN ranks
  * highest, -0.0 below 0.0), mu (kind 1; float, unclamped); no RNG.  on_device applies to obs and action_out. */
 int b200rl_net_act_greedy(b200rl_net* net, const float* obs, int64_t n, void* action_out, int on_device);
 

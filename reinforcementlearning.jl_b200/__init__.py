@@ -9,7 +9,7 @@ from .core import (AbstractHook, AbstractPolicy, BatchStepsPerEpisode, ComposedH
                    StopSignal, TimePerStep, TotalBatchRewardPerEpisode, run)
 from .envs import B200VecEnv, cartpole_params, mountaincar_params, pendulum_params
 from .explorers import EpsilonGreedyExplorer, GreedyExplorer
-from .learners import (ACT_RELU, ACT_TANH, KIND_CATEGORICAL, KIND_GAUSSIAN, KIND_Q, Agent, DQNLearner, EvaluationPolicy, InsertSampleRatioController,
+from .learners import (ACT_RELU, ACT_TANH, KIND_CATEGORICAL, KIND_DUELING, KIND_GAUSSIAN, KIND_Q, Agent, DQNLearner, EvaluationPolicy, InsertSampleRatioController,
                        Network, OnPolicyAgent, QBasedPolicy, Trajectory, dqn_config, evaluate, onpolicy_config)
 from . import checkpoint, core, explorers, learners, sharding
 from .returns import discount_rewards, discount_rewards_reduced, generalized_advantage_estimation

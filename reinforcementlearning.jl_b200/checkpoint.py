@@ -47,7 +47,7 @@ def checkpoint(env=None, net=None, agent=None):
     if net is not None:
         for name, w in _NET_FIELDS.items():
             out["net/" + name] = net.get(w)
-        if net.kind == R.KIND_Q:
+        if net.is_q:
             out["net/target"] = net.get(R.NET_TARGET)
     if agent is not None:
         c3 = np.zeros(3, np.int64)
@@ -73,7 +73,7 @@ def restore(ckpt, env=None, net=None, agent=None):
     if net is not None:
         for name, w in _NET_FIELDS.items():
             net.set(w, ckpt["net/" + name])
-        if net.kind == R.KIND_Q and "net/target" in ckpt:
+        if net.is_q and "net/target" in ckpt:
             net.set(R.NET_TARGET, ckpt["net/target"])
     if agent is not None:
         c3 = np.ascontiguousarray(ckpt["agent/counters"], np.int64)

@@ -150,7 +150,7 @@ __global__ void finalize_norm2_kernel(const double* __restrict__ sums2, double c
 // ------------------------------------------------------------------ network handle ---------
 struct b200rl_net {
     b200rl_ctx* ctx;
-    int kind;  // 0 actor-critic categorical, 1 actor-critic gaussian, 2 Q-network
+    int kind;  // 0 actor-critic categorical, 1 actor-critic gaussian, 2 Q-network, 3 dueling Q-network
     MlpDesc actor, critic;
     int64_t np;
     float *params, *grad, *m, *v, *beta_t, *target;
@@ -161,16 +161,21 @@ struct b200rl_net {
     uint64_t n_updates;
 };
 
+// kinds 2 and 3 are Q-networks (one flat vector, a target network, the DQN entry points); 0 and 1 actor-critic pairs
+static bool is_q_kind(int kind) { return kind == 2 || kind == 3; }
+
 static int make_descs(const b200rl_net_desc* d, MlpDesc* actor, MlpDesc* critic) {
     REQUIRE(d, B200RL_ERR_INVALID, "null desc");
-    REQUIRE(d->kind >= 0 && d->kind <= 2, B200RL_ERR_INVALID, "kind must be 0 (actor-critic categorical), 1 (gaussian) or 2 (Q-network)");
+    REQUIRE(d->kind >= 0 && d->kind <= 3, B200RL_ERR_INVALID,
+            "kind must be 0 (actor-critic categorical), 1 (gaussian), 2 (Q-network) or 3 (dueling Q-network)");
     REQUIRE(d->n_in >= 1 && d->n_in <= kInMax, B200RL_ERR_UNSUPPORTED, "n_in must be 1..4");
     REQUIRE(d->hidden == 64 || d->hidden == 128, B200RL_ERR_UNSUPPORTED, "hidden must be 64 or 128");
     REQUIRE(d->act == 0 || d->act == 1, B200RL_ERR_INVALID, "act must be 0 (relu) or 1 (tanh)");
     if (d->kind == 1) REQUIRE(d->n_out == 1, B200RL_ERR_UNSUPPORTED, "gaussian policy supports a 1-d action");
+    else if (d->kind == 3) REQUIRE(d->n_out >= 1 && d->n_out + 1 <= kOutMax, B200RL_ERR_UNSUPPORTED, "dueling Q-network: n_out (actions) must be 1..3");
     else REQUIRE(d->n_out >= 1 && d->n_out <= kOutMax, B200RL_ERR_UNSUPPORTED, "n_out must be 1..4");
-    *actor = MlpDesc{d->n_in, d->hidden, d->act, d->kind == 1 ? 2 : d->n_out, d->kind == 1 ? 1 : 0};
-    *critic = MlpDesc{d->n_in, d->hidden, d->act, 1, 0};
+    *actor = MlpDesc{d->n_in, d->hidden, d->act, d->kind == 1 ? 2 : d->n_out, d->kind == 1 ? 1 : 0, d->kind == 3 ? 1 : 0};
+    *critic = MlpDesc{d->n_in, d->hidden, d->act, 1, 0, 0};
     return B200RL_OK;
 }
 
@@ -180,7 +185,7 @@ int b200rl_net_nparams(const b200rl_net_desc* d, int64_t* out) {
     MlpDesc a, c;
     TRY(make_descs(d, &a, &c));
     REQUIRE(out, B200RL_ERR_INVALID, "null out");
-    *out = d->kind == 2 ? a.nparams() : a.nparams() + c.nparams();
+    *out = is_q_kind(d->kind) ? a.nparams() : a.nparams() + c.nparams();
     return B200RL_OK;
 }
 
@@ -194,7 +199,7 @@ int b200rl_net_destroy(b200rl_net* n) {
     return B200RL_OK;
 }
 
-/* Replaces FluxApproximator(model, optimiser) (+ TargetNetwork for kind 2): takes the flat
+/* Replaces FluxApproximator(model, optimiser) (+ TargetNetwork for kinds 2 and 3): takes the flat
  * Flux.destructure parameter vector; optimiser = Adam(1e-3, (0.9, 0.999), 1e-8), clip 0.5 until
  * b200rl_net_configure_optimizer is called. */
 int b200rl_net_create(b200rl_ctx* ctx, const b200rl_net_desc* d, const float* params_host, b200rl_net** out) {
@@ -205,22 +210,22 @@ int b200rl_net_create(b200rl_ctx* ctx, const b200rl_net_desc* d, const float* pa
     n->ctx = ctx; n->kind = d ? d->kind : 0;
     int s = make_descs(d, &n->actor, &n->critic);
     if (s != B200RL_OK) { delete n; return s; }
-    n->np = n->kind == 2 ? n->actor.nparams() : n->actor.nparams() + n->critic.nparams();
+    n->np = is_q_kind(n->kind) ? n->actor.nparams() : n->actor.nparams() + n->critic.nparams();
     n->lr = 1e-3f; n->b1 = 0.9f; n->b2 = 0.999f; n->eps = 1e-8f; n->max_grad_norm = 0.5f;
     size_t bytes = (size_t)n->np * sizeof(float);
-    n->n_partials = n->kind == 2 ? nn_dqn_max_partials(ctx, n->actor.H) : nn_grid_ctas(ctx, n->actor.H);
+    n->n_partials = is_q_kind(n->kind) ? nn_dqn_max_partials(ctx, n->actor.H) : nn_grid_ctas(ctx, n->actor.H);
     int n_loss_rows = 2 * (n->n_partials > ctx->sm_count ? n->n_partials : ctx->sm_count);
 #define NET_TRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { b200rl_set_error("%s -> %s", #x, cudaGetErrorString(_e)); b200rl_net_destroy(n); return B200RL_ERR_CUDA; } } while (0)
     NET_TRY(cudaMalloc(&n->params, bytes)); NET_TRY(cudaMalloc(&n->grad, bytes)); NET_TRY(cudaMalloc(&n->m, bytes)); NET_TRY(cudaMalloc(&n->v, bytes));
     NET_TRY(cudaMalloc(&n->beta_t, 2 * sizeof(float)));
-    if (n->kind == 2) NET_TRY(cudaMalloc(&n->target, bytes));
+    if (is_q_kind(n->kind)) NET_TRY(cudaMalloc(&n->target, bytes));
     NET_TRY(cudaMalloc(&n->partial, (size_t)n->n_partials * bytes));
     NET_TRY(cudaMalloc(&n->loss_partial, (size_t)n_loss_rows * 4 * sizeof(float)));
     NET_TRY(cudaMalloc(&n->loss4, 4 * sizeof(float))); NET_TRY(cudaMalloc(&n->gnorm, sizeof(float)));
     NET_TRY(cudaMalloc(&n->cta_sumsq, 256 * sizeof(double))); NET_TRY(cudaMalloc(&n->counter2, 4 * sizeof(unsigned int)));
     NET_TRY(cudaMemsetAsync(n->counter2, 0, 4 * sizeof(unsigned int), ctx->stream));
     NET_TRY(cudaMemcpyAsync(n->params, params_host, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    if (n->kind == 2) NET_TRY(cudaMemcpyAsync(n->target, params_host, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (is_q_kind(n->kind)) NET_TRY(cudaMemcpyAsync(n->target, params_host, bytes, cudaMemcpyHostToDevice, ctx->stream));
     NET_TRY(cudaMemsetAsync(n->grad, 0, bytes, ctx->stream)); NET_TRY(cudaMemsetAsync(n->m, 0, bytes, ctx->stream));
     NET_TRY(cudaMemsetAsync(n->v, 0, bytes, ctx->stream));
     NET_TRY(cudaMemsetAsync(n->partial, 0, (size_t)n->n_partials * bytes, ctx->stream));
@@ -319,7 +324,7 @@ static int stage_obs(b200rl_net* n, const float* obs, int64_t N, int on_device, 
  * rng = (4, N) uint64 DEVICE policy streams (advanced in place).  Outputs may be NULL.  on_device applies to obs and outputs. */
 int b200rl_net_act(b200rl_net* n, const float* obs, int64_t N, uint64_t* rng_dev, void* action_out, float* logp_out, float* value_out,
                    float* heads_out, int on_device) {
-    REQUIRE(n && obs && rng_dev && n->kind != 2, B200RL_ERR_INVALID, "bad argument (actor-critic nets only)");
+    REQUIRE(n && obs && rng_dev && !is_q_kind(n->kind), B200RL_ERR_INVALID, "bad argument (actor-critic nets only)");
     TRY(ctx_bind(n->ctx));
     AcHyper hp{0.1f, 1.f, 0.5f, 0.001f, 0.f, __builtin_inff(), 0, 0};
     const float* dobs;
@@ -339,12 +344,12 @@ int b200rl_net_act(b200rl_net* n, const float* obs, int64_t N, uint64_t* rng_dev
     return B200RL_OK;
 }
 
-/* critic V(s) (kinds 0/1: out (N)) or Q(s, .) (kind 2: out (n_out, N)); use_target selects the target network */
+/* critic V(s) (kinds 0/1: out (N)) or Q(s, .) (kinds 2, 3: out (n_out, N); kind 3 the combined Q); use_target selects the target network */
 int b200rl_net_values(b200rl_net* n, const float* obs, int64_t N, float* out, int use_target, int on_device) {
     REQUIRE(n && obs && out, B200RL_ERR_INVALID, "null argument");
     TRY(ctx_bind(n->ctx));
-    const MlpDesc& d = n->kind == 2 ? n->actor : n->critic;
-    const float* p = n->kind == 2 ? (use_target ? n->target : n->params) : n->params + n->actor.nparams();
+    const MlpDesc& d = is_q_kind(n->kind) ? n->actor : n->critic;
+    const float* p = is_q_kind(n->kind) ? (use_target ? n->target : n->params) : n->params + n->actor.nparams();
     REQUIRE(p, B200RL_ERR_INVALID, "no target network");
     const float* dobs;
     size_t ob = (size_t)N * d.nout * 4;
@@ -359,7 +364,7 @@ int b200rl_net_values(b200rl_net* n, const float* obs, int64_t N, float* out, in
 
 /* epsilon-greedy action selection on Q(s, .) (EpsilonGreedyExplorer / QBasedPolicy plan!); all pointers DEVICE */
 int b200rl_net_q_act(b200rl_net* n, const float* obs_dev, int64_t N, uint64_t* rng_dev, float epsilon, int32_t* action_out_dev) {
-    REQUIRE(n && obs_dev && action_out_dev && n->kind == 2, B200RL_ERR_INVALID, "bad argument (Q-network only)");
+    REQUIRE(n && obs_dev && action_out_dev && is_q_kind(n->kind), B200RL_ERR_INVALID, "bad argument (Q-network only)");
     REQUIRE(epsilon <= 0.f || rng_dev, B200RL_ERR_INVALID, "rng required for epsilon > 0");
     TRY(ctx_bind(n->ctx));
     void* s;
@@ -369,7 +374,7 @@ int b200rl_net_q_act(b200rl_net* n, const float* obs_dev, int64_t N, uint64_t* r
 
 /* BatchExplorer(EpsilonGreedyExplorer) with the decay schedule evaluated per column on the device; all pointers DEVICE */
 int b200rl_net_q_explore(b200rl_net* n, const float* obs_dev, int64_t N, uint64_t* rng_dev, const b200rl_explorer* ex, int32_t* action_out_dev) {
-    REQUIRE(n && obs_dev && action_out_dev && rng_dev && ex && n->kind == 2, B200RL_ERR_INVALID, "bad argument (Q-network only)");
+    REQUIRE(n && obs_dev && action_out_dev && rng_dev && ex && is_q_kind(n->kind), B200RL_ERR_INVALID, "bad argument (Q-network only)");
     REQUIRE(N > 0, B200RL_ERR_INVALID, "empty batch");
     REQUIRE((ex->kind == 0 || ex->kind == 1) && ex->warmup_steps >= 0 && ex->decay_steps >= 0, B200RL_ERR_INVALID, "bad explorer schedule");
     REQUIRE(ex->eps_stable >= 0.0 && ex->eps_stable <= 1.0 && ex->eps_init >= 0.0 && ex->eps_init <= 1.0, B200RL_ERR_INVALID, "epsilon outside [0, 1]");
@@ -379,7 +384,7 @@ int b200rl_net_q_explore(b200rl_net* n, const float* obs_dev, int64_t N, uint64_
     return nn_q_explore(n->ctx, n->actor, n->params, obs_dev, N, (unsigned long long*)rng_dev, *ex, action_out_dev, (float*)s);
 }
 
-/* plan!(greedy policy, obs): findmax of the logits / Q-values (kinds 0, 2), mu (kind 1); no RNG.  Same forward pass as
+/* plan!(greedy policy, obs): findmax of the logits / Q-values (kinds 0, 2, 3), mu (kind 1); no RNG.  Same forward pass as
  * b200rl_net_values / the head outputs of b200rl_net_act. */
 int b200rl_net_act_greedy(b200rl_net* n, const float* obs, int64_t N, void* action_out, int on_device) {
     REQUIRE(n && obs && action_out, B200RL_ERR_INVALID, "null argument");
@@ -410,7 +415,7 @@ int b200rl_evaluate(b200rl_net* n, b200rl_env* env, const b200rl_eval_config* cf
     REQUIRE(b200rl_env_internal_dtype(env) == B200RL_F32, B200RL_ERR_UNSUPPORTED, "the networks read Float32 observations: construct the env with T = Float32");
     REQUIRE(b200rl_env_internal_kind(env) != B200RL_ENV_ACROBOT, B200RL_ERR_UNSUPPORTED, "AcrobotEnv has 6 observations (networks take at most 4)");
     REQUIRE(cfg->mode == 0 || cfg->mode == 1, B200RL_ERR_INVALID, "mode must be 0 (greedy) or 1 (sample)");
-    REQUIRE(!(cfg->mode == 1 && n->kind == 2), B200RL_ERR_UNSUPPORTED, "mode 1 samples a policy head: evaluate a Q-network with mode 0 or QBasedPolicy");
+    REQUIRE(!(cfg->mode == 1 && is_q_kind(n->kind)), B200RL_ERR_UNSUPPORTED, "mode 1 samples a policy head: evaluate a Q-network with mode 0 or QBasedPolicy");
     REQUIRE(b200rl_env_internal_nobs(env) == n->actor.in, B200RL_ERR_INVALID, "network input width != observation width");
     const bool cont = b200rl_env_internal_continuous(env);
     REQUIRE(cont == (n->kind == 1), B200RL_ERR_INVALID, "head kind != action-space kind (Gaussian head <-> continuous actions)");
@@ -494,7 +499,7 @@ int b200rl_evaluate(b200rl_net* n, b200rl_env* env, const b200rl_eval_config* cf
 int b200rl_net_ac_step(b200rl_net* n, const b200rl_onpolicy_config* cfg, const float* states, const void* actions, const float* logp_old,
                        const float* adv, const float* ret, int64_t total, const int32_t* idx, int64_t B, float adv_mean, float adv_inv_std,
                        int apply_update, float* losses_out) {
-    REQUIRE(n && cfg && states && actions && adv && ret && n->kind != 2, B200RL_ERR_INVALID, "bad argument");
+    REQUIRE(n && cfg && states && actions && adv && ret && !is_q_kind(n->kind), B200RL_ERR_INVALID, "bad argument");
     TRY(ctx_bind(n->ctx));
     b200rl_ctx* ctx = n->ctx;
     int ns = n->actor.in;
@@ -595,7 +600,7 @@ int b200rl_onpolicy_create(b200rl_ctx* ctx, b200rl_net* net, b200rl_env* env, co
                            b200rl_onpolicy** out) {
     TRY(ctx_bind(ctx));
     REQUIRE(net && env && cfg && policy_rng && out, B200RL_ERR_INVALID, "null argument");
-    REQUIRE(net->kind != 2, B200RL_ERR_INVALID, "needs an actor-critic network");
+    REQUIRE(!is_q_kind(net->kind), B200RL_ERR_INVALID, "needs an actor-critic network");
     REQUIRE(net->ctx == ctx && b200rl_env_internal_ctx(env) == ctx, B200RL_ERR_INVALID, "net/env belong to another ctx");
     REQUIRE(b200rl_env_internal_dtype(env) == B200RL_F32, B200RL_ERR_UNSUPPORTED, "the learners read Float32 observations: construct the env with T = Float32");
     REQUIRE(cfg->update_freq >= 1 && cfg->n_epochs >= 1 && cfg->n_microbatches >= 1, B200RL_ERR_INVALID, "bad config");
@@ -1129,7 +1134,7 @@ static int dqn_stats(b200rl_net* n, const float* td, int64_t B, float* stats4) {
 }
 
 int b200rl_dqn_update(b200rl_net* n, b200rl_traj* t, const b200rl_dqn_config* cfg, float* stats_host) {
-    REQUIRE(n && t && cfg && n->kind == 2, B200RL_ERR_INVALID, "bad argument (needs a Q-network)");
+    REQUIRE(n && t && cfg && is_q_kind(n->kind), B200RL_ERR_INVALID, "bad argument (needs a Q-network)");
     REQUIRE(n->ctx == b200rl_traj_internal_ctx(t), B200RL_ERR_INVALID, "net/trajectory belong to different ctx");
     TRY(check_nstep_gamma(t, cfg));
     TRY(ctx_bind(n->ctx));
@@ -1267,7 +1272,7 @@ int b200rl_replay_destroy(b200rl_replay* r) {
 int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl_traj* traj, const b200rl_dqn_config* cfg, b200rl_replay** out) {
     TRY(ctx_bind(ctx));
     REQUIRE(q && env && traj && cfg && out, B200RL_ERR_INVALID, "null argument");
-    REQUIRE(q->kind == 2, B200RL_ERR_INVALID, "needs a Q-network (kind 2)");
+    REQUIRE(is_q_kind(q->kind), B200RL_ERR_INVALID, "needs a Q-network (kind 2 or 3)");
     REQUIRE(q->ctx == ctx && b200rl_env_internal_ctx(env) == ctx && b200rl_traj_internal_ctx(traj) == ctx, B200RL_ERR_INVALID,
             "net/env/trajectory belong to another ctx");
     REQUIRE(b200rl_env_internal_dtype(env) == B200RL_F32, B200RL_ERR_UNSUPPORTED, "the Q-network reads Float32 observations: construct the env with T = Float32");

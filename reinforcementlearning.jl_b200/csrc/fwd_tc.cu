@@ -11,6 +11,7 @@
 // Both kernels are built from the same device functions (tc_fwd.cuh, env_device.cuh) and compiled with the env flags
 // (-fmad=false): stepping through plan!/act! one launch at a time or through the fused rollout gives bit-identical results.
 #include "common.cuh"
+#include "duel.cuh"
 #include "env_device.cuh"
 #include "explore.cuh"
 #include "greedy.cuh"
@@ -109,6 +110,7 @@ forward_tc_kernel(MlpDesc actor, MlpDesc critic, const float* __restrict__ param
                 float z[kOutMax];
 #pragma unroll
                 for (int o = 0; o < kOutMax; ++o) z[o] = sm.net.b3[o] + sm.Zp[o * TM + tid] + sm.Zp[(kOutMax + o) * TM + tid];
+                if (mode == 1 && d.duel) duel::combine(z, d.nout);   // dueling Q-network: the combined Q, not the head rows
                 if (head_out && (mode == 1 || role == 0))
                     for (int o = 0; o < d.nout; ++o) head_out[(int64_t)d.nout * i + o] = z[o];
                 if (mode == 0 && role == 1) {
@@ -181,8 +183,8 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
     const int cta = blockIdx.x, nctas = gridDim.x;
     const int64_t N = g.N;
     const int64_t ntiles = (N + TM - 1) / TM;
-    load_net(sm.net[0], g.actor, g.params, ACT == B200RL_ACT_RELU ? kScale : 1.0f);
-    load_net(sm.net[1], g.critic, g.params + g.actor.nparams(), ACT == B200RL_ACT_RELU ? kScale : 1.0f);
+    load_net<false>(sm.net[0], g.actor, g.params, ACT == B200RL_ACT_RELU ? kScale : 1.0f);
+    load_net<false>(sm.net[1], g.critic, g.params + g.actor.nparams(), ACT == B200RL_ACT_RELU ? kScale : 1.0f);
     // resident env state
     int nslots = 0;
     for (int k = 0; k < kSlots; ++k)
@@ -411,9 +413,10 @@ struct EvalArgs {
     int32_t* counts;                    // (N), may be null
 };
 
-// MODE 0: greedy (greedy.cuh, no draw), 1: sample_head on the policy streams
+// MODE 0: greedy (greedy.cuh, no draw), 1: sample_head on the policy streams.  DUEL (MODE 0 only): a dueling Q-network, its head
+// rows combined into Q (duel.cuh) before the selection; the instantiations without it are the code of the other kinds.
 // (layer 1 and the head epilogue not unrolled: the relu variants would exceed 128 registers and spill)
-template <class Env, int ACT, int MODE>
+template <class Env, int ACT, int MODE, bool DUEL = false>
 __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename Env::P p, EnvArrays ea) {
     using act_t = typename Env::act_t;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -425,7 +428,7 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename
     const int64_t N = g.N;
     const int nctas = gridDim.x;
     const int64_t ntiles = (N + TM - 1) / TM;
-    load_net(sm.net, g.actor, g.params, ACT == B200RL_ACT_RELU ? kScale : 1.0f);
+    load_net<DUEL>(sm.net, g.actor, g.params, ACT == B200RL_ACT_RELU ? kScale : 1.0f);
     if (owner) { sm.fin_cnt[s] = 0; sm.fin_len[s] = 0; sm.fin_ret[s] = 0.f; }
 #pragma unroll 1
     for (int64_t base = blockIdx.x; base < ntiles; base += (int64_t)nctas * kSlots) {   // tiles base + k * nctas, k < kSlots
@@ -489,6 +492,7 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename
                     float z[kOutMax];
 #pragma unroll
                     for (int o = 0; o < kOutMax; ++o) z[o] = sm.net.b3[o] + sm.Zp[o * TM + s] + sm.Zp[(kOutMax + o) * TM + s];
+                    if (DUEL) duel::combine(z, g.actor.nout);
                     uint32_t a_bits;
                     if (MODE == 0) {
                         a_bits = greedy::greedy_action(g.actor, z);
@@ -584,12 +588,17 @@ template <class Env> int launch_evaluate(b200rl_ctx* ctx, const EvalArgs& g, con
         CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_TANH, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_RELU, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_TANH, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_RELU, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_TANH, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     const int64_t groups = ((g.N + TM - 1) / TM + kSlots - 1) / kSlots;
     int grid = 2 * ctx->sm_count;
     if ((int64_t)grid > groups) grid = (int)groups;
     const bool relu = g.actor.act == B200RL_ACT_RELU;
-    if (mode == 0) {
+    if (mode == 0 && g.actor.duel) {
+        if (relu) evaluate_tc_kernel<Env, B200RL_ACT_RELU, 0, true><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
+        else evaluate_tc_kernel<Env, B200RL_ACT_TANH, 0, true><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
+    } else if (mode == 0) {
         if (relu) evaluate_tc_kernel<Env, B200RL_ACT_RELU, 0><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
         else evaluate_tc_kernel<Env, B200RL_ACT_TANH, 0><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
     } else {
@@ -652,7 +661,9 @@ struct ReplayArgs {
     int stride;                            // min(2 nsteps + 1, cap + 1)
 };
 
-template <class Env, int ACT>
+// DUEL: a dueling Q-network, its head rows combined into Q (duel.cuh) before the selection (the instantiations without it are the
+// code of a plain Q-network)
+template <class Env, int ACT, bool DUEL = false>
 __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, typename Env::P p, EnvArrays ea) {
     using act_t = typename Env::act_t;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -667,7 +678,7 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
     const long long step0 = g.greedy ? 0 : *g.step_dev;
     const Ring& r = g.ring;
     const int64_t F = r.frames();
-    load_net(sm.net, g.q, g.params, ACT == B200RL_ACT_RELU ? kScale : 1.0f);
+    load_net<DUEL>(sm.net, g.q, g.params, ACT == B200RL_ACT_RELU ? kScale : 1.0f);
     if (owner) { sm.fin_cnt[s] = 0; sm.fin_len[s] = 0; sm.fin_ret[s] = 0.f; sm.dv[s] = 0; }
 #pragma unroll 1
     for (int64_t base = blockIdx.x; base < ntiles; base += (int64_t)nctas * kSlots) {
@@ -731,6 +742,7 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
                     float z[kOutMax];
 #pragma unroll
                     for (int o = 0; o < kOutMax; ++o) z[o] = sm.net.b3[o] + sm.Zp[o * TM + s] + sm.Zp[(kOutMax + o) * TM + s];
+                    if (DUEL) duel::combine(z, g.q.nout);
                     int a1;
                     if (g.greedy) {
                         int best = 0;      // q_act_kernel with epsilon = 0: the first maximum under `>`
@@ -840,11 +852,16 @@ template <class Env> int launch_replay_collect(b200rl_ctx* ctx, const ReplayArgs
     if (first_use_on_device(attr_devices, ctx->device)) {
         CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_TANH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_RELU, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_TANH, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     const int64_t groups = ((g.N + TM - 1) / TM + kSlots - 1) / kSlots;
     int grid = 2 * ctx->sm_count;
     if ((int64_t)grid > groups) grid = (int)groups;
-    if (g.q.act == B200RL_ACT_RELU) replay_collect_tc_kernel<Env, B200RL_ACT_RELU><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
+    if (g.q.duel) {
+        if (g.q.act == B200RL_ACT_RELU) replay_collect_tc_kernel<Env, B200RL_ACT_RELU, true><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
+        else replay_collect_tc_kernel<Env, B200RL_ACT_TANH, true><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
+    } else if (g.q.act == B200RL_ACT_RELU) replay_collect_tc_kernel<Env, B200RL_ACT_RELU><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
     else replay_collect_tc_kernel<Env, B200RL_ACT_TANH><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
     LAUNCH_CHECK(ctx);
     return B200RL_OK;
@@ -852,7 +869,7 @@ template <class Env> int launch_replay_collect(b200rl_ctx* ctx, const ReplayArgs
 
 }  // namespace
 
-bool nn_tc_supported(const MlpDesc& d) { return d.H == 64 && d.in <= kInMax && d.nout <= kOutMax; }
+bool nn_tc_supported(const MlpDesc& d) { return d.H == 64 && d.in <= kInMax && d.rows() <= kOutMax; }
 
 int nn_tc_forward(b200rl_ctx* ctx, int grid, const MlpDesc& actor, const MlpDesc& critic, const float* params, const AcHyper& hp, int mode,
                   const float* obs, int64_t N, unsigned long long* rng, void* action_out, float* logp_out, float* value_out, float* head_out,

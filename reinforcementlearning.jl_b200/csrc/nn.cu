@@ -13,6 +13,7 @@
 // (RLCore/src/utils/networks.jl:405-432), Gaussian head + diagnormlogpdf (networks.jl:44-116,
 // distributions.jl:9-34), clip_by_global_norm! (basic.jl:19-29), TargetNetwork sync
 // (policies/learners/target_network.jl:70-88).
+#include "duel.cuh"
 #include "explore.cuh"
 #include "nn.cuh"
 #include "perm.cuh"
@@ -60,15 +61,6 @@ __device__ __forceinline__ uint32_t mix32(uint32_t h) {
 using b200perm::perm_index;
 using b200perm::perm_index_bits;
 
-// head parameter addressing inside the flat parameter vector
-__device__ __forceinline__ int64_t head_base(const MlpDesc& d) { return (int64_t)d.H * d.in + d.H + (int64_t)d.H * d.H + d.H; }
-__device__ __forceinline__ int64_t head_w(const MlpDesc& d, int o, int j) {
-    return head_base(d) + (d.heads2 ? (int64_t)o * (d.H + 1) + j : (int64_t)o + (int64_t)d.nout * j);
-}
-__device__ __forceinline__ int64_t head_b(const MlpDesc& d, int o) {
-    return head_base(d) + (d.heads2 ? (int64_t)o * (d.H + 1) + d.H : (int64_t)d.nout * d.H + o);
-}
-
 template <int H, bool BWD> __device__ void load_weights(Smem<H, BWD>& sm, const MlpDesc& d, const float* __restrict__ p) {
     const int tid = threadIdx.x;
     const float* W1 = p;
@@ -84,9 +76,9 @@ template <int H, bool BWD> __device__ void load_weights(Smem<H, BWD>& sm, const 
     }
     for (int k = tid; k < H * kOutMax; k += NT) {
         int j = k / kOutMax, o = k % kOutMax;
-        sm.W3[k] = o < d.nout ? p[head_w(d, o, j)] : 0.f;
+        sm.W3[k] = o < d.rows() ? p[head_w(d, o, j)] : 0.f;
     }
-    if (tid < kOutMax) sm.b3[tid] = tid < d.nout ? p[head_b(d, tid)] : 0.f;
+    if (tid < kOutMax) sm.b3[tid] = tid < d.rows() ? p[head_b(d, tid)] : 0.f;
 }
 
 // ---- forward pieces -----------------------------------------------------------------------
@@ -183,7 +175,7 @@ template <int H, bool BWD> __device__ void forward_tile(Smem<H, BWD>& sm, const 
     store_tile<H>(sm.H2, acc, tx, ty);
     __syncthreads();
     // head: one (output, sample) pair per thread
-    for (int pidx = threadIdx.x; pidx < d.nout * C::TM; pidx += NT) {
+    for (int pidx = threadIdx.x; pidx < d.rows() * C::TM; pidx += NT) {
         int o = pidx / C::TM, s = pidx % C::TM;
         float z = sm.b3[o];
 #pragma unroll 8
@@ -213,7 +205,7 @@ template <int H> __device__ void backward_tile(Smem<H, true>& sm, const MlpDesc&
     for (int r = 0; r < (kOutMax * H + NT - 1) / NT; ++r) {
         int idx = tid + NT * r;
         int o = idx / H, j = idx % H;
-        if (o < d.nout) {
+        if (o < d.rows()) {
             float a = 0.f;
             const float* dz = sm.Dz + o * C::LDA;
             const float* h = sm.H2 + j * C::LDA;
@@ -226,7 +218,7 @@ template <int H> __device__ void backward_tile(Smem<H, true>& sm, const MlpDesc&
             g.w3[r] += a;
         }
     }
-    if (tid < d.nout) {
+    if (tid < d.rows()) {
         float a = 0.f;
         for (int s = 0; s < C::TM; ++s) a += sm.Dz[tid * C::LDA + s];
         g.b3 += a;
@@ -372,9 +364,9 @@ template <int H> __device__ void write_grad(const GradAcc<H>& g, const MlpDesc& 
     for (int r = 0; r < (kOutMax * H + NT - 1) / NT; ++r) {
         int idx = tid + NT * r;
         int o = idx / H, j = idx % H;
-        if (o < d.nout) out[head_w(d, o, j)] = g.w3[r];
+        if (o < d.rows()) out[head_w(d, o, j)] = g.w3[r];
     }
-    if (tid < d.nout) out[head_b(d, tid)] = g.b3;
+    if (tid < d.rows()) out[head_b(d, tid)] = g.b3;
 }
 
 __device__ __forceinline__ float block_sum(float v, float* red) {
@@ -628,7 +620,13 @@ forward_kernel(MlpDesc actor, MlpDesc critic, const float* __restrict__ params, 
         if (tid < C::TM) {
             int64_t i = tile * C::TM + tid;
             if (i < N) {
-                if (head_out && (mode == 1 || role == 0))
+                if (head_out && mode == 1 && d.duel) {   // dueling Q-network: the combined Q, not the head rows
+                    float z[kOutMax];
+#pragma unroll
+                    for (int o = 0; o < kOutMax; ++o) z[o] = sm.Out[o * C::LDA + tid];
+                    duel::combine(z, d.nout);
+                    for (int o = 0; o < d.nout; ++o) head_out[(int64_t)d.nout * i + o] = z[o];
+                } else if (head_out && (mode == 1 || role == 0))
                     for (int o = 0; o < d.nout; ++o) head_out[(int64_t)d.nout * i + o] = sm.Out[o * C::LDA + tid];
                 if (mode == 0 && role == 1) {
                     if (value_out) value_out[i] = sm.Out[tid];
@@ -902,9 +900,13 @@ dqn_loss_grad_kernel(MlpDesc q, const float* __restrict__ params, const float* _
                 }
                 float R = r[j] + (DISC ? disc[j] : gamma) * (t[j] ? 0.f : 1.f) * qn;
                 int ai = a[j] - 1;
+                float z[kOutMax];
+#pragma unroll
+                for (int o = 0; o < kOutMax; ++o) z[o] = sm.Out[o * C::LDA + tid];
+                if (q.duel) duel::combine(z, na);
                 float qv = 0.f;
 #pragma unroll
-                for (int o = 0; o < kOutMax; ++o) if (o == ai) qv = sm.Out[o * C::LDA + tid];
+                for (int o = 0; o < kOutMax; ++o) if (o == ai) qv = z[o];
                 float e = R - qv;
                 td_out[j] = e;
                 float wi = w ? w[j] : 1.f;
@@ -914,8 +916,11 @@ dqn_loss_grad_kernel(MlpDesc q, const float* __restrict__ params, const float* _
                     else { l = ae - 0.5f; dl = e > 0.f ? -1.f : 1.f; }
                 } else { l = e * e; dl = -2.0f * e; }
                 l0 += wi * l;
+                if (q.duel) duel::backward(wi * inv_B * dl, ai, na, dz);
+                else {
 #pragma unroll
-                for (int o = 0; o < kOutMax; ++o) if (o == ai) dz[o] = wi * inv_B * dl;
+                    for (int o = 0; o < kOutMax; ++o) if (o == ai) dz[o] = wi * inv_B * dl;
+                }
             }
 #pragma unroll
             for (int o = 0; o < kOutMax; ++o) sm.Dz[o * C::LDA + tid] = dz[o];
@@ -1022,7 +1027,8 @@ static int launch_dqn(b200rl_ctx* ctx, int grid, const MlpDesc& q, const float* 
 
 static int check_desc(const MlpDesc& d) {
     REQUIRE(d.in >= 1 && d.in <= kInMax, B200RL_ERR_UNSUPPORTED, "observation width must be 1..4");
-    REQUIRE(d.nout >= 1 && d.nout <= kOutMax, B200RL_ERR_UNSUPPORTED, "head width must be 1..4");
+    REQUIRE(d.nout >= 1 && d.rows() <= kOutMax, B200RL_ERR_UNSUPPORTED, d.duel ? "dueling head supports 1..3 actions" : "head width must be 1..4");
+    REQUIRE(!(d.duel && d.heads2), B200RL_ERR_UNSUPPORTED, "a dueling head is a Q-network head");
     REQUIRE(d.H == 64 || d.H == 128, B200RL_ERR_UNSUPPORTED, "hidden width must be 64 or 128");
     REQUIRE(!d.heads2 || d.nout == 2, B200RL_ERR_UNSUPPORTED, "gaussian head supports 1-d actions");
     return B200RL_OK;

@@ -5,19 +5,39 @@
 //   W1 (H x in), b1 (H), W2 (H x H), b2 (H), then
 //   single head:     W3 (n_out x H), b3 (n_out)                      [categorical logits / value / Q]
 //   gaussian heads:  Wmu (1 x H), bmu (1), Wsig (1 x H), bsig (1)    [GaussianNetwork mu / sigma, 1-d action]
-// (ActorCritic RLCore/src/utils/networks.jl:15-20, GaussianNetwork :44-116.)
+//   dueling heads:   Wv (1 x H), bv (1), Wa (n_out x H), ba (n_out)  [DuelingNetwork val / adv, combined by duel.cuh]
+// (ActorCritic RLCore/src/utils/networks.jl:15-20, GaussianNetwork :44-116, DuelingNetwork :500-522.)
 #pragma once
 #include "common.cuh"
 
 constexpr int kInMax = 4;    // observation width <= 4 (CartPole 4, Pendulum 3, MountainCar 2)
-constexpr int kOutMax = 4;   // head width <= 4
+constexpr int kOutMax = 4;   // head rows <= 4 (a dueling head has n_out + 1 rows: n_out <= 3)
 
 enum { B200RL_ACT_RELU = 0, B200RL_ACT_TANH = 1 };
 
 struct MlpDesc {
     int in, H, act, nout, heads2;  // heads2: two 1-wide heads (gaussian mu / sigma)
-    __host__ __device__ int64_t nparams() const { return (int64_t)H * in + H + (int64_t)H * H + H + (int64_t)nout * H + nout; }
+    int duel;                      // 1: dueling Q-network, head rows {val, adv_1 .. adv_nout}; nout stays the width of Q
+    __host__ __device__ int rows() const { return nout + duel; }   // rows the head computes
+    __host__ __device__ int64_t nparams() const { return (int64_t)H * in + H + (int64_t)H * H + H + (int64_t)rows() * H + rows(); }
 };
+
+// head row o (0 .. rows()-1), weight column j / bias, inside the flat parameter vector.  The one place that knows the head
+// layouts: the FFMA kernels (nn.cu), the tensor-core forward (tc_fwd.cuh) and the tensor-core backward (nn_tc.cu) all use it.
+// MAY_DUEL = false: a kernel that never sees a dueling network (the actor-critic ones) compiles without the dueling branch.
+template <bool MAY_DUEL = true>
+__host__ __device__ __forceinline__ int rows_of(const MlpDesc& d) { return MAY_DUEL ? d.rows() : d.nout; }
+__host__ __device__ __forceinline__ int64_t head_base(const MlpDesc& d) { return (int64_t)d.H * d.in + d.H + (int64_t)d.H * d.H + d.H; }
+template <bool MAY_DUEL = true>
+__host__ __device__ __forceinline__ int64_t head_w(const MlpDesc& d, int o, int j) {
+    if (MAY_DUEL && d.duel) return head_base(d) + (o == 0 ? (int64_t)j : (int64_t)(d.H + 1) + (o - 1) + (int64_t)d.nout * j);
+    return head_base(d) + (d.heads2 ? (int64_t)o * (d.H + 1) + j : (int64_t)o + (int64_t)d.nout * j);
+}
+template <bool MAY_DUEL = true>
+__host__ __device__ __forceinline__ int64_t head_b(const MlpDesc& d, int o) {
+    if (MAY_DUEL && d.duel) return head_base(d) + (o == 0 ? (int64_t)d.H : (int64_t)(d.H + 1) + (int64_t)d.nout * d.H + (o - 1));
+    return head_base(d) + (d.heads2 ? (int64_t)o * (d.H + 1) + d.H : (int64_t)d.nout * d.H + o);
+}
 
 struct AcHyper {  // scalars of the actor-critic losses (SURVEY Appendix B)
     float clip_range, w_actor, w_critic, w_entropy, min_sigma, max_sigma;

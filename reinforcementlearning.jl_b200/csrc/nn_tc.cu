@@ -41,13 +41,6 @@ __device__ __forceinline__ float normlogpdf1(float mu, float sigma, float x) {
     float s = sigma + 1e-8f, v = s * s, dd = x - mu;
     return -0.5f * ((logf(v) + (dd * dd) / v) + kLog2Pi);
 }
-__device__ __forceinline__ int64_t head_base(const MlpDesc& d) { return (int64_t)d.H * d.in + d.H + (int64_t)d.H * d.H + d.H; }
-__device__ __forceinline__ int64_t head_w(const MlpDesc& d, int o, int j) {
-    return head_base(d) + (d.heads2 ? (int64_t)o * (d.H + 1) + j : (int64_t)o + (int64_t)d.nout * j);
-}
-__device__ __forceinline__ int64_t head_b(const MlpDesc& d, int o) {
-    return head_base(d) + (d.heads2 ? (int64_t)o * (d.H + 1) + d.H : (int64_t)d.nout * d.H + o);
-}
 __device__ __forceinline__ uint32_t wimg_off(int n, int k) { return (uint32_t)((n >> 3) * GW_S + (k >> 3) * G_F + (n & 7) * 16 + (k & 7) * 2); }
 
 // =====================================================================================================
@@ -325,9 +318,9 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         for (int k = tid; k < H; k += NT7_ALL) { sm.b1[k] = b1[k] * s1; sm.b2[k] = b2[k]; }
         for (int k = tid; k < H * kNo; k += NT7_ALL) {
             int j = k / kNo, o = k % kNo;
-            sm.W3[k] = o < d.nout ? p[head_w(d, o, j)] : 0.f;
+            sm.W3[k] = o < d.nout ? p[head_w<false>(d, o, j)] : 0.f;
         }
-        if (tid < kNo) sm.b3[tid] = tid < d.nout ? p[head_b(d, tid)] : 0.f;
+        if (tid < kNo) sm.b3[tid] = tid < d.nout ? p[head_b<false>(d, tid)] : 0.f;
         for (int k = tid; k < H * H; k += NT7_ALL) {
             int o = k % H, i = k / H;
             const float w = W2[k] * kScaleW;
@@ -767,7 +760,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             float a = 0.f;
 #pragma unroll
             for (int g = 0; g < 8; ++g) a += seg[(m * 8 + g) * 64 + col];
-            if (m < d.nout) out[head_w(d, m, col)] = a;
+            if (m < d.nout) out[head_w<false>(d, m, col)] = a;
         }
         worker_sync();
     }
@@ -777,7 +770,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         float a = (red[warp * TM + lane] + red[warp * TM + 32 + lane]) + (red[warp * TM + 64 + lane] + red[warp * TM + 96 + lane]);
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-        if (lane == 0) out[head_b(d, warp)] = a;
+        if (lane == 0) out[head_b<false>(d, warp)] = a;
     }
     // loss sums (worker-only block reduction)
     float t0 = l0, t1 = l1;

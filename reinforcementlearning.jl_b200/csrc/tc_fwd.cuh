@@ -51,13 +51,6 @@ __device__ __forceinline__ float normlogpdf1(float mu, float sigma, float x) {  
     float s = sigma + 1e-8f, v = __fmul_rn(s, s), dd = x - mu;
     return __fmul_rn(-0.5f, (logf(v) + __fmul_rn(dd, dd) / v) + kLog2Pi);
 }
-__device__ __forceinline__ int64_t head_base(const MlpDesc& d) { return (int64_t)d.H * d.in + d.H + (int64_t)d.H * d.H + d.H; }
-__device__ __forceinline__ int64_t head_w(const MlpDesc& d, int o, int j) {
-    return head_base(d) + (d.heads2 ? (int64_t)o * (d.H + 1) + j : (int64_t)o + (int64_t)d.nout * j);
-}
-__device__ __forceinline__ int64_t head_b(const MlpDesc& d, int o) {
-    return head_base(d) + (d.heads2 ? (int64_t)o * (d.H + 1) + d.H : (int64_t)d.nout * d.H + o);
-}
 __device__ __forceinline__ uint32_t wimg_off(int n, int k) { return (uint32_t)((n >> 3) * GW_S + (k >> 3) * G_F + (n & 7) * 16 + (k & 7) * 2); }
 // FP32 accumulator of one block, row r, column col: 16-byte units XOR-swizzled by the row, so that 8 consecutive rows read
 // at the same column hit 8 different bank groups
@@ -65,6 +58,8 @@ __device__ __forceinline__ uint32_t dacc_off(int r, int col) { return (uint32_t)
 
 // s1: scale folded into W1 / b1 (kScale for relu trunks: relu(S z) = S relu(z) exactly for a power of two S, so layer 1 then
 // produces the scaled H1 operand without a multiply per feature; 1 otherwise)
+// MAY_DUEL = false: the caller never loads a dueling network (nn.cuh head_w)
+template <bool MAY_DUEL = true>
 __device__ inline void load_net(NetSm& w, const MlpDesc& d, const float* __restrict__ p, float s1) {
     const int tid = threadIdx.x;
     const float* b1 = p + (int64_t)H * d.in;
@@ -74,9 +69,9 @@ __device__ inline void load_net(NetSm& w, const MlpDesc& d, const float* __restr
     for (int k = tid; k < H; k += NT) { w.b1[k] = __fmul_rn(b1[k], s1); w.b2[k] = b2[k]; }
     for (int k = tid; k < H * kOutMax; k += NT) {
         int j = k / kOutMax, o = k % kOutMax;
-        w.W3[k] = o < d.nout ? p[head_w(d, o, j)] : 0.f;
+        w.W3[k] = o < rows_of<MAY_DUEL>(d) ? p[head_w<MAY_DUEL>(d, o, j)] : 0.f;
     }
-    if (tid < kOutMax) w.b3[tid] = tid < d.nout ? p[head_b(d, tid)] : 0.f;
+    if (tid < kOutMax) w.b3[tid] = tid < rows_of<MAY_DUEL>(d) ? p[head_b<MAY_DUEL>(d, tid)] : 0.f;
     for (int k = tid; k < H * H; k += NT) {   // W2[o + H*i]: B operand of H2pre[s][o] = sum_i H1[s][i] W2[o][i]
         int o = k % H, i = k / H;
         const float v = __fmul_rn(W2[k], kScale);

@@ -307,9 +307,13 @@ mutable struct B200Network
     h::Ptr{Cvoid}
     desc::NetDescC
 end
-"FluxApproximator stand-in: `params` is `Flux.destructure(ActorCritic(actor, critic))[1]` (Float32)."
+"""FluxApproximator stand-in: `params` is `Flux.destructure(ActorCritic(actor, critic))[1]` (Float32).
+`kind`: `:categorical`, `:gaussian`, `:q` (a Q-network) or `:dueling` (`DuelingNetwork(base = Chain(Dense(n_in, hidden, act),
+Dense(hidden, hidden, act)), val = Dense(hidden, 1), adv = Dense(hidden, n_out))`, networks.jl:500-522; `n_out` = number of
+actions, 1..3; `params = Flux.destructure(model)[1]` as it is).  `:q` and `:dueling` carry a target network."""
 function B200Network(ctx::B200Context; n_in, hidden, n_out, params::Vector{Float32}, act::Symbol = :relu, kind::Symbol = :categorical)
-    d = NetDescC(n_in, hidden, act === :relu ? 0 : 1, n_out, kind === :categorical ? 0 : kind === :gaussian ? 1 : 2)
+    k = kind === :categorical ? 0 : kind === :gaussian ? 1 : kind === :dueling ? 3 : 2
+    d = NetDescC(n_in, hidden, act === :relu ? 0 : 1, n_out, k)
     out = Ref{Ptr{Cvoid}}(C_NULL)
     GC.@preserve params check(ccall((:b200rl_net_create, LIB), Cint, (Ptr{Cvoid}, Ref{NetDescC}, Ptr{Float32}, Ref{Ptr{Cvoid}}),
                                     ctx.h, Ref(d), params, out))
@@ -541,7 +545,7 @@ struct DQNConfigC
     per_alpha::Cfloat; per_beta::Cfloat; per_eps::Cfloat
     huber::Int32; double_dqn::Int32; target_update_freq::Int32
 end
-"DQNLearner / PrioritizedDQNLearner: `net` is a `kind = :q` B200Network (FluxApproximator + TargetNetwork, target_network.jl:27-88)."
+"DQNLearner / PrioritizedDQNLearner: `net` is a `kind = :q` or `kind = :dueling` B200Network (FluxApproximator + TargetNetwork, target_network.jl:27-88)."
 struct B200DQNLearner <: RLCore.AbstractLearner
     net::B200Network
     cfg::DQNConfigC

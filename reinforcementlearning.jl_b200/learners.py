@@ -13,7 +13,8 @@ from .envs import _NOBS
 from .explorers import EpsilonGreedyExplorer, GreedyExplorer
 
 ACT_RELU, ACT_TANH = 0, 1
-KIND_CATEGORICAL, KIND_GAUSSIAN, KIND_Q = 0, 1, 2
+KIND_CATEGORICAL, KIND_GAUSSIAN, KIND_Q, KIND_DUELING = 0, 1, 2, 3
+Q_KINDS = (KIND_Q, KIND_DUELING)     # Q-networks: a target copy, the DQN learner, QBasedPolicy
 NET_PARAMS, NET_GRAD, NET_M, NET_V, NET_BETA_T, NET_TARGET = range(6)
 
 
@@ -32,7 +33,10 @@ def dqn_config(gamma=0.99, lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-8, max_grad_n
 
 
 class Network:
-    """b200rl_net: parameters + Adam state (+ target copy) on the device."""
+    """b200rl_net: parameters + Adam state (+ target copy) on the device.
+
+    kind KIND_DUELING: DuelingNetwork(base = trunk, val = Dense(hidden, 1), adv = Dense(hidden, n_out)) with n_out = number of
+    actions (1..3); ``params`` is ``Flux.destructure`` of it as it is, and everything that reads Q sees (val + adv) - mean(adv)."""
 
     def __init__(self, ctx, n_in, hidden, n_out, params, act=ACT_RELU, kind=KIND_CATEGORICAL):
         self.ctx, self.lib = ctx, ctx.lib
@@ -47,6 +51,10 @@ class Network:
         L.check(self.lib.b200rl_net_create(ctx.h, C.byref(self.desc), L.ptr(params), C.byref(h)))
         self.h = h
         self.kind, self.n_in, self.n_out = kind, n_in, n_out
+
+    @property
+    def is_q(self):
+        return self.kind in Q_KINDS
 
     @staticmethod
     def count_params(ctx, n_in, hidden, n_out, act=ACT_RELU, kind=KIND_CATEGORICAL):
@@ -108,7 +116,7 @@ class Network:
     def values(self, obs, use_target=False):
         obs = np.asfortranarray(obs, np.float32)
         n = obs.shape[1]
-        out = np.empty((self.n_out, n), np.float32, order="F") if self.kind == KIND_Q else np.empty(n, np.float32)
+        out = np.empty((self.n_out, n), np.float32, order="F") if self.is_q else np.empty(n, np.float32)
         L.check(self.lib.b200rl_net_values(self.h, L.ptr(obs), n, L.ptr(out), int(use_target), 0))
         return out
 
