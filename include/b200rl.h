@@ -292,18 +292,27 @@ int b200rl_net_act(b200rl_net* net, const float* obs, int64_t n, uint64_t* rng_d
 int b200rl_net_values(b200rl_net* net, const float* obs, int64_t n, float* out, int use_target, int on_device);
 /* QBasedPolicy + EpsilonGreedyExplorer (q_based_policy.jl:13-49, explorers/epsilon_greedy_explorer.jl:69-131); DEVICE pointers */
 int b200rl_net_q_act(b200rl_net* net, const float* obs_dev, int64_t n, uint64_t* rng_dev, float epsilon, int32_t* action_out_dev);
-/* EpsilonGreedyExplorer{kind, is_break_tie} with its decay schedule, applied to a batch the way BatchExplorer does
- * (explorers/epsilon_greedy_explorer.jl:47-112, explorers/batch_explorer.jl:15-21): the inner explorer is called once per
- * column, so column i is planned with get_eps(step + i) (Float64 schedule, :linear | :exp) and the caller advances
- * `step` by n afterwards.  Per column: u = rand(rng) is always drawn; u >= eps ? findmax(values)[2] (or, is_break_tie,
- * rand(rng, find_all_max(values)[2])) : rand(rng, 1:n_actions).  Column i draws from its own stream rng_dev[:, i]
- * (the reference draws all columns from one stream — not parallel; DESIGN.md §3). */
+/* A value-based explorer applied to a batch the way BatchExplorer does (explorers/batch_explorer.jl:15-21): the inner explorer
+ * is called once per column, column i draws from its own stream rng_dev[:, i] (the reference draws all columns from one
+ * stream — not parallel; DESIGN.md §3), and for the kinds with a step column i is planned at step + i and the caller advances
+ * `step` by n afterwards.  Per column, on Q = the column's Q-values (n_actions of them):
+ *   kind 0 / 1  EpsilonGreedyExplorer{:linear | :exp, is_break_tie} (explorers/epsilon_greedy_explorer.jl:47-112): eps =
+ *               get_eps(step + i) (Float64 schedule); u = rand(rng) is always drawn; u >= eps ? findmax(Q)[2] (or, is_break_tie,
+ *               rand(rng, find_all_max(Q)[2])) : rand(rng, 1:n_actions)
+ *   kind 2      EpsilonSpeedyExplorer(beta) (ReinforcementLearningFarm): the same selection without break-tie, with
+ *               eps = exp((beta * -1) * (step + i)) (Float64)
+ *   kind 3      WeightedSoftmaxExplorer(): sample(rng, Weights(softmax(Q), 1f0)) — one Float64 draw, Float32 softmax
+ *   kind 4      GumbelSoftmaxExplorer(): argmax(logsoftmax(Q) .- log.(-log.(rand(rng, Float32, n_actions)))) — n_actions draws
+ * Kinds 3 and 4 have no step (it is advanced but never read).  The fields a kind 2-4 explorer does not read (the epsilon schedule,
+ * is_break_tie, and beta for kinds 3 / 4) must be 0.  Refused: an unknown kind, a bad schedule (kinds 0 / 1), a non-finite beta
+ * (kind 2), a nonzero field the kind does not read. */
 typedef struct {
     double eps_stable, eps_init;
     int64_t warmup_steps, decay_steps;
     int64_t step;            /* explorer.step before this call (the reference starts at 1) */
-    int32_t kind;            /* 0 :linear, 1 :exp */
+    int32_t kind;            /* 0 :linear, 1 :exp, 2 speedy, 3 weighted softmax, 4 Gumbel softmax */
     int32_t is_break_tie;
+    double beta;             /* kind 2: EpsilonSpeedyExplorer's beta */
 } b200rl_explorer;
 int b200rl_net_q_explore(b200rl_net* net, const float* obs_dev, int64_t n, uint64_t* rng_dev, const b200rl_explorer* explorer,
                          int32_t* action_out_dev);
@@ -412,7 +421,7 @@ typedef struct b200rl_replay b200rl_replay;
  * refused by run).  The trajectory needs a sampler; a change of its n-step setting between runs re-captures the graphs. */
 int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl_traj* traj, const b200rl_dqn_config* cfg,
                          b200rl_replay** out);
-/* explorer_rng_dev: (4, N) DEVICE explorer streams (one per env, advanced).  ex: EpsilonGreedyExplorer (its step is advanced
+/* explorer_rng_dev: (4, N) DEVICE explorer streams (one per env, advanced).  ex: any b200rl_explorer kind (its step is advanced
  * by n_steps * N), NULL = GreedyExplorer (findmax, no draw).  ctl: counters advanced.  stats4 (may be NULL; synchronises):
  * loss, grad_norm, mean |td|, n_updates of the last update in the window (untouched when the window ran none).  Refuses a bad
  * explorer schedule or controller values before any side effect.  A CUDA error part-way through returns with the device state

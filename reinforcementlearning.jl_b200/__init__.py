@@ -8,7 +8,7 @@ from .core import (AbstractHook, AbstractPolicy, BatchStepsPerEpisode, ComposedH
                    RandomPolicy, StopAfterNEpisodes, StopAfterNoImprovement, StopAfterNSeconds, StopAfterNSteps, StopIfAll, StopIfAny,
                    StopSignal, TimePerStep, TotalBatchRewardPerEpisode, run)
 from .envs import B200VecEnv, cartpole_params, mountaincar_params, pendulum_params
-from .explorers import EpsilonGreedyExplorer, GreedyExplorer
+from .explorers import EpsilonGreedyExplorer, EpsilonSpeedyExplorer, GreedyExplorer, GumbelSoftmaxExplorer, WeightedSoftmaxExplorer
 from .learners import (ACT_RELU, ACT_TANH, KIND_CATEGORICAL, KIND_DUELING, KIND_GAUSSIAN, KIND_Q, Agent, DQNLearner, EvaluationPolicy, InsertSampleRatioController,
                        Network, OnPolicyAgent, QBasedPolicy, Trajectory, dqn_config, evaluate, onpolicy_config)
 from . import checkpoint, core, explorers, learners, sharding

@@ -51,9 +51,10 @@ class DQNConfig(C.Structure):
 
 
 class Explorer(C.Structure):
-    """b200rl_explorer: EpsilonGreedyExplorer{kind, is_break_tie} fields + the step before the call."""
+    """b200rl_explorer: kind (0 :linear, 1 :exp, 2 speedy, 3 weighted softmax, 4 Gumbel softmax), the EpsilonGreedyExplorer
+    fields, the step before the call and EpsilonSpeedyExplorer's beta."""
     _fields_ = [("eps_stable", C.c_double), ("eps_init", C.c_double), ("warmup_steps", C.c_int64), ("decay_steps", C.c_int64),
-                ("step", C.c_int64), ("kind", C.c_int32), ("is_break_tie", C.c_int32)]
+                ("step", C.c_int64), ("kind", C.c_int32), ("is_break_tie", C.c_int32), ("beta", C.c_double)]
 
 
 class InsertSampleRatio(C.Structure):

@@ -372,12 +372,27 @@ int b200rl_net_q_act(b200rl_net* n, const float* obs_dev, int64_t N, uint64_t* r
     return nn_q_act(n->ctx, n->actor, n->params, obs_dev, N, (unsigned long long*)rng_dev, epsilon, action_out_dev, (float*)s);
 }
 
-/* BatchExplorer(EpsilonGreedyExplorer) with the decay schedule evaluated per column on the device; all pointers DEVICE */
+// the explorer fields a kind reads: a known kind, a schedule with epsilons in [0, 1] (kinds 0 / 1), a finite beta (kind 2).  The
+// fields kinds 2-4 do not read must be zero, so that a struct filled for one explorer is not silently run as another.
+static int check_explorer(const b200rl_explorer* ex) {
+    REQUIRE(ex->kind >= 0 && ex->kind <= 4, B200RL_ERR_INVALID, "unknown explorer kind (0 :linear, 1 :exp, 2 speedy, 3 weighted softmax, 4 Gumbel softmax)");
+    if (ex->kind <= 1) {
+        REQUIRE(ex->warmup_steps >= 0 && ex->decay_steps >= 0, B200RL_ERR_INVALID, "bad explorer schedule");
+        REQUIRE(ex->eps_stable >= 0.0 && ex->eps_stable <= 1.0 && ex->eps_init >= 0.0 && ex->eps_init <= 1.0, B200RL_ERR_INVALID, "epsilon outside [0, 1]");
+        return B200RL_OK;
+    }
+    REQUIRE(ex->eps_stable == 0.0 && ex->eps_init == 0.0 && ex->warmup_steps == 0 && ex->decay_steps == 0 && ex->is_break_tie == 0,
+            B200RL_ERR_INVALID, "explorer kinds 2-4 take no epsilon schedule or break-tie (those fields must be 0)");
+    if (ex->kind == 2) REQUIRE(std::isfinite(ex->beta), B200RL_ERR_INVALID, "EpsilonSpeedyExplorer beta must be finite");
+    else REQUIRE(ex->beta == 0.0, B200RL_ERR_INVALID, "the softmax explorers take no beta (must be 0)");
+    return B200RL_OK;
+}
+
+/* BatchExplorer(explorer) with the explorer's schedule evaluated per column on the device; all pointers DEVICE */
 int b200rl_net_q_explore(b200rl_net* n, const float* obs_dev, int64_t N, uint64_t* rng_dev, const b200rl_explorer* ex, int32_t* action_out_dev) {
     REQUIRE(n && obs_dev && action_out_dev && rng_dev && ex && is_q_kind(n->kind), B200RL_ERR_INVALID, "bad argument (Q-network only)");
     REQUIRE(N > 0, B200RL_ERR_INVALID, "empty batch");
-    REQUIRE((ex->kind == 0 || ex->kind == 1) && ex->warmup_steps >= 0 && ex->decay_steps >= 0, B200RL_ERR_INVALID, "bad explorer schedule");
-    REQUIRE(ex->eps_stable >= 0.0 && ex->eps_stable <= 1.0 && ex->eps_init >= 0.0 && ex->eps_init <= 1.0, B200RL_ERR_INVALID, "epsilon outside [0, 1]");
+    TRY(check_explorer(ex));
     TRY(ctx_bind(n->ctx));
     void* s;
     TRY(ctx_scratch(n->ctx, (size_t)N * n->actor.nout * 4 + 256, &s));
@@ -1307,9 +1322,8 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
     REQUIRE(r && ctl, B200RL_ERR_INVALID, "null argument");
     REQUIRE(n_steps >= 0, B200RL_ERR_INVALID, "n_steps must be >= 0");
     if (ex) {
-        REQUIRE(explorer_rng_dev, B200RL_ERR_INVALID, "an epsilon-greedy explorer needs the (4, N) device explorer streams");
-        REQUIRE((ex->kind == 0 || ex->kind == 1) && ex->warmup_steps >= 0 && ex->decay_steps >= 0, B200RL_ERR_INVALID, "bad explorer schedule");
-        REQUIRE(ex->eps_stable >= 0.0 && ex->eps_stable <= 1.0 && ex->eps_init >= 0.0 && ex->eps_init <= 1.0, B200RL_ERR_INVALID, "epsilon outside [0, 1]");
+        REQUIRE(explorer_rng_dev, B200RL_ERR_INVALID, "an explorer other than GreedyExplorer needs the (4, N) device explorer streams");
+        TRY(check_explorer(ex));
         REQUIRE(n_steps <= ((1ll << 62) - (ex->step > 0 ? ex->step : 0)) / r->N, B200RL_ERR_INVALID, "explorer step would overflow");
     }
     REQUIRE(replay::controller_ok(*ctl), B200RL_ERR_INVALID, "bad controller values (ratio finite in [0, 1e6], counters >= 0)");

@@ -10,7 +10,7 @@
 
 #include "../../include/b200rl.h"
 
-#define B200RL_ABI_VERSION 1
+#define B200RL_ABI_VERSION 2
 
 void b200rl_set_error(const char* fmt, ...);
 

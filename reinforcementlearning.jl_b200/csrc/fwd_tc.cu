@@ -644,13 +644,20 @@ template <class Env> struct SmemReplay {
     int red_i[8], red_l[8];
     long long red_v[8];
 };
+// b200rl_explorer without its trailing beta, which the kernel takes as its last parameter: the parameters the ϵ-greedy
+// instantiations read keep the offsets they had before the explorer struct grew
+struct ReplayExplorer {
+    double eps_stable, eps_init;
+    int64_t warmup_steps, decay_steps, step;
+    int32_t kind, is_break_tie;
+};
 struct ReplayArgs {
     MlpDesc q;
     const float* params;
     int64_t N;
     int nsteps;
     int greedy;                            // 1: GreedyExplorer (findmax with `>`, no draw)
-    b200rl_explorer ex;
+    ReplayExplorer ex;
     const long long* step_dev;             // explorer step before the window (device)
     unsigned long long* xrng;              // (4, N) explorer streams
     Ring ring;
@@ -662,9 +669,10 @@ struct ReplayArgs {
 };
 
 // DUEL: a dueling Q-network, its head rows combined into Q (duel.cuh) before the selection (the instantiations without it are the
-// code of a plain Q-network)
-template <class Env, int ACT, bool DUEL = false>
-__global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, typename Env::P p, EnvArrays ea) {
+// code of a plain Q-network).  XEXT: the explorer kinds 2-4 (speedy, weighted / Gumbel softmax; explore::select<true>) — the
+// instantiations without it compile the ϵ-greedy kinds 0 / 1 only.
+template <class Env, int ACT, bool DUEL = false, bool XEXT = false>
+__global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, typename Env::P p, EnvArrays ea, double beta) {
     using act_t = typename Env::act_t;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     SmemReplay<Env>& sm = *reinterpret_cast<SmemReplay<Env>*>(smem_raw);
@@ -750,7 +758,13 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
                         a1 = best + 1;
                     } else {
                         unsigned long long xr[4] = {sl.xrng[s], sl.xrng[TM + s], sl.xrng[2 * TM + s], sl.xrng[3 * TM + s]};
-                        a1 = explore::select(g.ex, step0 + (long long)step * N + i, z, g.q.nout, xr);
+                        if constexpr (XEXT) {
+                            const b200rl_explorer ex{g.ex.eps_stable, g.ex.eps_init, g.ex.warmup_steps, g.ex.decay_steps, g.ex.step, g.ex.kind,
+                                                     g.ex.is_break_tie, beta};
+                            a1 = explore::select<true>(ex, step0 + (long long)step * N + i, z, g.q.nout, xr);
+                        } else {
+                            a1 = explore::select<false>(g.ex, step0 + (long long)step * N + i, z, g.q.nout, xr);
+                        }
                         sl.xrng[s] = xr[0]; sl.xrng[TM + s] = xr[1]; sl.xrng[2 * TM + s] = xr[2]; sl.xrng[3 * TM + s] = xr[3];
                     }
                     // act!(env, a) + fused auto-reset: the sequence of env_step_kernel<Env, false, true>
@@ -846,25 +860,30 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
     }
 }
 
-template <class Env> int launch_replay_collect(b200rl_ctx* ctx, const ReplayArgs& g, const typename Env::P& p, const EnvArrays& ea) {
+template <class Env, bool XEXT> int launch_replay_collect_x(b200rl_ctx* ctx, const ReplayArgs& g, const typename Env::P& p, const EnvArrays& ea,
+                                                           double beta) {
     const size_t smem = sizeof(SmemReplay<Env>) + 128;
-    static unsigned long long attr_devices = 0;   // once per device
+    static unsigned long long attr_devices = 0;   // once per device (and per XEXT)
     if (first_use_on_device(attr_devices, ctx->device)) {
-        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_TANH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_RELU, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_TANH, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_RELU, false, XEXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_TANH, false, XEXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_RELU, true, XEXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_TANH, true, XEXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     const int64_t groups = ((g.N + TM - 1) / TM + kSlots - 1) / kSlots;
     int grid = 2 * ctx->sm_count;
     if ((int64_t)grid > groups) grid = (int)groups;
     if (g.q.duel) {
-        if (g.q.act == B200RL_ACT_RELU) replay_collect_tc_kernel<Env, B200RL_ACT_RELU, true><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
-        else replay_collect_tc_kernel<Env, B200RL_ACT_TANH, true><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
-    } else if (g.q.act == B200RL_ACT_RELU) replay_collect_tc_kernel<Env, B200RL_ACT_RELU><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
-    else replay_collect_tc_kernel<Env, B200RL_ACT_TANH><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
+        if (g.q.act == B200RL_ACT_RELU) replay_collect_tc_kernel<Env, B200RL_ACT_RELU, true, XEXT><<<grid, NT, smem, ctx->stream>>>(g, p, ea, beta);
+        else replay_collect_tc_kernel<Env, B200RL_ACT_TANH, true, XEXT><<<grid, NT, smem, ctx->stream>>>(g, p, ea, beta);
+    } else if (g.q.act == B200RL_ACT_RELU) replay_collect_tc_kernel<Env, B200RL_ACT_RELU, false, XEXT><<<grid, NT, smem, ctx->stream>>>(g, p, ea, beta);
+    else replay_collect_tc_kernel<Env, B200RL_ACT_TANH, false, XEXT><<<grid, NT, smem, ctx->stream>>>(g, p, ea, beta);
     LAUNCH_CHECK(ctx);
     return B200RL_OK;
+}
+template <class Env> int launch_replay_collect(b200rl_ctx* ctx, const ReplayArgs& g, const typename Env::P& p, const EnvArrays& ea, double beta) {
+    if (!g.greedy && g.ex.kind >= 2) return launch_replay_collect_x<Env, true>(ctx, g, p, ea, beta);
+    return launch_replay_collect_x<Env, false>(ctx, g, p, ea, 0.0);
 }
 
 }  // namespace
@@ -991,13 +1010,14 @@ int nn_tc_replay_collect(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& q, con
     EnvView v;
     TRY(b200rl_env_internal_view(env, &v));
     if (!nn_tc_supported(q) || v.dtype != B200RL_F32 || v.continuous || ring.ns > kInMax) return B200RL_ERR_UNSUPPORTED;
-    ReplayArgs g{q, params, v.N, nsteps, ex ? 0 : 1, ex ? *ex : b200rl_explorer{}, step_dev, xrng, ring, default_priority, prioritized,
-                 keys, vals, stride};
+    const b200rl_explorer e = ex ? *ex : b200rl_explorer{};
+    ReplayArgs g{q, params, v.N, nsteps, ex ? 0 : 1, ReplayExplorer{e.eps_stable, e.eps_init, e.warmup_steps, e.decay_steps, e.step, e.kind, e.is_break_tie},
+                 step_dev, xrng, ring, default_priority, prioritized, keys, vals, stride};
     int st = B200RL_ERR_UNSUPPORTED;
     switch (v.kind) {
-        case B200RL_ENV_CARTPOLE: st = launch_replay_collect<CartPoleD<float, false>>(ctx, g, v.p.cp32, v.a); break;
-        case B200RL_ENV_PENDULUM: st = launch_replay_collect<PendulumD<false>>(ctx, g, v.p.pend, v.a); break;
-        case B200RL_ENV_MOUNTAINCAR: st = launch_replay_collect<MountainCarD<false>>(ctx, g, v.p.mc, v.a); break;
+        case B200RL_ENV_CARTPOLE: st = launch_replay_collect<CartPoleD<float, false>>(ctx, g, v.p.cp32, v.a, e.beta); break;
+        case B200RL_ENV_PENDULUM: st = launch_replay_collect<PendulumD<false>>(ctx, g, v.p.pend, v.a, e.beta); break;
+        case B200RL_ENV_MOUNTAINCAR: st = launch_replay_collect<MountainCarD<false>>(ctx, g, v.p.mc, v.a, e.beta); break;
     }
     if (st == B200RL_OK) b200rl_env_internal_add_steps(env, (uint64_t)nsteps);
     return st;

@@ -1,5 +1,6 @@
 """Host mirror of the reference's explorers for the DQN action path
-(RLCore/src/policies/explorers/epsilon_greedy_explorer.jl:47-204, batch_explorer.jl:15-21).
+(RLCore/src/policies/explorers/epsilon_greedy_explorer.jl:47-204, weighted_softmax_explorer.jl, gumbel_softmax_explorer.jl,
+batch_explorer.jl:15-21; ReinforcementLearningFarm's EpsilonSpeedyExplorer).
 
 The explorer object is host state in the reference too (a mutable struct holding the schedule and
 the step counter); the per-column work — evaluating get_ϵ(step + i), the uniform draw and the
@@ -7,6 +8,8 @@ arg-max / random choice for every env of the batch — happens in ``b200rl_net_q
 device.  ``get_eps`` / ``prob`` are the reference's scalar Float64 formulas (Python floats are
 IEEE doubles, evaluated left to right like the Julia code)."""
 import math
+
+import numpy as np
 
 from . import _lib as L
 
@@ -78,8 +81,83 @@ class EpsilonGreedyExplorer:
 
     def as_struct(self):
         return L.Explorer(self.eps_stable, self.eps_init, self.warmup_steps, self.decay_steps, self.step,
-                          0 if self.kind == "linear" else 1, int(self.is_break_tie))
+                          0 if self.kind == "linear" else 1, int(self.is_break_tie), 0.0)
 
     def advance(self, n):
         """The batch call planned n columns: the inner explorer's step moved n times (batch_explorer.jl:15-21)."""
         self.step += int(n)
+
+
+class EpsilonSpeedyExplorer:
+    """EpsilonSpeedyExplorer(β) (ReinforcementLearningFarm, explorers/epsilon_speedy_explorer.jl:19-53): ϵ-greedy with
+    get_ϵ = exp(β_neg * step), β_neg = β * -1, step starting at 1; findmax without break-tie."""
+    is_break_tie = False
+
+    def __init__(self, beta, step=1):
+        self.beta, self.step = float(beta), int(step)
+        if not math.isfinite(self.beta):
+            raise ValueError("beta must be finite")
+
+    def get_eps(self, step=None):
+        step = self.step if step is None else step
+        return math.exp(self.beta * -1 * float(step))
+
+    def prob(self, values, action=None):
+        """prob(s, values[, action]): the Categorical's probability vector (ϵ/n everywhere, + 1 - ϵ at findmax)."""
+        eps, n = self.get_eps(), len(values)
+        probs = [eps / n] * n
+        probs[_findmax(values)] += 1 - eps
+        return probs if action is None else probs[action - 1]
+
+    def as_struct(self):
+        return L.Explorer(0.0, 0.0, 0, 0, self.step, 2, 0, self.beta)
+
+    def advance(self, n):
+        """The batch call planned n columns: the inner explorer's step moved n times (batch_explorer.jl:15-21)."""
+        self.step += int(n)
+
+
+def softmax(values):
+    """NNlib's softmax of a Float32 vector as the device computes it: m = the largest non-NaN entry (-Inf if none),
+    e_j = exp(Q_j - m) (or, m = +Inf, 1 where Q_j = +Inf and 0 elsewhere), p_j = e_j / (e_1 + e_2 + ...) left to right, every
+    operation rounded once in Float32 (numpy's exp may differ from the device's in the last bit)."""
+    q = np.asarray(values, np.float32)
+    m = np.float32(-np.inf)
+    for v in q:
+        if v > m:
+            m = v
+    with np.errstate(invalid="ignore", over="ignore"):
+        if m == np.inf:
+            e = np.where(q == np.inf, np.float32(1), np.float32(0)).astype(np.float32)
+        else:
+            e = np.exp((q - m).astype(np.float32)).astype(np.float32)
+        s = e[0]
+        for v in e[1:]:
+            s = np.float32(s + v)
+        return (e / s).astype(np.float32)
+
+
+class WeightedSoftmaxExplorer:
+    """WeightedSoftmaxExplorer() (weighted_softmax_explorer.jl:20-21): sample(rng, Weights(softmax(values), 1f0)) per column
+    (one Float64 draw); no step."""
+
+    def prob(self, values):
+        """prob(s, values) = softmax(values) (weighted_softmax_explorer.jl:28)"""
+        return softmax(values)
+
+    def as_struct(self):
+        return L.Explorer(0.0, 0.0, 0, 0, 0, 3, 0, 0.0)
+
+    def advance(self, n):
+        pass
+
+
+class GumbelSoftmaxExplorer:
+    """GumbelSoftmaxExplorer() (gumbel_softmax_explorer.jl:12-16): argmax(logsoftmax(values) .- log.(-log.(u))) with
+    u = rand(rng, Float32, n) per column; no step."""
+
+    def as_struct(self):
+        return L.Explorer(0.0, 0.0, 0, 0, 0, 4, 0, 0.0)
+
+    def advance(self, n):
+        pass

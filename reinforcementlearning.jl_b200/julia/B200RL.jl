@@ -26,7 +26,7 @@ import ReinforcementLearningEnvironments as RLEnvs
 using ReinforcementLearningBase: AbstractEnv, AbstractPolicy, Observation, DefaultPlayer, (..), ×   # `..` / `×`: DomainSets, re-exported by RLBase (space.jl:6)
 using ReinforcementLearningCore: AbstractStage, PreExperimentStage, PostExperimentStage, PreActStage, PostActStage,
     AbstractStopCondition, AbstractHook, AbstractResetCondition, ResetIfEnvTerminated, StopAfterNEpisodes, StopAfterNSteps,
-    EpsilonGreedyExplorer, GreedyExplorer, AbstractExplorer
+    EpsilonGreedyExplorer, GreedyExplorer, AbstractExplorer, WeightedSoftmaxExplorer, GumbelSoftmaxExplorer
 
 export B200Context, B200VecEnv, B200Network, B200OnPolicyAgent, B200RandomPolicy, B200Trajectory, B200DQNLearner, B200QBasedPolicy,
     B200Agent, B200EpisodeStats, InsertSampleRatio, B200GreedyPolicy, evaluate, replay!, set_nstep!
@@ -559,17 +559,34 @@ update!(l::B200DQNLearner, t::B200Trajectory) =
 
 struct ExplorerC
     eps_stable::Cdouble; eps_init::Cdouble; warmup_steps::Int64; decay_steps::Int64; step::Int64; kind::Int32; is_break_tie::Int32
+    beta::Cdouble
 end
 ExplorerC(s::EpsilonGreedyExplorer{K,B}) where {K,B} =
-    ExplorerC(s.ϵ_stable, s.ϵ_init, s.warmup_steps, s.decay_steps, s.step, K === :linear ? 0 : 1, B ? 1 : 0)
+    ExplorerC(s.ϵ_stable, s.ϵ_init, s.warmup_steps, s.decay_steps, s.step, K === :linear ? 0 : 1, B ? 1 : 0, 0.0)
+ExplorerC(::WeightedSoftmaxExplorer) = ExplorerC(0.0, 0.0, 0, 0, 0, 3, 0, 0.0)
+ExplorerC(::GumbelSoftmaxExplorer) = ExplorerC(0.0, 0.0, 0, 0, 0, 4, 0, 0.0)
+# ReinforcementLearningFarm's EpsilonSpeedyExplorer(β) (its step is a Ref), matched by name so that this package does not depend
+# on ReinforcementLearningFarm
+is_speedy(s) = nameof(typeof(s)) === :EpsilonSpeedyExplorer
+function ExplorerC(s::AbstractExplorer)
+    is_speedy(s) || throw(ArgumentError("$(typeof(s)) has no device explorer"))
+    ExplorerC(0.0, 0.0, 0, 0, s.step[], 2, 0, s.β)
+end
+# the explorers b200rl_net_q_explore / b200rl_replay_run plan with (GreedyExplorer: b200rl_net_q_act / a NULL explorer)
+device_explorer(s) = s isa Union{EpsilonGreedyExplorer,WeightedSoftmaxExplorer,GumbelSoftmaxExplorer} || is_speedy(s)
+# advance the inner explorer's step to where the device call left it (the softmax explorers have no step)
+set_step!(s::EpsilonGreedyExplorer, step) = (s.step = step; nothing)
+set_step!(s::Union{WeightedSoftmaxExplorer,GumbelSoftmaxExplorer}, step) = nothing
+set_step!(s::AbstractExplorer, step) = (s.step[] = step; nothing)      # EpsilonSpeedyExplorer
 
 """
     B200QBasedPolicy(ctx, learner, explorer, n; explorer_seeds)
 
 `QBasedPolicy(learner, explorer)` (q_based_policy.jl:13-49) for a batched env.  `explorer` is the reference's own
-`EpsilonGreedyExplorer{kind, is_break_tie}` (or `GreedyExplorer()`): its schedule fields are read on every `plan!` and its
-`step` is advanced by `n`, the way `BatchExplorer` calls the inner explorer once per column (batch_explorer.jl:15-21); the
-forward pass, `get_ϵ(step + i)`, the draws and the arg-max run in one device call.
+`EpsilonGreedyExplorer{kind, is_break_tie}`, `WeightedSoftmaxExplorer()`, `GumbelSoftmaxExplorer()`, ReinforcementLearningFarm's
+`EpsilonSpeedyExplorer(β)` or `GreedyExplorer()`: its fields are read on every `plan!` and its step (if it has one) is advanced
+by `n`, the way `BatchExplorer` calls the inner explorer once per column (batch_explorer.jl:15-21); the forward pass, the
+per-column schedule, the draws and the selection run in one device call.
 """
 mutable struct B200QBasedPolicy{E<:AbstractExplorer} <: AbstractPolicy
     ctx::B200Context
@@ -596,11 +613,11 @@ function B200QBasedPolicy(ctx::B200Context, learner::B200DQNLearner, explorer::A
         ccall((:b200rl_free, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), x.ctx.h, x.d_action)
     end
 end
-function RLBase.plan!(p::B200QBasedPolicy{<:EpsilonGreedyExplorer}, env::B200VecEnv)
+function RLBase.plan!(p::B200QBasedPolicy, env::B200VecEnv)
     ex = ExplorerC(p.explorer)
     check(ccall((:b200rl_net_q_explore, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Ptr{Cvoid}, Ref{ExplorerC}, Ptr{Cvoid}),
                 p.learner.net.h, device_ptr(env, OBS), p.n, p.d_rng, Ref(ex), p.d_action))
-    p.explorer.step += p.n
+    set_step!(p.explorer, ex.step + p.n)
     DeviceActions(p.d_action)
 end
 function RLBase.plan!(p::B200QBasedPolicy{GreedyExplorer}, env::B200VecEnv)
@@ -722,7 +739,7 @@ advance.  `false` (nothing done) when the agent / env are outside the device loo
 function replay!(a::B200Agent, env::B200VecEnv, n_steps::Integer)
     p, t, c = a.policy, a.trajectory, a.trajectory.controller
     (a.fused && env isa B200VecEnv{Float32} && env.auto_reset && !env.continuous && t.batch_size > 0 && t.lanes == env.n &&
-     p.explorer isa Union{EpsilonGreedyExplorer,GreedyExplorer}) || return false
+     (device_explorer(p.explorer) || p.explorer isa GreedyExplorer)) || return false
     if a.replay == C_NULL || a.replay_env != env.h
         a.replay == C_NULL || ccall((:b200rl_replay_destroy, LIB), Cint, (Ptr{Cvoid},), a.replay)
         a.replay = C_NULL
@@ -734,11 +751,11 @@ function replay!(a::B200Agent, env::B200VecEnv, n_steps::Integer)
         a.replay, a.replay_env = h[], env.h
     end
     ctl = Ref(InsertSampleRatioC(c.ratio, c.threshold, c.n_inserted, c.n_sampled))
-    if p.explorer isa EpsilonGreedyExplorer
+    if device_explorer(p.explorer)
         ex = Ref(ExplorerC(p.explorer))
         check(ccall((:b200rl_replay_run, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ref{ExplorerC}, Ref{InsertSampleRatioC}, Int64, Ptr{Cfloat}),
                     a.replay, p.d_rng, ex, ctl, n_steps, C_NULL))
-        p.explorer.step = ex[].step
+        set_step!(p.explorer, ex[].step)
     else                                                           # GreedyExplorer: findmax, no draw
         check(ccall((:b200rl_replay_run, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ref{InsertSampleRatioC}, Int64, Ptr{Cfloat}),
                     a.replay, p.d_rng, C_NULL, ctl, n_steps, C_NULL))

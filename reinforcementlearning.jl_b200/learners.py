@@ -10,7 +10,8 @@ import numpy as np
 from . import _lib as L
 from .core import AbstractPolicy, FusedAction, PostActStage, PreActStage, PreEpisodeStage, PreExperimentStage
 from .envs import _NOBS
-from .explorers import EpsilonGreedyExplorer, GreedyExplorer
+from .explorers import (EpsilonGreedyExplorer, EpsilonSpeedyExplorer, GreedyExplorer, GumbelSoftmaxExplorer,
+                        WeightedSoftmaxExplorer)
 
 ACT_RELU, ACT_TANH = 0, 1
 KIND_CATEGORICAL, KIND_GAUSSIAN, KIND_Q, KIND_DUELING = 0, 1, 2, 3
@@ -593,6 +594,10 @@ def evaluate(net, env, n_steps, max_episodes=1, mode="greedy", rng=None):
     return dict(returns=returns, lengths=lengths, counts=counts)
 
 
+# the explorers b200rl_replay_run plans with (b200rl_explorer kinds 0 / 1, 2, 3, 4); GreedyExplorer runs as ex = NULL
+DEVICE_EXPLORERS = (EpsilonGreedyExplorer, EpsilonSpeedyExplorer, WeightedSoftmaxExplorer, GumbelSoftmaxExplorer)
+
+
 class Agent(AbstractPolicy):
     """Agent(policy, trajectory) (agent_base.jl:18-66) for a device-resident replay trajectory: pushes the env's
     transition frames (state / action / reward / terminal never visit the host) and lets the policy's learner train
@@ -610,10 +615,11 @@ class Agent(AbstractPolicy):
         if not hasattr(trajectory, "controller"):
             trajectory.controller = InsertSampleRatioController()
         self._host_act = None
-        # run() may hand whole stretches of the loop to run_replay (b200rl_replay_run): a DQN learner behind an epsilon-greedy
-        # or greedy explorer whose actions stay on the device.  The env's side is checked per run (replay_supported).
+        # run() may hand whole stretches of the loop to run_replay (b200rl_replay_run): a DQN learner behind one of the device
+        # explorers (epsilon-greedy, speedy, weighted / Gumbel softmax, greedy) whose actions stay on the device.  The env's side is
+        # checked per run (replay_supported).
         self.fusable = (not host_actions and isinstance(policy, QBasedPolicy) and isinstance(policy.learner, DQNLearner)
-                        and type(policy.explorer) in (EpsilonGreedyExplorer, GreedyExplorer))
+                        and type(policy.explorer) in DEVICE_EXPLORERS + (GreedyExplorer,))
         self._replay, self._replay_key = None, None
 
     def close(self):
@@ -656,12 +662,12 @@ class Agent(AbstractPolicy):
         (want_stats, synchronises) or None."""
         pol, c = self.policy, self.trajectory.controller
         h = self._handle(env)
-        ex = pol.explorer.as_struct() if isinstance(pol.explorer, EpsilonGreedyExplorer) else None
+        ex = pol.explorer.as_struct() if type(pol.explorer) in DEVICE_EXPLORERS else None
         ctl = L.InsertSampleRatio(c.ratio, c.threshold, c.n_inserted, c.n_sampled)
         stats = np.full(4, np.nan, np.float32) if want_stats else None
         L.check(pol.lib.b200rl_replay_run(h, C.c_void_p(pol._d_rng), None if ex is None else C.byref(ex), C.byref(ctl), int(n_steps),
                                           L.ptr(stats)))
-        if ex is not None:
+        if ex is not None and hasattr(pol.explorer, "step"):
             pol.explorer.step = ex.step
         c.n_inserted, c.n_sampled = ctl.n_inserted, ctl.n_sampled
         if stats is None or np.isnan(stats[3]):
