@@ -47,6 +47,7 @@ int b200rl_env_internal_max_timeout(const b200rl_env* e);
 int b200rl_env_internal_dtype(const b200rl_env* e);
 void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n);
 int b200rl_env_internal_n_actions(const b200rl_env* e);
+float b200rl_env_internal_action_bound(const b200rl_env* e);
 static void* env_field(b200rl_env* e, int f);
 static bool fused_rollout_enabled() {   // B200RL_FUSED_ROLLOUT=0: step through plan!/act! launches instead (same results)
     static int v = -1;
@@ -477,7 +478,7 @@ int b200rl_evaluate(b200rl_net* n, b200rl_env* env, const b200rl_eval_config* cf
         const float* obs = (const float*)env_field(env, B200RL_FIELD_OBS);
         const float* rew = (const float*)env_field(env, B200RL_FIELD_REWARD);
         const uint8_t* flags = (const uint8_t*)env_field(env, B200RL_FIELD_FLAGS);
-        const float bound = b200rl_env_internal_kind(env) == B200RL_ENV_PENDULUM ? 2.0f : 1.0f;   // action_space -2.0..2.0 | -1.0..1.0
+        const float bound = b200rl_env_internal_action_bound(env);
         for (int k = 0; k < nsteps; ++k) {
             const void* a_env = act;
             if (mode == 0) {
@@ -683,8 +684,8 @@ int b200rl_onpolicy_act(b200rl_onpolicy* a) {
     REQUIRE(a, B200RL_ERR_INVALID, "null agent");
     TRY(ctx_bind(a->ctx));
     char* act_col = (char*)a->actions + (size_t)a->N * a->t * 4;
-    if (a->continuous) {  // the env asserts a in -2.0..2.0; the stored (unclamped) action keeps its log-prob
-        const float bound = b200rl_env_internal_kind(a->env) == B200RL_ENV_PENDULUM ? 2.0f : 1.0f;   // action_space -2.0..2.0 | -1.0..1.0
+    if (a->continuous) {  // the env asserts a in its action space; the stored (unclamped) action keeps its log-prob
+        const float bound = b200rl_env_internal_action_bound(a->env);
         clamp_copy_kernel<<<grid_for(a->N, 256), 256, 0, a->ctx->stream>>>(a->act_clamped, (const float*)act_col, a->N, -bound, bound);
         LAUNCH_CHECK(a->ctx);
         return b200rl_env_step(a->env, a->act_clamped, 1, 1);

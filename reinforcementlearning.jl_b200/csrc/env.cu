@@ -22,48 +22,19 @@ namespace {
 constexpr int kBlock = 256;
 
 // ------------------------------------------------------------------ kernels -----------
-// Block-level accumulation of episode statistics: one atomicAdd triple per CTA that saw a
-// finished episode (device-side TotalRewardPerEpisode / BatchStepsPerEpisode, hooks.jl:146-231).
-__device__ __forceinline__ void block_episode_stats(double* stats, bool finished, float ret, int len) {
-    __shared__ float s_ret[kBlock / 32];
-    __shared__ int s_len[kBlock / 32];
-    __shared__ int s_cnt[kBlock / 32];
-    unsigned m = __ballot_sync(0xffffffffu, finished);
-    float r = finished ? ret : 0.f;
-    int l = finished ? len : 0;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        r += __shfl_xor_sync(0xffffffffu, r, o);
-        l += __shfl_xor_sync(0xffffffffu, l, o);
-    }
-    int w = threadIdx.x >> 5;
-    if ((threadIdx.x & 31) == 0) { s_ret[w] = r; s_len[w] = l; s_cnt[w] = __popc(m); }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double rr = 0; long long ll = 0; int cc = 0;
-#pragma unroll
-        for (int k = 0; k < kBlock / 32; ++k) { rr += s_ret[k]; ll += s_len[k]; cc += s_cnt[k]; }
-        if (cc) {
-            atomicAdd(&stats[0], (double)cc);
-            atomicAdd(&stats[1], rr);
-            atomicAdd(&stats[2], (double)ll);
-        }
-    }
-}
-
 template <class Env, bool RANDOM, bool AUTO>
 __global__ void __launch_bounds__(kBlock) env_step_kernel(typename Env::P p, EnvArrays a, int64_t N, const void* actions_v) {
     using T = typename Env::real;
     using act_t = typename Env::act_t;
+    __shared__ StatsScratch<kBlock / 32> red;
     int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
     bool active = i < N;
-    bool finished = false;
+    int fin_cnt = 0, fin_len = 0;
     float fin_ret = 0.f;
-    int fin_len = 0;
     if (active) {
         typename Env::S s = Env::load(a.state, i);
         int t = a.t[i];
-        uint8_t prev = a.flags[i];
+        int f = a.flags[i];
         Xo g;
         bool have_rng = false;
         act_t act;
@@ -78,34 +49,24 @@ __global__ void __launch_bounds__(kBlock) env_step_kernel(typename Env::P p, Env
             if (!ok) *a.err = 1;  // `@assert a in action_space(env)` -> flag, env left untouched
         }
         if (ok) {
-            bool done;
-            T rew;
-            Env::step(p, s, t, act, done, rew);
-            // MaxTimeoutEnv: terminated also when current_t (= t + 1) > max_t; reward untouched
-            if (a.max_timeout > 0 && t + 1 > a.max_timeout) done = true;
-            float ret = a.ep_ret[i] + (float)rew;
-            uint8_t f = done ? 1 : 0;
-            if (done && !((prev & 1) && !(prev & 2))) { finished = true; fin_ret = ret; fin_len = t; }
-            if (done) ret = 0.f;
-            if (AUTO && done) {  // fused soft reset (MultiThreadEnv reset!(env; is_force=false))
+            float ret = a.ep_ret[i];
+            const ActStep<T> r = act_step<Env, AUTO>(p, a.max_timeout, s, t, f, ret, act, fin_cnt, fin_ret, fin_len, [&](auto&& reset) {
                 if (!have_rng) { g = load_rng(a.rng, i); have_rng = true; }
-                Env::reset(p, s, g, act);
-                t = 0;
-                f = 3;
-            }
+                reset(g);
+            });
             Env::store(a.state, i, s);
             if (!Env::kObsIsState) Env::write_obs(a.obs, i, N, s);
             a.t[i] = t;
-            a.flags[i] = f;
-            reinterpret_cast<T*>(a.reward)[i] = rew;
+            a.flags[i] = (uint8_t)f;
+            reinterpret_cast<T*>(a.reward)[i] = r.rew;
             reinterpret_cast<act_t*>(a.action)[i] = act;
             a.ep_ret[i] = ret;
-            if (a.traj_reward) reinterpret_cast<T*>(a.traj_reward)[i] = rew;
-            if (a.traj_terminal) a.traj_terminal[i] = done ? 1 : 0;
+            if (a.traj_reward) reinterpret_cast<T*>(a.traj_reward)[i] = r.rew;
+            if (a.traj_terminal) a.traj_terminal[i] = r.done ? 1 : 0;
         }
         if (have_rng) store_rng(a.rng, i, g);
     }
-    block_episode_stats(a.stats, finished, fin_ret, fin_len);
+    cta_episode_stats(a.stats, fin_cnt, fin_ret, fin_len, red);
 }
 
 // envs whose reset! also sets the reward field (AcrobotEnv.jl:105: env.reward = -1); the others derive reward(env) from `done`
@@ -544,6 +505,13 @@ int b200rl_env_internal_n_actions(const b200rl_env* e) {   // size of a discrete
     if (e->continuous) return 0;
     if (e->kind == B200RL_ENV_PENDULUM) return e->dtype == B200RL_F64 ? e->p.pend64.n_actions : e->p.pend.n_actions;
     return e->kind == B200RL_ENV_CARTPOLE ? 2 : 3;
+}
+float b200rl_env_internal_action_bound(const b200rl_env* e) {   // continuous action space -bound..bound
+    switch (e->kind) {
+        case B200RL_ENV_PENDULUM: return PendulumD<true>::kActionBound;
+        case B200RL_ENV_MOUNTAINCAR: return MountainCarD<true>::kActionBound;
+    }
+    return CartPoleD<float, true>::kActionBound;
 }
 b200rl_ctx* b200rl_env_internal_ctx(const b200rl_env* e) { return e->ctx; }
 bool b200rl_env_internal_continuous(const b200rl_env* e) { return e->continuous; }

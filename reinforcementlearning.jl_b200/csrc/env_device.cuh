@@ -1,9 +1,10 @@
-// env_device.cuh — device code of the classic-control envs (state structs, reset!, _step!, observation), shared by the
-// batched step / reset kernels (env.cu) and the fused rollout kernel (rollout.cu).  Arithmetic follows the reference line by
-// line with Julia's promotion rules (which sub-expressions are Float64 for T = Float32) — see DESIGN.md §K1 and
+// env_device.cuh — device code of the classic-control envs (state structs, reset!, _step!, observation) and the act! step
+// around them, shared by the batched step / reset kernels (env.cu) and the fused rollout, evaluation and DQN collect kernels
+// (fwd_tc.cu).  Arithmetic follows the reference line by line with Julia's promotion rules (which sub-expressions are Float64
+// for T = Float32) — see DESIGN.md §K1 and
 //   RLEnvs/src/environments/examples/CartPoleEnv.jl:98-140, PendulumEnv.jl:84-122, MountainCarEnv.jl:99-135.
 // Every translation unit that includes this header MUST be compiled with -fmad=false -prec-div=true -prec-sqrt=true
-// -ftz=false (no contraction: Julia never contracts a*b+c); build.py does that for env.cu and rollout.cu.
+// -ftz=false (no contraction: Julia never contracts a*b+c); build.py does that for env.cu and fwd_tc.cu.
 #pragma once
 #include <type_traits>
 
@@ -47,12 +48,13 @@ template <class T, bool CONT = false> struct CartPoleD {
     using act_t = typename std::conditional<CONT, T, int32_t>::type;
     static constexpr int NS = 4, NOBS = 4;
     static constexpr bool kObsIsState = true;
+    static constexpr float kActionBound = 1.0f;   // CONT: action_space -1.0..1.0
     struct P { T g, M, m, l, pml, fmag, dt, ththr, xthr; int max_steps; };
     struct S { T x, xd, th, thd; };
     __device__ static S load(const void* st, int64_t i);
     __device__ static void store(void* st, int64_t i, const S& s);
     __device__ static bool valid(const P&, act_t a) {
-        if (CONT) return (T)a >= (T)-1 && (T)a <= (T)1;   // a in -1.0..1.0 (NaN fails)
+        if (CONT) return (T)a >= (T)-kActionBound && (T)a <= (T)kActionBound;   // NaN fails
         return a == 1 || a == 2;
     }
     __device__ static unsigned long long n_random(const P&) { return 2; }
@@ -129,6 +131,7 @@ template <bool CONT, class T = float> struct PendulumD {
     using V2 = typename vec2_of<T>::type;
     static constexpr int NS = 2, NOBS = 3;
     static constexpr bool kObsIsState = false;
+    static constexpr float kActionBound = 2.0f;   // CONT: action_space -2.0..2.0 (PendulumEnv.jl:73)
     using P = PendPT<T>;
     struct S { T th, thd; T torque; };
     __device__ static S load(const void* st, int64_t i) {
@@ -140,7 +143,7 @@ template <bool CONT, class T = float> struct PendulumD {
         reinterpret_cast<V2*>(st)[i] = v;
     }
     __device__ static bool valid(const P& p, act_t a) {
-        if (CONT) return (T)a >= (T)-2 && (T)a <= (T)2;   // a in -2.0..2.0 (NaN fails)
+        if (CONT) return (T)a >= (T)-kActionBound && (T)a <= (T)kActionBound;   // NaN fails
         return (int)a >= 1 && (int)a <= p.n_actions;
     }
     __device__ static unsigned long long n_random(const P& p) { return (unsigned long long)p.n_actions; }
@@ -192,6 +195,7 @@ template <bool CONT = false, class T = float> struct MountainCarD {
     using V2 = typename vec2_of<T>::type;
     static constexpr int NS = 2, NOBS = 2;
     static constexpr bool kObsIsState = true;
+    static constexpr float kActionBound = 1.0f;   // CONT: force in -1.0..1.0
     using P = MountainCarPT<T>;
     struct S { T x, v; };
     __device__ static S load(const void* st, int64_t i) {
@@ -203,7 +207,7 @@ template <bool CONT = false, class T = float> struct MountainCarD {
         reinterpret_cast<V2*>(st)[i] = v;
     }
     __device__ static bool valid(const P&, act_t a) {
-        if (CONT) return (T)a >= (T)-1 && (T)a <= (T)1;
+        if (CONT) return (T)a >= (T)-kActionBound && (T)a <= (T)kActionBound;
         return a >= 1 && a <= 3;
     }
     __device__ static unsigned long long n_random(const P&) { return 3; }
@@ -329,6 +333,74 @@ struct AcrobotD {
         o[0] = jld::jcos(s.th1); o[1] = jld::jsin(s.th1); o[2] = jld::jcos(s.th2); o[3] = jld::jsin(s.th2); o[4] = s.dth1; o[5] = s.dth2;
     }
 };
+
+// What one act! step reports besides the env it updated
+template <class T> struct ActStep {
+    T rew;
+    bool done;      // terminated, the MaxTimeoutEnv cut included
+    float ret;      // episode return up to and including this step
+    int len;        // env.t after the step: the episode's length when done
+};
+
+// act!(env, a) of one env: _step!, the MaxTimeoutEnv cut (terminated also when current_t = t + 1 > max_t, reward untouched,
+// wrappers/MaxTimeoutEnv.jl:17-28), the running episode return and the flags byte (bit0 terminal, bit1 auto-reset).  An episode
+// that finishes here — done, and not the terminal state of an env that was not reset since — is added to the caller's tally
+// (fin_cnt, fin_ret, fin_len).  AUTO: a terminating step is followed by MultiThreadEnv's soft reset (reset!(env; is_force = false)):
+// with_rng(f) calls f(Xo&) on the env's stream, which the caller may fetch only then; the reset may redraw `act` (env.action).
+template <class Env, bool AUTO, class WithRng>
+__device__ __forceinline__ ActStep<typename Env::real> act_step(const typename Env::P& p, int max_timeout, typename Env::S& s, int& t,
+                                                                int& flags, float& ep_ret, typename Env::act_t& act, int& fin_cnt,
+                                                                float& fin_ret, int& fin_len, WithRng&& with_rng) {
+    ActStep<typename Env::real> r;
+    Env::step(p, s, t, act, r.done, r.rew);
+    if (max_timeout > 0 && t + 1 > max_timeout) r.done = true;
+    r.ret = ep_ret + (float)r.rew;
+    r.len = t;
+    if (r.done && !((flags & 1) && !(flags & 2))) { fin_cnt += 1; fin_ret += r.ret; fin_len += t; }
+    ep_ret = r.done ? 0.f : r.ret;
+    flags = r.done ? 1 : 0;
+    if (AUTO && r.done) {
+        with_rng([&](Xo& g) { Env::reset(p, s, g, act); });
+        t = 0;
+        flags = 3;
+    }
+    return r;
+}
+
+#ifdef __CUDACC__
+// Episode statistics of one CTA (device-side TotalRewardPerEpisode / BatchStepsPerEpisode, hooks.jl:146-231): each thread's
+// finished-episode count, return and length -> warp sums (the returns in float) -> double sums over the warps in warp order -> one
+// atomicAdd triple per CTA that saw a finished episode.  `red` is the caller's shared scratch; every thread of the CTA calls this.
+// dv / red_dv / dv_out (optional): one more per-thread count, summed the same way and added to *dv_out when non-zero.
+template <int NWARPS> struct StatsScratch { float ret[NWARPS]; int cnt[NWARPS], len[NWARPS]; };
+template <int NWARPS>
+__device__ __forceinline__ void cta_episode_stats(double* stats, int cnt, float ret, int len, StatsScratch<NWARPS>& red, long long dv = 0,
+                                                  long long* red_dv = nullptr, unsigned long long* dv_out = nullptr) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+        len += __shfl_xor_sync(0xffffffffu, len, o);
+        ret += __shfl_xor_sync(0xffffffffu, ret, o);
+        if (red_dv) dv += __shfl_xor_sync(0xffffffffu, dv, o);
+    }
+    const int w = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) == 0) {
+        red.cnt[w] = cnt; red.ret[w] = ret; red.len[w] = len;
+        if (red_dv) red_dv[w] = dv;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double cc = 0, rr = 0, ll = 0;
+        long long vv = 0;
+        for (int k = 0; k < NWARPS; ++k) {
+            cc += red.cnt[k]; rr += red.ret[k]; ll += red.len[k];
+            if (red_dv) vv += red_dv[k];
+        }
+        if (cc > 0) { atomicAdd(&stats[0], cc); atomicAdd(&stats[1], rr); atomicAdd(&stats[2], ll); }
+        if (vv != 0) atomicAdd(dv_out, (unsigned long long)vv);
+    }
+}
+#endif
 
 // what the fused consumers (fwd_tc.cu) need to know about a b200rl_env handle
 struct EnvView {

@@ -7,9 +7,11 @@
 //                        both networks too.  Replaces 2 launches per env step (agent_base.jl:45-66 stage loop, run.jl:52-68).
 //   evaluate_tc_kernel : n_steps x { obs -> actor -> greedy | sampled action -> env step (+ fused auto-reset) -> per-env episode
 //                        records }: the actor alone, no rollout tensors (b200rl_evaluate).
+//   replay_collect_tc_kernel : n_steps x { obs -> Q -> explorer action -> env step (+ fused auto-reset) -> replay ring push }.
 //
-// Both kernels are built from the same device functions (tc_fwd.cuh, env_device.cuh) and compiled with the env flags
-// (-fmad=false): stepping through plan!/act! one launch at a time or through the fused rollout gives bit-identical results.
+// The kernels share one tile forward (tile_forward), one resident env slot with its load / write-back (EnvSlot) and the act! step
+// of env_device.cuh, and are compiled with the env flags (-fmad=false): stepping through plan!/act! one launch at a time or
+// through a fused kernel gives bit-identical results.
 #include "common.cuh"
 #include "duel.cuh"
 #include "env_device.cuh"
@@ -23,6 +25,7 @@ using namespace envdev;
 
 int b200rl_env_internal_view(b200rl_env* e, envdev::EnvView* out);
 void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n);
+int b200rl_env_internal_n_actions(const b200rl_env* e);
 
 namespace {
 
@@ -42,6 +45,36 @@ __device__ __forceinline__ void store_rng32(unsigned long long* rng, int64_t i, 
     ulonglong2* p = reinterpret_cast<ulonglong2*>(rng + 4 * i);
     p[0] = make_ulonglong2(s[0], s[1]);
     p[1] = make_ulonglong2(s[2], s[3]);
+}
+
+// One tile of TM samples through one network: the observations in X ([i][s], published by a barrier before the call) -> layer 1 ->
+// the GEMM of both warpgroups -> the head partial sums of both 32-feature halves in Zp ([half][o][s]).  Called by all NT threads;
+// ends with a barrier, after which Zp may be read (tile_heads) and the next tile's X writes are ordered behind this tile's reads.
+// UNROLL: as layer1_to_smem / head_partials.
+template <int ACT, int UNROLL = (ACT == B200RL_ACT_RELU ? 2 : 1)>
+__device__ __forceinline__ void tile_forward(const NetSm& net, int act_rt, int c, int s, uint8_t* T, const float* X, float* Zp) {
+    {
+        float x[kInMax];
+#pragma unroll
+        for (int k = 0; k < kInMax; ++k) x[k] = X[k * TM + s];
+        layer1_to_smem<ACT, UNROLL>(net, act_rt, x, c, s, T);
+    }
+    wg::fence_proxy_async();
+    __syncthreads();
+    gemm_block(T + c * BLK, net, c);   // warpgroup c: samples 64c .. 64c+63
+    __syncthreads();
+    {
+        float zp[kOutMax];
+        head_partials<ACT, UNROLL>(net, act_rt, c, s, T, zp);
+#pragma unroll
+        for (int o = 0; o < kOutMax; ++o) Zp[(c * kOutMax + o) * TM + s] = zp[o];
+    }
+    __syncthreads();
+}
+// head outputs of sample s after tile_forward
+__device__ __forceinline__ void tile_heads(const NetSm& net, const float* Zp, int s, float (&z)[kOutMax]) {
+#pragma unroll
+    for (int o = 0; o < kOutMax; ++o) z[o] = net.b3[o] + Zp[o * TM + s] + Zp[(kOutMax + o) * TM + s];
 }
 
 // mode 0: actor-critic rollout step (CTA role = blockIdx & 1), mode 1: plain forward of `actor` -> head_out
@@ -87,29 +120,12 @@ forward_tc_kernel(MlpDesc actor, MlpDesc critic, const float* __restrict__ param
             for (int k = 0; k < kInMax; ++k) sm.X[k * TM + tid] = x[k];
         }
         __syncthreads();
-        {
-            float x[kInMax];
-#pragma unroll
-            for (int k = 0; k < kInMax; ++k) x[k] = sm.X[k * TM + s];
-            layer1_to_smem<ACT>(sm.net, d.act, x, c, s, sm.T);
-        }
-        wg::fence_proxy_async();
-        __syncthreads();
-        gemm_block(sm.T + c * BLK, sm.net, c);   // warpgroup c: samples 64c .. 64c+63
-        __syncthreads();
-        {
-            float zp[kOutMax];
-            head_partials<ACT>(sm.net, d.act, c, s, sm.T, zp);
-#pragma unroll
-            for (int o = 0; o < kOutMax; ++o) sm.Zp[(c * kOutMax + o) * TM + s] = zp[o];
-        }
-        __syncthreads();               // accumulator reads done before the next tile's layer 1 overwrites the image
-        if (tid < TM) {
+        tile_forward<ACT>(sm.net, d.act, c, s, sm.T, sm.X, sm.Zp);   // (its last barrier: the head reads are done before the next
+        if (tid < TM) {                                              //  tile's layer 1 overwrites the image)
             int64_t i = tile * TM + tid;
             if (i < N) {
                 float z[kOutMax];
-#pragma unroll
-                for (int o = 0; o < kOutMax; ++o) z[o] = sm.net.b3[o] + sm.Zp[o * TM + tid] + sm.Zp[(kOutMax + o) * TM + tid];
+                tile_heads(sm.net, sm.Zp, tid, z);
                 if (mode == 1 && d.duel) duel::combine(z, d.nout);   // dueling Q-network: the combined Q, not the head rows
                 if (head_out && (mode == 1 || role == 0))
                     for (int o = 0; o < d.nout; ++o) head_out[(int64_t)d.nout * i + o] = z[o];
@@ -131,27 +147,123 @@ forward_tc_kernel(MlpDesc actor, MlpDesc critic, const float* __restrict__ param
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// fused rollout
-constexpr int kSlots = 2;   // tiles of 128 envs a CTA keeps resident
+// resident env slots of the fused kernels: a CTA keeps up to kSlots tiles of 128 envs (tiles base + k * nctas) in shared memory,
+// one entry per env, owned by thread s = the env's sample in the tile
+constexpr int kSlots = 2;
 
-template <class Env> struct SlotState {   // env state of one tile, one entry per env (owner thread = sample s)
+// a 4-word stream of env s in a slot's transposed [word][env] layout
+__device__ __forceinline__ void get_stream(const unsigned long long* w, int s, unsigned long long (&x)[4]) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) x[k] = w[k * TM + s];
+}
+__device__ __forceinline__ void put_stream(unsigned long long* w, int s, const unsigned long long (&x)[4]) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) w[k * TM + s] = x[k];
+}
+
+template <class E> struct EnvSlot {   // the env part of a slot; each kernel's slot type adds its own fields
+    using Env = E;
     typename Env::S st[TM];
     int t[TM];
     int flags[TM];
     float ep_ret[TM];
     float last_rew[TM];
     uint32_t last_act[TM];                 // env.action after the last act! (a reset may have redrawn it), raw bits
-    unsigned long long erng[4 * TM];   // env stream  [word][env]
-    unsigned long long prng[4 * TM];   // policy stream
+    unsigned long long erng[4 * TM];       // env stream
+};
+
+__device__ __forceinline__ int group_slots(int64_t base, int nctas, int64_t ntiles) {   // resident tiles of the group at `base`
+    int n = 0;
+    for (int k = 0; k < kSlots; ++k)
+        if (base + (int64_t)k * nctas < ntiles) n = k + 1;
+    return n;
+}
+// Owner thread s: loads the env part of env i of each resident tile into its slot; more(slot, i) loads the kernel's own fields.
+template <class Slot, class More>
+__device__ __forceinline__ void load_group(Slot* slot, int nslots, int64_t base, int nctas, const EnvArrays& ea, int64_t N, int s, More&& more) {
+    for (int k = 0; k < nslots; ++k) {
+        const int64_t i = (base + (int64_t)k * nctas) * TM + s;
+        if (i < N) {
+            Slot& sl = slot[k];
+            sl.st[s] = Slot::Env::load(ea.state, i);
+            sl.t[s] = ea.t[i];
+            sl.flags[s] = ea.flags[i];
+            sl.ep_ret[s] = ea.ep_ret[i];
+            unsigned long long e[4];
+            load_rng32(ea.rng, i, e);
+            put_stream(sl.erng, s, e);
+            more(sl, i);
+        }
+    }
+}
+// ... and writes it back: reward and action are the last step's, so only when the window stepped (`stepped`).
+template <class Slot, class More>
+__device__ __forceinline__ void store_group(const Slot* slot, int nslots, int64_t base, int nctas, const EnvArrays& ea, int64_t N, int s,
+                                            bool stepped, More&& more) {
+    using Env = typename Slot::Env;
+    for (int k = 0; k < nslots; ++k) {
+        const int64_t i = (base + (int64_t)k * nctas) * TM + s;
+        if (i < N) {
+            const Slot& sl = slot[k];
+            Env::store(ea.state, i, sl.st[s]);
+            if (!Env::kObsIsState) Env::write_obs(ea.obs, i, N, sl.st[s]);
+            ea.t[i] = sl.t[s];
+            ea.flags[i] = (uint8_t)sl.flags[s];
+            ea.ep_ret[i] = sl.ep_ret[s];
+            unsigned long long e[4];
+            get_stream(sl.erng, s, e);
+            store_rng32(ea.rng, i, e);
+            if (stepped) {
+                reinterpret_cast<float*>(ea.reward)[i] = sl.last_rew[s];
+                reinterpret_cast<uint32_t*>(ea.action)[i] = sl.last_act[s];
+            }
+            more(sl, i);
+        }
+    }
+}
+
+// the action the env receives for the head's raw action bits: the 1-based index, or the continuous action clamped to the action space
+template <class Env> __device__ __forceinline__ typename Env::act_t env_action(uint32_t a_bits) {
+    using act_t = typename Env::act_t;
+    if (std::is_same<act_t, float>::value) return (act_t)fminf(fmaxf(__uint_as_float(a_bits), -Env::kActionBound), Env::kActionBound);
+    return (act_t)(int32_t)a_bits;
+}
+// act!(env, a) of owner thread s's env in its slot: the act! step of env_step_kernel<Env, false, true>, the fused auto-reset drawing
+// from the slot's env stream, a finished episode added to the thread's tally
+template <class Env>
+__device__ __forceinline__ ActStep<float> slot_act(EnvSlot<Env>& sl, int s, const typename Env::P& p, int max_timeout, typename Env::act_t act,
+                                                   int& fin_cnt, float& fin_ret, int& fin_len) {
+    typename Env::S st = sl.st[s];
+    int t = sl.t[s], f = sl.flags[s];
+    float ret = sl.ep_ret[s];
+    const ActStep<float> r = act_step<Env, true>(p, max_timeout, st, t, f, ret, act, fin_cnt, fin_ret, fin_len, [&](auto&& reset) {
+        unsigned long long w[4];
+        get_stream(sl.erng, s, w);
+        Xo e{w[0], w[1], w[2], w[3]};
+        reset(e);
+        const unsigned long long o[4] = {e.s0, e.s1, e.s2, e.s3};
+        put_stream(sl.erng, s, o);
+    });
+    sl.st[s] = st; sl.t[s] = t; sl.flags[s] = f; sl.ep_ret[s] = ret;
+    sl.last_rew[s] = r.rew;
+    uint32_t bits;
+    memcpy(&bits, &act, 4);
+    sl.last_act[s] = bits;
+    return r;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// fused rollout
+template <class Env> struct RollSlot : EnvSlot<Env> {
+    unsigned long long prng[4 * TM];       // policy stream
 };
 template <class Env> struct SmemRoll {
     alignas(128) uint8_t T[TILE_BYTES];    // A operand / accumulator image of the tile being evaluated (tc_fwd.cuh)
     NetSm net[2];                          // actor, critic
     float X[kInMax * TM];
     float Zp[2][2 * kOutMax * TM];         // [net][half][o][s]
-    SlotState<Env> slot[kSlots];
-    float red_f[8];
-    int red_i[8], red_l[8];
+    RollSlot<Env> slot[kSlots];
+    StatsScratch<NT / 32> red;
 };
 
 struct RollArgs {
@@ -161,19 +273,18 @@ struct RollArgs {
     int64_t N;
     int t0, nsteps, T;          // rollout columns t0 .. t0 + nsteps - 1 of T
     int final_bootstrap;        // also write states[:, :, t0 + nsteps] and V of it (only when t0 + nsteps == T)
-    float act_lo, act_hi;       // continuous actions: the env receives clamp(a, lo, hi), the rollout keeps a
     unsigned long long* policy_rng;   // (4, N)
     float* states;              // (NOBS, N, T + 1)
-    void* actions;              // (N, T) int32 | f32
+    void* actions;              // (N, T) int32 | f32: continuous actions as sampled (the env receives them clamped, env_action)
     float* logp;                // (N, T)
     float* values;              // (N, T + 1)
     float* rewards;             // (N, T)
     uint8_t* terminals;         // (N, T)
 };
 
+// A CTA owns one group of up to kSlots tiles for the whole launch (the caller bounds N by it).
 template <class Env, int ACT>
 __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename Env::P p, EnvArrays ea) {
-    using act_t = typename Env::act_t;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     SmemRoll<Env>& sm = *reinterpret_cast<SmemRoll<Env>*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -182,33 +293,18 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
     const bool owner = c == 0;              // warps 0..3: thread s also owns env s of the tile
     const int cta = blockIdx.x, nctas = gridDim.x;
     const int64_t N = g.N;
-    const int64_t ntiles = (N + TM - 1) / TM;
     load_net<false>(sm.net[0], g.actor, g.params, ACT == B200RL_ACT_RELU ? kScale : 1.0f);
     load_net<false>(sm.net[1], g.critic, g.params + g.actor.nparams(), ACT == B200RL_ACT_RELU ? kScale : 1.0f);
-    // resident env state
-    int nslots = 0;
-    for (int k = 0; k < kSlots; ++k)
-        if ((int64_t)cta + (int64_t)k * nctas < ntiles) nslots = k + 1;
-    if (owner) {
-        for (int k = 0; k < nslots; ++k) {
-            const int64_t i = ((int64_t)cta + (int64_t)k * nctas) * TM + s;
-            SlotState<Env>& sl = sm.slot[k];
-            if (i < N) {
-                sl.st[s] = Env::load(ea.state, i);
-                sl.t[s] = ea.t[i];
-                sl.flags[s] = ea.flags[i];
-                sl.ep_ret[s] = ea.ep_ret[i];
-                Xo e = load_rng(ea.rng, i);
-                sl.erng[s] = e.s0; sl.erng[TM + s] = e.s1; sl.erng[2 * TM + s] = e.s2; sl.erng[3 * TM + s] = e.s3;
-                unsigned long long pr[4];
-                load_rng32(g.policy_rng, i, pr);
-                sl.prng[s] = pr[0]; sl.prng[TM + s] = pr[1]; sl.prng[2 * TM + s] = pr[2]; sl.prng[3 * TM + s] = pr[3];
-            }
-        }
-    }
+    const int nslots = group_slots(cta, nctas, (N + TM - 1) / TM);
+    if (owner)
+        load_group(sm.slot, nslots, cta, nctas, ea, N, s, [&](RollSlot<Env>& sl, int64_t i) {
+            unsigned long long pr[4];
+            load_rng32(g.policy_rng, i, pr);
+            put_stream(sl.prng, s, pr);
+        });
     wg::fence_proxy_async();
     __syncthreads();
-    // episode statistics of this thread's envs (device-side TotalRewardPerEpisode / BatchStepsPerEpisode, hooks.jl:146-231)
+    // episode statistics of this thread's envs
     int fin_cnt = 0, fin_len = 0;
     float fin_ret = 0.f;
     const int ns = Env::NOBS;
@@ -219,7 +315,7 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
         const bool boot = step == g.nsteps;      // extra pass: V(s_T) only
 #pragma unroll 1
         for (int k = 0; k < nslots; ++k) {
-            SlotState<Env>& sl = sm.slot[k];
+            RollSlot<Env>& sl = sm.slot[k];
             const int64_t i = ((int64_t)cta + (int64_t)k * nctas) * TM + s;
             const bool live = i < N;
             // ---- observation of this step -> X (shared) and column t of the rollout states ------------------------
@@ -238,27 +334,14 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
                 for (int j = 0; j < kInMax; ++j) sm.X[j * TM + s] = o[j];
             }
             __syncthreads();
-            float x[kInMax];
-#pragma unroll
-            for (int j = 0; j < kInMax; ++j) x[j] = sm.X[j * TM + s];
-            uint32_t a_bits = 0;
-            if (!boot) {
-                // ---- actor ---------------------------------------------------------------------------------------
-                layer1_to_smem<ACT>(sm.net[0], g.actor.act, x, c, s, sm.T);
-                wg::fence_proxy_async();
-                __syncthreads();
-                gemm_block(sm.T + c * BLK, sm.net[0], c);   // warpgroup c: samples 64c .. 64c+63
-                __syncthreads();
-                {
-                    float zp[kOutMax];
-                    head_partials<ACT>(sm.net[0], g.actor.act, c, s, sm.T, zp);
-#pragma unroll
-                    for (int o = 0; o < kOutMax; ++o) sm.Zp[0][(c * kOutMax + o) * TM + s] = zp[o];
-                }
-                __syncthreads();
-            }
+            if (!boot) tile_forward<ACT>(sm.net[0], g.actor.act, c, s, sm.T, sm.X, sm.Zp[0]);   // actor
             // ---- critic GEMM (warpgroup 1, both blocks) while the owner threads (warpgroup 0) sample the action and step the env
-            layer1_to_smem<ACT>(sm.net[1], g.critic.act, x, c, s, sm.T);
+            {
+                float x[kInMax];
+#pragma unroll
+                for (int j = 0; j < kInMax; ++j) x[j] = sm.X[j * TM + s];
+                layer1_to_smem<ACT>(sm.net[1], g.critic.act, x, c, s, sm.T);
+            }
             wg::fence_proxy_async();
             __syncthreads();
             if (!owner) {
@@ -267,41 +350,17 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
             }
             if (owner && live && !boot) {
                 float z[kOutMax];
-#pragma unroll
-                for (int o = 0; o < kOutMax; ++o) z[o] = sm.net[0].b3[o] + sm.Zp[0][o * TM + s] + sm.Zp[0][(kOutMax + o) * TM + s];
-                unsigned long long pr[4] = {sl.prng[s], sl.prng[TM + s], sl.prng[2 * TM + s], sl.prng[3 * TM + s]};
+                tile_heads(sm.net[0], sm.Zp[0], s, z);
+                unsigned long long pr[4];
+                get_stream(sl.prng, s, pr);
                 float lp;
-                a_bits = sample_head(g.actor, g.hp, z, pr, lp);
-                sl.prng[s] = pr[0]; sl.prng[TM + s] = pr[1]; sl.prng[2 * TM + s] = pr[2]; sl.prng[3 * TM + s] = pr[3];
+                const uint32_t a_bits = sample_head(g.actor, g.hp, z, pr, lp);
+                put_stream(sl.prng, s, pr);
                 reinterpret_cast<uint32_t*>(g.actions)[(size_t)N * t + i] = a_bits;
                 g.logp[(size_t)N * t + i] = lp;
-                // act!(env, a) + fused soft reset (MultiThreadEnv): same sequence as env_step_kernel<Env, false, true>
-                act_t act;
-                if (std::is_same<act_t, float>::value) act = (act_t)fminf(fmaxf(__uint_as_float(a_bits), g.act_lo), g.act_hi);
-                else act = (act_t)(int32_t)a_bits;
-                typename Env::S st = sl.st[s];
-                int tt = sl.t[s];
-                const int prev = sl.flags[s];
-                bool done;
-                float rew;
-                Env::step(p, st, tt, act, done, rew);
-                if (ea.max_timeout > 0 && tt + 1 > ea.max_timeout) done = true;
-                float ret = sl.ep_ret[s] + rew;
-                int f = done ? 1 : 0;
-                if (done && !((prev & 1) && !(prev & 2))) { fin_cnt += 1; fin_ret += ret; fin_len += tt; }
-                if (done) {
-                    ret = 0.f;
-                    Xo e{sl.erng[s], sl.erng[TM + s], sl.erng[2 * TM + s], sl.erng[3 * TM + s]};
-                    Env::reset(p, st, e, act);
-                    sl.erng[s] = e.s0; sl.erng[TM + s] = e.s1; sl.erng[2 * TM + s] = e.s2; sl.erng[3 * TM + s] = e.s3;
-                    tt = 0;
-                    f = 3;
-                }
-                sl.st[s] = st; sl.t[s] = tt; sl.flags[s] = f; sl.ep_ret[s] = ret;
-                g.rewards[(size_t)N * t + i] = rew;
-                g.terminals[(size_t)N * t + i] = done ? 1 : 0;
-                sl.last_rew[s] = rew;
-                { act_t tmp = act; uint32_t bits; memcpy(&bits, &tmp, 4); sl.last_act[s] = bits; }
+                const ActStep<float> r = slot_act(sl, s, p, ea.max_timeout, env_action<Env>(a_bits), fin_cnt, fin_ret, fin_len);
+                g.rewards[(size_t)N * t + i] = r.rew;
+                g.terminals[(size_t)N * t + i] = r.done ? 1 : 0;
             }
             __syncthreads();
             {
@@ -314,61 +373,13 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
             // (the next pass's X / Zp writes are ordered behind this read by its first __syncthreads)
         }
     }
-    // ---- write the env back ---------------------------------------------------------------------------------------
-    if (owner) {
-        for (int k = 0; k < nslots; ++k) {
-            const int64_t i = ((int64_t)cta + (int64_t)k * nctas) * TM + s;
-            SlotState<Env>& sl = sm.slot[k];
-            if (i < N) {
-                Env::store(ea.state, i, sl.st[s]);
-                if (!Env::kObsIsState) Env::write_obs(ea.obs, i, N, sl.st[s]);
-                ea.t[i] = sl.t[s];
-                ea.flags[i] = (uint8_t)sl.flags[s];
-                ea.ep_ret[i] = sl.ep_ret[s];
-                store_rng(ea.rng, i, Xo{sl.erng[s], sl.erng[TM + s], sl.erng[2 * TM + s], sl.erng[3 * TM + s]});
-                unsigned long long pr[4] = {sl.prng[s], sl.prng[TM + s], sl.prng[2 * TM + s], sl.prng[3 * TM + s]};
-                store_rng32(g.policy_rng, i, pr);
-                if (g.nsteps > 0) {
-                    reinterpret_cast<float*>(ea.reward)[i] = sl.last_rew[s];
-                    reinterpret_cast<uint32_t*>(ea.action)[i] = sl.last_act[s];
-                }
-            }
-        }
-    }
-    // episode statistics: one atomicAdd triple per CTA
-    {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            fin_cnt += __shfl_xor_sync(0xffffffffu, fin_cnt, o);
-            fin_len += __shfl_xor_sync(0xffffffffu, fin_len, o);
-            fin_ret += __shfl_xor_sync(0xffffffffu, fin_ret, o);
-        }
-        __syncthreads();
-        if (lane == 0) { sm.red_i[warp] = fin_cnt; sm.red_f[warp] = fin_ret; sm.red_l[warp] = fin_len; }
-        __syncthreads();
-        if (tid == 0) {
-            double cc = 0, rr = 0, ll = 0;
-            for (int w = 0; w < NT / 32; ++w) { cc += sm.red_i[w]; rr += sm.red_f[w]; ll += sm.red_l[w]; }
-            if (cc > 0) { atomicAdd(&ea.stats[0], cc); atomicAdd(&ea.stats[1], rr); atomicAdd(&ea.stats[2], ll); }
-        }
-    }
-}
-
-template <class Env> int launch_rollout(b200rl_ctx* ctx, const RollArgs& g, const typename Env::P& p, const EnvArrays& ea) {
-    const size_t smem = sizeof(SmemRoll<Env>) + 128;
-    static unsigned long long attr_devices = 0;   // once per device: the attribute call is not free and may serialise with running kernels
-    if (first_use_on_device(attr_devices, ctx->device)) {
-        CUDA_TRY(cudaFuncSetAttribute(rollout_tc_kernel<Env, B200RL_ACT_RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(rollout_tc_kernel<Env, B200RL_ACT_TANH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    }
-    const int64_t ntiles = (g.N + TM - 1) / TM;
-    int grid = 2 * ctx->sm_count;
-    if ((int64_t)grid > ntiles) grid = (int)ntiles;
-    // the activation is a template parameter (nn_tc_rollout only comes here when both trunks share it)
-    if (g.actor.act == B200RL_ACT_RELU) rollout_tc_kernel<Env, B200RL_ACT_RELU><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
-    else rollout_tc_kernel<Env, B200RL_ACT_TANH><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
-    LAUNCH_CHECK(ctx);
-    return B200RL_OK;
+    if (owner)
+        store_group(sm.slot, nslots, cta, nctas, ea, N, s, g.nsteps > 0, [&](const RollSlot<Env>& sl, int64_t i) {
+            unsigned long long pr[4];
+            get_stream(sl.prng, s, pr);
+            store_rng32(g.policy_rng, i, pr);
+        });
+    cta_episode_stats(ea.stats, fin_cnt, fin_ret, fin_len, sm.red);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -377,15 +388,8 @@ template <class Env> int launch_rollout(b200rl_ctx* ctx, const RollArgs& g, cons
 // group of up to kSlots resident tiles, writes the group back and takes the next one (no limit on N).  The head outputs come
 // from the device functions, template activation and operand scale of forward_tc_kernel's mode 1, so the staged greedy
 // policy (b200rl_net_act_greedy -> nn_mlp_forward) and this kernel pick the same actions bit for bit.
-template <class Env> struct EvalSlot {     // env state of one tile, one entry per env (owner thread = sample s)
-    typename Env::S st[TM];
-    int t[TM];
-    int flags[TM];
-    float ep_ret[TM];
-    float last_rew[TM];
-    uint32_t last_act[TM];
+template <class Env> struct EvalSlot : EnvSlot<Env> {
     int cnt[TM];                           // episodes finished in the window
-    unsigned long long erng[4 * TM];       // env stream  [word][env]
     unsigned long long prng[4 * TM];       // policy stream (MODE 1)
 };
 template <class Env> struct SmemEval {
@@ -396,8 +400,7 @@ template <class Env> struct SmemEval {
     EvalSlot<Env> slot[kSlots];
     int fin_cnt[TM], fin_len[TM];          // episode statistics of owner thread s (shared memory: no registers held across the window)
     float fin_ret[TM];
-    float red_f[8];
-    int red_i[8], red_l[8];
+    StatsScratch<NT / 32> red;
 };
 
 struct EvalArgs {
@@ -406,7 +409,6 @@ struct EvalArgs {
     AcHyper hp;
     int64_t N;
     int nsteps, K;
-    float act_lo, act_hi;               // continuous actions: the env receives clamp(a, lo, hi)
     unsigned long long* policy_rng;     // (4, N), MODE 1
     float* returns;                     // (K, N), may be null
     int32_t* lengths;                   // (K, N), may be null
@@ -418,7 +420,6 @@ struct EvalArgs {
 // (layer 1 and the head epilogue not unrolled: the relu variants would exceed 128 registers and spill)
 template <class Env, int ACT, int MODE, bool DUEL = false>
 __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename Env::P p, EnvArrays ea) {
-    using act_t = typename Env::act_t;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     SmemEval<Env>& sm = *reinterpret_cast<SmemEval<Env>*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -431,30 +432,17 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename
     load_net<DUEL>(sm.net, g.actor, g.params, ACT == B200RL_ACT_RELU ? kScale : 1.0f);
     if (owner) { sm.fin_cnt[s] = 0; sm.fin_len[s] = 0; sm.fin_ret[s] = 0.f; }
 #pragma unroll 1
-    for (int64_t base = blockIdx.x; base < ntiles; base += (int64_t)nctas * kSlots) {   // tiles base + k * nctas, k < kSlots
-        int nslots = 0;
-        for (int k = 0; k < kSlots; ++k)
-            if (base + (int64_t)k * nctas < ntiles) nslots = k + 1;
-        if (owner) {
-            for (int k = 0; k < nslots; ++k) {
-                const int64_t i = (base + (int64_t)k * nctas) * TM + s;
-                EvalSlot<Env>& sl = sm.slot[k];
-                if (i < N) {
-                    sl.st[s] = Env::load(ea.state, i);
-                    sl.t[s] = ea.t[i];
-                    sl.flags[s] = ea.flags[i];
-                    sl.ep_ret[s] = ea.ep_ret[i];
-                    sl.cnt[s] = 0;
-                    Xo e = load_rng(ea.rng, i);
-                    sl.erng[s] = e.s0; sl.erng[TM + s] = e.s1; sl.erng[2 * TM + s] = e.s2; sl.erng[3 * TM + s] = e.s3;
-                    if (MODE == 1) {
-                        unsigned long long pr[4];
-                        load_rng32(g.policy_rng, i, pr);
-                        sl.prng[s] = pr[0]; sl.prng[TM + s] = pr[1]; sl.prng[2 * TM + s] = pr[2]; sl.prng[3 * TM + s] = pr[3];
-                    }
+    for (int64_t base = blockIdx.x; base < ntiles; base += (int64_t)nctas * kSlots) {
+        const int nslots = group_slots(base, nctas, ntiles);
+        if (owner)
+            load_group(sm.slot, nslots, base, nctas, ea, N, s, [&](EvalSlot<Env>& sl, int64_t i) {
+                sl.cnt[s] = 0;
+                if (MODE == 1) {
+                    unsigned long long pr[4];
+                    load_rng32(g.policy_rng, i, pr);
+                    put_stream(sl.prng, s, pr);
                 }
-            }
-        }
+            });
         wg::fence_proxy_async();            // (the first pass: the weight image written by load_net, read by wgmma)
         __syncthreads();
 #pragma unroll 1
@@ -469,146 +457,48 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename
                     for (int j = 0; j < kInMax; ++j) sm.X[j * TM + s] = o[j];
                 }
                 __syncthreads();
-                {
-                    float x[kInMax];
-#pragma unroll
-                    for (int j = 0; j < kInMax; ++j) x[j] = sm.X[j * TM + s];
-                    layer1_to_smem<ACT, 1>(sm.net, g.actor.act, x, c, s, sm.T);
-                }
-                wg::fence_proxy_async();
-                __syncthreads();
-                gemm_block(sm.T + c * BLK, sm.net, c);   // warpgroup c: samples 64c .. 64c+63
-                __syncthreads();
-                {
-                    float zp[kOutMax];
-                    head_partials<ACT, 1>(sm.net, g.actor.act, c, s, sm.T, zp);
-#pragma unroll
-                    for (int o = 0; o < kOutMax; ++o) sm.Zp[(c * kOutMax + o) * TM + s] = zp[o];
-                }
-                __syncthreads();   // (the next pass's X / tile image writes are ordered behind these reads by its first barrier)
+                tile_forward<ACT, 1>(sm.net, g.actor.act, c, s, sm.T, sm.X, sm.Zp);
                 const int64_t i = (base + (int64_t)k * nctas) * TM + s;
                 if (owner && i < N) {
                     EvalSlot<Env>& sl = sm.slot[k];
                     float z[kOutMax];
-#pragma unroll
-                    for (int o = 0; o < kOutMax; ++o) z[o] = sm.net.b3[o] + sm.Zp[o * TM + s] + sm.Zp[(kOutMax + o) * TM + s];
+                    tile_heads(sm.net, sm.Zp, s, z);
                     if (DUEL) duel::combine(z, g.actor.nout);
                     uint32_t a_bits;
                     if (MODE == 0) {
                         a_bits = greedy::greedy_action(g.actor, z);
                     } else {
-                        unsigned long long pr[4] = {sl.prng[s], sl.prng[TM + s], sl.prng[2 * TM + s], sl.prng[3 * TM + s]};
+                        unsigned long long pr[4];
+                        get_stream(sl.prng, s, pr);
                         float lp;
                         a_bits = sample_head(g.actor, g.hp, z, pr, lp);
-                        sl.prng[s] = pr[0]; sl.prng[TM + s] = pr[1]; sl.prng[2 * TM + s] = pr[2]; sl.prng[3 * TM + s] = pr[3];
+                        put_stream(sl.prng, s, pr);
                     }
-                    // act!(env, a) + fused soft reset: the sequence of env_step_kernel<Env, false, true> (and rollout_tc_kernel)
-                    act_t act;
-                    if (std::is_same<act_t, float>::value) act = (act_t)fminf(fmaxf(__uint_as_float(a_bits), g.act_lo), g.act_hi);
-                    else act = (act_t)(int32_t)a_bits;
-                    typename Env::S st = sl.st[s];
-                    int tt = sl.t[s];
-                    const int prev = sl.flags[s];
-                    bool done;
-                    float rew;
-                    Env::step(p, st, tt, act, done, rew);
-                    if (ea.max_timeout > 0 && tt + 1 > ea.max_timeout) done = true;
-                    float ret = sl.ep_ret[s] + rew;
-                    int f = done ? 1 : 0;
-                    if (done && !((prev & 1) && !(prev & 2))) { sm.fin_cnt[s] += 1; sm.fin_ret[s] += ret; sm.fin_len[s] += tt; }
-                    if (done) {
+                    const ActStep<float> r = slot_act(sl, s, p, ea.max_timeout, env_action<Env>(a_bits), sm.fin_cnt[s], sm.fin_ret[s], sm.fin_len[s]);
+                    if (r.done) {
                         const int e = sl.cnt[s];   // record of the episode that ends: its return and env.t
                         if (e < g.K) {
-                            if (g.returns) g.returns[(size_t)g.K * i + e] = ret;
-                            if (g.lengths) g.lengths[(size_t)g.K * i + e] = tt;
+                            if (g.returns) g.returns[(size_t)g.K * i + e] = r.ret;
+                            if (g.lengths) g.lengths[(size_t)g.K * i + e] = r.len;
                         }
                         sl.cnt[s] = e + 1;
-                        ret = 0.f;
-                        Xo ex{sl.erng[s], sl.erng[TM + s], sl.erng[2 * TM + s], sl.erng[3 * TM + s]};
-                        Env::reset(p, st, ex, act);
-                        sl.erng[s] = ex.s0; sl.erng[TM + s] = ex.s1; sl.erng[2 * TM + s] = ex.s2; sl.erng[3 * TM + s] = ex.s3;
-                        tt = 0;
-                        f = 3;
                     }
-                    sl.st[s] = st; sl.t[s] = tt; sl.flags[s] = f; sl.ep_ret[s] = ret;
-                    sl.last_rew[s] = rew;
-                    { act_t tmp = act; uint32_t bits; memcpy(&bits, &tmp, 4); sl.last_act[s] = bits; }
                 }
             }
         }
-        // ---- write the group back (each owner thread touches only its own entries: no barrier before the next group's loads)
-        if (owner) {
-            for (int k = 0; k < nslots; ++k) {
-                const int64_t i = (base + (int64_t)k * nctas) * TM + s;
-                EvalSlot<Env>& sl = sm.slot[k];
-                if (i < N) {
-                    Env::store(ea.state, i, sl.st[s]);
-                    if (!Env::kObsIsState) Env::write_obs(ea.obs, i, N, sl.st[s]);
-                    ea.t[i] = sl.t[s];
-                    ea.flags[i] = (uint8_t)sl.flags[s];
-                    ea.ep_ret[i] = sl.ep_ret[s];
-                    store_rng(ea.rng, i, Xo{sl.erng[s], sl.erng[TM + s], sl.erng[2 * TM + s], sl.erng[3 * TM + s]});
-                    if (MODE == 1) {
-                        unsigned long long pr[4] = {sl.prng[s], sl.prng[TM + s], sl.prng[2 * TM + s], sl.prng[3 * TM + s]};
-                        store_rng32(g.policy_rng, i, pr);
-                    }
-                    reinterpret_cast<float*>(ea.reward)[i] = sl.last_rew[s];
-                    reinterpret_cast<uint32_t*>(ea.action)[i] = sl.last_act[s];
-                    if (g.counts) g.counts[i] = sl.cnt[s];
+        // (each owner thread touches only its own entries: no barrier before the next group's loads)
+        if (owner)
+            store_group(sm.slot, nslots, base, nctas, ea, N, s, g.nsteps > 0, [&](const EvalSlot<Env>& sl, int64_t i) {
+                if (MODE == 1) {
+                    unsigned long long pr[4];
+                    get_stream(sl.prng, s, pr);
+                    store_rng32(g.policy_rng, i, pr);
                 }
-            }
-        }
+                if (g.counts) g.counts[i] = sl.cnt[s];
+            });
     }
-    // episode statistics: one atomicAdd triple per CTA
-    {
-        int fin_cnt = owner ? sm.fin_cnt[s] : 0, fin_len = owner ? sm.fin_len[s] : 0;
-        float fin_ret = owner ? sm.fin_ret[s] : 0.f;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            fin_cnt += __shfl_xor_sync(0xffffffffu, fin_cnt, o);
-            fin_len += __shfl_xor_sync(0xffffffffu, fin_len, o);
-            fin_ret += __shfl_xor_sync(0xffffffffu, fin_ret, o);
-        }
-        __syncthreads();
-        if (lane == 0) { sm.red_i[warp] = fin_cnt; sm.red_f[warp] = fin_ret; sm.red_l[warp] = fin_len; }
-        __syncthreads();
-        if (tid == 0) {
-            double cc = 0, rr = 0, ll = 0;
-            for (int w = 0; w < NT / 32; ++w) { cc += sm.red_i[w]; rr += sm.red_f[w]; ll += sm.red_l[w]; }
-            if (cc > 0) { atomicAdd(&ea.stats[0], cc); atomicAdd(&ea.stats[1], rr); atomicAdd(&ea.stats[2], ll); }
-        }
-    }
+    cta_episode_stats(ea.stats, owner ? sm.fin_cnt[s] : 0, owner ? sm.fin_ret[s] : 0.f, owner ? sm.fin_len[s] : 0, sm.red);
 }
-
-template <class Env> int launch_evaluate(b200rl_ctx* ctx, const EvalArgs& g, const typename Env::P& p, const EnvArrays& ea, int mode) {
-    const size_t smem = sizeof(SmemEval<Env>) + 128;
-    static unsigned long long attr_devices = 0;   // once per device
-    if (first_use_on_device(attr_devices, ctx->device)) {
-        CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_RELU, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_TANH, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_RELU, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_TANH, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_RELU, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(evaluate_tc_kernel<Env, B200RL_ACT_TANH, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    }
-    const int64_t groups = ((g.N + TM - 1) / TM + kSlots - 1) / kSlots;
-    int grid = 2 * ctx->sm_count;
-    if ((int64_t)grid > groups) grid = (int)groups;
-    const bool relu = g.actor.act == B200RL_ACT_RELU;
-    if (mode == 0 && g.actor.duel) {
-        if (relu) evaluate_tc_kernel<Env, B200RL_ACT_RELU, 0, true><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
-        else evaluate_tc_kernel<Env, B200RL_ACT_TANH, 0, true><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
-    } else if (mode == 0) {
-        if (relu) evaluate_tc_kernel<Env, B200RL_ACT_RELU, 0><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
-        else evaluate_tc_kernel<Env, B200RL_ACT_TANH, 0><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
-    } else {
-        if (relu) evaluate_tc_kernel<Env, B200RL_ACT_RELU, 1><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
-        else evaluate_tc_kernel<Env, B200RL_ACT_TANH, 1><<<grid, NT, smem, ctx->stream>>>(g, p, ea);
-    }
-    LAUNCH_CHECK(ctx);
-    return B200RL_OK;
-}
-
 
 // ---------------------------------------------------------------------------------------------------------------------
 // fused DQN collect (b200rl_replay_run): nsteps x { obs -> Q -> BatchExplorer column (explore.cuh) | findmax (GreedyExplorer) ->
@@ -619,17 +509,10 @@ template <class Env> int launch_evaluate(b200rl_ctx* ctx, const EvalArgs& g, con
 // contiguous run mod cap + 1, at most cap + 1 of them, no duplicates — and the caller rebuilds the tree once from the children,
 // which gives the tree the per-step rebuilds give.  The head outputs are those of nn_mlp_forward's tensor-core path (see
 // evaluate_tc_kernel), so the actions equal the staged q_explore / q_act selection bit for bit.
-template <class Env> struct ReplaySlot {
-    typename Env::S st[TM];
-    int t[TM];
-    int flags[TM];
-    float ep_ret[TM];
-    float last_rew[TM];
-    int32_t last_act[TM];
+template <class Env> struct ReplaySlot : EnvSlot<Env> {
     int p0[TM];                            // slot of the first touched leaf of the lane (head - 1 at the start)
     int adv[TM];                           // frames written in the window
-    unsigned long long erng[4 * TM];       // env stream      [word][env]
-    unsigned long long xrng[4 * TM];       // explorer stream [word][env]
+    unsigned long long xrng[4 * TM];       // explorer stream
 };
 template <class Env> struct SmemReplay {
     alignas(128) uint8_t T[TILE_BYTES];
@@ -640,9 +523,8 @@ template <class Env> struct SmemReplay {
     int fin_cnt[TM], fin_len[TM];
     float fin_ret[TM];
     long long dv[TM];                      // change of the sampleable count, per owner thread
-    float red_f[8];
-    int red_i[8], red_l[8];
-    long long red_v[8];
+    StatsScratch<NT / 32> red;
+    long long red_dv[NT / 32];
 };
 // b200rl_explorer without its trailing beta, which the kernel takes as its last parameter: the parameters the ϵ-greedy
 // instantiations read keep the offsets they had before the explorer struct grew
@@ -673,7 +555,6 @@ struct ReplayArgs {
 // instantiations without it compile the ϵ-greedy kinds 0 / 1 only.
 template <class Env, int ACT, bool DUEL = false, bool XEXT = false>
 __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, typename Env::P p, EnvArrays ea, double beta) {
-    using act_t = typename Env::act_t;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     SmemReplay<Env>& sm = *reinterpret_cast<SmemReplay<Env>*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -690,10 +571,9 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
     if (owner) { sm.fin_cnt[s] = 0; sm.fin_len[s] = 0; sm.fin_ret[s] = 0.f; sm.dv[s] = 0; }
 #pragma unroll 1
     for (int64_t base = blockIdx.x; base < ntiles; base += (int64_t)nctas * kSlots) {
-        int nslots = 0;
-        for (int k = 0; k < kSlots; ++k)
-            if (base + (int64_t)k * nctas < ntiles) nslots = k + 1;
-        if (owner) {
+        const int nslots = group_slots(base, nctas, ntiles);
+        // (the load of load_group written out: through load_group, ptxas spills 8 / 20 B in the Pendulum dueling relu instantiation)
+        if (owner)
             for (int k = 0; k < nslots; ++k) {
                 const int64_t i = (base + (int64_t)k * nctas) * TM + s;
                 ReplaySlot<Env>& sl = sm.slot[k];
@@ -713,7 +593,6 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
                     }
                 }
             }
-        }
         wg::fence_proxy_async();
         __syncthreads();
 #pragma unroll 1
@@ -727,29 +606,12 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
                     for (int j = 0; j < kInMax; ++j) sm.X[j * TM + s] = o[j];
                 }
                 __syncthreads();
-                {
-                    float x[kInMax];
-#pragma unroll
-                    for (int j = 0; j < kInMax; ++j) x[j] = sm.X[j * TM + s];
-                    layer1_to_smem<ACT, 1>(sm.net, g.q.act, x, c, s, sm.T);
-                }
-                wg::fence_proxy_async();
-                __syncthreads();
-                gemm_block(sm.T + c * BLK, sm.net, c);
-                __syncthreads();
-                {
-                    float zp[kOutMax];
-                    head_partials<ACT, 1>(sm.net, g.q.act, c, s, sm.T, zp);
-#pragma unroll
-                    for (int o = 0; o < kOutMax; ++o) sm.Zp[(c * kOutMax + o) * TM + s] = zp[o];
-                }
-                __syncthreads();
+                tile_forward<ACT, 1>(sm.net, g.q.act, c, s, sm.T, sm.X, sm.Zp);
                 const int64_t i = (base + (int64_t)k * nctas) * TM + s;
                 if (owner && i < N) {
                     ReplaySlot<Env>& sl = sm.slot[k];
                     float z[kOutMax];
-#pragma unroll
-                    for (int o = 0; o < kOutMax; ++o) z[o] = sm.net.b3[o] + sm.Zp[o * TM + s] + sm.Zp[(kOutMax + o) * TM + s];
+                    tile_heads(sm.net, sm.Zp, s, z);
                     if (DUEL) duel::combine(z, g.q.nout);
                     int a1;
                     if (g.greedy) {
@@ -757,7 +619,8 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
                         for (int o = 1; o < g.q.nout; ++o) if (z[o] > z[best]) best = o;
                         a1 = best + 1;
                     } else {
-                        unsigned long long xr[4] = {sl.xrng[s], sl.xrng[TM + s], sl.xrng[2 * TM + s], sl.xrng[3 * TM + s]};
+                        unsigned long long xr[4];
+                        get_stream(sl.xrng, s, xr);
                         if constexpr (XEXT) {
                             const b200rl_explorer ex{g.ex.eps_stable, g.ex.eps_init, g.ex.warmup_steps, g.ex.decay_steps, g.ex.step, g.ex.kind,
                                                      g.ex.is_break_tie, beta};
@@ -765,125 +628,95 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
                         } else {
                             a1 = explore::select<false>(g.ex, step0 + (long long)step * N + i, z, g.q.nout, xr);
                         }
-                        sl.xrng[s] = xr[0]; sl.xrng[TM + s] = xr[1]; sl.xrng[2 * TM + s] = xr[2]; sl.xrng[3 * TM + s] = xr[3];
+                        put_stream(sl.xrng, s, xr);
                     }
-                    // act!(env, a) + fused auto-reset: the sequence of env_step_kernel<Env, false, true>
-                    act_t act = (act_t)a1;
-                    typename Env::S st = sl.st[s];
-                    int tt = sl.t[s];
-                    const int prev = sl.flags[s];
-                    bool done;
-                    float rew;
-                    Env::step(p, st, tt, act, done, rew);
-                    if (ea.max_timeout > 0 && tt + 1 > ea.max_timeout) done = true;
-                    float ret = sl.ep_ret[s] + rew;
-                    int f = done ? 1 : 0;
-                    if (done && !((prev & 1) && !(prev & 2))) { sm.fin_cnt[s] += 1; sm.fin_ret[s] += ret; sm.fin_len[s] += tt; }
-                    if (done) {
-                        ret = 0.f;
-                        Xo ex{sl.erng[s], sl.erng[TM + s], sl.erng[2 * TM + s], sl.erng[3 * TM + s]};
-                        Env::reset(p, st, ex, act);
-                        sl.erng[s] = ex.s0; sl.erng[TM + s] = ex.s1; sl.erng[2 * TM + s] = ex.s2; sl.erng[3 * TM + s] = ex.s3;
-                        tt = 0;
-                        f = 3;
-                    }
-                    sl.st[s] = st; sl.t[s] = tt; sl.flags[s] = f; sl.ep_ret[s] = ret;
-                    sl.last_rew[s] = rew;
-                    sl.last_act[s] = (int32_t)act;
-                    // push!(trajectory, (state = s', action, reward, terminal)) of lane i
+                    const ActStep<float> res = slot_act(sl, s, p, ea.max_timeout, (typename Env::act_t)a1, sm.fin_cnt[s], sm.fin_ret[s], sm.fin_len[s]);
+                    // push!(trajectory, (state = s', action = env.action, reward, terminal)) of lane i
                     float nobs[kInMax];
-                    Env::observe(st, nobs);
+                    Env::observe(sl.st[s], nobs);
                     RingLeaves lv;
                     int adv = 0;
-                    sm.dv[s] += ring::push_sart(r, i, (int32_t)act, rew, (uint8_t)f, nobs, g.default_priority, lv, &adv);
+                    sm.dv[s] += ring::push_sart(r, i, (int32_t)sl.last_act[s], res.rew, (uint8_t)sl.flags[s], nobs, g.default_priority, lv, &adv);
                     sl.adv[s] += adv;
                     if (g.prioritized)
                         for (int j = 0; j < 3; ++j) if (lv.key[j] >= 0) r.tree[r.L + lv.key[j]] = lv.val[j];
                 }
             }
         }
-        if (owner) {
-            for (int k = 0; k < nslots; ++k) {
-                const int64_t i = (base + (int64_t)k * nctas) * TM + s;
-                ReplaySlot<Env>& sl = sm.slot[k];
-                if (i < N) {
-                    Env::store(ea.state, i, sl.st[s]);
-                    if (!Env::kObsIsState) Env::write_obs(ea.obs, i, N, sl.st[s]);
-                    ea.t[i] = sl.t[s];
-                    ea.flags[i] = (uint8_t)sl.flags[s];
-                    ea.ep_ret[i] = sl.ep_ret[s];
-                    store_rng(ea.rng, i, Xo{sl.erng[s], sl.erng[TM + s], sl.erng[2 * TM + s], sl.erng[3 * TM + s]});
-                    if (!g.greedy) {
-                        unsigned long long xr[4] = {sl.xrng[s], sl.xrng[TM + s], sl.xrng[2 * TM + s], sl.xrng[3 * TM + s]};
-                        store_rng32(g.xrng, i, xr);
-                    }
-                    if (g.nsteps > 0) {
-                        reinterpret_cast<float*>(ea.reward)[i] = sl.last_rew[s];
-                        reinterpret_cast<int32_t*>(ea.action)[i] = sl.last_act[s];
-                    }
-                    if (g.prioritized) {   // the lane's touched slots p0, p0 + 1, ... (mod cap + 1), one key each
-                        const int n_touched = (int)min((int64_t)sl.adv[s] + 1, F);
-                        for (int j = 0; j < g.stride; ++j) {
-                            int64_t key = -1;
-                            float v = 0.f;
-                            if (j < n_touched) { key = (((int64_t)sl.p0[s] + j) % F) * r.lanes + i; v = r.tree[r.L + key]; }
-                            g.keys[(int64_t)j * N + i] = key;
-                            g.vals[(int64_t)j * N + i] = v;
-                        }
+        if (owner)
+            store_group(sm.slot, nslots, base, nctas, ea, N, s, g.nsteps > 0, [&](const ReplaySlot<Env>& sl, int64_t i) {
+                if (!g.greedy) {
+                    unsigned long long xr[4];
+                    get_stream(sl.xrng, s, xr);
+                    store_rng32(g.xrng, i, xr);
+                }
+                if (g.prioritized) {   // the lane's touched slots p0, p0 + 1, ... (mod cap + 1), one key each
+                    const int n_touched = (int)min((int64_t)sl.adv[s] + 1, F);
+                    for (int j = 0; j < g.stride; ++j) {
+                        int64_t key = -1;
+                        float v = 0.f;
+                        if (j < n_touched) { key = (((int64_t)sl.p0[s] + j) % F) * r.lanes + i; v = r.tree[r.L + key]; }
+                        g.keys[(int64_t)j * N + i] = key;
+                        g.vals[(int64_t)j * N + i] = v;
                     }
                 }
-            }
-        }
+            });
     }
     // episode statistics and the sampleable count: one atomic each per CTA
-    {
-        int fin_cnt = owner ? sm.fin_cnt[s] : 0, fin_len = owner ? sm.fin_len[s] : 0;
-        float fin_ret = owner ? sm.fin_ret[s] : 0.f;
-        long long dv = owner ? sm.dv[s] : 0;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            fin_cnt += __shfl_xor_sync(0xffffffffu, fin_cnt, o);
-            fin_len += __shfl_xor_sync(0xffffffffu, fin_len, o);
-            fin_ret += __shfl_xor_sync(0xffffffffu, fin_ret, o);
-            dv += __shfl_xor_sync(0xffffffffu, dv, o);
-        }
-        __syncthreads();
-        if (lane == 0) { sm.red_i[warp] = fin_cnt; sm.red_f[warp] = fin_ret; sm.red_l[warp] = fin_len; sm.red_v[warp] = dv; }
-        __syncthreads();
-        if (tid == 0) {
-            double cc = 0, rr = 0, ll = 0;
-            long long vv = 0;
-            for (int w = 0; w < NT / 32; ++w) { cc += sm.red_i[w]; rr += sm.red_f[w]; ll += sm.red_l[w]; vv += sm.red_v[w]; }
-            if (cc > 0) { atomicAdd(&ea.stats[0], cc); atomicAdd(&ea.stats[1], rr); atomicAdd(&ea.stats[2], ll); }
-            if (vv != 0) atomicAdd((unsigned long long*)r.n_valid, (unsigned long long)vv);
-        }
-    }
+    cta_episode_stats(ea.stats, owner ? sm.fin_cnt[s] : 0, owner ? sm.fin_ret[s] : 0.f, owner ? sm.fin_len[s] : 0, sm.red,
+                      owner ? sm.dv[s] : 0, sm.red_dv, (unsigned long long*)r.n_valid);
 }
 
-template <class Env, bool XEXT> int launch_replay_collect_x(b200rl_ctx* ctx, const ReplayArgs& g, const typename Env::P& p, const EnvArrays& ea,
-                                                           double beta) {
-    const size_t smem = sizeof(SmemReplay<Env>) + 128;
-    static unsigned long long attr_devices = 0;   // once per device (and per XEXT)
-    if (first_use_on_device(attr_devices, ctx->device)) {
-        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_RELU, false, XEXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_TANH, false, XEXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_RELU, true, XEXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(replay_collect_tc_kernel<Env, B200RL_ACT_TANH, true, XEXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    }
-    const int64_t groups = ((g.N + TM - 1) / TM + kSlots - 1) / kSlots;
+// ---------------------------------------------------------------------------------------------------------------------
+// host side of the fused kernels
+// Launches `kernel` on min(2 per SM, units) CTAs of NT threads with sizeof(Smem) of dynamic shared memory; the instantiation's
+// shared-memory limit is raised on its first launch on a device (the attribute call is not free and may serialise with running kernels).
+template <auto kernel, class Smem, class... Args> int launch_fused(b200rl_ctx* ctx, int64_t units, const Args&... args) {
+    const size_t smem = sizeof(Smem) + 128;
+    static unsigned long long attr_devices = 0;
+    if (first_use_on_device(attr_devices, ctx->device))
+        CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int grid = 2 * ctx->sm_count;
-    if ((int64_t)grid > groups) grid = (int)groups;
-    if (g.q.duel) {
-        if (g.q.act == B200RL_ACT_RELU) replay_collect_tc_kernel<Env, B200RL_ACT_RELU, true, XEXT><<<grid, NT, smem, ctx->stream>>>(g, p, ea, beta);
-        else replay_collect_tc_kernel<Env, B200RL_ACT_TANH, true, XEXT><<<grid, NT, smem, ctx->stream>>>(g, p, ea, beta);
-    } else if (g.q.act == B200RL_ACT_RELU) replay_collect_tc_kernel<Env, B200RL_ACT_RELU, false, XEXT><<<grid, NT, smem, ctx->stream>>>(g, p, ea, beta);
-    else replay_collect_tc_kernel<Env, B200RL_ACT_TANH, false, XEXT><<<grid, NT, smem, ctx->stream>>>(g, p, ea, beta);
+    if ((int64_t)grid > units) grid = (int)units;
+    kernel<<<grid, NT, smem, ctx->stream>>>(args...);
     LAUNCH_CHECK(ctx);
     return B200RL_OK;
 }
-template <class Env> int launch_replay_collect(b200rl_ctx* ctx, const ReplayArgs& g, const typename Env::P& p, const EnvArrays& ea, double beta) {
-    if (!g.greedy && g.ex.kind >= 2) return launch_replay_collect_x<Env, true>(ctx, g, p, ea, beta);
-    return launch_replay_collect_x<Env, false>(ctx, g, p, ea, 0.0);
+
+template <class Env> struct EnvTag { using type = Env; };
+// Calls f(EnvTag<Env>{}, params) with the Float32 device env type of the handle and its parameters (a continuous variant reads the
+// parameter block of its discrete kind, which has the same layout).  The caller has checked v.dtype == B200RL_F32.
+template <class F> int with_f32_env(const EnvView& v, F&& f) {
+    switch (v.kind) {
+        case B200RL_ENV_CARTPOLE: {
+            if (!v.continuous) return f(EnvTag<CartPoleD<float, false>>{}, v.p.cp32);
+            CartPoleD<float, true>::P q;
+            static_assert(sizeof q == sizeof v.p.cp32, "same params layout");
+            memcpy(&q, &v.p.cp32, sizeof q);
+            return f(EnvTag<CartPoleD<float, true>>{}, q);
+        }
+        case B200RL_ENV_PENDULUM:
+            return v.continuous ? f(EnvTag<PendulumD<true>>{}, v.p.pend) : f(EnvTag<PendulumD<false>>{}, v.p.pend);
+        case B200RL_ENV_MOUNTAINCAR: {
+            if (!v.continuous) return f(EnvTag<MountainCarD<false>>{}, v.p.mc);
+            MountainCarD<true>::P q;
+            static_assert(sizeof q == sizeof v.p.mc, "same params layout");
+            memcpy(&q, &v.p.mc, sizeof q);
+            return f(EnvTag<MountainCarD<true>>{}, q);
+        }
+    }
+    return B200RL_ERR_UNSUPPORTED;
+}
+
+template <class Env, bool XEXT>
+int launch_replay_collect(b200rl_ctx* ctx, int64_t groups, const ReplayArgs& g, const typename Env::P& p, const EnvArrays& ea, double beta) {
+    constexpr int RELU = B200RL_ACT_RELU, TANH = B200RL_ACT_TANH;
+    const bool relu = g.q.act == RELU;
+    if (g.q.duel)
+        return relu ? launch_fused<replay_collect_tc_kernel<Env, RELU, true, XEXT>, SmemReplay<Env>>(ctx, groups, g, p, ea, beta)
+                    : launch_fused<replay_collect_tc_kernel<Env, TANH, true, XEXT>, SmemReplay<Env>>(ctx, groups, g, p, ea, beta);
+    return relu ? launch_fused<replay_collect_tc_kernel<Env, RELU, false, XEXT>, SmemReplay<Env>>(ctx, groups, g, p, ea, beta)
+                : launch_fused<replay_collect_tc_kernel<Env, TANH, false, XEXT>, SmemReplay<Env>>(ctx, groups, g, p, ea, beta);
 }
 
 }  // namespace
@@ -924,39 +757,14 @@ int nn_tc_rollout(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const 
     const int64_t ntiles = (v.N + TM - 1) / TM;
     if (ntiles > (int64_t)kSlots * 2 * ctx->sm_count) return B200RL_ERR_UNSUPPORTED;
     if ((actor.heads2 != 0) != (v.continuous != 0)) return B200RL_ERR_UNSUPPORTED;   // Gaussian head <-> continuous action space
-    RollArgs g{actor, critic, params, hp, v.N, t0, nsteps, T, final_bootstrap, -1.0f, 1.0f, policy_rng, states, actions, logp, values, rewards, terminals};
-    int st = B200RL_ERR_UNSUPPORTED;
-    switch (v.kind) {
-        case B200RL_ENV_CARTPOLE:
-            if (v.continuous) {
-                CartPoleD<float, true>::P q;
-                memcpy(&q, &v.p.cp32, sizeof q);
-                st = launch_rollout<CartPoleD<float, true>>(ctx, g, q, v.a);
-            } else {
-                if (actor.nout != 2) return B200RL_ERR_UNSUPPORTED;
-                st = launch_rollout<CartPoleD<float, false>>(ctx, g, v.p.cp32, v.a);
-            }
-            break;
-        case B200RL_ENV_PENDULUM:
-            if (v.continuous) {
-                g.act_lo = -2.0f; g.act_hi = 2.0f;      // PendulumEnv.jl:73: action_space -2.0..2.0
-                st = launch_rollout<PendulumD<true>>(ctx, g, v.p.pend, v.a);
-            } else {
-                if (actor.nout != v.p.pend.n_actions) return B200RL_ERR_UNSUPPORTED;
-                st = launch_rollout<PendulumD<false>>(ctx, g, v.p.pend, v.a);
-            }
-            break;
-        case B200RL_ENV_MOUNTAINCAR:
-            if (v.continuous) {
-                MountainCarD<true>::P q;
-                memcpy(&q, &v.p.mc, sizeof q);
-                st = launch_rollout<MountainCarD<true>>(ctx, g, q, v.a);
-            } else {
-                if (actor.nout != 3) return B200RL_ERR_UNSUPPORTED;
-                st = launch_rollout<MountainCarD<false>>(ctx, g, v.p.mc, v.a);
-            }
-            break;
-    }
+    if (!v.continuous && actor.nout != b200rl_env_internal_n_actions(env)) return B200RL_ERR_UNSUPPORTED;
+    const RollArgs g{actor, critic, params, hp, v.N, t0, nsteps, T, final_bootstrap, policy_rng, states, actions, logp, values, rewards, terminals};
+    const int st = with_f32_env(v, [&](auto env_type, const auto& p) {
+        using Env = typename decltype(env_type)::type;
+        // the activation is a template parameter (both trunks share it, checked above)
+        return actor.act == B200RL_ACT_RELU ? launch_fused<rollout_tc_kernel<Env, B200RL_ACT_RELU>, SmemRoll<Env>>(ctx, ntiles, g, p, v.a)
+                                            : launch_fused<rollout_tc_kernel<Env, B200RL_ACT_TANH>, SmemRoll<Env>>(ctx, ntiles, g, p, v.a);
+    });
     if (st == B200RL_OK) b200rl_env_internal_add_steps(env, (uint64_t)nsteps);
     return st;
 }
@@ -968,36 +776,21 @@ int nn_tc_evaluate(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const
     EnvView v;
     TRY(b200rl_env_internal_view(env, &v));
     if (!nn_tc_supported(actor) || v.dtype != B200RL_F32) return B200RL_ERR_UNSUPPORTED;
-    EvalArgs g{actor, params, hp, v.N, nsteps, K, -1.0f, 1.0f, policy_rng, returns, lengths, counts};
-    int st = B200RL_ERR_UNSUPPORTED;
-    switch (v.kind) {
-        case B200RL_ENV_CARTPOLE:
-            if (v.continuous) {
-                CartPoleD<float, true>::P q;
-                memcpy(&q, &v.p.cp32, sizeof q);
-                st = launch_evaluate<CartPoleD<float, true>>(ctx, g, q, v.a, mode);
-            } else {
-                st = launch_evaluate<CartPoleD<float, false>>(ctx, g, v.p.cp32, v.a, mode);
-            }
-            break;
-        case B200RL_ENV_PENDULUM:
-            if (v.continuous) {
-                g.act_lo = -2.0f; g.act_hi = 2.0f;      // PendulumEnv.jl:73: action_space -2.0..2.0
-                st = launch_evaluate<PendulumD<true>>(ctx, g, v.p.pend, v.a, mode);
-            } else {
-                st = launch_evaluate<PendulumD<false>>(ctx, g, v.p.pend, v.a, mode);
-            }
-            break;
-        case B200RL_ENV_MOUNTAINCAR:
-            if (v.continuous) {
-                MountainCarD<true>::P q;
-                memcpy(&q, &v.p.mc, sizeof q);
-                st = launch_evaluate<MountainCarD<true>>(ctx, g, q, v.a, mode);
-            } else {
-                st = launch_evaluate<MountainCarD<false>>(ctx, g, v.p.mc, v.a, mode);
-            }
-            break;
-    }
+    const EvalArgs g{actor, params, hp, v.N, nsteps, K, policy_rng, returns, lengths, counts};
+    const int64_t groups = ((v.N + TM - 1) / TM + kSlots - 1) / kSlots;
+    const int st = with_f32_env(v, [&](auto env_type, const auto& p) {
+        using Env = typename decltype(env_type)::type;
+        constexpr int RELU = B200RL_ACT_RELU, TANH = B200RL_ACT_TANH;
+        const bool relu = actor.act == RELU;
+        if (mode == 0 && actor.duel)
+            return relu ? launch_fused<evaluate_tc_kernel<Env, RELU, 0, true>, SmemEval<Env>>(ctx, groups, g, p, v.a)
+                        : launch_fused<evaluate_tc_kernel<Env, TANH, 0, true>, SmemEval<Env>>(ctx, groups, g, p, v.a);
+        if (mode == 0)
+            return relu ? launch_fused<evaluate_tc_kernel<Env, RELU, 0>, SmemEval<Env>>(ctx, groups, g, p, v.a)
+                        : launch_fused<evaluate_tc_kernel<Env, TANH, 0>, SmemEval<Env>>(ctx, groups, g, p, v.a);
+        return relu ? launch_fused<evaluate_tc_kernel<Env, RELU, 1>, SmemEval<Env>>(ctx, groups, g, p, v.a)
+                    : launch_fused<evaluate_tc_kernel<Env, TANH, 1>, SmemEval<Env>>(ctx, groups, g, p, v.a);
+    });
     if (st == B200RL_OK) b200rl_env_internal_add_steps(env, (uint64_t)nsteps);
     return st;
 }
@@ -1011,14 +804,15 @@ int nn_tc_replay_collect(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& q, con
     TRY(b200rl_env_internal_view(env, &v));
     if (!nn_tc_supported(q) || v.dtype != B200RL_F32 || v.continuous || ring.ns > kInMax) return B200RL_ERR_UNSUPPORTED;
     const b200rl_explorer e = ex ? *ex : b200rl_explorer{};
-    ReplayArgs g{q, params, v.N, nsteps, ex ? 0 : 1, ReplayExplorer{e.eps_stable, e.eps_init, e.warmup_steps, e.decay_steps, e.step, e.kind, e.is_break_tie},
-                 step_dev, xrng, ring, default_priority, prioritized, keys, vals, stride};
-    int st = B200RL_ERR_UNSUPPORTED;
-    switch (v.kind) {
-        case B200RL_ENV_CARTPOLE: st = launch_replay_collect<CartPoleD<float, false>>(ctx, g, v.p.cp32, v.a, e.beta); break;
-        case B200RL_ENV_PENDULUM: st = launch_replay_collect<PendulumD<false>>(ctx, g, v.p.pend, v.a, e.beta); break;
-        case B200RL_ENV_MOUNTAINCAR: st = launch_replay_collect<MountainCarD<false>>(ctx, g, v.p.mc, v.a, e.beta); break;
-    }
+    const ReplayArgs g{q, params, v.N, nsteps, ex ? 0 : 1, ReplayExplorer{e.eps_stable, e.eps_init, e.warmup_steps, e.decay_steps, e.step, e.kind, e.is_break_tie},
+                       step_dev, xrng, ring, default_priority, prioritized, keys, vals, stride};
+    const int64_t groups = ((v.N + TM - 1) / TM + kSlots - 1) / kSlots;
+    const int st = with_f32_env(v, [&](auto env_type, const auto& p) {
+        using Env = typename decltype(env_type)::type;
+        if constexpr (std::is_floating_point<typename Env::act_t>::value) return (int)B200RL_ERR_UNSUPPORTED;   // (rejected above)
+        else if (!g.greedy && g.ex.kind >= 2) return launch_replay_collect<Env, true>(ctx, groups, g, p, v.a, e.beta);
+        else return launch_replay_collect<Env, false>(ctx, groups, g, p, v.a, 0.0);
+    });
     if (st == B200RL_OK) b200rl_env_internal_add_steps(env, (uint64_t)nsteps);
     return st;
 }

@@ -1,6 +1,6 @@
 // tests/hostdev/hostdev.cpp — TEST INFRASTRUCTURE.  The product's device headers compiled for the host (see cuda_runtime.h here) behind
-// a flat C interface: Julia math kernels, Xoshiro samplers, env reset!/_step! per env, and the minibatch permutation.  The control flow
-// around the per-env primitives (auto-reset after a terminating step) restates env.cu's step kernel in the obvious serial way.
+// a flat C interface: Julia math kernels, Xoshiro samplers, env reset! and the act! step (auto-reset included) per env, and the
+// minibatch permutation.
 #include <cuda_runtime.h>
 
 #include <vector>
@@ -30,8 +30,8 @@ int64_t hd_rand_oneto(uint64_t* s, uint64_t n) {
 }  // extern "C"
 
 namespace {
-// One env object per index, stepped serially: t += 1 inside Env::step; a terminating step keeps its reward / terminal and (auto-reset)
-// the state becomes the fresh episode's — exactly what the oracle's `step(actions, auto_reset = true)` and the kernel do.
+// One env object per index, stepped serially through the kernels' act! step: a terminating step keeps its reward / terminal and
+// (auto-reset) the state becomes the fresh episode's — what the oracle's `step(actions, auto_reset = true)` does.
 template <class Env>
 void run_env(const typename Env::P& p, int64_t n, int steps, uint64_t* rng, const void* actions, int random_policy, void* state_io,
              typename Env::real* reward_out, uint8_t* terminal_out, int32_t* t_io, void* action_out, int do_reset_first) {
@@ -43,15 +43,14 @@ void run_env(const typename Env::P& p, int64_t n, int steps, uint64_t* rng, cons
         int t = t_io[i];
         act_t last = 0;
         if (do_reset_first) { Env::reset(p, s, g, last); t = 0; }
-        real rew = 0;
-        bool done = false;
+        int flags = 0, fin_cnt = 0, fin_len = 0;
+        float ep_ret = 0.f, fin_ret = 0.f;
         for (int k = 0; k < steps; ++k) {
             act_t a = random_policy ? Env::from_index(p, jld::rand_oneto(g, Env::n_random(p))) : reinterpret_cast<const act_t*>(actions)[(int64_t)k * n + i];
-            Env::step(p, s, t, a, done, rew);
-            last = a;
-            reward_out[(int64_t)k * n + i] = rew;
-            terminal_out[(int64_t)k * n + i] = done ? 1 : 0;
-            if (done) { act_t dummy = 0; Env::reset(p, s, g, dummy); t = 0; }
+            last = a;   // the action taken, not the one a reset redraws
+            const ActStep<real> r = act_step<Env, true>(p, 0, s, t, flags, ep_ret, a, fin_cnt, fin_ret, fin_len, [&](auto&& reset) { reset(g); });
+            reward_out[(int64_t)k * n + i] = r.rew;
+            terminal_out[(int64_t)k * n + i] = r.done ? 1 : 0;
         }
         Env::store(state_io, i, s);
         t_io[i] = t;
