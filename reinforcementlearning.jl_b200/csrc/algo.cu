@@ -12,48 +12,12 @@
 #include <map>
 
 #include "greedy.cuh"
+#include "internal.h"
 #include "nn.cuh"
 #include "replay_schedule.h"
 #include "ring.cuh"
 
-// other translation units
-int b200rl_gae_fused_internal(b200rl_ctx* ctx, float* adv, float* ret, const float* r, const float* v, const uint8_t* term, float gamma,
-                              float lambda, int64_t S, int64_t n_time, double* partials, float* norm2);
-int b200rl_gae_fused_partials_count(int64_t S);
-int b200rl_env_internal_set_traj_targets(b200rl_env* e, void* reward_col, uint8_t* terminal_col);
-int64_t b200rl_env_internal_n(const b200rl_env* e);
-int b200rl_env_internal_kind(const b200rl_env* e);
-int b200rl_env_internal_nobs(const b200rl_env* e);
-b200rl_ctx* b200rl_env_internal_ctx(const b200rl_env* e);
-bool b200rl_env_internal_continuous(const b200rl_env* e);
-struct TrajBatchView { const float* s; const int32_t* a; const float* r; const uint8_t* t; const float* s2; const float* w; int64_t B; int ns; };
-TrajBatchView b200rl_traj_internal_batch(b200rl_traj* t);
-bool b200rl_traj_internal_prioritized(b200rl_traj* t);
-b200rl_ctx* b200rl_traj_internal_ctx(b200rl_traj* t);
-int64_t b200rl_traj_internal_lanes(b200rl_traj* t);
-void b200rl_traj_internal_add_pushed(b200rl_traj* t, int64_t n);
-int64_t b200rl_traj_internal_pushed(b200rl_traj* t);
-Ring b200rl_traj_internal_ring(b200rl_traj* t);
-float b200rl_traj_internal_default_priority(b200rl_traj* t);
-void b200rl_traj_internal_nstep(b200rl_traj* t, int* n, float* gamma);
-const float* b200rl_traj_internal_discount(b200rl_traj* t);
-int b200rl_traj_internal_tree_rebuild(b200rl_traj* t, const int64_t* keys, const float* vals, int64_t n);
-uint64_t b200rl_env_internal_steps(const b200rl_env* e);
-int b200rl_traj_internal_priority_from_td(b200rl_traj* t, const float* td_dev, float eps, float alpha);
-int b200rl_comm_allreduce_internal(b200rl_ctx* ctx, void* buf, int64_t n, int is_double);
-int b200rl_comm_world(b200rl_ctx* ctx);
-int b200rl_env_internal_kind(const b200rl_env* e);
-int b200rl_env_internal_max_timeout(const b200rl_env* e);
-int b200rl_env_internal_dtype(const b200rl_env* e);
-void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n);
-int b200rl_env_internal_n_actions(const b200rl_env* e);
-float b200rl_env_internal_action_bound(const b200rl_env* e);
-static void* env_field(b200rl_env* e, int f);
-static bool fused_rollout_enabled() {   // B200RL_FUSED_ROLLOUT=0: step through plan!/act! launches instead (same results)
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("B200RL_FUSED_ROLLOUT"); v = (e && e[0] == '0') ? 0 : 1; }
-    return v != 0;
-}
+static void* env_field(b200rl_env* e, int f) { void* p = nullptr; b200rl_env_ptr(e, f, &p); return p; }
 
 namespace {
 __global__ void clamp_copy_kernel(float* __restrict__ dst, const float* __restrict__ src, int64_t n, float lo, float hi) {
@@ -162,6 +126,111 @@ struct b200rl_net {
     uint64_t n_updates;
 };
 
+// One optimiser step on the gradient partials of a loss + backward launch: reduce [-> all-reduce over the ranks] ->
+// clip_by_global_norm! -> Adam.  One kernel (nn_reduce_clip_adam) when its CTAs can all be co-resident and the ranks, if any,
+// exchange over the peer memory; the staged kernels otherwise.  stats_row (may be null, and then so is tick): the row {4 loss sums,
+// grad norm} of this step; tick: the device update counter, incremented once by the step.
+static int optimiser_step(b200rl_net* n, int n_partials, int n_loss, float max_grad_norm, float lr, float b1, float b2, float eps,
+                          float* stats_row, unsigned int* tick) {
+    b200rl_ctx* ctx = n->ctx;
+    const int world = b200rl_comm_world(ctx);
+    P2PTable peers;
+    if ((world == 1 || b200rl_comm_p2p_table(ctx, &peers)) && (int)grid_for(n->np, 256) <= ctx->sm_count)
+        return nn_reduce_clip_adam(ctx, n->partial, n_partials, n->np, n->params, n->grad, n->m, n->v, n->beta_t, n->loss_partial, n_loss, n->loss4,
+                                   max_grad_norm, lr, b1, b2, eps, n->gnorm, n->cta_sumsq, n->counter2, stats_row, tick);
+    TRY(nn_reduce_partials(ctx, n->partial, n_partials, n->np, n->grad, n->loss_partial, n_loss, n->loss4));
+    if (world > 1) {
+        TRY(b200rl_comm_allreduce_internal(ctx, n->grad, n->np, 0));
+        TRY(b200rl_comm_allreduce_internal(ctx, n->loss4, 4, 0));
+    }
+    TRY(nn_clip_adam(ctx, n->params, n->grad, n->m, n->v, n->beta_t, n->np, max_grad_norm, lr, b1, b2, eps, 1.0f, n->gnorm));
+    if (stats_row) {
+        stats_row_kernel<<<1, 32, 0, ctx->stream>>>(stats_row, n->loss4, n->gnorm, tick);
+        LAUNCH_CHECK(ctx);
+    }
+    return B200RL_OK;
+}
+
+// ------------------------------------------------------------------ CUDA-graph replay unit --
+// A stretch of launches (the body) that an agent loop runs over and over, replayed as one CUDA graph per unit id.  The first
+// use of an id runs the body eagerly (lazy module loading, function attributes, scratch growth), the second captures it, every
+// later one launches the graph.  Capture does not execute, so the host counters the captured calls advanced are measured,
+// rolled back, and advanced by the same amount on every launch: the host sees what an eager run leaves.  A capture or
+// instantiation that fails switches the unit to eager launches for good.
+struct HostCounters {
+    uint64_t launches, net_updates, env_steps, agent_updates;
+    int64_t pushed;
+    HostCounters operator-(const HostCounters& o) const {
+        return {launches - o.launches, net_updates - o.net_updates, env_steps - o.env_steps, agent_updates - o.agent_updates, pushed - o.pushed};
+    }
+};
+struct CounterSet {   // where a body's host counters live; traj and agent_updates may be null
+    b200rl_ctx* ctx; b200rl_net* net; b200rl_env* env; b200rl_traj* traj; uint64_t* agent_updates;
+    HostCounters read() const {
+        return {ctx->launches, net->n_updates, b200rl_env_internal_steps(env), agent_updates ? *agent_updates : 0,
+                traj ? b200rl_traj_internal_pushed(traj) : 0};
+    }
+    void add(const HostCounters& d) const {
+        ctx->launches += d.launches; net->n_updates += d.net_updates;
+        b200rl_env_internal_add_steps(env, d.env_steps);
+        if (agent_updates) *agent_updates += d.agent_updates;
+        if (traj) b200rl_traj_internal_add_pushed(traj, d.pushed);
+    }
+};
+class GraphUnit {
+    struct Unit { cudaGraphExec_t exec = nullptr; bool warmed = false; HostCounters delta{}; };
+    std::map<int64_t, Unit> units_;
+    std::vector<unsigned char> key_;
+    bool failed_ = false;
+    void drop() {
+        for (auto& kv : units_) if (kv.second.exec) { cudaGraphExecDestroy(kv.second.exec); kv.second.exec = nullptr; }
+    }
+public:
+    ~GraphUnit() { drop(); }
+    bool active() const {
+        for (const auto& kv : units_) if (kv.second.exec) return true;
+        return false;
+    }
+    // what the captured launches bake in besides the handles (compared bytewise): a change re-captures every unit
+    void rekey(const void* key, size_t bytes) {
+        const unsigned char* k = (const unsigned char*)key;
+        if (key_.size() == bytes && memcmp(key_.data(), k, bytes) == 0) return;
+        drop();
+        key_.assign(k, k + bytes);
+    }
+    // capturable = false: run the body eagerly (a measurement run, or launches a graph cannot hold)
+    template <class Body>
+    int run(int64_t id, const CounterSet& cs, bool capturable, Body&& body) {
+        b200rl_ctx* ctx = cs.ctx;
+        Unit& u = units_[id];
+        if (!u.warmed || !capturable || failed_ || ctx->phase_base >= 0) {
+            u.warmed = true;
+            return body();
+        }
+        if (!u.exec) {
+            const HostCounters c0 = cs.read();
+            CUDA_TRY(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
+            const int st = body();
+            cudaGraph_t g = nullptr;
+            const cudaError_t ce = cudaStreamEndCapture(ctx->stream, &g);
+            u.delta = cs.read() - c0;
+            cs.add(c0 - cs.read());
+            cudaError_t ie = cudaErrorUnknown;
+            if (st == B200RL_OK && ce == cudaSuccess && g) ie = cudaGraphInstantiate(&u.exec, g, 0);
+            if (g) cudaGraphDestroy(g);
+            if (ie != cudaSuccess) {
+                cudaGetLastError();
+                u.exec = nullptr;
+                failed_ = true;
+                return body();
+            }
+        }
+        CUDA_TRY(cudaGraphLaunch(u.exec, ctx->stream));
+        cs.add(u.delta);
+        return B200RL_OK;
+    }
+};
+
 // kinds 2 and 3 are Q-networks (one flat vector, a target network, the DQN entry points); 0 and 1 actor-critic pairs
 static bool is_q_kind(int kind) { return kind == 2 || kind == 3; }
 
@@ -216,7 +285,7 @@ int b200rl_net_create(b200rl_ctx* ctx, const b200rl_net_desc* d, const float* pa
     size_t bytes = (size_t)n->np * sizeof(float);
     n->n_partials = is_q_kind(n->kind) ? nn_dqn_max_partials(ctx, n->actor.H) : nn_grid_ctas(ctx, n->actor.H);
     int n_loss_rows = 2 * (n->n_partials > ctx->sm_count ? n->n_partials : ctx->sm_count);
-#define NET_TRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { b200rl_set_error("%s -> %s", #x, cudaGetErrorString(_e)); b200rl_net_destroy(n); return B200RL_ERR_CUDA; } } while (0)
+#define NET_TRY(x) CUDA_TRY_OR(x, b200rl_net_destroy(n))
     NET_TRY(cudaMalloc(&n->params, bytes)); NET_TRY(cudaMalloc(&n->grad, bytes)); NET_TRY(cudaMalloc(&n->m, bytes)); NET_TRY(cudaMalloc(&n->v, bytes));
     NET_TRY(cudaMalloc(&n->beta_t, 2 * sizeof(float)));
     if (is_q_kind(n->kind)) NET_TRY(cudaMalloc(&n->target, bytes));
@@ -310,6 +379,18 @@ int b200rl_net_target_sync(b200rl_net* n, float rho) {
     return nn_target_sync(n->ctx, n->target, n->params, n->np, rho);
 }
 
+// the loss scalars of an agent's config; kSamplerHyper: what plan! outside an agent samples with (b200rl_net_act, b200rl_evaluate)
+static AcHyper ac_hyper(const b200rl_onpolicy_config& c) {
+    return AcHyper{c.clip_range, c.w_actor, c.w_critic, c.w_entropy, c.min_sigma, c.max_sigma, c.normalize_advantage, c.algo};
+}
+static constexpr AcHyper kSamplerHyper{0.1f, 1.f, 0.5f, 0.001f, 0.f, __builtin_inff(), 0, 0};
+// per-minibatch stats row [actor_loss, critic_loss, entropy, loss, grad_norm, 0] from the device row s = {4 loss sums, grad norm}
+static void decode_stats_row(const b200rl_onpolicy_config& c, const float* s, float invB, float* o) {
+    o[0] = s[0] * invB; o[1] = s[2] * invB; o[2] = s[1] * invB;
+    o[3] = c.w_actor * o[0] + c.w_critic * o[1] - c.w_entropy * o[2];
+    o[4] = s[4]; o[5] = 0.f;
+}
+
 static int stage_obs(b200rl_net* n, const float* obs, int64_t N, int on_device, const float** dev, size_t extra, void** extra_dev) {
     size_t ob = (size_t)N * n->actor.in * 4;
     if (on_device && extra == 0) { *dev = obs; return B200RL_OK; }
@@ -327,7 +408,7 @@ int b200rl_net_act(b200rl_net* n, const float* obs, int64_t N, uint64_t* rng_dev
                    float* heads_out, int on_device) {
     REQUIRE(n && obs && rng_dev && !is_q_kind(n->kind), B200RL_ERR_INVALID, "bad argument (actor-critic nets only)");
     TRY(ctx_bind(n->ctx));
-    AcHyper hp{0.1f, 1.f, 0.5f, 0.001f, 0.f, __builtin_inff(), 0, 0};
+    const AcHyper& hp = kSamplerHyper;
     const float* dobs;
     size_t ho = (size_t)N * n->actor.nout * 4;
     void* ex = nullptr;
@@ -463,7 +544,7 @@ int b200rl_evaluate(b200rl_net* n, b200rl_env* env, const b200rl_eval_config* cf
         if (dret && rec_bytes) CUDA_TRY(cudaMemcpyAsync(dret, returns_out, rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
         if (dlen && rec_bytes) CUDA_TRY(cudaMemcpyAsync(dlen, lengths_out, rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
     }
-    AcHyper hp{0.1f, 1.f, 0.5f, 0.001f, 0.f, __builtin_inff(), 0, 0};   // b200rl_net_act's sampler
+    const AcHyper& hp = kSamplerHyper;
     unsigned long long* prng = (unsigned long long*)policy_rng_dev;
     TRY(b200rl_env_reset(env, 1));   // reset!(env; is_force = true), run.jl:46
     int st = nn_tc_enabled() ? nn_tc_evaluate(ctx, env, n->actor, n->params, hp, mode, nsteps, K, prng, dret, dlen, dcnt) : B200RL_ERR_UNSUPPORTED;
@@ -542,7 +623,7 @@ int b200rl_net_ac_step(b200rl_net* n, const b200rl_onpolicy_config* cfg, const f
     float nm[2] = {adv_mean, adv_inv_std};
     CUDA_TRY(cudaMemcpyAsync(base + o_n, nm, 8, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));  // host buffers (incl. the local iota) are borrowed for this call only
-    AcHyper hp{cfg->clip_range, cfg->w_actor, cfg->w_critic, cfg->w_entropy, cfg->min_sigma, cfg->max_sigma, cfg->normalize_advantage, cfg->algo};
+    const AcHyper hp = ac_hyper(*cfg);
     AcBatch b{(const float*)(base + o_s), ns, base + o_a, logp_old ? (const float*)(base + o_l) : nullptr, (const float*)(base + o_ad),
               (const float*)(base + o_r), (const int32_t*)(base + o_i), (uint32_t)total, 0u, 0u, nullptr, nullptr, Beff, 1.0f / (float)Beff,
               (const float*)(base + o_n)};
@@ -554,14 +635,11 @@ int b200rl_net_ac_step(b200rl_net* n, const b200rl_onpolicy_config* cfg, const f
         n->n_updates += 1;
     }
     if (losses_out) {
-        float l4[4], gn = 0.f;
-        CUDA_TRY(cudaMemcpyAsync(l4, n->loss4, 16, cudaMemcpyDeviceToHost, ctx->stream));
-        if (apply_update) CUDA_TRY(cudaMemcpyAsync(&gn, n->gnorm, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        float s[5] = {};   // {4 loss sums, grad norm}
+        CUDA_TRY(cudaMemcpyAsync(s, n->loss4, 16, cudaMemcpyDeviceToHost, ctx->stream));
+        if (apply_update) CUDA_TRY(cudaMemcpyAsync(s + 4, n->gnorm, 4, cudaMemcpyDeviceToHost, ctx->stream));
         CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-        float invB = 1.0f / (float)Beff;
-        losses_out[0] = l4[0] * invB; losses_out[1] = l4[2] * invB; losses_out[2] = l4[1] * invB;
-        losses_out[3] = cfg->w_actor * losses_out[0] + cfg->w_critic * losses_out[1] - cfg->w_entropy * losses_out[2];
-        losses_out[4] = gn; losses_out[5] = 0.f;
+        decode_stats_row(*cfg, s, 1.0f / (float)Beff, losses_out);
     }
     return B200RL_OK;
 }
@@ -587,11 +665,37 @@ struct b200rl_onpolicy {
     float4* rec;                 // packed 32-byte records of the rollout (written after GAE, gathered by K7)
     unsigned int* upd_dev;       // device copy of n_updates: keys the minibatch permutation, ticked by the last optimiser step of an update
     uint64_t n_updates;
-    // CUDA graph of one whole iteration (collect(T) + update) for b200rl_onpolicy_iterate
-    cudaGraph_t graph; cudaGraphExec_t graph_exec; bool warmed; int graph_tc; uint64_t graph_env_gen; uint64_t graph_launches; int graph_failed;
+    GraphUnit graph;             // one whole iteration (collect(T) + update) for b200rl_onpolicy_iterate
 };
 
-static void* env_field(b200rl_env* e, int f) { void* p = nullptr; b200rl_env_ptr(e, f, &p); return p; }
+// the (n_epochs * n_microbatches, 6) stats rows of the last update (synchronises)
+static int read_stats(b200rl_onpolicy* a, float* stats_host) {
+    std::vector<float> tmp((size_t)a->stats_rows * 8);
+    CUDA_TRY(cudaMemcpyAsync(tmp.data(), a->stats_dev, tmp.size() * 4, cudaMemcpyDeviceToHost, a->ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(a->ctx->stream));
+    const float invB = 1.0f / ((float)(a->N * a->T / a->cfg.n_microbatches) * (float)b200rl_comm_world(a->ctx));
+    for (int r = 0; r < a->stats_rows; ++r) decode_stats_row(a->cfg, tmp.data() + (size_t)r * 8, invB, stats_host + (size_t)r * 6);
+    return B200RL_OK;
+}
+
+/* rollout tensors by field id: 0 state (ns, N, T+1) | 1 action (N, T) | 2 logp (N, T) | 3 reward (N, T) | 4 terminal (N, T) u8 |
+ * 5 value (N, T+1) | 6 advantage (N, T) | 7 return (N, T) | 8 policy rng (4, N) u64 | 9 advantage norm {mean, inv_std} */
+static int rollout_field(b200rl_onpolicy* a, int field, void** p, size_t* bytes) {
+    const size_t N = (size_t)a->N, T = (size_t)a->T;
+    switch (field) {
+        case 0: *p = a->states; *bytes = N * a->ns * (T + 1) * 4; return B200RL_OK;
+        case 1: *p = a->actions; *bytes = N * T * 4; return B200RL_OK;
+        case 2: *p = a->logp; *bytes = N * T * 4; return B200RL_OK;
+        case 3: *p = a->rewards; *bytes = N * T * 4; return B200RL_OK;
+        case 4: *p = a->terminals; *bytes = N * T; return B200RL_OK;
+        case 5: *p = a->values; *bytes = N * (T + 1) * 4; return B200RL_OK;
+        case 6: *p = a->adv; *bytes = N * T * 4; return B200RL_OK;
+        case 7: *p = a->ret; *bytes = N * T * 4; return B200RL_OK;
+        case 8: *p = a->rng; *bytes = N * 32; return B200RL_OK;
+        case 9: *p = a->norm2; *bytes = 8; return B200RL_OK;
+    }
+    REQUIRE(false, B200RL_ERR_INVALID, "unknown field");
+}
 
 extern "C" {
 
@@ -603,8 +707,6 @@ int b200rl_onpolicy_destroy(b200rl_onpolicy* a) {
     cudaFree(a->rng); cudaFree(a->states); cudaFree(a->actions); cudaFree(a->logp); cudaFree(a->rewards); cudaFree(a->terminals);
     cudaFree(a->values); cudaFree(a->adv); cudaFree(a->ret); cudaFree(a->act_clamped); cudaFree(a->norm_partials); cudaFree(a->norm_sums);
     cudaFree(a->norm2); cudaFree(a->perm_dev); cudaFree(a->stats_dev); cudaFree(a->rec); cudaFree(a->upd_dev);
-    if (a->graph_exec) cudaGraphExecDestroy(a->graph_exec);
-    if (a->graph) cudaGraphDestroy(a->graph);
     delete a;
     return B200RL_OK;
 }
@@ -627,11 +729,10 @@ int b200rl_onpolicy_create(b200rl_ctx* ctx, b200rl_net* net, b200rl_env* env, co
     int64_t N = b200rl_env_internal_n(env);
     REQUIRE((N * cfg->update_freq) % cfg->n_microbatches == 0, B200RL_ERR_INVALID, "N*T must be divisible by n_microbatches");
     REQUIRE(N * (int64_t)cfg->update_freq < (1ll << 31), B200RL_ERR_UNSUPPORTED, "rollout too large for 32-bit sample indices");
-    b200rl_onpolicy* a = new b200rl_onpolicy();
-    memset(a, 0, sizeof *a);
+    b200rl_onpolicy* a = new b200rl_onpolicy();   // (value-initialised: every pointer and counter starts at zero)
     a->ctx = ctx; a->net = net; a->env = env; a->cfg = *cfg; a->N = N; a->T = cfg->update_freq; a->t = 0; a->ns = nobs; a->continuous = cont;
     size_t NT_ = (size_t)N * a->T;
-#define A_TRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { b200rl_set_error("%s -> %s", #x, cudaGetErrorString(_e)); b200rl_onpolicy_destroy(a); return _e == cudaErrorMemoryAllocation ? B200RL_ERR_OOM : B200RL_ERR_CUDA; } } while (0)
+#define A_TRY(x) CUDA_TRY_OR(x, b200rl_onpolicy_destroy(a))
     A_TRY(cudaMalloc(&a->rng, (size_t)N * 32));
     A_TRY(cudaMalloc(&a->states, (size_t)N * nobs * (a->T + 1) * 4));
     A_TRY(cudaMalloc(&a->actions, NT_ * 4)); A_TRY(cudaMalloc(&a->logp, NT_ * 4)); A_TRY(cudaMalloc(&a->rewards, NT_ * 4));
@@ -667,10 +768,8 @@ int b200rl_onpolicy_plan(b200rl_onpolicy* a, void* actions_host) {
     a->bootstrap_done = false;
     int64_t N = a->N;
     const float* obs = (const float*)env_field(a->env, B200RL_FIELD_OBS);
-    AcHyper hp{a->cfg.clip_range, a->cfg.w_actor, a->cfg.w_critic, a->cfg.w_entropy, a->cfg.min_sigma, a->cfg.max_sigma,
-               a->cfg.normalize_advantage, a->cfg.algo};
     char* act_col = (char*)a->actions + (size_t)N * a->t * 4;
-    TRY(nn_policy_act(a->ctx, a->net->actor, a->net->critic, a->net->params, hp, obs, N, a->rng, act_col, a->logp + (size_t)N * a->t,
+    TRY(nn_policy_act(a->ctx, a->net->actor, a->net->critic, a->net->params, ac_hyper(a->cfg), obs, N, a->rng, act_col, a->logp + (size_t)N * a->t,
                       a->values + (size_t)N * a->t, nullptr, a->states + (size_t)N * a->ns * a->t));
     TRY(b200rl_env_internal_set_traj_targets(a->env, a->rewards + (size_t)N * a->t, a->terminals + (size_t)N * a->t));
     if (actions_host) {
@@ -703,13 +802,11 @@ int b200rl_onpolicy_push(b200rl_onpolicy* a) {
 /* n x (plan! -> act! -> push!) without leaving the device */
 int b200rl_onpolicy_collect(b200rl_onpolicy* a, int n_steps) {
     REQUIRE(a && n_steps >= 0, B200RL_ERR_INVALID, "bad argument");
-    if (n_steps > 0 && nn_tc_enabled() && fused_rollout_enabled()) {   // one launch for the whole stretch (fwd_tc.cu)
+    if (n_steps > 0 && nn_tc_enabled()) {   // one launch for the whole stretch (fwd_tc.cu)
         REQUIRE(a->t + n_steps <= a->T, B200RL_ERR_INVALID, "rollout is full: call b200rl_onpolicy_update first");
         TRY(ctx_bind(a->ctx));
-        AcHyper hp{a->cfg.clip_range, a->cfg.w_actor, a->cfg.w_critic, a->cfg.w_entropy, a->cfg.min_sigma, a->cfg.max_sigma,
-                   a->cfg.normalize_advantage, a->cfg.algo};
         const int fin = a->t + n_steps == a->T ? 1 : 0;
-        int st = nn_tc_rollout(a->ctx, a->env, a->net->actor, a->net->critic, a->net->params, hp, a->rng, a->t, n_steps, a->T, fin, a->states,
+        int st = nn_tc_rollout(a->ctx, a->env, a->net->actor, a->net->critic, a->net->params, ac_hyper(a->cfg), a->rng, a->t, n_steps, a->T, fin, a->states,
                                a->actions, a->logp, a->values, a->rewards, a->terminals);
         if (st == B200RL_OK) {
             a->t += n_steps;
@@ -764,7 +861,7 @@ int b200rl_onpolicy_update(b200rl_onpolicy* a, const int32_t* perm_host, float* 
     // GAE + returns + normalisation sums
     int n_part = b200rl_gae_fused_partials_count(N) / 2;
     TRY(b200rl_gae_fused_internal(ctx, a->adv, a->ret, a->rewards, a->values, a->terminals, c.gamma, c.lambda, N, T,
-                                  c.normalize_advantage ? a->norm_partials : nullptr, nullptr));
+                                  c.normalize_advantage ? a->norm_partials : nullptr));
     if (c.algo == 1) {  // A2C: critic target = discounted gains bootstrapped with V(s_{T+1})
         TRY(b200rl_discount_rewards_f32(ctx, a->ret, a->rewards, a->terminals, a->values + (size_t)N * T, c.gamma, N, T, 2, 1));
     }
@@ -790,7 +887,7 @@ int b200rl_onpolicy_update(b200rl_onpolicy* a, const int32_t* perm_host, float* 
         CUDA_TRY(cudaMemcpyAsync(a->perm_dev, perm_host, (size_t)c.n_epochs * NT_ * 4, cudaMemcpyHostToDevice, ctx->stream));
     }
     TRY(phase(1));
-    AcHyper hp{c.clip_range, c.w_actor, c.w_critic, c.w_entropy, c.min_sigma, c.max_sigma, c.normalize_advantage, c.algo};
+    const AcHyper hp = ac_hyper(c);
     int64_t B = NT_ / c.n_microbatches;
     int row = 0;
     for (int e = 0; e < c.n_epochs; ++e) {
@@ -803,50 +900,22 @@ int b200rl_onpolicy_update(b200rl_onpolicy* a, const int32_t* perm_host, float* 
                       1.0f / ((float)B * (float)world), a->norm2};
             float* stats_row = a->stats_dev + (size_t)row * 8;
             unsigned int* tick = row == a->stats_rows - 1 ? a->upd_dev : nullptr;   // the last optimiser step closes the update
-            // one launch: loss + backward + [peer exchange] + clip + Adam (tensor-core path)
+            // one launch: loss + backward + [peer exchange] + clip + Adam (tensor-core path); otherwise loss + backward, then the
+            // optimiser step
             int ctas = nn_ac_loss_grad_step(ctx, n->actor, n->critic, n->params, hp, b, n->partial, n->loss_partial, n->grad, n->m, n->v, n->beta_t,
                                             n->loss4, c.max_grad_norm, c.lr, c.beta1, c.beta2, c.eps, n->gnorm, n->cta_sumsq, n->counter2, stats_row, tick);
-            if (ctas > 0) {
-                TRY(phase(2 + 2 * row));
-                TRY(phase(3 + 2 * row));
-                n->n_updates += 1;
-                continue;
-            }
-            if (ctas != B200RL_ERR_UNSUPPORTED) return ctas;
-            ctas = nn_ac_loss_grad(ctx, n->actor, n->critic, n->params, hp, b, n->partial, n->loss_partial);
+            const bool staged = ctas == B200RL_ERR_UNSUPPORTED;
+            if (staged) ctas = nn_ac_loss_grad(ctx, n->actor, n->critic, n->params, hp, b, n->partial, n->loss_partial);
             if (ctas < 0) return ctas;
             TRY(phase(2 + 2 * row));
-            P2PTable peers;
-            if (world > 1 && !b200rl_comm_p2p_table(ctx, &peers)) {   // no peer exchange attached: reduce -> NCCL all-reduce -> clip + Adam
-                TRY(nn_reduce_partials(ctx, n->partial, ctas, n->np, n->grad, n->loss_partial, 2 * ctas, n->loss4));
-                TRY(b200rl_comm_allreduce_internal(ctx, n->grad, n->np, 0));
-                TRY(b200rl_comm_allreduce_internal(ctx, n->loss4, 4, 0));
-                TRY(nn_clip_adam(ctx, n->params, n->grad, n->m, n->v, n->beta_t, n->np, c.max_grad_norm, c.lr, c.beta1, c.beta2, c.eps, 1.0f, n->gnorm));
-                stats_row_kernel<<<1, 32, 0, ctx->stream>>>(stats_row, n->loss4, n->gnorm, tick);
-                LAUNCH_CHECK(ctx);
-            } else {   // one kernel: reduce [-> exchange with the peers over NVLink] -> clip -> Adam -> stats row
-                TRY(nn_reduce_clip_adam(ctx, n->partial, ctas, n->np, n->params, n->grad, n->m, n->v, n->beta_t, n->loss_partial, 2 * ctas, n->loss4,
-                                        c.max_grad_norm, c.lr, c.beta1, c.beta2, c.eps, n->gnorm, n->cta_sumsq, n->counter2, stats_row, tick));
-            }
+            if (staged) TRY(optimiser_step(n, ctas, 2 * ctas, c.max_grad_norm, c.lr, c.beta1, c.beta2, c.eps, stats_row, tick));
             TRY(phase(3 + 2 * row));
             n->n_updates += 1;
         }
     }
     a->n_updates += 1;
     a->t = 0;
-    if (stats_host) {
-        std::vector<float> tmp((size_t)a->stats_rows * 8);
-        CUDA_TRY(cudaMemcpyAsync(tmp.data(), a->stats_dev, tmp.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-        float invB = 1.0f / ((float)B * (float)world);
-        for (int r = 0; r < a->stats_rows; ++r) {
-            float* o = stats_host + (size_t)r * 6;
-            const float* s = tmp.data() + (size_t)r * 8;
-            o[0] = s[0] * invB; o[1] = s[2] * invB; o[2] = s[1] * invB;
-            o[3] = c.w_actor * o[0] + c.w_critic * o[1] - c.w_entropy * o[2];
-            o[4] = s[4]; o[5] = 0.f;
-        }
-    }
+    if (stats_host) TRY(read_stats(a, stats_host));
     return B200RL_OK;
 }
 
@@ -857,110 +926,41 @@ int b200rl_onpolicy_update(b200rl_onpolicy* a, const int32_t* perm_host, float* 
  * sequence numbers, self-resetting grid barrier), so the captured launches are replayable as they are.  The first
  * iteration ever runs eagerly (lazy module loading, scratch growth, function attributes), the second is captured.
  * stats_host: optional (n_epochs * n_microbatches, 6) rows of the LAST iteration (forces a sync).
- * Falls back to eager launches when capture is impossible (NCCL path without the peer exchange, B200RL_GRAPH=0). */
+ * Falls back to eager launches when capture is impossible (NCCL path without the peer exchange). */
 int b200rl_onpolicy_iterate(b200rl_onpolicy* a, int n_iters, float* stats_host) {
     REQUIRE(a && n_iters >= 0, B200RL_ERR_INVALID, "bad argument");
     REQUIRE(a->t == 0, B200RL_ERR_INVALID, "iterate needs an empty rollout (t = 0)");
     TRY(ctx_bind(a->ctx));
     b200rl_ctx* ctx = a->ctx;
-    static int graph_env = -1;
-    if (graph_env < 0) { const char* e = getenv("B200RL_GRAPH"); graph_env = (e && e[0] == '0') ? 0 : 1; }
     P2PTable peers;
-    const bool capturable = graph_env && !a->graph_failed && ctx->phase_base < 0 && (b200rl_comm_world(ctx) == 1 || b200rl_comm_p2p_table(ctx, &peers));
-    const int rows = a->stats_rows;
+    const bool capturable = b200rl_comm_world(ctx) == 1 || b200rl_comm_p2p_table(ctx, &peers);
+    const int key[2] = {nn_tc_enabled() ? 1 : 0, b200rl_env_internal_max_timeout(a->env)};   // launch arguments the graph bakes in
+    a->graph.rekey(key, sizeof key);
+    const CounterSet counters{ctx, a->net, a->env, nullptr, &a->n_updates};
     for (int it = 0; it < n_iters; ++it) {
-        if (!capturable || !a->warmed) {
+        TRY(a->graph.run(0, counters, capturable, [&]() -> int {
+            a->t = 0; a->bootstrap_done = false;   // (a no-op, unless a capture that failed part-way left the rollout filled)
             TRY(b200rl_onpolicy_collect(a, a->T));
-            TRY(b200rl_onpolicy_update(a, nullptr, nullptr));
-            a->warmed = true;
-            continue;
-        }
-        const int tc_now = nn_tc_enabled() ? 1 : 0;
-        const uint64_t env_gen = (uint64_t)b200rl_env_internal_max_timeout(a->env);
-        if (a->graph_exec && (a->graph_tc != tc_now || a->graph_env_gen != env_gen)) {   // a launch argument changed: re-capture
-            cudaGraphExecDestroy(a->graph_exec); a->graph_exec = nullptr;
-            cudaGraphDestroy(a->graph); a->graph = nullptr;
-        }
-        if (!a->graph_exec) {
-            // capture does not execute: the host-side bookkeeping the captured calls did is rolled back and redone per replay
-            const uint64_t l0 = ctx->launches, nu0 = a->n_updates, nnu0 = a->net->n_updates;
-            CUDA_TRY(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
-            int st = b200rl_onpolicy_collect(a, a->T);
-            if (st == B200RL_OK) st = b200rl_onpolicy_update(a, nullptr, nullptr);
-            cudaGraph_t g = nullptr;
-            cudaError_t ce = cudaStreamEndCapture(ctx->stream, &g);
-            a->graph_launches = ctx->launches - l0;
-            ctx->launches = l0; a->n_updates = nu0; a->net->n_updates = nnu0; a->t = 0; a->bootstrap_done = false;
-            b200rl_env_internal_add_steps(a->env, (uint64_t)0 - (uint64_t)a->T);
-            if (st != B200RL_OK || ce != cudaSuccess || !g) {
-                if (g) cudaGraphDestroy(g);
-                cudaGetLastError();
-                a->graph_failed = 1;   // stay on eager launches
-                TRY(b200rl_onpolicy_collect(a, a->T));
-                TRY(b200rl_onpolicy_update(a, nullptr, nullptr));
-                continue;
-            }
-            cudaError_t ie = cudaGraphInstantiate(&a->graph_exec, g, 0);
-            if (ie != cudaSuccess) {
-                cudaGraphDestroy(g);
-                cudaGetLastError();
-                a->graph_exec = nullptr; a->graph_failed = 1;
-                TRY(b200rl_onpolicy_collect(a, a->T));
-                TRY(b200rl_onpolicy_update(a, nullptr, nullptr));
-                continue;
-            }
-            a->graph = g; a->graph_tc = tc_now; a->graph_env_gen = env_gen;
-        }
-        CUDA_TRY(cudaGraphLaunch(a->graph_exec, ctx->stream));
-        ctx->launches += a->graph_launches;
-        a->n_updates += 1; a->net->n_updates += (uint64_t)rows;
-        b200rl_env_internal_add_steps(a->env, (uint64_t)a->T);
+            return b200rl_onpolicy_update(a, nullptr, nullptr);
+        }));
     }
-    if (stats_host && n_iters > 0) {
-        const b200rl_onpolicy_config& c = a->cfg;
-        std::vector<float> tmp((size_t)rows * 8);
-        CUDA_TRY(cudaMemcpyAsync(tmp.data(), a->stats_dev, tmp.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-        float invB = 1.0f / ((float)(a->N * a->T / c.n_microbatches) * (float)b200rl_comm_world(ctx));
-        for (int r = 0; r < rows; ++r) {
-            float* o = stats_host + (size_t)r * 6;
-            const float* s = tmp.data() + (size_t)r * 8;
-            o[0] = s[0] * invB; o[1] = s[2] * invB; o[2] = s[1] * invB;
-            o[3] = c.w_actor * o[0] + c.w_critic * o[1] - c.w_entropy * o[2];
-            o[4] = s[4]; o[5] = 0.f;
-        }
-    }
+    if (stats_host && n_iters > 0) TRY(read_stats(a, stats_host));
     return B200RL_OK;
 }
 /* 1 when b200rl_onpolicy_iterate replays a captured graph, 0 when it launches eagerly (diagnostic for tests / bench) */
 int b200rl_onpolicy_graph_active(b200rl_onpolicy* a, int* out) {
     REQUIRE(a && out, B200RL_ERR_INVALID, "null argument");
-    *out = a->graph_exec ? 1 : 0;
+    *out = a->graph.active() ? 1 : 0;
     return B200RL_OK;
 }
 
-/* rollout tensors for inspection / parity tests.  field: 0 state (ns, N, T+1) | 1 action (N, T) |
- * 2 logp (N, T) | 3 reward (N, T) | 4 terminal (N, T) u8 | 5 value (N, T+1) | 6 advantage (N, T) |
- * 7 return (N, T) | 8 policy rng (4, N) u64 | 9 advantage norm {mean, inv_std} */
+/* rollout tensors for inspection / parity tests (fields: rollout_field) */
 int b200rl_onpolicy_get(b200rl_onpolicy* a, int field, void* host_dst, size_t bytes) {
     REQUIRE(a && host_dst, B200RL_ERR_INVALID, "null argument");
     TRY(ctx_bind(a->ctx));
-    size_t N = (size_t)a->N, T = (size_t)a->T;
-    const void* src = nullptr;
-    size_t need = 0;
-    switch (field) {
-        case 0: src = a->states; need = N * a->ns * (T + 1) * 4; break;
-        case 1: src = a->actions; need = N * T * 4; break;
-        case 2: src = a->logp; need = N * T * 4; break;
-        case 3: src = a->rewards; need = N * T * 4; break;
-        case 4: src = a->terminals; need = N * T; break;
-        case 5: src = a->values; need = N * (T + 1) * 4; break;
-        case 6: src = a->adv; need = N * T * 4; break;
-        case 7: src = a->ret; need = N * T * 4; break;
-        case 8: src = a->rng; need = N * 32; break;
-        case 9: src = a->norm2; need = 8; break;
-        default: REQUIRE(false, B200RL_ERR_INVALID, "unknown field");
-    }
+    void* src;
+    size_t need;
+    TRY(rollout_field(a, field, &src, &need));
     REQUIRE(bytes >= need, B200RL_ERR_INVALID, "destination too small");
     CUDA_TRY(cudaMemcpyAsync(host_dst, src, need, cudaMemcpyDeviceToHost, a->ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(a->ctx->stream));
@@ -970,20 +970,11 @@ int b200rl_onpolicy_get(b200rl_onpolicy* a, int field, void* host_dst, size_t by
 /* checkpoint import: fields 0-5 and 8 of b200rl_onpolicy_get (advantages / returns / normalisation are recomputed by update) */
 int b200rl_onpolicy_set(b200rl_onpolicy* a, int field, const void* host_src, size_t bytes) {
     REQUIRE(a && host_src, B200RL_ERR_INVALID, "null argument");
+    REQUIRE(field != 6 && field != 7 && field != 9, B200RL_ERR_INVALID, "field not settable");
     TRY(ctx_bind(a->ctx));
-    size_t N = (size_t)a->N, T = (size_t)a->T;
-    void* dst = nullptr;
-    size_t need = 0;
-    switch (field) {
-        case 0: dst = a->states; need = N * a->ns * (T + 1) * 4; break;
-        case 1: dst = a->actions; need = N * T * 4; break;
-        case 2: dst = a->logp; need = N * T * 4; break;
-        case 3: dst = a->rewards; need = N * T * 4; break;
-        case 4: dst = a->terminals; need = N * T; break;
-        case 5: dst = a->values; need = N * (T + 1) * 4; break;
-        case 8: dst = a->rng; need = N * 32; break;
-        default: REQUIRE(false, B200RL_ERR_INVALID, "field not settable");
-    }
+    void* dst;
+    size_t need;
+    TRY(rollout_field(a, field, &dst, &need));
     REQUIRE(bytes >= need, B200RL_ERR_INVALID, "source too small");
     CUDA_TRY(cudaMemcpyAsync(dst, host_src, need, cudaMemcpyHostToDevice, a->ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(a->ctx->stream));
@@ -1018,7 +1009,7 @@ int b200rl_onpolicy_time_kernel(b200rl_onpolicy* a, int which, int reps, float* 
     b200rl_net* n = a->net;
     const b200rl_onpolicy_config& c = a->cfg;
     int64_t N = a->N, T = a->T, NT_ = N * T, B = NT_ / c.n_microbatches;
-    AcHyper hp{c.clip_range, c.w_actor, c.w_critic, c.w_entropy, c.min_sigma, c.max_sigma, c.normalize_advantage, c.algo};
+    const AcHyper hp = ac_hyper(c);
     const float* obs = (const float*)env_field(a->env, B200RL_FIELD_OBS);
     int ctas = (nn_tc_enabled() && nn_tc_bwd_supported(n->actor, n->critic)) ? nn_tc_partial_rows(2 * (ctx->sm_count / 2), n->actor, hp, B) : nn_grid_ctas(ctx, n->actor.H);
     void* rng_copy = nullptr;
@@ -1039,18 +1030,9 @@ int b200rl_onpolicy_time_kernel(b200rl_onpolicy* a, int which, int reps, float* 
                 return nn_policy_act(ctx, n->actor, n->critic, n->params, hp, obs, N, (unsigned long long*)rng_copy, o, o + N, o + 2 * N, nullptr, nullptr);
             }
             case 2: return b200rl_env_step(a->env, a->actions, 1, 1);
-            case 3: return b200rl_gae_fused_internal(ctx, a->adv, a->ret, a->rewards, a->values, a->terminals, c.gamma, c.lambda, N, T, a->norm_partials, nullptr);
-            case 4: {   // the optimiser step as update() runs it (lr = 0: parameters stay put), incl. the peer exchange of a sharded run
-                P2PTable peers;
-                if (b200rl_comm_world(ctx) > 1 && !b200rl_comm_p2p_table(ctx, &peers)) {
-                    TRY(nn_reduce_partials(ctx, n->partial, ctas, n->np, n->grad, n->loss_partial, 2 * ctas, n->loss4));
-                    TRY(b200rl_comm_allreduce_internal(ctx, n->grad, n->np, 0));
-                    TRY(b200rl_comm_allreduce_internal(ctx, n->loss4, 4, 0));
-                    return nn_clip_adam(ctx, n->params, n->grad, n->m, n->v, n->beta_t, n->np, c.max_grad_norm, 0.0f, c.beta1, c.beta2, c.eps, 1.0f, n->gnorm);
-                }
-                return nn_reduce_clip_adam(ctx, n->partial, ctas, n->np, n->params, n->grad, n->m, n->v, n->beta_t, n->loss_partial, 2 * ctas, n->loss4,
-                                           c.max_grad_norm, 0.0f, c.beta1, c.beta2, c.eps, n->gnorm, n->cta_sumsq, n->counter2, nullptr, nullptr);
-            }
+            case 3: return b200rl_gae_fused_internal(ctx, a->adv, a->ret, a->rewards, a->values, a->terminals, c.gamma, c.lambda, N, T, a->norm_partials);
+            // the optimiser step as update() runs it (lr = 0: parameters stay put), incl. the peer exchange of a sharded run
+            case 4: return optimiser_step(n, ctas, 2 * ctas, c.max_grad_norm, 0.0f, c.beta1, c.beta2, c.eps, nullptr, nullptr);
         }
         b200rl_set_error("unknown kernel id");
         return B200RL_ERR_INVALID;
@@ -1100,20 +1082,7 @@ static int dqn_update_seq(b200rl_net* n, b200rl_traj* t, const b200rl_dqn_config
     int np_ = nn_dqn_loss_grad(ctx, n->actor, n->params, n->target, b.s, b.a, b.r, b.t, b.s2, b.w, b.B, 1.0f / ((float)b.B * (float)world), cfg->gamma,
                                cfg->huber, cfg->double_dqn, n->partial, n->loss_partial, td, b200rl_traj_internal_discount(t));
     if (np_ < 0) return np_;
-    P2PTable peers;
-    const unsigned adam_grid = grid_for(n->np, 256);
-    if ((world == 1 || b200rl_comm_p2p_table(ctx, &peers)) && (int)adam_grid <= ctx->sm_count) {
-        // one kernel: partial reduce [-> peer exchange] -> global-norm clip -> Adam (the optimiser step of the on-policy path)
-        TRY(nn_reduce_clip_adam(ctx, n->partial, np_, n->np, n->params, n->grad, n->m, n->v, n->beta_t, n->loss_partial, np_, n->loss4, cfg->max_grad_norm,
-                                cfg->lr, cfg->beta1, cfg->beta2, cfg->eps, n->gnorm, n->cta_sumsq, n->counter2, nullptr, nullptr));
-    } else {
-        TRY(nn_reduce_partials(ctx, n->partial, np_, n->np, n->grad, n->loss_partial, np_, n->loss4));
-        if (world > 1) {
-            TRY(b200rl_comm_allreduce_internal(ctx, n->grad, n->np, 0));
-            TRY(b200rl_comm_allreduce_internal(ctx, n->loss4, 4, 0));
-        }
-        TRY(nn_clip_adam(ctx, n->params, n->grad, n->m, n->v, n->beta_t, n->np, cfg->max_grad_norm, cfg->lr, cfg->beta1, cfg->beta2, cfg->eps, 1.0f, n->gnorm));
-    }
+    TRY(optimiser_step(n, np_, np_, cfg->max_grad_norm, cfg->lr, cfg->beta1, cfg->beta2, cfg->eps, nullptr, nullptr));
     if (b200rl_traj_internal_prioritized(t)) TRY(b200rl_traj_internal_priority_from_td(t, td, cfg->per_eps, cfg->per_alpha));
     n->n_updates += 1;
     if (upd_dev) TRY(nn_target_sync_counted(ctx, n->target, n->params, n->np, cfg->rho, upd_dev, cfg->target_update_freq));
@@ -1179,12 +1148,6 @@ namespace {
 __global__ void add_i64_kernel(long long* __restrict__ v, long long d) { *v += d; }
 }  // namespace
 
-struct ReplayGraph {   // one "1 step + m updates" unit
-    cudaGraph_t graph = nullptr;
-    cudaGraphExec_t exec = nullptr;
-    uint64_t launches = 0;   // kernels in the graph (ctx->launches advances by this per replay)
-    int uses = 0;
-};
 // what the captured launches bake in besides the handles: a change means re-capture
 struct ReplayKey {
     int tc, max_timeout, greedy, pad;
@@ -1193,7 +1156,6 @@ struct ReplayKey {
     const void* rng;
     const void* scratch;
     const void* keys;
-    bool operator!=(const ReplayKey& o) const { return memcmp(this, &o, sizeof *this) != 0; }
 };
 struct b200rl_replay {
     b200rl_ctx* ctx;
@@ -1209,18 +1171,8 @@ struct b200rl_replay {
     int64_t* keys; float* vals;   // (stride, N) sum-tree leaves a fused collect window touched (prioritised ring)
     int stride_cap;               // rows of keys / vals allocated
     long long h_counters[2];
-    std::map<int64_t, ReplayGraph> graphs;
-    ReplayKey key;
-    bool graph_failed;
+    GraphUnit graphs;             // "1 step + m updates" units, by m
 };
-
-static void replay_drop_graphs(b200rl_replay* r) {
-    for (auto& kv : r->graphs) {
-        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-        if (kv.second.graph) cudaGraphDestroy(kv.second.graph);
-        kv.second.exec = nullptr; kv.second.graph = nullptr;
-    }
-}
 
 // plan! -> act! -> push!(trajectory): the launches of the stage protocol (QBasedPolicy.plan_device, env.act_, Agent.push)
 static int replay_collect_step(b200rl_replay* r, uint64_t* rng, const b200rl_explorer* ex) {
@@ -1279,7 +1231,6 @@ int b200rl_replay_destroy(b200rl_replay* r) {
     if (!r) return B200RL_OK;
     cudaSetDevice(r->ctx->device);
     cudaStreamSynchronize(r->ctx->stream);
-    replay_drop_graphs(r);
     cudaFree(r->action); cudaFree(r->ex_step_dev); cudaFree(r->upd_dev); cudaFree(r->td_keep); cudaFree(r->keys); cudaFree(r->vals);
     delete r;
     return B200RL_OK;
@@ -1303,13 +1254,9 @@ int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl
     REQUIRE(b.ns == q->actor.in, B200RL_ERR_INVALID, "trajectory state width != network input width");
     REQUIRE(b200rl_comm_world(ctx) == 1, B200RL_ERR_UNSUPPORTED, "the replay agent loop runs on one GPU (communicator world > 1)");
     TRY(check_nstep_gamma(traj, cfg));
-    b200rl_replay* r = new b200rl_replay();
+    b200rl_replay* r = new b200rl_replay();   // (value-initialised: every pointer and counter starts at zero)
     r->ctx = ctx; r->net = q; r->env = env; r->traj = traj; r->cfg = *cfg; r->N = N; r->B = b.B;
-    r->action = nullptr; r->ex_step_dev = nullptr; r->upd_dev = nullptr; r->td_keep = nullptr; r->keys = nullptr; r->vals = nullptr;
-    r->stride_cap = 0;
-    memset(&r->key, 0, sizeof r->key);
-    r->graph_failed = false;
-#define R_TRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { b200rl_set_error("%s -> %s", #x, cudaGetErrorString(_e)); b200rl_replay_destroy(r); return _e == cudaErrorMemoryAllocation ? B200RL_ERR_OOM : B200RL_ERR_CUDA; } } while (0)
+#define R_TRY(x) CUDA_TRY_OR(x, b200rl_replay_destroy(r))
     R_TRY(cudaMalloc(&r->action, (size_t)N * 4));
     R_TRY(cudaMalloc(&r->ex_step_dev, sizeof(long long)));
     R_TRY(cudaMalloc(&r->upd_dev, sizeof(unsigned long long)));
@@ -1367,15 +1314,13 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
     key.rng = explorer_rng_dev;
     key.scratch = ctx->scratch;
     key.keys = r->keys;
-    if (key != r->key) { replay_drop_graphs(r); r->key = key; }
+    r->graphs.rekey(&key, sizeof key);
     // device copies of the counters the launches read
     r->h_counters[0] = ex ? (long long)ex->step : 0;
     r->h_counters[1] = (long long)n->n_updates;
     CUDA_TRY(cudaMemcpyAsync(r->ex_step_dev, &r->h_counters[0], sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemcpyAsync(r->upd_dev, &r->h_counters[1], sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
-    static int graph_env = -1;
-    if (graph_env < 0) { const char* e = getenv("B200RL_GRAPH"); graph_env = (e && e[0] == '0') ? 0 : 1; }
-    const bool capturable = graph_env && !r->graph_failed && ctx->phase_base < 0;
+    const CounterSet counters{ctx, n, r->env, r->traj, nullptr};
     bool updated = false;
     for (int64_t j = 0; j < n_steps;) {
         const int64_t m = ms[(size_t)j];
@@ -1388,40 +1333,7 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
         }
         ++j;
         updated = true;
-        ReplayGraph& G = r->graphs[m];
-        if (!capturable || G.uses++ == 0) {   // first use eager (lazy loading, function attributes)
-            TRY(replay_unit(r, explorer_rng_dev, ex, m));
-            continue;
-        }
-        if (!G.exec) {
-            // capture does not execute: the host-side bookkeeping of the captured calls is measured, rolled back and redone per replay
-            const uint64_t l0 = ctx->launches, nu0 = n->n_updates, es0 = b200rl_env_internal_steps(r->env);
-            const int64_t p0 = b200rl_traj_internal_pushed(r->traj);
-            CUDA_TRY(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
-            int st = replay_unit(r, explorer_rng_dev, ex, m);
-            cudaGraph_t g = nullptr;
-            cudaError_t ce = cudaStreamEndCapture(ctx->stream, &g);
-            G.launches = ctx->launches - l0;
-            ctx->launches = l0; n->n_updates = nu0;
-            b200rl_env_internal_add_steps(r->env, es0 - b200rl_env_internal_steps(r->env));
-            b200rl_traj_internal_add_pushed(r->traj, p0 - b200rl_traj_internal_pushed(r->traj));
-            cudaError_t ie = cudaErrorUnknown;
-            if (st == B200RL_OK && ce == cudaSuccess && g) ie = cudaGraphInstantiate(&G.exec, g, 0);
-            if (ie != cudaSuccess) {
-                if (g) cudaGraphDestroy(g);
-                cudaGetLastError();
-                G.exec = nullptr;
-                r->graph_failed = true;   // stay on eager launches
-                TRY(replay_unit(r, explorer_rng_dev, ex, m));
-                continue;
-            }
-            G.graph = g;
-        }
-        CUDA_TRY(cudaGraphLaunch(G.exec, ctx->stream));
-        ctx->launches += G.launches;
-        n->n_updates += (uint64_t)m;
-        b200rl_env_internal_add_steps(r->env, 1);
-        b200rl_traj_internal_add_pushed(r->traj, 1);
+        TRY(r->graphs.run(m, counters, true, [&] { return replay_unit(r, explorer_rng_dev, ex, m); }));
     }
     *ctl = c;
     if (ex) ex->step += n_steps * r->N;
@@ -1431,8 +1343,7 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
 
 int b200rl_replay_graph_active(b200rl_replay* r, int* out) {
     REQUIRE(r && out, B200RL_ERR_INVALID, "null argument");
-    *out = 0;
-    for (auto& kv : r->graphs) if (kv.second.exec) *out = 1;
+    *out = r->graphs.active() ? 1 : 0;
     return B200RL_OK;
 }
 

@@ -6,6 +6,7 @@
 #include <dlfcn.h>
 
 #include "common.cuh"
+#include "internal.h"
 
 namespace {
 typedef struct ncclComm* ncclComm_t;

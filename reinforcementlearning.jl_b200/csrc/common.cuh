@@ -22,6 +22,16 @@ void b200rl_set_error(const char* fmt, ...);
             return _e == cudaErrorMemoryAllocation ? B200RL_ERR_OOM : B200RL_ERR_CUDA;      \
         }                                                                                   \
     } while (0)
+// CUDA_TRY inside a create: `cleanup` (the destroy of the half-built handle) runs before the error is returned
+#define CUDA_TRY_OR(expr, cleanup)                                                          \
+    do {                                                                                    \
+        cudaError_t _e = (expr);                                                            \
+        if (_e != cudaSuccess) {                                                            \
+            b200rl_set_error("%s:%d %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e)); \
+            cleanup;                                                                        \
+            return _e == cudaErrorMemoryAllocation ? B200RL_ERR_OOM : B200RL_ERR_CUDA;      \
+        }                                                                                   \
+    } while (0)
 
 #define REQUIRE(cond, code, msg)                 \
     do {                                         \

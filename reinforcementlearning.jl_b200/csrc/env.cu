@@ -13,6 +13,7 @@
 
 #include "common.cuh"
 #include "env_device.cuh"
+#include "internal.h"
 
 using jld::Xo;
 using namespace envdev;
@@ -481,7 +482,7 @@ int b200rl_env_episode_stats(b200rl_env* e, double* out4, int reset_after) {
 
 }  // extern "C"
 
-// internal hooks for other translation units (fused consumers)
+// internal hooks for other translation units (fused consumers; internal.h)
 int b200rl_env_internal_set_traj_targets(b200rl_env* e, void* reward_col, uint8_t* terminal_col) {
     e->a.traj_reward = reward_col;
     e->a.traj_terminal = terminal_col;

@@ -17,15 +17,12 @@
 #include "env_device.cuh"
 #include "explore.cuh"
 #include "greedy.cuh"
+#include "internal.h"
 #include "ring.cuh"
 #include "tc_fwd.cuh"
 
 using namespace tcfwd;
 using namespace envdev;
-
-int b200rl_env_internal_view(b200rl_env* e, envdev::EnvView* out);
-void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n);
-int b200rl_env_internal_n_actions(const b200rl_env* e);
 
 namespace {
 

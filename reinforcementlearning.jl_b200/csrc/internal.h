@@ -1,0 +1,47 @@
+// internal.h — what the translation units of libb200rl.so export to each other outside the C ABI: the accessors of the env,
+// trajectory, returns and communicator handles.  Included by the units that define them too, so that the compiler checks every
+// declaration against its definition.
+#pragma once
+#include "common.cuh"
+
+struct Ring;                              // ring.cuh
+namespace envdev { struct EnvView; }     // env_device.cuh
+
+// ---- env.cu
+int b200rl_env_internal_set_traj_targets(b200rl_env* e, void* reward_col, uint8_t* terminal_col);
+int b200rl_env_internal_view(b200rl_env* e, envdev::EnvView* out);
+void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n);
+uint64_t b200rl_env_internal_steps(const b200rl_env* e);
+int b200rl_env_internal_max_timeout(const b200rl_env* e);
+int b200rl_env_internal_dtype(const b200rl_env* e);
+int64_t b200rl_env_internal_n(const b200rl_env* e);
+int b200rl_env_internal_kind(const b200rl_env* e);
+int b200rl_env_internal_nobs(const b200rl_env* e);
+int b200rl_env_internal_n_actions(const b200rl_env* e);
+float b200rl_env_internal_action_bound(const b200rl_env* e);
+b200rl_ctx* b200rl_env_internal_ctx(const b200rl_env* e);
+bool b200rl_env_internal_continuous(const b200rl_env* e);
+
+// ---- traj.cu
+struct TrajBatchView { const float* s; const int32_t* a; const float* r; const uint8_t* t; const float* s2; const float* w; int64_t B; int ns; };
+TrajBatchView b200rl_traj_internal_batch(b200rl_traj* t);
+bool b200rl_traj_internal_prioritized(b200rl_traj* t);
+b200rl_ctx* b200rl_traj_internal_ctx(b200rl_traj* t);
+int64_t b200rl_traj_internal_lanes(b200rl_traj* t);
+void b200rl_traj_internal_add_pushed(b200rl_traj* t, int64_t n);
+int64_t b200rl_traj_internal_pushed(b200rl_traj* t);
+Ring b200rl_traj_internal_ring(b200rl_traj* t);
+float b200rl_traj_internal_default_priority(b200rl_traj* t);
+void b200rl_traj_internal_nstep(b200rl_traj* t, int* n, float* gamma);
+const float* b200rl_traj_internal_discount(b200rl_traj* t);
+int b200rl_traj_internal_tree_rebuild(b200rl_traj* t, const int64_t* keys, const float* vals, int64_t n);
+int b200rl_traj_internal_priority_from_td(b200rl_traj* t, const float* td_dev, float eps, float alpha);
+
+// ---- returns.cu
+int b200rl_gae_fused_internal(b200rl_ctx* ctx, float* adv, float* ret, const float* r, const float* v, const uint8_t* term, float gamma,
+                              float lambda, int64_t S, int64_t n_time, double* partials);
+int b200rl_gae_fused_partials_count(int64_t S);
+
+// ---- comm.cu
+int b200rl_comm_allreduce_internal(b200rl_ctx* ctx, void* buf, int64_t n, int is_double);
+void b200rl_comm_destroy_internal(b200rl_ctx* ctx);

@@ -14,6 +14,7 @@
 // The fused variant also emits returns = adv + v and per-CTA partial sums for the advantage
 // normalisation used by the PPO update (no second pass over the advantages).
 #include "common.cuh"
+#include "internal.h"
 #include "jl_device.cuh"
 
 namespace {
@@ -188,20 +189,6 @@ __global__ void __launch_bounds__(kBlock) scan_few_series(T* __restrict__ out, c
     if (MODE == 1 && lane == 0) out[s] = carry;
 }
 
-// Final reduce of the per-CTA partials in CTA order -> {mean, 1/clamp(std,1e-8,1000)} as float2.
-__global__ void finalize_norm_kernel(const double* __restrict__ partials, int n_partials, double count, float* __restrict__ out2) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    double a = 0, b = 0;
-    for (int k = 0; k < n_partials; ++k) { a += partials[2 * k]; b += partials[2 * k + 1]; }
-    double mean = a / count;
-    double var = (b - count * mean * mean) / (count - 1.0);
-    if (var < 0) var = 0;
-    float sd = (float)sqrt(var);
-    sd = sd < 1e-8f ? 1e-8f : (sd > 1000.0f ? 1000.0f : sd);
-    out2[0] = (float)mean;
-    out2[1] = 1.0f / sd;
-}
-
 template <class T, int MODE>
 int run_scan(b200rl_ctx* ctx, T* out, const T* r, const T* v, const uint8_t* term, const T* init, T gamma, T lambda, int64_t R,
              int64_t C, int dims, int on_device) {
@@ -248,19 +235,13 @@ int run_scan(b200rl_ctx* ctx, T* out, const T* r, const T* v, const uint8_t* ter
 
 }  // namespace
 
-// internal: fused GAE for the (N, T) rollout layout — advantages, returns and the
-// normalisation constants {mean, inv_std} in `norm2` (device float[2]).  `partials` must
-// hold 2 * ceil(S / 128) doubles.
+// internal: fused GAE for the (N, T) rollout layout — advantages, returns and, when `partials` is not null, the per-CTA
+// {sum, sum of squares} of the advantages for the normalisation (2 * ceil(S / 128) doubles; algo.cu reduces them).
 int b200rl_gae_fused_internal(b200rl_ctx* ctx, float* adv, float* ret, const float* r, const float* v, const uint8_t* term,
-                              float gamma, float lambda, int64_t S, int64_t n_time, double* partials, float* norm2) {
-    unsigned grid = grid_for(S, kBlock);
-    scan_series_fastest<float, 2><<<grid, kBlock, 0, ctx->stream>>>(adv, r, v, term, nullptr, gamma, lambda, S, n_time, ret,
-                                                                  partials);
+                              float gamma, float lambda, int64_t S, int64_t n_time, double* partials) {
+    scan_series_fastest<float, 2><<<grid_for(S, kBlock), kBlock, 0, ctx->stream>>>(adv, r, v, term, nullptr, gamma, lambda, S, n_time, ret,
+                                                                                 partials);
     LAUNCH_CHECK(ctx);
-    if (norm2) {
-        finalize_norm_kernel<<<1, 32, 0, ctx->stream>>>(partials, (int)grid, (double)S * (double)n_time, norm2);
-        LAUNCH_CHECK(ctx);
-    }
     return B200RL_OK;
 }
 int b200rl_gae_fused_partials_count(int64_t S) { return 2 * (int)grid_for(S, kBlock); }
