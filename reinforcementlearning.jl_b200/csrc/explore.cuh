@@ -42,6 +42,18 @@ inline float fdiv(float a, float b) { return a / b; }
 inline float d2f(double a) { return (float)a; }
 #endif
 
+// Xoshiro256++ on a 4-word state held in registers.  Streams live in memory as 4 consecutive words per column (rng + 4 i),
+// moved as two 16-byte vectors.
+__host__ __device__ __forceinline__ void xo_load(const unsigned long long* rng, int64_t i, unsigned long long (&s)[4]) {
+    const ulonglong2* p = reinterpret_cast<const ulonglong2*>(rng + 4 * i);
+    ulonglong2 a = p[0], b = p[1];
+    s[0] = a.x; s[1] = a.y; s[2] = b.x; s[3] = b.y;
+}
+__host__ __device__ __forceinline__ void xo_store(unsigned long long* rng, int64_t i, const unsigned long long (&s)[4]) {
+    ulonglong2* p = reinterpret_cast<ulonglong2*>(rng + 4 * i);
+    p[0] = make_ulonglong2(s[0], s[1]);
+    p[1] = make_ulonglong2(s[2], s[3]);
+}
 __host__ __device__ __forceinline__ unsigned long long xo_next(unsigned long long (&s)[4]) {
     unsigned long long tmp = s[0] + s[3];
     unsigned long long res = ((tmp << 23) | (tmp >> 41)) + s[0];
@@ -55,8 +67,8 @@ __host__ __device__ __forceinline__ double xo_f64(unsigned long long (&s)[4]) { 
 // rand(rng, Float32): jl_device.cuh's rand_f32 on this stream layout (an output of 0 happens: its top 24 bits all zero)
 __host__ __device__ __forceinline__ float xo_f32(unsigned long long (&s)[4]) { return (float)((unsigned)(xo_next(s) >> 32) >> 8) * 0x1p-24f; }
 
-// rand(rng, Base.OneTo(n)) — Lemire nearly-divisionless on UInt64 (Julia 1.10 SamplerRangeNDL), 1-based
-__host__ __device__ __forceinline__ int xo_oneto(unsigned long long (&s)[4], unsigned long long n) {
+// rand(rng, Base.OneTo(n)) - 1 — Lemire nearly-divisionless on UInt64 (Julia 1.10 SamplerRangeNDL), 0-based, n up to 2^64 - 1
+__host__ __device__ __forceinline__ unsigned long long xo_below(unsigned long long (&s)[4], unsigned long long n) {
     unsigned long long x = xo_next(s);
     unsigned long long hi = mul64hi(x, n), lo = x * n;
     if (lo < n) {
@@ -67,8 +79,10 @@ __host__ __device__ __forceinline__ int xo_oneto(unsigned long long (&s)[4], uns
             lo = x * n;
         }
     }
-    return (int)hi + 1;
+    return hi;
 }
+// rand(rng, Base.OneTo(n)), 1-based, for n within int (action counts)
+__host__ __device__ __forceinline__ int xo_oneto(unsigned long long (&s)[4], unsigned long long n) { return (int)xo_below(s, n) + 1; }
 
 // get_ϵ(s::EpsilonGreedyExplorer{:linear | :exp}, step) (epsilon_greedy_explorer.jl:69-91): Float64, left to right
 // Ex: b200rl_explorer, or any struct with its schedule fields (the fused collect's kernel argument)

@@ -18,6 +18,7 @@
 #include "explore.cuh"
 #include "greedy.cuh"
 #include "internal.h"
+#include "policy.cuh"
 #include "ring.cuh"
 #include "tc_fwd.cuh"
 
@@ -32,17 +33,6 @@ struct SmemFwd {
     float X[kInMax * TM];                 // [i][s]
     float Zp[2 * kOutMax * TM];           // head partials [half][o][s]
 };
-
-__device__ __forceinline__ void load_rng32(const unsigned long long* rng, int64_t i, unsigned long long (&s)[4]) {
-    const ulonglong2* p = reinterpret_cast<const ulonglong2*>(rng + 4 * i);
-    ulonglong2 a = p[0], b = p[1];
-    s[0] = a.x; s[1] = a.y; s[2] = b.x; s[3] = b.y;
-}
-__device__ __forceinline__ void store_rng32(unsigned long long* rng, int64_t i, const unsigned long long (&s)[4]) {
-    ulonglong2* p = reinterpret_cast<ulonglong2*>(rng + 4 * i);
-    p[0] = make_ulonglong2(s[0], s[1]);
-    p[1] = make_ulonglong2(s[2], s[3]);
-}
 
 // One tile of TM samples through one network: the observations in X ([i][s], published by a barrier before the call) -> layer 1 ->
 // the GEMM of both warpgroups -> the head partial sums of both 32-feature halves in Zp ([half][o][s]).  Called by all NT threads;
@@ -130,12 +120,12 @@ forward_tc_kernel(MlpDesc actor, MlpDesc critic, const float* __restrict__ param
                     if (value_out) value_out[i] = z[0];
                 } else if (mode == 0) {
                     unsigned long long st[4];
-                    load_rng32(rng, i, st);
+                    explore::xo_load(rng, i, st);
                     float lp;
-                    uint32_t a = sample_head(actor, hp, z, st, lp);
+                    uint32_t a = policy::sample_head(actor.heads2, actor.nout, hp, z, st, lp);
                     if (action_out) reinterpret_cast<uint32_t*>(action_out)[i] = a;
                     if (logp_out) logp_out[i] = lp;
-                    store_rng32(rng, i, st);
+                    explore::xo_store(rng, i, st);
                 }
             }
         }
@@ -187,7 +177,7 @@ __device__ __forceinline__ void load_group(Slot* slot, int nslots, int64_t base,
             sl.flags[s] = ea.flags[i];
             sl.ep_ret[s] = ea.ep_ret[i];
             unsigned long long e[4];
-            load_rng32(ea.rng, i, e);
+            explore::xo_load(ea.rng, i, e);
             put_stream(sl.erng, s, e);
             more(sl, i);
         }
@@ -209,7 +199,7 @@ __device__ __forceinline__ void store_group(const Slot* slot, int nslots, int64_
             ea.ep_ret[i] = sl.ep_ret[s];
             unsigned long long e[4];
             get_stream(sl.erng, s, e);
-            store_rng32(ea.rng, i, e);
+            explore::xo_store(ea.rng, i, e);
             if (stepped) {
                 reinterpret_cast<float*>(ea.reward)[i] = sl.last_rew[s];
                 reinterpret_cast<uint32_t*>(ea.action)[i] = sl.last_act[s];
@@ -296,7 +286,7 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
     if (owner)
         load_group(sm.slot, nslots, cta, nctas, ea, N, s, [&](RollSlot<Env>& sl, int64_t i) {
             unsigned long long pr[4];
-            load_rng32(g.policy_rng, i, pr);
+            explore::xo_load(g.policy_rng, i, pr);
             put_stream(sl.prng, s, pr);
         });
     wg::fence_proxy_async();
@@ -351,7 +341,7 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
                 unsigned long long pr[4];
                 get_stream(sl.prng, s, pr);
                 float lp;
-                const uint32_t a_bits = sample_head(g.actor, g.hp, z, pr, lp);
+                const uint32_t a_bits = policy::sample_head(g.actor.heads2, g.actor.nout, g.hp, z, pr, lp);
                 put_stream(sl.prng, s, pr);
                 reinterpret_cast<uint32_t*>(g.actions)[(size_t)N * t + i] = a_bits;
                 g.logp[(size_t)N * t + i] = lp;
@@ -374,7 +364,7 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
         store_group(sm.slot, nslots, cta, nctas, ea, N, s, g.nsteps > 0, [&](const RollSlot<Env>& sl, int64_t i) {
             unsigned long long pr[4];
             get_stream(sl.prng, s, pr);
-            store_rng32(g.policy_rng, i, pr);
+            explore::xo_store(g.policy_rng, i, pr);
         });
     cta_episode_stats(ea.stats, fin_cnt, fin_ret, fin_len, sm.red);
 }
@@ -436,7 +426,7 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename
                 sl.cnt[s] = 0;
                 if (MODE == 1) {
                     unsigned long long pr[4];
-                    load_rng32(g.policy_rng, i, pr);
+                    explore::xo_load(g.policy_rng, i, pr);
                     put_stream(sl.prng, s, pr);
                 }
             });
@@ -468,7 +458,7 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename
                         unsigned long long pr[4];
                         get_stream(sl.prng, s, pr);
                         float lp;
-                        a_bits = sample_head(g.actor, g.hp, z, pr, lp);
+                        a_bits = policy::sample_head(g.actor.heads2, g.actor.nout, g.hp, z, pr, lp);
                         put_stream(sl.prng, s, pr);
                     }
                     const ActStep<float> r = slot_act(sl, s, p, ea.max_timeout, env_action<Env>(a_bits), sm.fin_cnt[s], sm.fin_ret[s], sm.fin_len[s]);
@@ -489,7 +479,7 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename
                 if (MODE == 1) {
                     unsigned long long pr[4];
                     get_stream(sl.prng, s, pr);
-                    store_rng32(g.policy_rng, i, pr);
+                    explore::xo_store(g.policy_rng, i, pr);
                 }
                 if (g.counts) g.counts[i] = sl.cnt[s];
             });
@@ -585,7 +575,7 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
                     sl.erng[s] = e.s0; sl.erng[TM + s] = e.s1; sl.erng[2 * TM + s] = e.s2; sl.erng[3 * TM + s] = e.s3;
                     if (!g.greedy) {
                         unsigned long long xr[4];
-                        load_rng32(g.xrng, i, xr);
+                        explore::xo_load(g.xrng, i, xr);
                         sl.xrng[s] = xr[0]; sl.xrng[TM + s] = xr[1]; sl.xrng[2 * TM + s] = xr[2]; sl.xrng[3 * TM + s] = xr[3];
                     }
                 }
@@ -645,7 +635,7 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
                 if (!g.greedy) {
                     unsigned long long xr[4];
                     get_stream(sl.xrng, s, xr);
-                    store_rng32(g.xrng, i, xr);
+                    explore::xo_store(g.xrng, i, xr);
                 }
                 if (g.prioritized) {   // the lane's touched slots p0, p0 + 1, ... (mod cap + 1), one key each
                     const int n_touched = (int)min((int64_t)sl.adv[s] + 1, F);

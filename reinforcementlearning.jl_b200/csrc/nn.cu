@@ -17,11 +17,11 @@
 #include "explore.cuh"
 #include "nn.cuh"
 #include "perm.cuh"
+#include "policy.cuh"
 
 namespace {
 
 constexpr int NT = 256;
-constexpr float kLog2Pi = 1.8378770664093453f;
 
 template <int H> struct Cfg {
     static constexpr int TM = (H == 64) ? 128 : 64;   // samples per tile
@@ -50,13 +50,6 @@ template <int H, bool BWD> struct Smem {
     float Red[64];
 };
 
-__device__ __forceinline__ float act_f(int act, float z) { return act == B200RL_ACT_RELU ? fmaxf(z, 0.f) : tanhf(z); }
-__device__ __forceinline__ float dact_f(int act, float h) { return act == B200RL_ACT_RELU ? (h > 0.f ? 1.f : 0.f) : 1.f - h * h; }
-
-__device__ __forceinline__ uint32_t mix32(uint32_t h) {
-    h ^= h >> 16; h *= 0x85EBCA6Bu; h ^= h >> 13; h *= 0xC2B2AE35u; h ^= h >> 16;
-    return h;
-}
 // minibatch permutation: perm.cuh
 using b200perm::perm_index;
 using b200perm::perm_index_bits;
@@ -369,27 +362,6 @@ template <int H> __device__ void write_grad(const GradAcc<H>& g, const MlpDesc& 
     if (tid < d.rows()) out[head_b(d, tid)] = g.b3;
 }
 
-__device__ __forceinline__ float block_sum(float v, float* red) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    float t = 0.f;
-    if (threadIdx.x == 0)
-        for (int k = 0; k < NT / 32; ++k) t += red[k];
-    return t;  // valid on thread 0
-}
-
-__device__ __forceinline__ float softplus_f(float x) { return x > 0.f ? x + log1pf(expf(-x)) : log1pf(expf(x)); }
-__device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + expf(-x)); }
-__device__ __forceinline__ float normlogpdf1(float mu, float sigma, float x) {  // diagnormlogpdf, d = 1
-    float s = sigma + 1e-8f;
-    float v = s * s;
-    float dd = x - mu;
-    return -0.5f * ((logf(v) + (dd * dd) / v) + kLog2Pi);
-}
-
 // ------------------------------------------------------------- actor-critic loss + grad -----
 template <int H>
 __global__ void __launch_bounds__(NT, (H == 64) ? 2 : 1)
@@ -465,81 +437,21 @@ ac_loss_grad_kernel(MlpDesc actor, MlpDesc critic, const float* __restrict__ par
             bool valid = (tile * C::TM + s) < b.B;
             float dz[kOutMax] = {0.f, 0.f, 0.f, 0.f};
             if (valid) {
-                if (role == 1) {
-                    float v = sm.Out[s];
-                    float err = sm.Aux[3 * C::TM + s] - v;
-                    l0 += err * err;
-                    dz[0] = -2.0f * hp.w_critic * b.inv_B * err;
-                } else {
-                    float A = sm.Aux[2 * C::TM + s];
-                    float lp_old = sm.Aux[C::TM + s];
-                    float logp_a, gsel_scale;  // gsel_scale = d(surrogate)/d(logp_a)
-                    if (!actor.heads2) {
-                        int na = actor.nout;
-                        float z[kOutMax], lp[kOutMax], pr[kOutMax];
-                        float m = -3.4e38f;
+                float z[kOutMax];
 #pragma unroll
-                        for (int o = 0; o < kOutMax; ++o) { z[o] = sm.Out[o * C::LDA + s]; if (o < na) m = fmaxf(m, z[o]); }
-                        float se = 0.f;
+                for (int o = 0; o < kOutMax; ++o) z[o] = sm.Out[o * C::LDA + s];
+                // one call per role with the role a constant: each accumulation then sees its own loss term, so the critic's
+                // l0 += err * err contracts to one FMA here (the tensor-core K7 adds the returned terms after the join)
+                auto loss = [&](int rl) {
+                    const policy::LossOut<kOutMax> r = policy::sample_loss(actor.heads2, actor.nout, rl, hp, b.inv_B, z, sm.Aux[s], sm.Aux[C::TM + s],
+                                                                           sm.Aux[2 * C::TM + s], sm.Aux[3 * C::TM + s]);
+                    l0 += r.l0;
+                    if (rl == 0) l1 += r.l1;
 #pragma unroll
-                        for (int o = 0; o < kOutMax; ++o) if (o < na) se += expf(z[o] - m);
-                        float ls = logf(se);
-                        float Hent = 0.f;
-#pragma unroll
-                        for (int o = 0; o < kOutMax; ++o) {
-                            lp[o] = (z[o] - m) - ls;
-                            pr[o] = o < na ? expf(lp[o]) : 0.f;
-                            if (o < na) Hent -= pr[o] * lp[o];
-                        }
-                        int a = __float_as_int(sm.Aux[s]) - 1;
-                        logp_a = 0.f;
-#pragma unroll
-                        for (int o = 0; o < kOutMax; ++o) if (o == a) logp_a = lp[o];
-                        l1 += Hent;
-                        if (hp.algo == 0) {
-                            float ratio = expf(logp_a - lp_old);
-                            float u = ratio * A;
-                            float rc = fminf(fmaxf(ratio, 1.0f - hp.clip_range), 1.0f + hp.clip_range);
-                            float c = rc * A;
-                            l0 += -fminf(u, c);
-                            bool inside = ratio >= 1.0f - hp.clip_range && ratio <= 1.0f + hp.clip_range;
-                            gsel_scale = (u < c || inside) ? u : 0.f;
-                        } else {
-                            l0 += -(logp_a * A);
-                            gsel_scale = A;
-                        }
-                        float dlogp = -hp.w_actor * b.inv_B * gsel_scale;
-#pragma unroll
-                        for (int o = 0; o < kOutMax; ++o)
-                            if (o < na) dz[o] = dlogp * ((o == a ? 1.f : 0.f) - pr[o]) + hp.w_entropy * b.inv_B * pr[o] * (lp[o] + Hent);
-                    } else {
-                        float mu = sm.Out[s], raw = sm.Out[C::LDA + s];
-                        float sp = softplus_f(raw);
-                        float sigma = fminf(fmaxf(sp, hp.min_sigma), hp.max_sigma);
-                        bool clamped = sp < hp.min_sigma || sp > hp.max_sigma;
-                        float a = sm.Aux[s];
-                        logp_a = normlogpdf1(mu, sigma, a);
-                        float Hent = logf(sigma) + 0.5f * (kLog2Pi + 1.0f);
-                        l1 += Hent;
-                        if (hp.algo == 0) {
-                            float ratio = expf(logp_a - lp_old);
-                            float u = ratio * A;
-                            float rc = fminf(fmaxf(ratio, 1.0f - hp.clip_range), 1.0f + hp.clip_range);
-                            float c = rc * A;
-                            l0 += -fminf(u, c);
-                            bool inside = ratio >= 1.0f - hp.clip_range && ratio <= 1.0f + hp.clip_range;
-                            gsel_scale = (u < c || inside) ? u : 0.f;
-                        } else {
-                            l0 += -(logp_a * A);
-                            gsel_scale = A;
-                        }
-                        float dlogp = -hp.w_actor * b.inv_B * gsel_scale;
-                        float sg = sigma + 1e-8f, dd = a - mu;
-                        dz[0] = dlogp * (dd / (sg * sg));
-                        float dsig = dlogp * (-1.0f / sg + (dd * dd) / (sg * sg * sg)) - hp.w_entropy * b.inv_B * (1.0f / sigma);
-                        dz[1] = clamped ? 0.f : dsig * sigmoid_f(raw);
-                    }
-                }
+                    for (int o = 0; o < kOutMax; ++o) dz[o] = r.dz[o];
+                };
+                if (role == 1) loss(1);
+                else loss(0);
             }
 #pragma unroll
             for (int o = 0; o < kOutMax; ++o) sm.Dz[o * C::LDA + s] = dz[o];
@@ -548,8 +460,8 @@ ac_loss_grad_kernel(MlpDesc actor, MlpDesc critic, const float* __restrict__ par
         backward_tile<H>(sm, d, g);
     }
     write_grad<H>(g, d, partial + (int64_t)cta * np_total + poff);
-    float t0 = block_sum(l0, sm.Red);
-    float t1 = block_sum(l1, sm.Red);
+    float t0 = block_sum<NT>(l0, sm.Red);
+    float t1 = block_sum<NT>(l1, sm.Red);
     if (tid == 0) {
         float* lp = loss_partial + (int64_t)blockIdx.x * 4;  // actor rows: {surrogate, entropy, 0, 0}; critic rows: {0, 0, sq.err, 0}
         lp[0] = role ? 0.f : t0; lp[1] = role ? 0.f : t1; lp[2] = role ? t0 : 0.f; lp[3] = 0.f;
@@ -557,27 +469,6 @@ ac_loss_grad_kernel(MlpDesc actor, MlpDesc critic, const float* __restrict__ par
 }
 
 // ------------------------------------------------------------- rollout inference ------------
-__device__ __forceinline__ void load_rng32(const unsigned long long* rng, int64_t i, unsigned long long (&s)[4]) {
-    const ulonglong2* p = reinterpret_cast<const ulonglong2*>(rng + 4 * i);
-    ulonglong2 a = p[0], b = p[1];
-    s[0] = a.x; s[1] = a.y; s[2] = b.x; s[3] = b.y;
-}
-__device__ __forceinline__ void store_rng32(unsigned long long* rng, int64_t i, const unsigned long long (&s)[4]) {
-    ulonglong2* p = reinterpret_cast<ulonglong2*>(rng + 4 * i);
-    p[0] = make_ulonglong2(s[0], s[1]);
-    p[1] = make_ulonglong2(s[2], s[3]);
-}
-__device__ __forceinline__ unsigned long long xo_next(unsigned long long (&s)[4]) {
-    unsigned long long tmp = s[0] + s[3];
-    unsigned long long res = ((tmp << 23) | (tmp >> 41)) + s[0];
-    unsigned long long t = s[1] << 17;
-    s[2] ^= s[0]; s[3] ^= s[1]; s[1] ^= s[2]; s[0] ^= s[3]; s[2] ^= t;
-    s[3] = (s[3] << 45) | (s[3] >> 19);
-    return res;
-}
-__device__ __forceinline__ double xo_f64(unsigned long long (&s)[4]) { return (double)(xo_next(s) >> 11) * 0x1p-53; }
-__device__ __forceinline__ float xo_f32(unsigned long long (&s)[4]) { return (float)((unsigned)(xo_next(s) >> 32) >> 8) * 0x1p-24f; }
-
 // mode 0: actor-critic rollout (roles), 1: plain forward of `actor` desc (single role) -> head_out
 template <int H>
 __global__ void __launch_bounds__(NT, (H == 64) ? 2 : 1)
@@ -632,41 +523,15 @@ forward_kernel(MlpDesc actor, MlpDesc critic, const float* __restrict__ params, 
                     if (value_out) value_out[i] = sm.Out[tid];
                 } else if (mode == 0) {
                     unsigned long long st[4];
-                    load_rng32(rng, i, st);
-                    if (!actor.heads2) {  // sample_categorical: argmax(-log(-log(u)) + logp), u Float64
-                        int na = actor.nout;
-                        float z[kOutMax], lp[kOutMax];
-                        float m = -3.4e38f;
+                    explore::xo_load(rng, i, st);
+                    float z[kOutMax];
 #pragma unroll
-                        for (int o = 0; o < kOutMax; ++o) { z[o] = sm.Out[o * C::LDA + tid]; if (o < na) m = fmaxf(m, z[o]); }
-                        float se = 0.f;
-#pragma unroll
-                        for (int o = 0; o < kOutMax; ++o) if (o < na) se += expf(z[o] - m);
-                        float ls = logf(se);
-                        int best = 0;
-                        double bv = 0.0;
-                        float blp = 0.f;
-#pragma unroll
-                        for (int o = 0; o < kOutMax; ++o) {
-                            if (o < na) {
-                                lp[o] = (z[o] - m) - ls;
-                                double u = xo_f64(st);
-                                double gv = -log(-log(u)) + (double)lp[o];
-                                if (o == 0 || gv > bv) { bv = gv; best = o; blp = lp[o]; }
-                            }
-                        }
-                        if (action_out) reinterpret_cast<int32_t*>(action_out)[i] = best + 1;
-                        if (logp_out) logp_out[i] = blp;
-                    } else {  // GaussianNetwork: a = mu + sigma * n
-                        float mu = sm.Out[tid], raw = sm.Out[C::LDA + tid];
-                        float sigma = fminf(fmaxf(softplus_f(raw), hp.min_sigma), hp.max_sigma);
-                        float u1 = xo_f32(st), u2 = xo_f32(st);
-                        float n = sqrtf(-2.0f * logf(1.0f - u1)) * cosf(6.2831855f * u2);
-                        float a = mu + sigma * n;
-                        if (action_out) reinterpret_cast<float*>(action_out)[i] = a;
-                        if (logp_out) logp_out[i] = normlogpdf1(mu, sigma, a);
-                    }
-                    store_rng32(rng, i, st);
+                    for (int o = 0; o < kOutMax; ++o) z[o] = sm.Out[o * C::LDA + tid];
+                    float lp;
+                    const uint32_t a = policy::sample_head(actor.heads2, actor.nout, hp, z, st, lp);
+                    if (action_out) reinterpret_cast<uint32_t*>(action_out)[i] = a;
+                    if (logp_out) logp_out[i] = lp;
+                    explore::xo_store(rng, i, st);
                 }
             }
         }
@@ -929,7 +794,7 @@ dqn_loss_grad_kernel(MlpDesc q, const float* __restrict__ params, const float* _
         backward_tile<H>(sm, q, g);
     }
     write_grad<H>(g, q, partial + (int64_t)cta * np);
-    float t0 = block_sum(l0, sm.Red);
+    float t0 = block_sum<NT>(l0, sm.Red);
     if (tid == 0) {
         float* lp = loss_partial + (int64_t)blockIdx.x * 4;
         lp[0] = t0; lp[1] = 0.f; lp[2] = 0.f; lp[3] = 0.f;
@@ -946,13 +811,13 @@ __global__ void q_act_kernel(const float* __restrict__ qv, int na, int64_t N, un
     for (int o = 1; o < na; ++o) if (qv[(int64_t)na * i + o] > qv[(int64_t)na * i + best]) best = o;
     if (epsilon > 0.f) {
         unsigned long long st[4];
-        load_rng32(rng, i, st);
-        double u = xo_f64(st);
+        explore::xo_load(rng, i, st);
+        double u = explore::xo_f64(st);
         if (u < (double)epsilon) {
-            unsigned long long x = xo_next(st);
+            unsigned long long x = explore::xo_next(st);
             best = (int)__umul64hi(x, (unsigned long long)na);
         }
-        store_rng32(rng, i, st);
+        explore::xo_store(rng, i, st);
     }
     action_out[i] = best + 1;
 }
@@ -967,9 +832,9 @@ __global__ void q_explore_kernel(const float* __restrict__ qv, int na, int64_t N
     if (i >= N) return;
     const long long step = step_dev ? *step_dev : ex.step;
     unsigned long long st[4];
-    load_rng32(rng, i, st);
+    explore::xo_load(rng, i, st);
     const int action = explore::select(ex, step + i, qv + (int64_t)na * i, na, st);
-    store_rng32(rng, i, st);
+    explore::xo_store(rng, i, st);
     action_out[i] = action;
 }
 

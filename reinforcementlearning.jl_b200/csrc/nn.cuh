@@ -9,6 +9,7 @@
 // (ActorCritic RLCore/src/utils/networks.jl:15-20, GaussianNetwork :44-116, DuelingNetwork :500-522.)
 #pragma once
 #include "common.cuh"
+#include "policy.cuh"   // AcHyper
 
 constexpr int kInMax = 4;    // observation width <= 4 (CartPole 4, Pendulum 3, MountainCar 2)
 constexpr int kOutMax = 4;   // head rows <= 4 (a dueling head has n_out + 1 rows: n_out <= 3)
@@ -38,12 +39,6 @@ __host__ __device__ __forceinline__ int64_t head_b(const MlpDesc& d, int o) {
     if (MAY_DUEL && d.duel) return head_base(d) + (o == 0 ? (int64_t)d.H : (int64_t)(d.H + 1) + (int64_t)d.nout * d.H + (o - 1));
     return head_base(d) + (d.heads2 ? (int64_t)o * (d.H + 1) + d.H : (int64_t)d.nout * d.H + o);
 }
-
-struct AcHyper {  // scalars of the actor-critic losses (SURVEY Appendix B)
-    float clip_range, w_actor, w_critic, w_entropy, min_sigma, max_sigma;
-    int normalize_adv;
-    int algo;  // 0 PPO clipped surrogate, 1 A2C (logp * advantage)
-};
 
 // One minibatch of the on-policy update: sample j is flat index perm(j) into the rollout
 // arrays (states (ns, total) column-major; actions / logp_old / adv / ret (total)).
@@ -84,6 +79,22 @@ int nn_ac_loss_grad_step(b200rl_ctx* ctx, const MlpDesc& actor, const MlpDesc& c
 
 #ifdef __CUDACC__
 __device__ __forceinline__ uint32_t ac_perm_key(const AcBatch& b) { return b.perm_key + (b.perm_epoch ? *b.perm_epoch * 1000003u : 0u); }
+// the trunk activation, and its derivative from the activation's output h
+__device__ __forceinline__ float act_f(int act, float z) { return act == B200RL_ACT_RELU ? fmaxf(z, 0.f) : tanhf(z); }
+__device__ __forceinline__ float dact_f(int act, float h) { return act == B200RL_ACT_RELU ? (h > 0.f ? 1.f : 0.f) : 1.f - h * h; }
+// sum of v over the NTHREADS threads of the CTA (warp shuffles, then the warp sums in order); valid on thread 0
+template <int NTHREADS>
+__device__ __forceinline__ float block_sum(float v, float* red) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float t = 0.f;
+    if (threadIdx.x == 0)
+        for (int k = 0; k < NTHREADS / 32; ++k) t += red[k];
+    return t;
+}
 #endif
 int nn_grid_ctas(b200rl_ctx* ctx, int H);  // persistent CTAs per role
 int nn_dqn_max_partials(b200rl_ctx* ctx, int H);

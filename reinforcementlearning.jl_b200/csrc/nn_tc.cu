@@ -12,36 +12,22 @@
 // heads (N <= 2) stay on FFMA.  The forward-only kernels (policy inference, fused rollout) live in fwd_tc.cu (same split).
 #include "nn.cuh"
 #include "perm.cuh"
+#include "policy.cuh"
+#include "tc_fwd.cuh"
 #include "tc_split.h"
 #include "wgmma.cuh"
 
 namespace {
 
-constexpr int NT = 256;
-constexpr int TM = 128;              // samples per tile = two wgmma M = 64 blocks
-constexpr int H = 64;
-constexpr int G_F = 128;             // weight image (fp16, K-major): byte stride between 8-element K chunks = one 8 x 16 B core matrix
-constexpr int GW_S = 8 * G_F;        // stride between 8-row groups (64 K elements = 8 chunks)
-constexpr int WIMG_BYTES = 16 * GW_S; // one [hi (64 rows) ; lo (64 rows)] x [K = 64] fp16 weight image = 16 KB
-constexpr float kScaleW = 64.0f;     // power-of-two operand scales (see the header comment)
-constexpr float kLog2Pi = 1.8378770664093453f;
-
-__device__ __forceinline__ float act_f(int act, float z) { return act == B200RL_ACT_RELU ? fmaxf(z, 0.f) : tanhf(z); }
-// two fp32 values -> packed fp16 pair {lo half = a, hi half = b}: the hi parts, and the fp16 of what they miss (the lo parts)
-__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-    const __half2 h = __floats2half2_rn(a, b);
-    const float2 back = __half22float2(h);
-    const __half2 l = __floats2half2_rn(a - back.x, b - back.y);
-    hi = *reinterpret_cast<const uint32_t*>(&h);
-    lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-__device__ __forceinline__ float half_bits_to_float(uint32_t bits16) { return __half2float(__ushort_as_half((unsigned short)bits16)); }
-__device__ __forceinline__ float softplus_f(float x) { return x > 0.f ? x + log1pf(expf(-x)) : log1pf(expf(x)); }
-__device__ __forceinline__ float normlogpdf1(float mu, float sigma, float x) {
-    float s = sigma + 1e-8f, v = s * s, dd = x - mu;
-    return -0.5f * ((logf(v) + (dd * dd) / v) + kLog2Pi);
-}
-__device__ __forceinline__ uint32_t wimg_off(int n, int k) { return (uint32_t)((n >> 3) * GW_S + (k >> 3) * G_F + (n & 7) * 16 + (k & 7) * 2); }
+// the W2 operand image and the fp16 split of the tensor-core forward (tc_fwd.cuh)
+using tcfwd::G_F;
+using tcfwd::GW_S;
+using tcfwd::WIMG_BYTES;
+using tcfwd::split2;
+using tcfwd::wimg_off;
+constexpr int TM = tcfwd::TM;        // samples per tile = two wgmma M = 64 blocks
+constexpr int H = tcfwd::H;
+constexpr float kScaleW = tcfwd::kScale;   // power-of-two operand scales (see the header comment)
 
 // =====================================================================================================
 // K7 on tensor cores: PPO / A2C loss + backward for one minibatch, all four tile GEMMs on wgmma.
@@ -130,26 +116,8 @@ __device__ __forceinline__ void store16_feat(uint8_t* img, int f0, int s, const 
     *reinterpret_cast<uint4*>(p) = make_uint4(v[0], v[1], v[2], v[3]);
     *reinterpret_cast<uint4*>(p + GS_T) = make_uint4(v[4], v[5], v[6], v[7]);
 }
-__device__ __forceinline__ float dact_f(int act, float h) { return act == B200RL_ACT_RELU ? (h > 0.f ? 1.f : 0.f) : 1.f - h * h; }
-
-__device__ __forceinline__ uint32_t mix32(uint32_t h) {
-    h ^= h >> 16; h *= 0x85EBCA6Bu; h ^= h >> 13; h *= 0xC2B2AE35u; h ^= h >> 16;
-    return h;
-}
 using b200perm::perm_index;
 using b200perm::perm_index_bits;
-__device__ __forceinline__ float block_sum512(float v, float* red) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    float t = 0.f;
-    if (threadIdx.x == 0)
-        for (int k = 0; k < NT7 / 32; ++k) t += red[k];
-    return t;
-}
-__device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + expf(-x)); }
 
 // sum over the 32 lanes of NV values each (NV a power of two <= 32... here 32): lane L ends with the totals of
 // values 2L*(NV/64).. — for NV = 32: lane L holds the total of value index L in v[0].
@@ -178,89 +146,6 @@ __device__ __forceinline__ void group_sync(int q) { asm volatile("bar.sync %0, 1
 // operand hand-over to the MMA warpgroup: 512 worker threads arrive without waiting, its 128 threads wait
 __device__ __forceinline__ void ready_arrive(int id) { asm volatile("bar.arrive %0, 640;" ::"r"(id) : "memory"); }
 __device__ __forceinline__ void ready_wait(int id) { asm volatile("bar.sync %0, 640;" ::"r"(id) : "memory"); }
-// per-sample loss and d(loss)/d(head outputs); identical arithmetic on every thread that evaluates a sample
-struct LossOut { float dz[kNo]; float l0, l1; };
-__device__ __forceinline__ LossOut sample_loss(const MlpDesc& actor, int role, const AcHyper& hp, float inv_B, const float (&z)[kNo],
-                                               float a_bits, float lp_old, float A, float ret) {
-    LossOut r;
-#pragma unroll
-    for (int o = 0; o < kNo; ++o) r.dz[o] = 0.f;
-    r.l0 = 0.f; r.l1 = 0.f;
-    if (role == 1) {
-        float err = ret - z[0];
-        r.l0 = err * err;
-        r.dz[0] = -2.0f * hp.w_critic * inv_B * err;
-        return r;
-    }
-    float logp_a, gsel;
-    if (!actor.heads2) {
-        int na = actor.nout;
-        float lp[kNo], pr[kNo];
-        float m = -3.4e38f;
-#pragma unroll
-        for (int o = 0; o < kNo; ++o) if (o < na) m = fmaxf(m, z[o]);
-        float se = 0.f;
-#pragma unroll
-        for (int o = 0; o < kNo; ++o) if (o < na) se += expf(z[o] - m);
-        float ls = logf(se);
-        float Hent = 0.f;
-#pragma unroll
-        for (int o = 0; o < kNo; ++o) {
-            lp[o] = (z[o] - m) - ls;
-            pr[o] = o < na ? expf(lp[o]) : 0.f;
-            if (o < na) Hent -= pr[o] * lp[o];
-        }
-        int a = __float_as_int(a_bits) - 1;
-        logp_a = 0.f;
-#pragma unroll
-        for (int o = 0; o < kNo; ++o) if (o == a) logp_a = lp[o];
-        r.l1 = Hent;
-        if (hp.algo == 0) {
-            float ratio = expf(logp_a - lp_old);
-            float u = ratio * A;
-            float rc = fminf(fmaxf(ratio, 1.0f - hp.clip_range), 1.0f + hp.clip_range);
-            float cc = rc * A;
-            r.l0 = -fminf(u, cc);
-            bool inside = ratio >= 1.0f - hp.clip_range && ratio <= 1.0f + hp.clip_range;
-            gsel = (u < cc || inside) ? u : 0.f;
-        } else {
-            r.l0 = -(logp_a * A);
-            gsel = A;
-        }
-        float dlogp = -hp.w_actor * inv_B * gsel;
-#pragma unroll
-        for (int o = 0; o < kNo; ++o)
-            if (o < na) r.dz[o] = dlogp * ((o == a ? 1.f : 0.f) - pr[o]) + hp.w_entropy * inv_B * pr[o] * (lp[o] + Hent);
-    } else {
-        float mu = z[0], raw = z[1];
-        float sp = softplus_f(raw);
-        float sigma = fminf(fmaxf(sp, hp.min_sigma), hp.max_sigma);
-        bool clamped = sp < hp.min_sigma || sp > hp.max_sigma;
-        float a = a_bits;
-        logp_a = normlogpdf1(mu, sigma, a);
-        float Hent = logf(sigma) + 0.5f * (kLog2Pi + 1.0f);
-        r.l1 = Hent;
-        if (hp.algo == 0) {
-            float ratio = expf(logp_a - lp_old);
-            float u = ratio * A;
-            float rc = fminf(fmaxf(ratio, 1.0f - hp.clip_range), 1.0f + hp.clip_range);
-            float cc = rc * A;
-            r.l0 = -fminf(u, cc);
-            bool inside = ratio >= 1.0f - hp.clip_range && ratio <= 1.0f + hp.clip_range;
-            gsel = (u < cc || inside) ? u : 0.f;
-        } else {
-            r.l0 = -(logp_a * A);
-            gsel = A;
-        }
-        float dlogp = -hp.w_actor * inv_B * gsel;
-        float sgm = sigma + 1e-8f, dd = a - mu;
-        r.dz[0] = dlogp * (dd / (sgm * sgm));
-        float dsig = dlogp * (-1.0f / sgm + (dd * dd) / (sgm * sgm * sgm)) - hp.w_entropy * inv_B * (1.0f / sigma);
-        r.dz[1] = clamped ? 0.f : dsig * sigmoid_f(raw);
-    }
-    return r;
-}
-
 #ifdef B200RL_K7_TIMING   // debug build only: per-phase cycle sums seen by one watched worker thread
 __device__ unsigned long long g_k7_phase[40];
 __device__ int g_k7_watch = 0;   // watched worker thread (low 16 bits) of CTA (high bits; CTAs below n_actor = actor) whose timeline is recorded
@@ -321,13 +206,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             sm.W3[k] = o < d.nout ? p[head_w<false>(d, o, j)] : 0.f;
         }
         if (tid < kNo) sm.b3[tid] = tid < d.nout ? p[head_b<false>(d, tid)] : 0.f;
-        for (int k = tid; k < H * H; k += NT7_ALL) {
-            int o = k % H, i = k / H;
-            const float w = W2[k] * kScaleW;
-            const __half wh = __float2half_rn(w), wl = __float2half_rn(w - __half2float(wh));
-            *reinterpret_cast<__half*>(sm.B1 + wimg_off(o, i)) = wh;
-            *reinterpret_cast<__half*>(sm.B1 + wimg_off(H + o, i)) = wl;
-        }
+        tcfwd::fill_w2_image<NT7_ALL>(sm.B1, W2);
     }
     // constant B operand of the db2 GEMM: feature 0 = 1.0 (fp16 0x3C00) for every sample, the rest 0 (the XT buffers are written whole by publish())
     for (int k = tid; k < 2 * TM; k += NT7_ALL)
@@ -604,7 +483,8 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             for (int o = 0; o < kNo; ++o)
                 z[o] = sm.b3[o] + ((sm.Zp[o * TM + s] + sm.Zp[(kNo + o) * TM + s]) + (sm.Zp[(2 * kNo + o) * TM + s] + sm.Zp[(3 * kNo + o) * TM + s]));
             const bool valid = (tile * TM + s) < b.B;
-            LossOut lo_ = sample_loss(actor, role, hp, b.inv_B, z, aux[0], aux[1], aux[2], aux[3]);
+            // (evaluated by all four feature-block threads of a sample: identical arithmetic on each)
+            const policy::LossOut<kNo> lo_ = policy::sample_loss(actor.heads2, actor.nout, role, hp, b.inv_B, z, aux[0], aux[1], aux[2], aux[3]);
             float dz[kNo];
 #pragma unroll
             for (int o = 0; o < kNo; ++o) dz[o] = valid ? lo_.dz[o] : 0.f;

@@ -10,8 +10,9 @@
 // Thread <-> data: warp w: sample quadrant q = w % 4 (samples 32q .. 32q+31), column half c = w / 4; thread = sample
 // s = 32q + lane, features 32c .. 32c+31.  The tile image holds, per 64-sample block, the A operand [hi 8 KB | lo 8 KB]; once
 // the block's wgmmas have completed, the warpgroup that ran them overwrites it with the FP32 accumulator (64 x 64).  Every
-// multiply-add is an explicit fmaf / separate op: the arithmetic does not depend on the contraction flags of the including
-// translation unit.
+// multiply-add of the forward pass is an explicit fmaf / separate op: its arithmetic does not depend on the contraction flags of
+// the including translation unit.  The operand format (split2, wimg_off, the W2 image) is shared with the tensor-core backward
+// (nn_tc.cu).
 #pragma once
 #include "nn.cuh"
 #include "wgmma.cuh"
@@ -27,7 +28,6 @@ constexpr int WIMG_BYTES = 16 * GW_S; // [hi (64 rows) ; lo (64 rows)] x [K = 64
 constexpr int BLK = 8 * GW_S * 2;     // one 64-sample block of the tile image: A operand [hi | lo], later its FP32 accumulator
 constexpr int TILE_BYTES = 2 * BLK;
 constexpr float kScale = 64.0f;       // power-of-two scale of both operands (exact; undone on the accumulator)
-constexpr float kLog2Pi = 1.8378770664093453f;
 
 struct NetSm {   // one network's weights in shared memory
     alignas(128) uint8_t B[WIMG_BYTES];        // 64 W2 as (n = out, k = in), K-major fp16: rows 0..63 hi, 64..127 lo (one N = 128 operand)
@@ -37,21 +37,29 @@ struct NetSm {   // one network's weights in shared memory
     float b3[kOutMax];
 };
 
-__device__ __forceinline__ float act_f(int act, float z) { return act == B200RL_ACT_RELU ? fmaxf(z, 0.f) : tanhf(z); }
-// two fp32 values -> packed fp16 pairs {low half = a, high half = b}: hi parts, and the fp16 of what they miss (lo parts)
+// two fp32 values -> packed fp16 pairs {low half = a, high half = b}: hi parts, and the fp16 of what they miss (lo parts).
+// (The subtraction is plain: in the tensor-core backward, compiled with contraction, it may fuse with the multiply that made
+// a or b, as it always has; the forward's operands come from rounded operations, so nothing can fuse there.)
 __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
     const __half2 h = __floats2half2_rn(a, b);
     const float2 back = __half22float2(h);
-    const __half2 l = __floats2half2_rn(__fsub_rn(a, back.x), __fsub_rn(b, back.y));
+    const __half2 l = __floats2half2_rn(a - back.x, b - back.y);
     hi = *reinterpret_cast<const uint32_t*>(&h);
     lo = *reinterpret_cast<const uint32_t*>(&l);
 }
-__device__ __forceinline__ float softplus_f(float x) { return x > 0.f ? x + log1pf(expf(-x)) : log1pf(expf(x)); }
-__device__ __forceinline__ float normlogpdf1(float mu, float sigma, float x) {   // distributions.jl:18-21, eps = 1f-8
-    float s = sigma + 1e-8f, v = __fmul_rn(s, s), dd = x - mu;
-    return __fmul_rn(-0.5f, (logf(v) + __fmul_rn(dd, dd) / v) + kLog2Pi);
-}
 __device__ __forceinline__ uint32_t wimg_off(int n, int k) { return (uint32_t)((n >> 3) * GW_S + (k >> 3) * G_F + (n & 7) * 16 + (k & 7) * 2); }
+// W2 (Flux layout W2[o + H*i]) -> the B operand image of a CTA of NTHREADS threads: kScale W2 as (n = out o, k = in i), K-major
+// fp16, rows 0..63 hi, 64..127 lo.  kScale is a power of two, so the product is exact with or without contraction.
+template <int NTHREADS>
+__device__ __forceinline__ void fill_w2_image(uint8_t* img, const float* W2) {
+    for (int k = threadIdx.x; k < H * H; k += NTHREADS) {
+        const int o = k % H, i = k / H;
+        const float v = W2[k] * kScale;
+        const __half vh = __float2half_rn(v), vl = __float2half_rn(v - __half2float(vh));
+        *reinterpret_cast<__half*>(img + wimg_off(o, i)) = vh;
+        *reinterpret_cast<__half*>(img + wimg_off(H + o, i)) = vl;
+    }
+}
 // FP32 accumulator of one block, row r, column col: 16-byte units XOR-swizzled by the row, so that 8 consecutive rows read
 // at the same column hit 8 different bank groups
 __device__ __forceinline__ uint32_t dacc_off(int r, int col) { return (uint32_t)(r * 256 + (((col >> 2) ^ (r & 15)) << 4) + (col & 3) * 4); }
@@ -72,26 +80,8 @@ __device__ inline void load_net(NetSm& w, const MlpDesc& d, const float* __restr
         w.W3[k] = o < rows_of<MAY_DUEL>(d) ? p[head_w<MAY_DUEL>(d, o, j)] : 0.f;
     }
     if (tid < kOutMax) w.b3[tid] = tid < rows_of<MAY_DUEL>(d) ? p[head_b<MAY_DUEL>(d, tid)] : 0.f;
-    for (int k = tid; k < H * H; k += NT) {   // W2[o + H*i]: B operand of H2pre[s][o] = sum_i H1[s][i] W2[o][i]
-        int o = k % H, i = k / H;
-        const float v = __fmul_rn(W2[k], kScale);
-        const __half vh = __float2half_rn(v), vl = __float2half_rn(__fsub_rn(v, __half2float(vh)));
-        *reinterpret_cast<__half*>(w.B + wimg_off(o, i)) = vh;
-        *reinterpret_cast<__half*>(w.B + wimg_off(H + o, i)) = vl;
-    }
+    fill_w2_image<NT>(w.B, W2);   // B operand of H2pre[s][o] = sum_i H1[s][i] W2[o][i]
 }
-
-// Xoshiro256++ on a 4-word state held in registers (policy stream of one env)
-__device__ __forceinline__ unsigned long long xo_next(unsigned long long (&s)[4]) {
-    unsigned long long tmp = s[0] + s[3];
-    unsigned long long res = ((tmp << 23) | (tmp >> 41)) + s[0];
-    unsigned long long t = s[1] << 17;
-    s[2] ^= s[0]; s[3] ^= s[1]; s[1] ^= s[2]; s[0] ^= s[3]; s[2] ^= t;
-    s[3] = (s[3] << 45) | (s[3] >> 19);
-    return res;
-}
-__device__ __forceinline__ double xo_f64(unsigned long long (&s)[4]) { return (double)(xo_next(s) >> 11) * 0x1p-53; }
-__device__ __forceinline__ float xo_f32(unsigned long long (&s)[4]) { return (float)((unsigned)(xo_next(s) >> 32) >> 8) * 0x1p-24f; }
 
 // layer 1 of this thread's sample: H1[32c .. 32c+32) = act(W1 x + b1) -> A operand of its block (hi at +0, lo at +8 KB; the
 // image layout of the weights, row = sample)
@@ -187,48 +177,6 @@ __device__ __forceinline__ void head_partials(const NetSm& w, int act_rt, int c,
             zp[0] = fmaf(ww.x, h2, zp[0]); zp[1] = fmaf(ww.y, h2, zp[1]); zp[2] = fmaf(ww.z, h2, zp[2]); zp[3] = fmaf(ww.w, h2, zp[3]);
         }
     }
-}
-
-// one Gumbel(0, 1) draw in Float64 (one out-of-line copy: the double-precision log is ~150 instructions)
-__device__ __noinline__ double gumbel64(double u) { return -log(-log(u)); }
-
-// policy head: sample an action and its log-probability from the head outputs z on the env's policy stream.
-// Categorical: sample_categorical (networks.jl:425-432), Float64 Gumbel noise; Gaussian: GaussianNetwork (networks.jl:64-116).
-// Returns the action as raw 32 bits (int32 1-based | float).
-__device__ __forceinline__ uint32_t sample_head(const MlpDesc& actor, const AcHyper& hp, const float (&z)[kOutMax], unsigned long long (&st)[4],
-                                                float& logp) {
-    if (!actor.heads2) {
-        const int na = actor.nout;
-        float lp[kOutMax];
-        float m = -3.4e38f;
-#pragma unroll
-        for (int o = 0; o < kOutMax; ++o) if (o < na) m = fmaxf(m, z[o]);
-        float se = 0.f;
-#pragma unroll
-        for (int o = 0; o < kOutMax; ++o) if (o < na) se += expf(z[o] - m);
-        float ls = logf(se);
-        int best = 0;
-        double bv = 0.0;
-        float blp = 0.f;
-#pragma unroll
-        for (int o = 0; o < kOutMax; ++o) {
-            if (o < na) {
-                lp[o] = (z[o] - m) - ls;
-                double u = xo_f64(st);
-                double gv = gumbel64(u) + (double)lp[o];
-                if (o == 0 || gv > bv) { bv = gv; best = o; blp = lp[o]; }
-            }
-        }
-        logp = blp;
-        return (uint32_t)(best + 1);
-    }
-    float mu = z[0], raw = z[1];
-    float sigma = fminf(fmaxf(softplus_f(raw), hp.min_sigma), hp.max_sigma);
-    float u1 = xo_f32(st), u2 = xo_f32(st);
-    float n = __fmul_rn(sqrtf(__fmul_rn(-2.0f, logf(1.0f - u1))), cosf(__fmul_rn(6.2831855f, u2)));
-    float a = __fadd_rn(mu, __fmul_rn(sigma, n));
-    logp = normlogpdf1(mu, sigma, a);
-    return __float_as_uint(a);
 }
 
 }  // namespace tcfwd

@@ -19,42 +19,12 @@
 // A push is one thread per lane (neighbouring lanes write neighbouring addresses unless their episode counts differ);
 // a sample is one thread per batch slot: Xoshiro draw -> (rejection | sum-tree descent) -> 2 x state gather + scalars.
 #include "common.cuh"
+#include "explore.cuh"   // the sampler streams (Xoshiro256++)
 #include "internal.h"
 #include "nstep.cuh"
 #include "ring.cuh"
 
 namespace {
-
-struct Xo4 { unsigned long long s[4]; };
-__device__ __forceinline__ Xo4 load_xo(const unsigned long long* rng, int64_t i) {
-    const ulonglong2* p = reinterpret_cast<const ulonglong2*>(rng + 4 * i);
-    ulonglong2 a = p[0], b = p[1];
-    Xo4 g; g.s[0] = a.x; g.s[1] = a.y; g.s[2] = b.x; g.s[3] = b.y;
-    return g;
-}
-__device__ __forceinline__ void store_xo(unsigned long long* rng, int64_t i, const Xo4& g) {
-    ulonglong2* p = reinterpret_cast<ulonglong2*>(rng + 4 * i);
-    p[0] = make_ulonglong2(g.s[0], g.s[1]);
-    p[1] = make_ulonglong2(g.s[2], g.s[3]);
-}
-__device__ __forceinline__ unsigned long long xo_next(Xo4& g) {
-    unsigned long long tmp = g.s[0] + g.s[3];
-    unsigned long long res = ((tmp << 23) | (tmp >> 41)) + g.s[0];
-    unsigned long long t = g.s[1] << 17;
-    g.s[2] ^= g.s[0]; g.s[3] ^= g.s[1]; g.s[1] ^= g.s[2]; g.s[0] ^= g.s[3]; g.s[2] ^= t;
-    g.s[3] = (g.s[3] << 45) | (g.s[3] >> 19);
-    return res;
-}
-// rand(rng, Base.OneTo(n)) - 1  (Lemire nearly-divisionless, Julia SamplerRangeNDL)
-__device__ __forceinline__ unsigned long long rand_below(Xo4& g, unsigned long long n) {
-    unsigned long long x = xo_next(g);
-    unsigned long long hi = __umul64hi(x, n), lo = x * n;
-    if (lo < n) {
-        unsigned long long t = (0ull - n) % n;
-        while (lo < t) { x = xo_next(g); hi = __umul64hi(x, n); lo = x * n; }
-    }
-    return hi;
-}
 
 // ---- push kernels: one thread per lane (ring.cuh); `keys`/`vals` (3 per lane) receive the sum-tree leaves to rewrite (key -1 = none)
 __device__ __forceinline__ void emit_leaves(int64_t e, const RingLeaves& lv, int64_t* __restrict__ keys, float* __restrict__ vals) {
@@ -150,13 +120,14 @@ __global__ void __launch_bounds__(128) sample_gather_kernel(Ring r, unsigned lon
     }
     int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= B) return;
-    Xo4 g = load_xo(slots, k);
+    unsigned long long g[4];
+    explore::xo_load(slots, k, g);
     const int64_t F = r.frames();
     int64_t key;
     float p = 0.f, w = 1.f;
     if (PRIO) {
         const float total = top[1];
-        float v = ((float)((unsigned)(xo_next(g) >> 32) >> 8) * 0x1p-24f) * total;  // rand(rng, Float32) * total
+        float v = explore::xo_f32(g) * total;  // rand(rng, Float32) * total
         int64_t node = 1;
         while (node < r.L) {     // never step into an empty subtree: float rounding cannot land on a zero-priority leaf
             const int64_t l = 2 * node;
@@ -175,7 +146,7 @@ __global__ void __launch_bounds__(128) sample_gather_kernel(Ring r, unsigned lon
         const unsigned long long n = (unsigned long long)(r.lanes * r.cap);
         key = -1;
         for (int tries = 0; tries < 4096; ++tries) {
-            const int64_t q = (int64_t)rand_below(g, n);
+            const int64_t q = (int64_t)explore::xo_below(g, n);
             const int64_t e = q % r.lanes, j = q / r.lanes;
             const int64_t cnt = r.count[e];
             if (j >= cnt - 1) continue;
@@ -184,7 +155,7 @@ __global__ void __launch_bounds__(128) sample_gather_kernel(Ring r, unsigned lon
         }
         if (key < 0) __trap();   // (practically) nothing sampleable
     }
-    store_xo(slots, k, g);
+    explore::xo_store(slots, k, g);
     const int64_t slot = key / r.lanes, e = key % r.lanes;
     NStepWindow win;
     if (NSTEP) win = nstep::window(r, key, nsa.n, nsa.gamma);
