@@ -264,8 +264,8 @@ int b200rl_traj_total_priority(b200rl_traj* traj, float* out);
  *         Flat vector: trunk, Wv (1 x hidden), bv, Wa (n_out x hidden), ba — Flux.destructure(DuelingNetwork(...)) as it is.
  * Trunks are Dense(n_in,hidden,act) -> Dense(hidden,hidden,act); act 0 relu, 1 tanh; hidden 64|128.
  * Parameters are one flat fp32 vector in Flux.destructure order (weights (out,in) column-major).
- * Q-network entry points (kinds 2 and 3): net_values, net_q_act, net_q_explore, net_act_greedy, evaluate mode 0, dqn_update,
- * dqn_last_td, replay_create.  Actor-critic entry points (kinds 0 and 1): net_act, net_ac_step, onpolicy_create, evaluate
+ * Q-network entry points (kinds 2 and 3): net_values, net_q_act, net_q_explore, net_act_greedy, evaluate mode 0, evaluate_explore,
+ * dqn_update, dqn_last_td, replay_create.  Actor-critic entry points (kinds 0 and 1): net_act, net_ac_step, onpolicy_create, evaluate
  * mode 1; they refuse kinds 2 and 3 before any side effect. */
 typedef struct { int32_t n_in, hidden, act, n_out, kind; } b200rl_net_desc;
 int b200rl_net_nparams(const b200rl_net_desc* desc, int64_t* out);
@@ -334,6 +334,17 @@ int b200rl_net_act_greedy(b200rl_net* net, const float* obs, int64_t n, void* ac
 typedef struct { int32_t mode, n_steps, max_episodes; } b200rl_eval_config;   /* mode 0 greedy, 1 sample */
 int b200rl_evaluate(b200rl_net* net, b200rl_env* env, const b200rl_eval_config* cfg, uint64_t* policy_rng_dev,
                     float* returns_out, int32_t* lengths_out, int32_t* counts_out, int on_device);
+/* run(QBasedPolicy(learner, explorer), env, StopAfterNSteps(n_steps)) for a Q-network (kinds 2 and 3; a dueling head combined into Q
+ * first): reset!(env; is_force = true) for every env, then n_steps x {plan!, act!} where plan! is b200rl_net_q_explore's BatchExplorer
+ * — column i at window step k is planned at explorer step ex->step + k N + i on its stream explorer_rng_dev[:, i] — or, ex = NULL,
+ * GreedyExplorer (the first maximum under `>`, b200rl_net_q_act with epsilon = 0; no draw, no streams needed).  Outputs, env side
+ * effects and on_device as b200rl_evaluate; the (4, N) DEVICE explorer streams are advanced in place and, on success, ex->step by
+ * N n_steps (as b200rl_replay_run).  The network (its update counter and target too) is only read.  Refused before any side effect:
+ * B200RL_ERR_UNSUPPORTED for Float64, Acrobot and continuous-action envs; B200RL_ERR_INVALID for a network that is not a Q-network,
+ * an input / head width that does not match the env, n_steps < 1, max_episodes < 0, an explorer without streams and a bad explorer
+ * (see b200rl_explorer).  One fused launch for hidden = 64 on the tensor-core path. */
+int b200rl_evaluate_explore(b200rl_net* net, b200rl_env* env, int32_t n_steps, int32_t max_episodes, b200rl_explorer* ex,
+                            uint64_t* explorer_rng_dev, float* returns_out, int32_t* lengths_out, int32_t* counts_out, int on_device);
 
 /* ---------------------------------------------------------------- on-policy agent -- */
 /* PPO (clipped surrogate) / A2C hyper-parameters; defaults of the in-tree example

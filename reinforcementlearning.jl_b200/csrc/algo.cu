@@ -249,6 +249,79 @@ static int make_descs(const b200rl_net_desc* d, MlpDesc* actor, MlpDesc* critic)
     return B200RL_OK;
 }
 
+// device buffers of an evaluation window: the records, and the staged path's per-env accumulators, actions and head outputs
+struct EvalBufs {
+    float* ret;                   // (K, N), null when the caller wants no returns
+    int32_t* len;                 // (K, N), null when the caller wants no lengths
+    int32_t* cnt;                 // (N)
+    float* acc_ret;
+    int32_t* acc_len;
+    uint32_t* act;
+    float* act_clamped;
+    float* heads;                 // (nout, N)
+};
+
+// The flow of b200rl_evaluate and b200rl_evaluate_explore after their checks: the device records (the caller's, on_device, or
+// scratch holding the caller's values, so that slots the window does not fill keep them), reset!(env; is_force = true) (run.jl:46),
+// the fused window fused(bufs) or, where it returns B200RL_ERR_UNSUPPORTED, n_steps x {plan!, act! (auto-reset), record} as staged
+// launches without a host sync, then the copy-out.  plan(k, bufs, &a_env) launches plan! of window step k and sets the actions the
+// env receives.
+template <class Fused, class Plan>
+static int eval_window(b200rl_ctx* ctx, b200rl_env* env, int nout, int nsteps, int K, float* returns_out, int32_t* lengths_out,
+                       int32_t* counts_out, int on_device, Fused&& fused, Plan&& plan) {
+    const int64_t N = b200rl_env_internal_n(env);
+    const size_t rec_bytes = (size_t)N * K * 4;
+    auto round256 = [](size_t b) { return (b + 255) / 256 * 256; };
+    // device buffers: the caller's (on_device) or scratch; the staged path also keeps per-env accumulators and its actions
+    size_t off = 0;
+    const size_t o_ret = off; off += on_device ? 0 : round256(rec_bytes);
+    const size_t o_len = off; off += on_device ? 0 : round256(rec_bytes);
+    const size_t o_cnt = off; off += round256((size_t)N * 4);
+    const size_t o_acc = off; off += round256((size_t)N * 4) * 2;
+    const size_t o_act = off; off += round256((size_t)N * 4) * 2;
+    const size_t o_heads = off; off += round256((size_t)N * nout * 4);
+    void* sc;
+    TRY(ctx_scratch(ctx, off, &sc));
+    char* base = (char*)sc;
+    EvalBufs b;
+    b.ret = returns_out ? (on_device ? returns_out : (float*)(base + o_ret)) : nullptr;
+    b.len = lengths_out ? (on_device ? lengths_out : (int32_t*)(base + o_len)) : nullptr;
+    b.cnt = (on_device && counts_out) ? counts_out : (int32_t*)(base + o_cnt);
+    b.acc_ret = (float*)(base + o_acc);
+    b.acc_len = (int32_t*)(base + o_acc + round256((size_t)N * 4));
+    b.act = (uint32_t*)(base + o_act);
+    b.act_clamped = (float*)(base + o_act + round256((size_t)N * 4));
+    b.heads = (float*)(base + o_heads);
+    if (!on_device) {   // record slots the window does not fill keep the caller's values
+        if (b.ret && rec_bytes) CUDA_TRY(cudaMemcpyAsync(b.ret, returns_out, rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
+        if (b.len && rec_bytes) CUDA_TRY(cudaMemcpyAsync(b.len, lengths_out, rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    TRY(b200rl_env_reset(env, 1));   // reset!(env; is_force = true), run.jl:46
+    int st = nn_tc_enabled() ? fused(b) : B200RL_ERR_UNSUPPORTED;
+    if (st == B200RL_ERR_UNSUPPORTED) {   // staged: plan! -> act! (auto-reset) -> record, n_steps times, no host sync
+        CUDA_TRY(cudaMemsetAsync(b.cnt, 0, (size_t)N * 4, ctx->stream));
+        CUDA_TRY(cudaMemsetAsync(b.acc_ret, 0, round256((size_t)N * 4) * 2, ctx->stream));
+        const float* rew = (const float*)env_field(env, B200RL_FIELD_REWARD);
+        const uint8_t* flags = (const uint8_t*)env_field(env, B200RL_FIELD_FLAGS);
+        for (int k = 0; k < nsteps; ++k) {
+            const void* a_env = b.act;
+            TRY(plan(k, b, &a_env));
+            TRY(b200rl_env_step(env, a_env, 1, 1));
+            eval_record_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(rew, flags, N, K, b.acc_ret, b.acc_len, b.cnt, b.ret, b.len);
+            LAUNCH_CHECK(ctx);
+        }
+    } else if (st != B200RL_OK) {
+        return st;
+    }
+    if (!on_device) {
+        if (returns_out && rec_bytes) CUDA_TRY(cudaMemcpyAsync(returns_out, b.ret, rec_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        if (lengths_out && rec_bytes) CUDA_TRY(cudaMemcpyAsync(lengths_out, b.len, rec_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        if (counts_out) CUDA_TRY(cudaMemcpyAsync(counts_out, b.cnt, (size_t)N * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    }
+    return B200RL_OK;
+}
+
 extern "C" {
 
 int b200rl_net_nparams(const b200rl_net_desc* d, int64_t* out) {
@@ -524,69 +597,66 @@ int b200rl_evaluate(b200rl_net* n, b200rl_env* env, const b200rl_eval_config* cf
     b200rl_ctx* ctx = n->ctx;
     const int64_t N = b200rl_env_internal_n(env);
     const int K = cfg->max_episodes, mode = cfg->mode, nsteps = cfg->n_steps;
-    const size_t rec_bytes = (size_t)N * K * 4;
-    auto round256 = [](size_t b) { return (b + 255) / 256 * 256; };
-    // device buffers: the caller's (on_device) or scratch; the staged path also keeps per-env accumulators and its actions
-    size_t off = 0;
-    const size_t o_ret = off; off += on_device ? 0 : round256(rec_bytes);
-    const size_t o_len = off; off += on_device ? 0 : round256(rec_bytes);
-    const size_t o_cnt = off; off += round256((size_t)N * 4);
-    const size_t o_acc = off; off += round256((size_t)N * 4) * 2;
-    const size_t o_act = off; off += round256((size_t)N * 4) * 2;
-    const size_t o_heads = off; off += round256((size_t)N * n->actor.nout * 4);
-    void* sc;
-    TRY(ctx_scratch(ctx, off, &sc));
-    char* base = (char*)sc;
-    float* dret = returns_out ? (on_device ? returns_out : (float*)(base + o_ret)) : nullptr;
-    int32_t* dlen = lengths_out ? (on_device ? lengths_out : (int32_t*)(base + o_len)) : nullptr;
-    int32_t* dcnt = (on_device && counts_out) ? counts_out : (int32_t*)(base + o_cnt);
-    if (!on_device) {   // record slots the window does not fill keep the caller's values
-        if (dret && rec_bytes) CUDA_TRY(cudaMemcpyAsync(dret, returns_out, rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
-        if (dlen && rec_bytes) CUDA_TRY(cudaMemcpyAsync(dlen, lengths_out, rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    }
     const AcHyper& hp = kSamplerHyper;
     unsigned long long* prng = (unsigned long long*)policy_rng_dev;
-    TRY(b200rl_env_reset(env, 1));   // reset!(env; is_force = true), run.jl:46
-    int st = nn_tc_enabled() ? nn_tc_evaluate(ctx, env, n->actor, n->params, hp, mode, nsteps, K, prng, dret, dlen, dcnt) : B200RL_ERR_UNSUPPORTED;
-    if (st == B200RL_ERR_UNSUPPORTED) {   // staged: plan! -> act! (auto-reset) -> record, n_steps times, no host sync
-        float* acc_ret = (float*)(base + o_acc);
-        int32_t* acc_len = (int32_t*)(base + o_acc + round256((size_t)N * 4));
-        uint32_t* act = (uint32_t*)(base + o_act);
-        float* act_clamped = (float*)(base + o_act + round256((size_t)N * 4));
-        float* heads = (float*)(base + o_heads);
-        CUDA_TRY(cudaMemsetAsync(dcnt, 0, (size_t)N * 4, ctx->stream));
-        CUDA_TRY(cudaMemsetAsync(acc_ret, 0, round256((size_t)N * 4) * 2, ctx->stream));
-        const float* obs = (const float*)env_field(env, B200RL_FIELD_OBS);
-        const float* rew = (const float*)env_field(env, B200RL_FIELD_REWARD);
-        const uint8_t* flags = (const uint8_t*)env_field(env, B200RL_FIELD_FLAGS);
-        const float bound = b200rl_env_internal_action_bound(env);
-        for (int k = 0; k < nsteps; ++k) {
-            const void* a_env = act;
+    const float* obs = (const float*)env_field(env, B200RL_FIELD_OBS);
+    const float bound = b200rl_env_internal_action_bound(env);
+    return eval_window(
+        ctx, env, n->actor.nout, nsteps, K, returns_out, lengths_out, counts_out, on_device,
+        [&](const EvalBufs& b) -> int { return nn_tc_evaluate(ctx, env, n->actor, n->params, hp, mode, nsteps, K, prng, b.ret, b.len, b.cnt); },
+        [&](int, const EvalBufs& b, const void** a_env) -> int {
             if (mode == 0) {
-                TRY(nn_mlp_forward(ctx, n->actor, n->params, obs, N, heads));
-                greedy_select_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(heads, n->actor, N, cont ? 1 : 0, -bound, bound, act);
+                TRY(nn_mlp_forward(ctx, n->actor, n->params, obs, N, b.heads));
+                greedy_select_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(b.heads, n->actor, N, cont ? 1 : 0, -bound, bound, b.act);
                 LAUNCH_CHECK(ctx);
             } else {
-                TRY(nn_policy_act(ctx, n->actor, n->critic, n->params, hp, obs, N, prng, act, nullptr, nullptr, nullptr, nullptr));
+                TRY(nn_policy_act(ctx, n->actor, n->critic, n->params, hp, obs, N, prng, b.act, nullptr, nullptr, nullptr, nullptr));
                 if (cont) {
-                    clamp_copy_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(act_clamped, (const float*)act, N, -bound, bound);
+                    clamp_copy_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(b.act_clamped, (const float*)b.act, N, -bound, bound);
                     LAUNCH_CHECK(ctx);
-                    a_env = act_clamped;
+                    *a_env = b.act_clamped;
                 }
             }
-            TRY(b200rl_env_step(env, a_env, 1, 1));
-            eval_record_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(rew, flags, N, K, acc_ret, acc_len, dcnt, dret, dlen);
-            LAUNCH_CHECK(ctx);
-        }
-    } else if (st != B200RL_OK) {
-        return st;
+            return B200RL_OK;
+        });
+}
+
+/* run(QBasedPolicy(learner, explorer), env, StopAfterNSteps(n_steps)); see b200rl.h.  Fused into one launch (fwd_tc.cu) for H = 64
+ * on the tensor-core path, otherwise q_explore | q_act, act! and record launches per step with the same arithmetic. */
+int b200rl_evaluate_explore(b200rl_net* n, b200rl_env* env, int32_t n_steps, int32_t max_episodes, b200rl_explorer* ex,
+                            uint64_t* explorer_rng_dev, float* returns_out, int32_t* lengths_out, int32_t* counts_out, int on_device) {
+    REQUIRE(n && env, B200RL_ERR_INVALID, "null argument");
+    REQUIRE(b200rl_env_internal_ctx(env) == n->ctx, B200RL_ERR_INVALID, "net/env belong to another ctx");
+    REQUIRE(b200rl_env_internal_dtype(env) == B200RL_F32, B200RL_ERR_UNSUPPORTED, "the Q-network reads Float32 observations: construct the env with T = Float32");
+    REQUIRE(b200rl_env_internal_kind(env) != B200RL_ENV_ACROBOT, B200RL_ERR_UNSUPPORTED, "AcrobotEnv has 6 observations (networks take at most 4)");
+    REQUIRE(!b200rl_env_internal_continuous(env), B200RL_ERR_UNSUPPORTED, "QBasedPolicy needs a discrete action space");
+    REQUIRE(is_q_kind(n->kind), B200RL_ERR_INVALID, "needs a Q-network (kind 2 or 3)");
+    REQUIRE(b200rl_env_internal_nobs(env) == n->actor.in, B200RL_ERR_INVALID, "network input width != observation width");
+    REQUIRE(n->actor.nout == b200rl_env_internal_n_actions(env), B200RL_ERR_INVALID, "Q head width != number of discrete actions");
+    REQUIRE(n_steps >= 1, B200RL_ERR_INVALID, "n_steps must be >= 1");
+    REQUIRE(max_episodes >= 0, B200RL_ERR_INVALID, "max_episodes must be >= 0");
+    const int64_t N = b200rl_env_internal_n(env);
+    if (ex) {
+        REQUIRE(explorer_rng_dev, B200RL_ERR_INVALID, "an explorer other than GreedyExplorer needs the (4, N) device explorer streams");
+        TRY(check_explorer(ex));
+        REQUIRE(n_steps <= ((1ll << 62) - (ex->step > 0 ? ex->step : 0)) / N, B200RL_ERR_INVALID, "explorer step would overflow");
     }
-    if (!on_device) {
-        if (returns_out && rec_bytes) CUDA_TRY(cudaMemcpyAsync(returns_out, dret, rec_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        if (lengths_out && rec_bytes) CUDA_TRY(cudaMemcpyAsync(lengths_out, dlen, rec_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        if (counts_out) CUDA_TRY(cudaMemcpyAsync(counts_out, dcnt, (size_t)N * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    }
+    TRY(ctx_bind(n->ctx));
+    b200rl_ctx* ctx = n->ctx;
+    unsigned long long* xrng = (unsigned long long*)explorer_rng_dev;
+    const float* obs = (const float*)env_field(env, B200RL_FIELD_OBS);
+    TRY(eval_window(
+        ctx, env, n->actor.nout, n_steps, max_episodes, returns_out, lengths_out, counts_out, on_device,
+        [&](const EvalBufs& b) -> int {
+            return nn_tc_evaluate(ctx, env, n->actor, n->params, kSamplerHyper, 2, n_steps, max_episodes, xrng, b.ret, b.len, b.cnt, ex);
+        },
+        [&](int k, const EvalBufs& b, const void**) -> int {
+            if (!ex) return nn_q_act(ctx, n->actor, n->params, obs, N, nullptr, 0.0f, (int32_t*)b.act, b.heads);   // GreedyExplorer
+            b200rl_explorer e = *ex;
+            e.step = ex->step + (int64_t)k * N;     // BatchExplorer: the inner explorer's step moved N times per plan!
+            return nn_q_explore(ctx, n->actor, n->params, obs, N, xrng, e, (int32_t*)b.act, b.heads);
+        }));
+    if (ex) ex->step += (int64_t)n_steps * N;
     return B200RL_OK;
 }
 

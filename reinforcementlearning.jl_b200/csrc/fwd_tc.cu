@@ -5,8 +5,9 @@
 //                        write the transition into column t of the rollout tensors }.  A CTA owns up to two tiles of 128
 //                        envs for the whole launch; their env state and both RNG streams stay in shared memory, the weights of
 //                        both networks too.  Replaces 2 launches per env step (agent_base.jl:45-66 stage loop, run.jl:52-68).
-//   evaluate_tc_kernel : n_steps x { obs -> actor -> greedy | sampled action -> env step (+ fused auto-reset) -> per-env episode
-//                        records }: the actor alone, no rollout tensors (b200rl_evaluate).
+//   evaluate_tc_kernel : n_steps x { obs -> actor -> greedy | sampled action (or Q -> explorer action) -> env step (+ fused
+//                        auto-reset) -> per-env episode records }: one network, no rollout tensors (b200rl_evaluate,
+//                        b200rl_evaluate_explore).
 //   replay_collect_tc_kernel : n_steps x { obs -> Q -> explorer action -> env step (+ fused auto-reset) -> replay ring push }.
 //
 // The kernels share one tile forward (tile_forward), one resident env slot with its load / write-back (EnvSlot) and the act! step
@@ -239,6 +240,38 @@ __device__ __forceinline__ ActStep<float> slot_act(EnvSlot<Env>& sl, int s, cons
     return r;
 }
 
+// b200rl_explorer without its trailing beta, which the kernels that plan with it take separately: the parameters the ϵ-greedy
+// instantiations read keep the offsets they had before the explorer struct grew
+struct QExplorer {
+    double eps_stable, eps_init;
+    int64_t warmup_steps, decay_steps, step;
+    int32_t kind, is_break_tie;
+};
+// plan!(QBasedPolicy) of owner thread s's column on its Q-values z, 1-based: GreedyExplorer (greedy: the first maximum under `>`,
+// q_act_kernel with epsilon = 0, no draw) or the BatchExplorer column of explore.cuh at explorer step `step` on the column's stream,
+// kept in the slot's transposed array w.  XEXT: the explorer kinds 2-4 (speedy, weighted / Gumbel softmax; explore::select<true>),
+// which read beta; without it only the ϵ-greedy kinds 0 / 1 are compiled.  The fused collect and the fused evaluation plan with it.
+template <bool XEXT>
+__device__ __forceinline__ int plan_q_column(bool greedy, const QExplorer& ex, double beta, long long step, const float* z, int na,
+                                             unsigned long long* w, int s) {
+    if (greedy) {
+        int best = 0;
+        for (int o = 1; o < na; ++o) if (z[o] > z[best]) best = o;
+        return best + 1;
+    }
+    unsigned long long xr[4];
+    get_stream(w, s, xr);
+    int a1;
+    if constexpr (XEXT) {
+        const b200rl_explorer e{ex.eps_stable, ex.eps_init, ex.warmup_steps, ex.decay_steps, ex.step, ex.kind, ex.is_break_tie, beta};
+        a1 = explore::select<true>(e, step, z, na, xr);
+    } else {
+        a1 = explore::select<false>(ex, step, z, na, xr);
+    }
+    put_stream(w, s, xr);
+    return a1;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // fused rollout
 template <class Env> struct RollSlot : EnvSlot<Env> {
@@ -377,7 +410,7 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
 // policy (b200rl_net_act_greedy -> nn_mlp_forward) and this kernel pick the same actions bit for bit.
 template <class Env> struct EvalSlot : EnvSlot<Env> {
     int cnt[TM];                           // episodes finished in the window
-    unsigned long long prng[4 * TM];       // policy stream (MODE 1)
+    unsigned long long prng[4 * TM];       // policy stream (MODE 1) | explorer stream (MODE 2)
 };
 template <class Env> struct SmemEval {
     alignas(128) uint8_t T[TILE_BYTES];
@@ -396,17 +429,32 @@ struct EvalArgs {
     AcHyper hp;
     int64_t N;
     int nsteps, K;
-    unsigned long long* policy_rng;     // (4, N), MODE 1
+    unsigned long long* policy_rng;     // (4, N): policy streams (MODE 1) | explorer streams (MODE 2, not greedy)
     float* returns;                     // (K, N), may be null
     int32_t* lengths;                   // (K, N), may be null
     int32_t* counts;                    // (N), may be null
 };
+// MODE 2: EvalArgs and the explorer of QBasedPolicy; column i at window step k plans at explorer step step0 + k N + i.  (A struct of
+// its own: the MODE 0 / 1 instantiations keep the kernel parameters, and the code, they had before MODE 2 existed.)
+struct EvalExploreArgs : EvalArgs {
+    int greedy;                         // 1: GreedyExplorer (the first maximum under `>`, no draw)
+    QExplorer ex;
+    double beta;
+    long long step0;
+};
+template <int MODE> using EvalArgsOf = typename std::conditional<MODE == 2, EvalExploreArgs, EvalArgs>::type;
+// the window reads and writes back a (4, N) stream per env: the policy streams (MODE 1) or the explorer streams (MODE 2, not greedy)
+template <int MODE> __device__ __forceinline__ bool eval_streams(const EvalArgsOf<MODE>& g) {
+    if constexpr (MODE == 2) return !g.greedy;
+    else return MODE == 1;
+}
 
-// MODE 0: greedy (greedy.cuh, no draw), 1: sample_head on the policy streams.  DUEL (MODE 0 only): a dueling Q-network, its head
-// rows combined into Q (duel.cuh) before the selection; the instantiations without it are the code of the other kinds.
+// MODE 0: greedy (greedy.cuh, no draw), 1: sample_head on the policy streams, 2: a Q-network planned by its explorer
+// (plan_q_column, b200rl_evaluate_explore).  DUEL (MODE 0 / 2): a dueling Q-network, its head rows combined into Q (duel.cuh) before
+// the selection; the instantiations without it are the code of the other kinds.  XEXT (MODE 2): the explorer kinds 2-4 compiled.
 // (layer 1 and the head epilogue not unrolled: the relu variants would exceed 128 registers and spill)
-template <class Env, int ACT, int MODE, bool DUEL = false>
-__global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename Env::P p, EnvArrays ea) {
+template <class Env, int ACT, int MODE, bool DUEL = false, bool XEXT = false>
+__global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgsOf<MODE> g, typename Env::P p, EnvArrays ea) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     SmemEval<Env>& sm = *reinterpret_cast<SmemEval<Env>*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -424,7 +472,7 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename
         if (owner)
             load_group(sm.slot, nslots, base, nctas, ea, N, s, [&](EvalSlot<Env>& sl, int64_t i) {
                 sl.cnt[s] = 0;
-                if (MODE == 1) {
+                if (eval_streams<MODE>(g)) {
                     unsigned long long pr[4];
                     explore::xo_load(g.policy_rng, i, pr);
                     put_stream(sl.prng, s, pr);
@@ -452,8 +500,10 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename
                     tile_heads(sm.net, sm.Zp, s, z);
                     if (DUEL) duel::combine(z, g.actor.nout);
                     uint32_t a_bits;
-                    if (MODE == 0) {
+                    if constexpr (MODE == 0) {
                         a_bits = greedy::greedy_action(g.actor, z);
+                    } else if constexpr (MODE == 2) {
+                        a_bits = (uint32_t)plan_q_column<XEXT>(g.greedy, g.ex, g.beta, g.step0 + (long long)step * N + i, z, g.actor.nout, sl.prng, s);
                     } else {
                         unsigned long long pr[4];
                         get_stream(sl.prng, s, pr);
@@ -476,7 +526,7 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgs g, typename
         // (each owner thread touches only its own entries: no barrier before the next group's loads)
         if (owner)
             store_group(sm.slot, nslots, base, nctas, ea, N, s, g.nsteps > 0, [&](const EvalSlot<Env>& sl, int64_t i) {
-                if (MODE == 1) {
+                if (eval_streams<MODE>(g)) {
                     unsigned long long pr[4];
                     get_stream(sl.prng, s, pr);
                     explore::xo_store(g.policy_rng, i, pr);
@@ -513,20 +563,13 @@ template <class Env> struct SmemReplay {
     StatsScratch<NT / 32> red;
     long long red_dv[NT / 32];
 };
-// b200rl_explorer without its trailing beta, which the kernel takes as its last parameter: the parameters the ϵ-greedy
-// instantiations read keep the offsets they had before the explorer struct grew
-struct ReplayExplorer {
-    double eps_stable, eps_init;
-    int64_t warmup_steps, decay_steps, step;
-    int32_t kind, is_break_tie;
-};
 struct ReplayArgs {
     MlpDesc q;
     const float* params;
     int64_t N;
     int nsteps;
     int greedy;                            // 1: GreedyExplorer (findmax with `>`, no draw)
-    ReplayExplorer ex;
+    QExplorer ex;                          // (beta: the kernel's last parameter)
     const long long* step_dev;             // explorer step before the window (device)
     unsigned long long* xrng;              // (4, N) explorer streams
     Ring ring;
@@ -600,23 +643,7 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
                     float z[kOutMax];
                     tile_heads(sm.net, sm.Zp, s, z);
                     if (DUEL) duel::combine(z, g.q.nout);
-                    int a1;
-                    if (g.greedy) {
-                        int best = 0;      // q_act_kernel with epsilon = 0: the first maximum under `>`
-                        for (int o = 1; o < g.q.nout; ++o) if (z[o] > z[best]) best = o;
-                        a1 = best + 1;
-                    } else {
-                        unsigned long long xr[4];
-                        get_stream(sl.xrng, s, xr);
-                        if constexpr (XEXT) {
-                            const b200rl_explorer ex{g.ex.eps_stable, g.ex.eps_init, g.ex.warmup_steps, g.ex.decay_steps, g.ex.step, g.ex.kind,
-                                                     g.ex.is_break_tie, beta};
-                            a1 = explore::select<true>(ex, step0 + (long long)step * N + i, z, g.q.nout, xr);
-                        } else {
-                            a1 = explore::select<false>(g.ex, step0 + (long long)step * N + i, z, g.q.nout, xr);
-                        }
-                        put_stream(sl.xrng, s, xr);
-                    }
+                    const int a1 = plan_q_column<XEXT>(g.greedy, g.ex, beta, step0 + (long long)step * N + i, z, g.q.nout, sl.xrng, s);
                     const ActStep<float> res = slot_act(sl, s, p, ea.max_timeout, (typename Env::act_t)a1, sm.fin_cnt[s], sm.fin_ret[s], sm.fin_len[s]);
                     // push!(trajectory, (state = s', action = env.action, reward, terminal)) of lane i
                     float nobs[kInMax];
@@ -695,6 +722,20 @@ template <class F> int with_f32_env(const EnvView& v, F&& f) {
     return B200RL_ERR_UNSUPPORTED;
 }
 
+// the evaluate_tc_kernel instantiation of the network's activation (and, MODE 0 / 2, of a dueling head)
+template <class Env, int MODE, bool XEXT = false>
+int launch_evaluate(b200rl_ctx* ctx, int64_t groups, const EvalArgsOf<MODE>& g, const typename Env::P& p, const EnvArrays& ea) {
+    constexpr int RELU = B200RL_ACT_RELU, TANH = B200RL_ACT_TANH;
+    const bool relu = g.actor.act == RELU;
+    if constexpr (MODE != 1) {
+        if (g.actor.duel)
+            return relu ? launch_fused<evaluate_tc_kernel<Env, RELU, MODE, true, XEXT>, SmemEval<Env>>(ctx, groups, g, p, ea)
+                        : launch_fused<evaluate_tc_kernel<Env, TANH, MODE, true, XEXT>, SmemEval<Env>>(ctx, groups, g, p, ea);
+    }
+    return relu ? launch_fused<evaluate_tc_kernel<Env, RELU, MODE, false, XEXT>, SmemEval<Env>>(ctx, groups, g, p, ea)
+                : launch_fused<evaluate_tc_kernel<Env, TANH, MODE, false, XEXT>, SmemEval<Env>>(ctx, groups, g, p, ea);
+}
+
 template <class Env, bool XEXT>
 int launch_replay_collect(b200rl_ctx* ctx, int64_t groups, const ReplayArgs& g, const typename Env::P& p, const EnvArrays& ea, double beta) {
     constexpr int RELU = B200RL_ACT_RELU, TANH = B200RL_ACT_TANH;
@@ -756,27 +797,26 @@ int nn_tc_rollout(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const 
     return st;
 }
 
-// Fused evaluation window (after the caller's forced reset).  The caller has validated net <-> env; B200RL_ERR_UNSUPPORTED
-// (no side effect, no error message) = outside the fused envelope: the caller steps through staged launches instead.
+// Fused evaluation window (after the caller's forced reset).  mode 0 greedy, 1 sampled, 2 a Q-network planned by the explorer `ex`
+// (null: GreedyExplorer) from ex->step on the streams policy_rng.  The caller has validated net <-> env <-> explorer;
+// B200RL_ERR_UNSUPPORTED (no side effect, no error message) = outside the fused envelope: the caller steps through staged launches.
 int nn_tc_evaluate(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const float* params, const AcHyper& hp, int mode, int nsteps,
-                   int K, unsigned long long* policy_rng, float* returns, int32_t* lengths, int32_t* counts) {
+                   int K, unsigned long long* policy_rng, float* returns, int32_t* lengths, int32_t* counts, const b200rl_explorer* ex) {
     EnvView v;
     TRY(b200rl_env_internal_view(env, &v));
-    if (!nn_tc_supported(actor) || v.dtype != B200RL_F32) return B200RL_ERR_UNSUPPORTED;
+    if (!nn_tc_supported(actor) || v.dtype != B200RL_F32 || (mode == 2 && v.continuous)) return B200RL_ERR_UNSUPPORTED;
+    const b200rl_explorer e = ex ? *ex : b200rl_explorer{};
     const EvalArgs g{actor, params, hp, v.N, nsteps, K, policy_rng, returns, lengths, counts};
+    const EvalExploreArgs gx{g, ex ? 0 : 1, QExplorer{e.eps_stable, e.eps_init, e.warmup_steps, e.decay_steps, e.step, e.kind, e.is_break_tie},
+                             e.beta, (long long)e.step};
     const int64_t groups = ((v.N + TM - 1) / TM + kSlots - 1) / kSlots;
     const int st = with_f32_env(v, [&](auto env_type, const auto& p) {
         using Env = typename decltype(env_type)::type;
-        constexpr int RELU = B200RL_ACT_RELU, TANH = B200RL_ACT_TANH;
-        const bool relu = actor.act == RELU;
-        if (mode == 0 && actor.duel)
-            return relu ? launch_fused<evaluate_tc_kernel<Env, RELU, 0, true>, SmemEval<Env>>(ctx, groups, g, p, v.a)
-                        : launch_fused<evaluate_tc_kernel<Env, TANH, 0, true>, SmemEval<Env>>(ctx, groups, g, p, v.a);
-        if (mode == 0)
-            return relu ? launch_fused<evaluate_tc_kernel<Env, RELU, 0>, SmemEval<Env>>(ctx, groups, g, p, v.a)
-                        : launch_fused<evaluate_tc_kernel<Env, TANH, 0>, SmemEval<Env>>(ctx, groups, g, p, v.a);
-        return relu ? launch_fused<evaluate_tc_kernel<Env, RELU, 1>, SmemEval<Env>>(ctx, groups, g, p, v.a)
-                    : launch_fused<evaluate_tc_kernel<Env, TANH, 1>, SmemEval<Env>>(ctx, groups, g, p, v.a);
+        if (mode == 0) return launch_evaluate<Env, 0>(ctx, groups, g, p, v.a);
+        if (mode == 1) return launch_evaluate<Env, 1>(ctx, groups, g, p, v.a);
+        if constexpr (std::is_floating_point<typename Env::act_t>::value) return (int)B200RL_ERR_UNSUPPORTED;   // (rejected above)
+        else if (ex && ex->kind >= 2) return launch_evaluate<Env, 2, true>(ctx, groups, gx, p, v.a);
+        else return launch_evaluate<Env, 2>(ctx, groups, gx, p, v.a);
     });
     if (st == B200RL_OK) b200rl_env_internal_add_steps(env, (uint64_t)nsteps);
     return st;
@@ -791,7 +831,7 @@ int nn_tc_replay_collect(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& q, con
     TRY(b200rl_env_internal_view(env, &v));
     if (!nn_tc_supported(q) || v.dtype != B200RL_F32 || v.continuous || ring.ns > kInMax) return B200RL_ERR_UNSUPPORTED;
     const b200rl_explorer e = ex ? *ex : b200rl_explorer{};
-    const ReplayArgs g{q, params, v.N, nsteps, ex ? 0 : 1, ReplayExplorer{e.eps_stable, e.eps_init, e.warmup_steps, e.decay_steps, e.step, e.kind, e.is_break_tie},
+    const ReplayArgs g{q, params, v.N, nsteps, ex ? 0 : 1, QExplorer{e.eps_stable, e.eps_init, e.warmup_steps, e.decay_steps, e.step, e.kind, e.is_break_tie},
                        step_dev, xrng, ring, default_priority, prioritized, keys, vals, stride};
     const int64_t groups = ((v.N + TM - 1) / TM + kSlots - 1) / kSlots;
     const int st = with_f32_env(v, [&](auto env_type, const auto& p) {

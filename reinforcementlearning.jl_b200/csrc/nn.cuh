@@ -144,10 +144,11 @@ struct b200rl_env;
 int nn_tc_rollout(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const MlpDesc& critic, const float* params, const AcHyper& hp,
                   unsigned long long* policy_rng, int t0, int nsteps, int T, int final_bootstrap, float* states, void* actions, float* logp,
                   float* values, float* rewards, uint8_t* terminals);
-// fused evaluation window (fwd_tc.cu): nsteps x {actor -> greedy (mode 0) | sampled (mode 1) action, env step, episode records};
-// B200RL_ERR_UNSUPPORTED = outside the fused envelope, step through staged launches instead
+// fused evaluation window (fwd_tc.cu): nsteps x {actor -> greedy (mode 0) | sampled (mode 1) action | Q-network -> explorer column
+// (mode 2; ex null: GreedyExplorer), env step, episode records}; B200RL_ERR_UNSUPPORTED = outside the fused envelope, step through
+// staged launches instead
 int nn_tc_evaluate(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const float* params, const AcHyper& hp, int mode, int nsteps,
-                   int K, unsigned long long* policy_rng, float* returns, int32_t* lengths, int32_t* counts);
+                   int K, unsigned long long* policy_rng, float* returns, int32_t* lengths, int32_t* counts, const b200rl_explorer* ex = nullptr);
 // fused DQN collect window (fwd_tc.cu): nsteps x {Q -> explorer column | findmax, env step, ring push} for H = 64; the touched
 // sum-tree leaves of each lane go to keys / vals (stride, N) for one tree rebuild.  B200RL_ERR_UNSUPPORTED = outside the envelope
 struct Ring;

@@ -689,6 +689,35 @@ function evaluate(net::B200Network, env::B200VecEnv; n_steps::Integer, max_episo
 end
 
 """
+    evaluate(p::B200QBasedPolicy, env; n_steps, max_episodes = 1)
+
+`run(p, env, StopAfterNSteps(n_steps))` in actor mode (docs/src/How_to_use_hooks.md:96-119): the Q-network planned by the policy's
+explorer on the policy's explorer streams, as one fused kernel launch where the network allows it (b200rl_evaluate_explore).  The
+same records as `evaluate(net, env; ...)`.  The streams and the explorer's step advance exactly as under `run`; the learner is only
+read.  To evaluate without touching a training policy, build a second `B200QBasedPolicy` over the same learner.
+"""
+function evaluate(p::B200QBasedPolicy, env::B200VecEnv; n_steps::Integer, max_episodes::Integer = 1)
+    n = env.n
+    returns = fill(NaN32, max_episodes, n)
+    lengths = fill(Int32(-1), max_episodes, n)
+    counts = zeros(Int32, n)
+    if device_explorer(p.explorer)
+        ex = Ref(ExplorerC(p.explorer))
+        GC.@preserve returns lengths counts check(ccall((:b200rl_evaluate_explore, LIB), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Int32, Int32, Ref{ExplorerC}, Ptr{Cvoid}, Ptr{Float32}, Ptr{Int32}, Ptr{Int32}, Cint),
+            p.learner.net.h, env.h, n_steps, max_episodes, ex, p.d_rng, returns, lengths, counts, 0))
+        set_step!(p.explorer, ex[].step)
+    elseif p.explorer isa GreedyExplorer                           # findmax, no draw
+        GC.@preserve returns lengths counts check(ccall((:b200rl_evaluate_explore, LIB), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Int32, Int32, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Float32}, Ptr{Int32}, Ptr{Int32}, Cint),
+            p.learner.net.h, env.h, n_steps, max_episodes, C_NULL, p.d_rng, returns, lengths, counts, 0))
+    else
+        throw(ArgumentError("$(typeof(p.explorer)) has no device explorer"))
+    end
+    (; returns, lengths, counts)
+end
+
+"""
     B200Agent(policy::B200QBasedPolicy, trajectory::B200Trajectory)
 
 `Agent(policy, trajectory)` (agent_base.jl:18-66) with a device-resident replay: transition frames never visit the host.  `_run` announces

@@ -565,7 +565,14 @@ def evaluate(net, env, n_steps, max_episodes=1, mode="greedy", rng=None):
     ``rng`` (mode "sample"): (N, 4) uint64 policy streams, advanced in place, or a device pointer (int) to them.
     Returns ``returns`` (K, N) float32 and ``lengths`` (K, N) int32 (the first K = max_episodes episodes of each env that
     end inside the window; slots no episode reaches hold NaN / -1) and ``counts`` (N,) int32 (episodes per env, may exceed K).
-    Average over the envs with ``counts >= K`` to avoid the bias towards short episodes of a fixed window."""
+    Average over the envs with ``counts >= K`` to avoid the bias towards short episodes of a fixed window.
+
+    ``net`` may also be a :class:`QBasedPolicy` (b200rl_evaluate_explore): its Q-network planned by its explorer on its explorer
+    streams, exactly as ``run(policy, env, StopAfterNSteps(n_steps))`` would — the streams and the explorer's step advance
+    (``explorer.advance(N * n_steps)``); ``mode`` and ``rng`` do not apply.  To evaluate without touching a training policy, build a
+    second QBasedPolicy over the same learner with its own explorer and streams."""
+    if isinstance(net, QBasedPolicy):
+        return _evaluate_q_based(net, env, n_steps, max_episodes)
     if mode not in EVAL_MODES:
         raise ValueError(f"mode must be one of {sorted(EVAL_MODES)}")
     ctx, lib, n, K = net.ctx, net.ctx.lib, env.n, int(max_episodes)
@@ -591,6 +598,22 @@ def evaluate(net, env, n_steps, max_episodes=1, mode="greedy", rng=None):
     finally:
         if host_rng is not None:
             ctx.free(d_rng)
+    return dict(returns=returns, lengths=lengths, counts=counts)
+
+
+def _evaluate_q_based(policy, env, n_steps, max_episodes):
+    ex = policy.explorer
+    if type(ex) not in DEVICE_EXPLORERS + (GreedyExplorer,):
+        raise TypeError(f"{type(ex).__name__} has no device explorer")
+    ctx, lib, n, K = policy.ctx, policy.lib, env.n, int(max_episodes)
+    returns = np.full((K, n), np.nan, np.float32, order="F")
+    lengths = np.full((K, n), -1, np.int32, order="F")
+    counts = np.zeros(n, np.int32)
+    st = ex.as_struct() if type(ex) in DEVICE_EXPLORERS else None
+    L.check(lib.b200rl_evaluate_explore(policy.learner.net.h, env.h, int(n_steps), K, None if st is None else C.byref(st),
+                                        C.c_void_p(policy._d_rng), L.ptr(returns), L.ptr(lengths), L.ptr(counts), 0))
+    if st is not None:
+        ex.advance(n * int(n_steps))
     return dict(returns=returns, lengths=lengths, counts=counts)
 
 
