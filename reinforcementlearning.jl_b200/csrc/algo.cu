@@ -121,31 +121,40 @@ struct b200rl_net {
     float *params, *grad, *m, *v, *beta_t, *target;
     float* partial; int n_partials;
     float* loss_partial; float* loss4; float* gnorm;
-    double* cta_sumsq; unsigned int* counter2;
+    double* cta_sumsq; unsigned int* counters;
     float lr, b1, b2, eps, max_grad_norm;
     uint64_t n_updates;
 };
 
+// The operands of one optimiser step on n with the hyperparameters of an on-policy or DQN config c.  stats_row (may be null, and
+// then so is tick): the row {4 loss sums, grad norm} of this step; tick: the device update counter, incremented once by the step.
+template <class Config>
+static OptStep opt_step(const b200rl_net* n, const Config& c, float* stats_row = nullptr, unsigned int* tick = nullptr) {
+    OptStep st = {};
+    st.params = n->params; st.grad = n->grad; st.m = n->m; st.v = n->v; st.beta_t = n->beta_t;
+    st.loss_out4 = n->loss4; st.stats_row = stats_row; st.gnorm_out = n->gnorm;
+    st.cta_sumsq = n->cta_sumsq; st.counters = n->counters; st.tick = tick;
+    st.max_norm = c.max_grad_norm; st.lr = c.lr; st.b1 = c.beta1; st.b2 = c.beta2; st.eps = c.eps;
+    return st;
+}
+
 // One optimiser step on the gradient partials of a loss + backward launch: reduce [-> all-reduce over the ranks] ->
 // clip_by_global_norm! -> Adam.  One kernel (nn_reduce_clip_adam) when its CTAs can all be co-resident and the ranks, if any,
-// exchange over the peer memory; the staged kernels otherwise.  stats_row (may be null, and then so is tick): the row {4 loss sums,
-// grad norm} of this step; tick: the device update counter, incremented once by the step.
-static int optimiser_step(b200rl_net* n, int n_partials, int n_loss, float max_grad_norm, float lr, float b1, float b2, float eps,
-                          float* stats_row, unsigned int* tick) {
+// exchange over the peer memory; the staged kernels otherwise.
+static int optimiser_step(b200rl_net* n, int n_partials, int n_loss, const OptStep& st) {
     b200rl_ctx* ctx = n->ctx;
     const int world = b200rl_comm_world(ctx);
     P2PTable peers;
     if ((world == 1 || b200rl_comm_p2p_table(ctx, &peers)) && (int)grid_for(n->np, 256) <= ctx->sm_count)
-        return nn_reduce_clip_adam(ctx, n->partial, n_partials, n->np, n->params, n->grad, n->m, n->v, n->beta_t, n->loss_partial, n_loss, n->loss4,
-                                   max_grad_norm, lr, b1, b2, eps, n->gnorm, n->cta_sumsq, n->counter2, stats_row, tick);
+        return nn_reduce_clip_adam(ctx, n->partial, n_partials, n->np, n->loss_partial, n_loss, st);
     TRY(nn_reduce_partials(ctx, n->partial, n_partials, n->np, n->grad, n->loss_partial, n_loss, n->loss4));
     if (world > 1) {
         TRY(b200rl_comm_allreduce_internal(ctx, n->grad, n->np, 0));
         TRY(b200rl_comm_allreduce_internal(ctx, n->loss4, 4, 0));
     }
-    TRY(nn_clip_adam(ctx, n->params, n->grad, n->m, n->v, n->beta_t, n->np, max_grad_norm, lr, b1, b2, eps, 1.0f, n->gnorm));
-    if (stats_row) {
-        stats_row_kernel<<<1, 32, 0, ctx->stream>>>(stats_row, n->loss4, n->gnorm, tick);
+    TRY(nn_clip_adam(ctx, n->np, st));
+    if (st.stats_row) {
+        stats_row_kernel<<<1, 32, 0, ctx->stream>>>(st.stats_row, n->loss4, n->gnorm, st.tick);
         LAUNCH_CHECK(ctx);
     }
     return B200RL_OK;
@@ -337,7 +346,7 @@ int b200rl_net_destroy(b200rl_net* n) {
     cudaSetDevice(n->ctx->device);
     cudaStreamSynchronize(n->ctx->stream);
     cudaFree(n->params); cudaFree(n->grad); cudaFree(n->m); cudaFree(n->v); cudaFree(n->beta_t); cudaFree(n->target);
-    cudaFree(n->partial); cudaFree(n->loss_partial); cudaFree(n->loss4); cudaFree(n->gnorm); cudaFree(n->cta_sumsq); cudaFree(n->counter2);
+    cudaFree(n->partial); cudaFree(n->loss_partial); cudaFree(n->loss4); cudaFree(n->gnorm); cudaFree(n->cta_sumsq); cudaFree(n->counters);
     delete n;
     return B200RL_OK;
 }
@@ -365,8 +374,8 @@ int b200rl_net_create(b200rl_ctx* ctx, const b200rl_net_desc* d, const float* pa
     NET_TRY(cudaMalloc(&n->partial, (size_t)n->n_partials * bytes));
     NET_TRY(cudaMalloc(&n->loss_partial, (size_t)n_loss_rows * 4 * sizeof(float)));
     NET_TRY(cudaMalloc(&n->loss4, 4 * sizeof(float))); NET_TRY(cudaMalloc(&n->gnorm, sizeof(float)));
-    NET_TRY(cudaMalloc(&n->cta_sumsq, 256 * sizeof(double))); NET_TRY(cudaMalloc(&n->counter2, 4 * sizeof(unsigned int)));
-    NET_TRY(cudaMemsetAsync(n->counter2, 0, 4 * sizeof(unsigned int), ctx->stream));
+    NET_TRY(cudaMalloc(&n->cta_sumsq, 256 * sizeof(double))); NET_TRY(cudaMalloc(&n->counters, 4 * sizeof(unsigned int)));
+    NET_TRY(cudaMemsetAsync(n->counters, 0, 4 * sizeof(unsigned int), ctx->stream));
     NET_TRY(cudaMemcpyAsync(n->params, params_host, bytes, cudaMemcpyHostToDevice, ctx->stream));
     if (is_q_kind(n->kind)) NET_TRY(cudaMemcpyAsync(n->target, params_host, bytes, cudaMemcpyHostToDevice, ctx->stream));
     NET_TRY(cudaMemsetAsync(n->grad, 0, bytes, ctx->stream)); NET_TRY(cudaMemsetAsync(n->m, 0, bytes, ctx->stream));
@@ -701,7 +710,7 @@ int b200rl_net_ac_step(b200rl_net* n, const b200rl_onpolicy_config* cfg, const f
     if (ctas < 0) return ctas;
     TRY(nn_reduce_partials(ctx, n->partial, ctas, n->np, n->grad, n->loss_partial, 2 * ctas, n->loss4));
     if (apply_update) {
-        TRY(nn_clip_adam(ctx, n->params, n->grad, n->m, n->v, n->beta_t, n->np, cfg->max_grad_norm, cfg->lr, cfg->beta1, cfg->beta2, cfg->eps, 1.0f, n->gnorm));
+        TRY(nn_clip_adam(ctx, n->np, opt_step(n, *cfg)));
         n->n_updates += 1;
     }
     if (losses_out) {
@@ -972,13 +981,13 @@ int b200rl_onpolicy_update(b200rl_onpolicy* a, const int32_t* perm_host, float* 
             unsigned int* tick = row == a->stats_rows - 1 ? a->upd_dev : nullptr;   // the last optimiser step closes the update
             // one launch: loss + backward + [peer exchange] + clip + Adam (tensor-core path); otherwise loss + backward, then the
             // optimiser step
-            int ctas = nn_ac_loss_grad_step(ctx, n->actor, n->critic, n->params, hp, b, n->partial, n->loss_partial, n->grad, n->m, n->v, n->beta_t,
-                                            n->loss4, c.max_grad_norm, c.lr, c.beta1, c.beta2, c.eps, n->gnorm, n->cta_sumsq, n->counter2, stats_row, tick);
+            const OptStep st = opt_step(n, c, stats_row, tick);
+            int ctas = nn_ac_loss_grad_step(ctx, n->actor, n->critic, hp, b, n->partial, n->loss_partial, st);
             const bool staged = ctas == B200RL_ERR_UNSUPPORTED;
             if (staged) ctas = nn_ac_loss_grad(ctx, n->actor, n->critic, n->params, hp, b, n->partial, n->loss_partial);
             if (ctas < 0) return ctas;
             TRY(phase(2 + 2 * row));
-            if (staged) TRY(optimiser_step(n, ctas, 2 * ctas, c.max_grad_norm, c.lr, c.beta1, c.beta2, c.eps, stats_row, tick));
+            if (staged) TRY(optimiser_step(n, ctas, 2 * ctas, st));
             TRY(phase(3 + 2 * row));
             n->n_updates += 1;
         }
@@ -1102,7 +1111,11 @@ int b200rl_onpolicy_time_kernel(b200rl_onpolicy* a, int which, int reps, float* 
             case 2: return b200rl_env_step(a->env, a->actions, 1, 1);
             case 3: return b200rl_gae_fused_internal(ctx, a->adv, a->ret, a->rewards, a->values, a->terminals, c.gamma, c.lambda, N, T, a->norm_partials);
             // the optimiser step as update() runs it (lr = 0: parameters stay put), incl. the peer exchange of a sharded run
-            case 4: return optimiser_step(n, ctas, 2 * ctas, c.max_grad_norm, 0.0f, c.beta1, c.beta2, c.eps, nullptr, nullptr);
+            case 4: {
+                OptStep st = opt_step(n, c);
+                st.lr = 0.0f;
+                return optimiser_step(n, ctas, 2 * ctas, st);
+            }
         }
         b200rl_set_error("unknown kernel id");
         return B200RL_ERR_INVALID;
@@ -1152,7 +1165,7 @@ static int dqn_update_seq(b200rl_net* n, b200rl_traj* t, const b200rl_dqn_config
     int np_ = nn_dqn_loss_grad(ctx, n->actor, n->params, n->target, b.s, b.a, b.r, b.t, b.s2, b.w, b.B, 1.0f / ((float)b.B * (float)world), cfg->gamma,
                                cfg->huber, cfg->double_dqn, n->partial, n->loss_partial, td, b200rl_traj_internal_discount(t));
     if (np_ < 0) return np_;
-    TRY(optimiser_step(n, np_, np_, cfg->max_grad_norm, cfg->lr, cfg->beta1, cfg->beta2, cfg->eps, nullptr, nullptr));
+    TRY(optimiser_step(n, np_, np_, opt_step(n, *cfg)));
     if (b200rl_traj_internal_prioritized(t)) TRY(b200rl_traj_internal_priority_from_td(t, td, cfg->per_eps, cfg->per_alpha));
     n->n_updates += 1;
     if (upd_dev) TRY(nn_target_sync_counted(ctx, n->target, n->params, n->np, cfg->rho, upd_dev, cfg->target_update_freq));

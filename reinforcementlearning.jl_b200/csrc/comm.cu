@@ -87,17 +87,7 @@ __global__ void __launch_bounds__(256) p2p_allreduce_small_kernel(P2PTable tab, 
         unsigned w[2] = {0u, 0u};
         memcpy(w, &mine, sizeof(T));
         for (int h = 0; h < W; ++h) p2p_push(tab, 1, slot, (size_t)i * W + h, w[h], seq);
-        T acc = 0;
-        for (int r = 0; r < tab.nranks; ++r) {
-            T val = mine;
-            if (r != tab.rank) {
-                unsigned u[2] = {0u, 0u};
-                for (int h = 0; h < W; ++h) u[h] = p2p_recv(tab, 1, slot, r, (size_t)i * W + h, seq);
-                memcpy(&val, u, sizeof(T));
-            }
-            acc += val;
-        }
-        buf[i] = acc;
+        buf[i] = p2p_sum_ranks(tab, 1, slot, (size_t)i * W, mine, seq);
     }
     __syncthreads();
     if (threadIdx.x == 0) *seq_ptr = seq;

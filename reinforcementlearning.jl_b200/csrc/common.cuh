@@ -146,4 +146,21 @@ __device__ __forceinline__ unsigned p2p_recv(const P2PTable& t, int area, unsign
         }
     }
 }
+// the exchange's sum of one element over the ranks, in rank order (bit-identical on every rank): `mine` for the own rank, the packets
+// of word_idx (sizeof(T) / 4 consecutive words) from the peers.  The caller pushes its own packets first.
+template <class T>
+__device__ __forceinline__ T p2p_sum_ranks(const P2PTable& t, int area, unsigned slot, size_t word_idx, T mine, unsigned seq) {
+    constexpr int W = sizeof(T) / 4;
+    T acc = 0;
+    for (int r = 0; r < t.nranks; ++r) {
+        T val = mine;
+        if (r != t.rank) {
+            unsigned u[W];
+            for (int h = 0; h < W; ++h) u[h] = p2p_recv(t, area, slot, r, word_idx + h, seq);
+            memcpy(&val, u, sizeof(T));
+        }
+        acc += val;
+    }
+    return acc;
+}
 #endif

@@ -556,15 +556,13 @@ __global__ void reduce_partials_kernel(const float* __restrict__ partial, int n_
 }
 
 // single CTA: gn = sqrt(sum g^2) (fixed tree, double), clip_by_global_norm!, Optimisers Adam
-__global__ void __launch_bounds__(1024) clip_adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
-                                                         float* __restrict__ v, float* __restrict__ beta_t, int64_t np, float max_norm,
-                                                         float lr, float b1, float b2, float eps, float grad_scale,
-                                                         float* __restrict__ gnorm_out) {
+__global__ void __launch_bounds__(1024) clip_adam_kernel(int64_t np, OptStep st) {
     __shared__ double red[32];
     __shared__ float s_scale;
+    const float lr = st.lr, b1 = st.b1, b2 = st.b2, eps = st.eps;   // (read first: see reduce_clip_adam_kernel)
     double acc = 0.0;
     for (int64_t k = threadIdx.x; k < np; k += blockDim.x) {
-        float x = g[k] * grad_scale;
+        float x = st.grad[k];
         acc += (double)x * (double)x;
     }
 #pragma unroll
@@ -575,24 +573,20 @@ __global__ void __launch_bounds__(1024) clip_adam_kernel(float* __restrict__ p, 
         double t = 0.0;
         for (int k = 0; k < (int)(blockDim.x >> 5); ++k) t += red[k];
         float gn = (float)sqrt(t);
-        float sc = 1.0f;
-        if (max_norm > 0.f && max_norm <= gn) sc = max_norm / fmaxf(max_norm, gn);
-        s_scale = sc;
-        if (gnorm_out) *gnorm_out = gn;
+        s_scale = optim::clip_scale(gn, st.max_norm);
+        if (st.gnorm_out) *st.gnorm_out = gn;
     }
     __syncthreads();
-    const float sc = s_scale * grad_scale;
-    const float bt1 = beta_t[0], bt2 = beta_t[1];
+    const float sc = s_scale;
+    const float bt1 = st.beta_t[0], bt2 = st.beta_t[1];
     for (int64_t k = threadIdx.x; k < np; k += blockDim.x) {
-        float gk = g[k] * sc;
-        g[k] = gk;
-        float mk = b1 * m[k] + (1.0f - b1) * gk;
-        float vk = b2 * v[k] + (1.0f - b2) * (gk * gk);
-        m[k] = mk; v[k] = vk;
-        p[k] -= mk / (1.0f - bt1) / (sqrtf(vk / (1.0f - bt2)) + eps) * lr;
+        float gk = st.grad[k] * sc;
+        st.grad[k] = gk;
+        const optim::AdamOut a = optim::adam_update(gk, st.m[k], st.v[k], st.params[k], lr, b1, b2, eps, bt1, bt2);
+        st.m[k] = a.m; st.v[k] = a.v; st.params[k] = a.p;
     }
     __syncthreads();
-    if (threadIdx.x == 0) { beta_t[0] = bt1 * b1; beta_t[1] = bt2 * b2; }
+    if (threadIdx.x == 0) optim::beta_advance(st.beta_t, bt1, bt2, b1, b2);
 }
 
 // Fused K8: partial reduce -> [peer exchange over NVLink] -> global norm -> clip -> Adam in ONE launch.  The CTAs meet at a
@@ -601,21 +595,16 @@ __global__ void __launch_bounds__(1024) clip_adam_kernel(float* __restrict__ p, 
 // XCHG (sharded run, SURVEY §8e): every thread pushes its element of the local gradient into the peers' inboxes as a
 // self-validating {value, sequence} packet (remote NVLink store), then reads the peers' packets from the own inbox and sums
 // in rank order — every rank computes the identical global gradient, so the replicas stay bit-identical without a broadcast.
+// (A template parameter, not a run-time branch: the single-GPU instantiation carries no exchange code.)
 template <bool XCHG>
-__global__ void __launch_bounds__(256) reduce_clip_adam_kernel(const float* __restrict__ partial, int n_partials, int64_t np, float* __restrict__ p,
-                                                              float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                                                              float* __restrict__ beta_t, const float* __restrict__ loss_partial, int n_loss,
-                                                              float* __restrict__ loss_out4, float max_norm, float lr, float b1, float b2, float eps,
-                                                              float* __restrict__ gnorm_out, double* __restrict__ cta_sumsq,
-                                                              unsigned int* __restrict__ counter, float* __restrict__ stats_row,
-                                                              P2PTable tab, unsigned int* __restrict__ seq_ptr, unsigned int* __restrict__ tick) {
+__global__ void __launch_bounds__(256) reduce_clip_adam_kernel(const float* __restrict__ partial, int n_partials, int64_t np,
+                                                              const float* __restrict__ loss_partial, int n_loss, OptStep st) {
     __shared__ double red[8];
     __shared__ float s_scale;
-    // The grid barrier counters reset themselves (the last CTA through the second counter zeroes both), the exchange sequence
-    // number and the update tick live in device memory: nothing here depends on host-side launch counts, so the launch can be
-    // captured in a CUDA graph and replayed, and no counter ever wraps.
-    const unsigned int target = gridDim.x;
-    const unsigned int seq = XCHG ? *seq_ptr + 1u : 0u;
+    // The hyperparameters are read first.  Defined this early, they make the compiler contract Adam's multiply-adds as it did when
+    // they were scalar kernel parameters, so the kernel keeps its rounding (K7, which reads them late, contracts the other product).
+    const float lr = st.lr, b1 = st.b1, b2 = st.b2, eps = st.eps;
+    const unsigned int seq = XCHG ? *st.seq_ptr + 1u : 0u;
     const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     float gk = 0.f;
     if (k < np) {
@@ -627,19 +616,12 @@ __global__ void __launch_bounds__(256) reduce_clip_adam_kernel(const float* __re
         for (int c = 0; c < n_loss; ++c) lsum += loss_partial[c * 4 + threadIdx.x];
     if (XCHG) {   // push the local chunk into every peer's inbox, then collect the peers' chunks from the own inbox
         const unsigned slot = seq & 1u;
-        if (k < np) p2p_push(tab, 0, slot, (size_t)k, __float_as_uint(gk), seq);
-        if (loss_thread) p2p_push(tab, 0, slot, (size_t)np + threadIdx.x, __float_as_uint(lsum), seq);   // the 4 loss sums ride along
-        float acc = 0.f, lacc = 0.f;
-        for (int r = 0; r < tab.nranks; ++r) {
-            if (k < np) acc += r == tab.rank ? gk : __uint_as_float(p2p_recv(tab, 0, slot, r, (size_t)k, seq));
-            if (loss_thread) lacc += r == tab.rank ? lsum : __uint_as_float(p2p_recv(tab, 0, slot, r, (size_t)np + threadIdx.x, seq));
-        }
-        gk = acc; lsum = lacc;
+        if (k < np) p2p_push(st.tab, 0, slot, (size_t)k, __float_as_uint(gk), seq);
+        if (loss_thread) p2p_push(st.tab, 0, slot, (size_t)np + threadIdx.x, __float_as_uint(lsum), seq);   // the 4 loss sums ride along
+        if (k < np) gk = p2p_sum_ranks(st.tab, 0, slot, (size_t)k, gk, seq);
+        if (loss_thread) lsum = p2p_sum_ranks(st.tab, 0, slot, (size_t)np + threadIdx.x, lsum, seq);
     }
-    if (loss_thread) {
-        if (loss_out4) loss_out4[threadIdx.x] = lsum;
-        if (stats_row) stats_row[threadIdx.x] = lsum;
-    }
+    if (loss_thread) optim::publish_loss(st, threadIdx.x, lsum);
     double acc = (double)gk * (double)gk;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -649,55 +631,34 @@ __global__ void __launch_bounds__(256) reduce_clip_adam_kernel(const float* __re
         if (threadIdx.x == 0) {
             double t = 0.0;
             for (int w = 0; w < 8; ++w) t += red[w];
-            cta_sumsq[blockIdx.x] = t;
-            __threadfence();
-            atomicAdd(counter, 1u);
-            unsigned int spins = 0;
-            while (*reinterpret_cast<volatile unsigned int*>(counter) < target)
-                if (++spins > (1u << 26)) __trap();
-            __threadfence();
+            st.cta_sumsq[blockIdx.x] = t;
+            optim::grid_barrier(st.counters, gridDim.x);
         }
         __syncwarp();
         // (one dependent L2 read per CTA was ~5 us of this ~14 us kernel; the loads now go out together, the adds keep the CTA order)
         double tot = 0.0;
         for (unsigned int c0 = 0; c0 < gridDim.x; c0 += 32) {
             const unsigned int c = c0 + threadIdx.x;
-            const double mine = c < gridDim.x ? *reinterpret_cast<volatile double*>(cta_sumsq + c) : 0.0;
+            const double mine = c < gridDim.x ? *reinterpret_cast<volatile double*>(st.cta_sumsq + c) : 0.0;
             const unsigned int n = min(32u, gridDim.x - c0);
             for (unsigned int l = 0; l < n; ++l) tot += __shfl_sync(0xffffffffu, mine, l);
         }
-    if (threadIdx.x == 0) {
-        float gn = (float)sqrt(tot);
-        float sc = 1.0f;
-        if (max_norm > 0.f && max_norm <= gn) sc = max_norm / fmaxf(max_norm, gn);
-        s_scale = sc;
-        if (blockIdx.x == 0) {
-            if (gnorm_out) *gnorm_out = gn;
-            if (stats_row) stats_row[4] = gn;
+        if (threadIdx.x == 0) {
+            const float gn = (float)sqrt(tot);
+            s_scale = optim::clip_scale(gn, st.max_norm);
+            if (blockIdx.x == 0) optim::publish_gnorm(st, gn);
         }
     }
-    }
     __syncthreads();
-    const float bt1 = beta_t[0], bt2 = beta_t[1];
+    const float bt1 = st.beta_t[0], bt2 = st.beta_t[1];
     if (k < np) {
         gk *= s_scale;
-        g[k] = gk;
-        float mk = b1 * m[k] + (1.0f - b1) * gk;
-        float vk = b2 * v[k] + (1.0f - b2) * (gk * gk);
-        m[k] = mk; v[k] = vk;
-        p[k] -= mk / (1.0f - bt1) / (sqrtf(vk / (1.0f - bt2)) + eps) * lr;
+        st.grad[k] = gk;
+        const optim::AdamOut a = optim::adam_update(gk, st.m[k], st.v[k], st.params[k], lr, b1, b2, eps, bt1, bt2);
+        st.m[k] = a.m; st.v[k] = a.v; st.params[k] = a.p;
     }
-    // beta^t advances once every CTA has read it: the last CTA to pass a second counter does it
     __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        if (atomicAdd(counter + 1, 1u) + 1u == target) {   // every CTA has left the first barrier and read beta^t / the sequence number
-            beta_t[0] = bt1 * b1; beta_t[1] = bt2 * b2;
-            counter[0] = 0u; counter[1] = 0u;
-            if (XCHG) *seq_ptr = seq;
-            if (tick) *tick += 1u;
-        }
-    }
+    if (threadIdx.x == 0) optim::close_step<2>(st, bt1, bt2, XCHG, seq);
 }
 
 __global__ void target_sync_kernel(float* __restrict__ target, const float* __restrict__ model, int64_t np, float rho) {
@@ -951,26 +912,23 @@ int nn_ac_loss_grad(b200rl_ctx* ctx, const MlpDesc& actor, const MlpDesc& critic
 
 // K7 + optimiser step in ONE launch (tensor-core path only; B200RL_FUSED_STEP=0 disables it).  A sharded run takes it only when
 // every rank owns its device (P2PTable::exclusive): the launch occupies all SMs and waits for the peers' packets inside itself.
-int nn_ac_loss_grad_step(b200rl_ctx* ctx, const MlpDesc& actor, const MlpDesc& critic, float* params, const AcHyper& hp, const AcBatch& b,
-                         float* partial, float* loss_partial, float* grad, float* m, float* v, float* beta_t, float* loss_out4,
-                         float max_grad_norm, float lr, float b1, float b2, float eps, float* gnorm_out, double* cta_sumsq,
-                         unsigned int* counter4, float* stats_row, unsigned int* tick) {
+// This is the one place that decides whether the fused step runs: nn_tc_ac_loss_grad takes the step as given.
+int nn_ac_loss_grad_step(b200rl_ctx* ctx, const MlpDesc& actor, const MlpDesc& critic, const AcHyper& hp, const AcBatch& b, float* partial,
+                         float* loss_partial, const OptStep& step) {
     if (g_fused_step < 0) { const char* e = getenv("B200RL_FUSED_STEP"); g_fused_step = (e && e[0] == '0') ? 0 : 1; }
-    if (!g_fused_step || !nn_tc_enabled() || !nn_tc_bwd_supported(actor, critic) || actor.H != critic.H || actor.in != critic.in) return B200RL_ERR_UNSUPPORTED;
-    if (check_desc(actor) != B200RL_OK || check_desc(critic) != B200RL_OK) return B200RL_ERR_UNSUPPORTED;
-    const int ctas = ctx->sm_count / 2;
+    const int grid = 2 * (ctx->sm_count / 2);
     const int64_t np = actor.nparams() + critic.nparams();
-    if ((np + 2 * ctas - 1) / (2 * ctas) > 512) return B200RL_ERR_UNSUPPORTED;
-    AcStep st = {};
-    st.params = params; st.grad = grad; st.m = m; st.v = v; st.beta_t = beta_t; st.loss_out4 = loss_out4; st.stats_row = stats_row;
-    st.gnorm_out = gnorm_out; st.cta_sumsq = cta_sumsq; st.counter = counter4; st.tick = tick; st.seq_ptr = nullptr;
-    st.max_norm = max_grad_norm; st.lr = lr; st.b1 = b1; st.b2 = b2; st.eps = eps;
+    if (!g_fused_step || !nn_tc_enabled() || !nn_tc_bwd_supported(actor, critic) || actor.H != critic.H || actor.in != critic.in ||
+        check_desc(actor) != B200RL_OK || check_desc(critic) != B200RL_OK || !nn_tc_step_fits(ctx, grid, actor, hp, b.B, np))
+        return B200RL_ERR_UNSUPPORTED;
+    OptStep st = step;
+    st.tab = {}; st.seq_ptr = nullptr;
     if (b200rl_comm_world(ctx) > 1) {   // sharded run: needs the attached peer exchange and one rank per device
         if (!b200rl_comm_p2p_table(ctx, &st.tab) || !st.tab.exclusive || (size_t)np + 4 > kP2PXCap) return B200RL_ERR_UNSUPPORTED;
         st.seq_ptr = b200rl_comm_p2p_seq_dev(ctx);
     }
-    int rc = nn_tc_ac_loss_grad(ctx, 2 * ctas, actor, critic, params, hp, b, partial, loss_partial, np, &st);
-    return rc != B200RL_OK ? rc : nn_tc_partial_rows(2 * ctas, actor, hp, b.B);
+    int rc = nn_tc_ac_loss_grad(ctx, grid, actor, critic, st.params, hp, b, partial, loss_partial, np, &st);
+    return rc != B200RL_OK ? rc : nn_tc_partial_rows(grid, actor, hp, b.B);
 }
 
 int nn_reduce_partials(b200rl_ctx* ctx, const float* partial, int n_partials, int64_t np, float* grad, const float* loss_partial,
@@ -980,29 +938,23 @@ int nn_reduce_partials(b200rl_ctx* ctx, const float* partial, int n_partials, in
     return B200RL_OK;
 }
 
-int nn_clip_adam(b200rl_ctx* ctx, float* params, float* grad, float* m, float* v, float* beta_t, int64_t np, float max_grad_norm, float lr,
-                 float b1, float b2, float eps, float grad_scale, float* gnorm_out) {
-    clip_adam_kernel<<<1, 1024, 0, ctx->stream>>>(params, grad, m, v, beta_t, np, max_grad_norm, lr, b1, b2, eps, grad_scale, gnorm_out);
+int nn_clip_adam(b200rl_ctx* ctx, int64_t np, const OptStep& st) {
+    clip_adam_kernel<<<1, 1024, 0, ctx->stream>>>(np, st);
     LAUNCH_CHECK(ctx);
     return B200RL_OK;
 }
 
-int nn_reduce_clip_adam(b200rl_ctx* ctx, const float* partial, int n_partials, int64_t np, float* params, float* grad, float* m, float* v,
-                        float* beta_t, const float* loss_partial, int n_loss, float* loss_out4, float max_grad_norm, float lr, float b1, float b2,
-                        float eps, float* gnorm_out, double* cta_sumsq, unsigned int* counter2, float* stats_row, unsigned int* tick) {
+int nn_reduce_clip_adam(b200rl_ctx* ctx, const float* partial, int n_partials, int64_t np, const float* loss_partial, int n_loss, const OptStep& step) {
     unsigned grid = grid_for(np, 256);
     REQUIRE((int)grid <= ctx->sm_count, B200RL_ERR_UNSUPPORTED, "fused reduce+Adam needs all CTAs co-resident");
-    P2PTable tab = {};
-    if (b200rl_comm_p2p_table(ctx, &tab)) {
+    OptStep st = step;
+    st.tab = {}; st.seq_ptr = nullptr;
+    const bool xchg = b200rl_comm_p2p_table(ctx, &st.tab);
+    if (xchg) {
         REQUIRE((size_t)np + 4 <= kP2PXCap, B200RL_ERR_UNSUPPORTED, "gradient larger than the peer exchange inbox");
-        reduce_clip_adam_kernel<true><<<grid, 256, 0, ctx->stream>>>(partial, n_partials, np, params, grad, m, v, beta_t, loss_partial, n_loss, loss_out4,
-                                                                    max_grad_norm, lr, b1, b2, eps, gnorm_out, cta_sumsq, counter2, stats_row, tab,
-                                                                    b200rl_comm_p2p_seq_dev(ctx), tick);
-    } else {
-        reduce_clip_adam_kernel<false><<<grid, 256, 0, ctx->stream>>>(partial, n_partials, np, params, grad, m, v, beta_t, loss_partial, n_loss, loss_out4,
-                                                                     max_grad_norm, lr, b1, b2, eps, gnorm_out, cta_sumsq, counter2, stats_row, tab,
-                                                                     nullptr, tick);
+        st.seq_ptr = b200rl_comm_p2p_seq_dev(ctx);
     }
+    (xchg ? reduce_clip_adam_kernel<true> : reduce_clip_adam_kernel<false>)<<<grid, 256, 0, ctx->stream>>>(partial, n_partials, np, loss_partial, n_loss, st);
     LAUNCH_CHECK(ctx);
     return B200RL_OK;
 }

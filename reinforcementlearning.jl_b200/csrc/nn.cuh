@@ -9,6 +9,7 @@
 // (ActorCritic RLCore/src/utils/networks.jl:15-20, GaussianNetwork :44-116, DuelingNetwork :500-522.)
 #pragma once
 #include "common.cuh"
+#include "optim.cuh"
 #include "policy.cuh"   // AcHyper
 
 constexpr int kInMax = 4;    // observation width <= 4 (CartPole 4, Pendulum 3, MountainCar 2)
@@ -56,27 +57,6 @@ struct AcBatch {
     const float* norm2;         // device {mean, inv_std} for advantage normalisation
 };
 
-// Optimiser step fused into the tail of the tensor-core K7 (nn_ac_loss_grad_step): reduce the per-CTA partials -> [NVLink peer
-// exchange] -> global norm -> clip_by_global_norm! -> Adam, behind two grid barriers inside the SAME launch (the persistent
-// CTAs, one per SM, are co-resident), instead of a second kernel (a launch, L2 round trips and a barrier per optimiser step).
-struct AcStep {
-    float* params; float* grad; float* m; float* v; float* beta_t;
-    float* loss_out4; float* stats_row; float* gnorm_out;     // each may be null
-    double* cta_sumsq;            // >= grid doubles (<= 256)
-    unsigned int* counter;        // 4 zero-initialised uints (self-resetting grid barriers)
-    unsigned int* tick;           // may be null: device update counter incremented once by the launch
-    unsigned int* seq_ptr;        // gradient-exchange sequence number (sharded run)
-    float max_norm, lr, b1, b2, eps;
-    P2PTable tab;                 // nranks <= 1: single GPU
-};
-// K7 + optimiser step in one launch.  Returns the number of gradient partials (> 0) like nn_ac_loss_grad, or
-// B200RL_ERR_UNSUPPORTED *without side effects* when the configuration is outside the fused path (the caller then runs
-// nn_ac_loss_grad + nn_reduce_clip_adam).
-int nn_ac_loss_grad_step(b200rl_ctx* ctx, const MlpDesc& actor, const MlpDesc& critic, float* params, const AcHyper& hp, const AcBatch& b,
-                         float* partial, float* loss_partial, float* grad, float* m, float* v, float* beta_t, float* loss_out4,
-                         float max_grad_norm, float lr, float b1, float b2, float eps, float* gnorm_out, double* cta_sumsq,
-                         unsigned int* counter4, float* stats_row, unsigned int* tick);
-
 #ifdef __CUDACC__
 __device__ __forceinline__ uint32_t ac_perm_key(const AcBatch& b) { return b.perm_key + (b.perm_epoch ? *b.perm_epoch * 1000003u : 0u); }
 // the trunk activation, and its derivative from the activation's output h
@@ -109,15 +89,30 @@ int nn_ac_loss_grad(b200rl_ctx* ctx, const MlpDesc& actor, const MlpDesc& critic
                     const AcBatch& b, float* partial /* [ctas][np] */, float* loss_partial /* [2*ctas][4] */);
 int nn_reduce_partials(b200rl_ctx* ctx, const float* partial, int n_partials, int64_t np, float* grad, const float* loss_partial,
                        int n_loss_partials, float* loss_out4);
-// clip_by_global_norm! + Optimisers Adam on a flat gradient (single CTA, deterministic)
-int nn_clip_adam(b200rl_ctx* ctx, float* params, float* grad, float* m, float* v, float* beta_t /* device [2] */, int64_t np,
-                 float max_grad_norm, float lr, float b1, float b2, float eps, float grad_scale, float* gnorm_out /* device */);
-// fused single-launch variant (single GPU, or a sharded run with the NVLink peer exchange attached; stats_row (may be null)
-// receives {4 loss sums, grad norm}): cta_sumsq >= grid doubles, counter2 = 2 zero-initialised uints (self-resetting grid barrier),
-// tick (may be null) = device counter incremented once by the launch (the agent's update counter that keys the permutation)
-int nn_reduce_clip_adam(b200rl_ctx* ctx, const float* partial, int n_partials, int64_t np, float* params, float* grad, float* m, float* v,
-                        float* beta_t, const float* loss_partial, int n_loss, float* loss_out4, float max_grad_norm, float lr, float b1, float b2,
-                        float eps, float* gnorm_out, double* cta_sumsq, unsigned int* counter2, float* stats_row, unsigned int* tick);
+
+// ---- optimiser step: [reduce the per-CTA partials -> peer exchange ->] global norm -> clip_by_global_norm! -> Adam (optim.cuh) ----
+// The operands of one step on a network's flat parameter vector.  The single-launch steps (K8, K7's tail) meet at self-resetting
+// grid barriers on `counters` and keep their sequence numbers and tick in device memory, so they can be captured and replayed.
+struct OptStep {
+    float* params; float* grad; float* m; float* v; float* beta_t /* device [2]: {beta1^t, beta2^t} */;
+    float* loss_out4; float* stats_row; float* gnorm_out;     // each may be null; stats_row receives {4 loss sums, grad norm}
+    double* cta_sumsq;            // >= grid doubles (<= 256)
+    unsigned int* counters;       // 4 zero-initialised uints (grid barriers: K8 uses 2, K7 3)
+    unsigned int* tick;           // may be null: device update counter incremented once by the step (keys the permutation)
+    unsigned int* seq_ptr;        // gradient-exchange sequence number (sharded run; set by the launcher)
+    float max_norm, lr, b1, b2, eps;
+    P2PTable tab;                 // nranks <= 1: single GPU (set by the launcher)
+};
+// clip_by_global_norm! + Adam on st.grad (single CTA, deterministic); writes st.gnorm_out
+int nn_clip_adam(b200rl_ctx* ctx, int64_t np, const OptStep& st);
+// reduce + [peer exchange +] clip + Adam in one launch, when its ceil(np / 256) CTAs are all co-resident (B200RL_ERR_UNSUPPORTED
+// otherwise); the peer exchange runs when one is attached
+int nn_reduce_clip_adam(b200rl_ctx* ctx, const float* partial, int n_partials, int64_t np, const float* loss_partial, int n_loss, const OptStep& st);
+// K7 + optimiser step in one launch.  Returns the number of gradient partials (> 0) like nn_ac_loss_grad, or
+// B200RL_ERR_UNSUPPORTED *without side effects* when the configuration is outside the fused path (the caller then runs
+// nn_ac_loss_grad + nn_reduce_clip_adam).
+int nn_ac_loss_grad_step(b200rl_ctx* ctx, const MlpDesc& actor, const MlpDesc& critic, const AcHyper& hp, const AcBatch& b, float* partial,
+                         float* loss_partial, const OptStep& st);
 int nn_target_sync(b200rl_ctx* ctx, float* target, const float* model, int64_t np, float rho);
 // target sync every `freq` optimiser steps, counted on the device: *upd_dev += 1, sync when it is a multiple of freq
 int nn_target_sync_counted(b200rl_ctx* ctx, float* target, const float* model, int64_t np, float rho, unsigned long long* upd_dev, int freq);
@@ -157,5 +152,8 @@ int nn_tc_replay_collect(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& q, con
                          int nsteps, int64_t* keys, float* vals, int stride);
 bool nn_tc_bwd_supported(const MlpDesc& actor, const MlpDesc& critic);
 int nn_tc_partial_rows(int grid, const MlpDesc& actor, const AcHyper& hp, int64_t B);   // gradient-partial rows the tensor-core K7 writes with `grid` CTAs
+// whether K7 with `grid` CTAs can run the optimiser step on np parameters in its tail (the launch geometry only; nn_ac_loss_grad_step
+// decides the rest)
+bool nn_tc_step_fits(b200rl_ctx* ctx, int grid, const MlpDesc& actor, const AcHyper& hp, int64_t B, int64_t np);
 int nn_tc_ac_loss_grad(b200rl_ctx* ctx, int grid, const MlpDesc& actor, const MlpDesc& critic, const float* params, const AcHyper& hp,
-                       const AcBatch& b, float* partial, float* loss_partial, int64_t np, const AcStep* step /* null: loss + backward only */);
+                       const AcBatch& b, float* partial, float* loss_partial, int64_t np, const OptStep* step /* null: loss + backward only */);

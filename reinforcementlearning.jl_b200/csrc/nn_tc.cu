@@ -40,6 +40,9 @@ constexpr float kScaleW = tcfwd::kScale;   // power-of-two operand scales (see t
 // One CTA per SM (640 threads, actor or critic), persistent, software-pipelined across tiles (see the loop).
 // Thread <-> data (workers): warp w: sample quadrant q = w % 4, feature block c = w / 4; thread = sample s = 32q + lane.
 constexpr int NT7 = 512;
+// the fused optimiser step stages the CTA's slice of every partial row through registers: at most kMaxStage floats per worker thread
+// (10 * 512 >= 64 * 74 with the BASELINE network; nn_tc_step_fits)
+constexpr int kMaxStage = 10;
 // The activation images: element (feature f, sample s) at
 //     (f / 8) * GS_T + (s / 8) * GF_T + (s % 8) * 16 + (f % 8) * 2
 // i.e. [feature block of 8][sample][8 features]: thread = sample writes 8 features as ONE 16-byte vector, and the 32 lanes of a
@@ -169,7 +172,7 @@ template <int ACT>
 __global__ void __launch_bounds__(NT7_ALL, 1)
 ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no __restrict__: the fused optimiser step rewrites them in the tail */, AcHyper hp, AcBatch b, float* partial,
                        float* __restrict__ loss_partial, int64_t np_total, float scale_base /* power of two ~ 1 / inv_B */,
-                       AcStep st /* st.params != null: the optimiser step runs in the tail of this launch */,
+                       OptStep st /* st.params != null: the optimiser step runs in the tail of this launch */,
                        int n_actor /* CTAs [0, n_actor) work on the actor, the rest on the critic */) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     SmemBwd& sm = *reinterpret_cast<SmemBwd*>(smem_raw);
@@ -665,23 +668,17 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         float* lp = loss_partial + (int64_t)blockIdx.x * 4;
         lp[0] = role ? 0.f : a0; lp[1] = role ? 0.f : a1; lp[2] = role ? a0 : 0.f; lp[3] = 0.f;
     }
-    // ---- fused optimiser step (K8 inside K7's tail): same arithmetic and summation orders as reduce_clip_adam_kernel ----------
+    // ---- fused optimiser step (K8 inside K7's tail): K8's arithmetic (optim.cuh) and its CTA-order gradient and loss sums; the
+    //      gradient-norm total is summed per lane, then by a butterfly, so it may round differently from K8's --------------------
     if (st.params) {
         const unsigned int G = gridDim.x;
         K7_T(24);                                // (everything since the last tile: drain, head-gradient reductions, partial rows)
         worker_sync();                           // every worker's partial / loss rows are written (CTA scope) ...
         K7_T(25);
-        if (tid == 0) {                          // grid barrier A: every CTA's rows are written
-            __threadfence();                     // ... and ordered before the arrival device-wide (fence cumulativity, as in cooperative groups)
-            atomicAdd(st.counter, 1u);
-            unsigned int spins = 0;
-            while (*reinterpret_cast<volatile unsigned int*>(st.counter) < G)
-                if (++spins > (1u << 26)) __trap();
-            __threadfence();
-        }
+        if (tid == 0) optim::grid_barrier(st.counters, G);   // grid barrier A: every CTA's rows are written
         worker_sync();
         K7_T(26);
-        const int per = (int)((np_total + G - 1) / G);           // parameters per CTA (<= 512: checked by the launcher)
+        const int per = (int)((np_total + G - 1) / G);           // parameters per CTA (<= NT7: nn_tc_step_fits)
         const int64_t k = (int64_t)blockIdx.x * per + tid;
         const bool mine = tid < per && k < np_total;
         const unsigned int seq = st.tab.nranks > 1 ? *st.seq_ptr + 1u : 0u;
@@ -691,7 +688,6 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         const int nstage = per * nrows;                                  // <= 64 * 76 floats with the BASELINE network
         const int64_t k0 = (int64_t)blockIdx.x * per;
         {   // (fixed trip count, loads first: a rolled loop would wait for each L2 round trip before issuing the next)
-            constexpr int kMaxStage = 10;                                // 10 * 512 >= 64 * 74 (checked by the launcher)
             float t[kMaxStage];
 #pragma unroll
             for (int j = 0; j < kMaxStage; ++j) {
@@ -743,17 +739,10 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             const unsigned slot = seq & 1u;
             if (mine) p2p_push(st.tab, 0, slot, (size_t)k, __float_as_uint(gk), seq);
             if (loss_thread) p2p_push(st.tab, 0, slot, (size_t)np_total + tid, __float_as_uint(lsum), seq);
-            float acc = 0.f, lacc = 0.f;
-            for (int r = 0; r < st.tab.nranks; ++r) {
-                if (mine) acc += r == st.tab.rank ? gk : __uint_as_float(p2p_recv(st.tab, 0, slot, r, (size_t)k, seq));
-                if (loss_thread) lacc += r == st.tab.rank ? lsum : __uint_as_float(p2p_recv(st.tab, 0, slot, r, (size_t)np_total + tid, seq));
-            }
-            gk = acc; lsum = lacc;
+            if (mine) gk = p2p_sum_ranks(st.tab, 0, slot, (size_t)k, gk, seq);
+            if (loss_thread) lsum = p2p_sum_ranks(st.tab, 0, slot, (size_t)np_total + tid, lsum, seq);
         }
-        if (loss_thread) {
-            if (st.loss_out4) st.loss_out4[tid] = lsum;
-            if (st.stats_row) st.stats_row[tid] = lsum;
-        }
+        if (loss_thread) optim::publish_loss(st, tid, lsum);
         double sq = (double)gk * (double)gk;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
@@ -765,12 +754,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
                 double t = 0.0;
                 for (int w = 0; w < NT7 / 32; ++w) t += sm.RedD[w];
                 st.cta_sumsq[blockIdx.x] = t;
-                __threadfence();
-                atomicAdd(st.counter + 1, 1u);
-                unsigned int spins = 0;
-                while (*reinterpret_cast<volatile unsigned int*>(st.counter + 1) < G)
-                    if (++spins > (1u << 26)) __trap();
-                __threadfence();
+                optim::grid_barrier(st.counters + 1, G);
             }
             __syncwarp();
             K7_T(29);
@@ -786,13 +770,8 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             for (int o = 16; o > 0; o >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, o);
             if (lane == 0) {
                 const float gn = (float)sqrt(tot);
-                float sc = 1.0f;
-                if (st.max_norm > 0.f && st.max_norm <= gn) sc = st.max_norm / fmaxf(st.max_norm, gn);
-                sm.step_scale = sc;
-                if (blockIdx.x == 0) {
-                    if (st.gnorm_out) *st.gnorm_out = gn;
-                    if (st.stats_row) st.stats_row[4] = gn;
-                }
+                sm.step_scale = optim::clip_scale(gn, st.max_norm);
+                if (blockIdx.x == 0) optim::publish_gnorm(st, gn);
             }
         }
         worker_sync();
@@ -801,21 +780,11 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         if (mine) {
             gk *= sm.step_scale;
             st.grad[k] = gk;
-            const float mk = st.b1 * m_k + (1.0f - st.b1) * gk;
-            const float vk = st.b2 * v_k + (1.0f - st.b2) * (gk * gk);
-            st.m[k] = mk; st.v[k] = vk;
-            st.params[k] = p_k - mk / (1.0f - bt1) / (sqrtf(vk / (1.0f - bt2)) + st.eps) * st.lr;
+            const optim::AdamOut a = optim::adam_update(gk, m_k, v_k, p_k, st.lr, st.b1, st.b2, st.eps, bt1, bt2);
+            st.m[k] = a.m; st.v[k] = a.v; st.params[k] = a.p;
         }
         worker_sync();
-        if (tid == 0) {                          // the last CTA through advances beta^t and re-arms the counters (every thread of
-                                                 // every CTA has read beta^t / the sequence number before its CTA arrives here)
-            if (atomicAdd(st.counter + 2, 1u) + 1u == G) {
-                st.beta_t[0] = bt1 * st.b1; st.beta_t[1] = bt2 * st.b2;
-                st.counter[0] = 0u; st.counter[1] = 0u; st.counter[2] = 0u;
-                if (st.tab.nranks > 1) *st.seq_ptr = seq;
-                if (st.tick) *st.tick += 1u;
-            }
-        }
+        if (tid == 0) optim::close_step<3>(st, bt1, bt2, st.tab.nranks > 1, seq);
         K7_T(31);
     }
     }  // worker warps
@@ -839,17 +808,17 @@ int nn_tc_partial_rows(int grid, const MlpDesc& actor, const AcHyper& hp, int64_
 bool nn_tc_bwd_supported(const MlpDesc& actor, const MlpDesc& critic) {
     return actor.H == 64 && critic.H == 64 && actor.in <= kInMax && actor.nout <= 2 && critic.nout == 1;
 }
+// the optimiser step in K7's tail: every CTA co-resident (one per SM) and at most 256 of them (cta_sumsq), one worker thread per
+// parameter of the CTA's slice, the slice of every partial row in kMaxStage registers per thread, the loss rows in two
+bool nn_tc_step_fits(b200rl_ctx* ctx, int grid, const MlpDesc& actor, const AcHyper& hp, int64_t B, int64_t np) {
+    const int64_t per = (np + grid - 1) / grid;
+    return grid <= ctx->sm_count && grid <= 256 && per <= NT7 && per * nn_tc_partial_rows(grid, actor, hp, B) <= kMaxStage * NT7 &&
+           4 * grid <= 2 * NT7;
+}
 int nn_tc_ac_loss_grad(b200rl_ctx* ctx, int grid, const MlpDesc& actor, const MlpDesc& critic, const float* params, const AcHyper& hp,
-                       const AcBatch& b, float* partial, float* loss_partial, int64_t np, const AcStep* step) {
-    AcStep st = {};
+                       const AcBatch& b, float* partial, float* loss_partial, int64_t np, const OptStep* step) {
+    const OptStep st = step ? *step : OptStep{};
     const int n_actor = nn_tc_actor_ctas(grid, actor, hp, (b.B + TM - 1) / TM);
-    if (step) {
-        st = *step;
-        const int64_t per = (np + grid - 1) / grid;
-        const int rows = n_actor > grid - n_actor ? n_actor : grid - n_actor;
-        REQUIRE(st.params == params && per <= NT7 && grid <= ctx->sm_count && per * rows <= 10 * NT7 && 4 * grid <= 2 * NT7 && grid <= 256, B200RL_ERR_UNSUPPORTED,
-                "fused optimiser step: bad configuration");
-    }
     size_t smem = sizeof(SmemBwd) + 128;
     static unsigned long long attr_devices = 0;   // once per device
     if (first_use_on_device(attr_devices, ctx->device)) {
