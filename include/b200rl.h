@@ -273,6 +273,10 @@ int b200rl_net_nparams(const b200rl_net_desc* desc, int64_t* out);
 int b200rl_net_create(b200rl_ctx* ctx, const b200rl_net_desc* desc, const float* params_host, b200rl_net** out);
 int b200rl_net_destroy(b200rl_net* net);
 int b200rl_net_configure_optimizer(b200rl_net* net, float lr, float beta1, float beta2, float eps, float max_grad_norm);
+/* actor-critic kinds (0, 1): the critic trunk's activation (0 relu, 1 tanh) when it differs from the actor's (desc->act), e.g.
+ * ActorCritic(Chain(Dense(.., relu), ..), Chain(Dense(.., tanh), ..)).  A mixed pair runs the staged launches and the
+ * runtime-activation learner kernel (the fused rollout returns B200RL_ERR_UNSUPPORTED for it). */
+int b200rl_net_set_critic_act(b200rl_net* net, int act);
 /* export / import (checkpoint hooks, docs/src/How_to_use_hooks.md:124-167).
  * which: 0 params | 1 last gradient | 2 Adam m | 3 Adam v | 4 beta^t (2) | 5 target params */
 int b200rl_net_get(b200rl_net* net, int which, float* host_dst, int64_t count);

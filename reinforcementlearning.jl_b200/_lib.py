@@ -143,6 +143,7 @@ SIGNATURES = {
     "b200rl_net_create": (_i32, [_vp, _vp, _vp, _pp]),
     "b200rl_net_destroy": (_i32, [_vp]),
     "b200rl_net_configure_optimizer": (_i32, [_vp, _f32, _f32, _f32, _f32, _f32]),
+    "b200rl_net_set_critic_act": (_i32, [_vp, _i32]),
     "b200rl_net_get": (_i32, [_vp, _i32, _vp, _i64]),
     "b200rl_net_set": (_i32, [_vp, _i32, _vp, _i64]),
     "b200rl_net_ptr": (_i32, [_vp, _i32, _pp]),

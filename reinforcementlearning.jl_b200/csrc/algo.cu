@@ -390,6 +390,14 @@ int b200rl_net_create(b200rl_ctx* ctx, const b200rl_net_desc* d, const float* pa
     return B200RL_OK;
 }
 
+int b200rl_net_set_critic_act(b200rl_net* n, int act) {
+    REQUIRE(n, B200RL_ERR_INVALID, "null net");
+    REQUIRE(!is_q_kind(n->kind), B200RL_ERR_INVALID, "only actor-critic networks have a critic trunk");
+    REQUIRE(act == 0 || act == 1, B200RL_ERR_INVALID, "act must be 0 (relu) or 1 (tanh)");
+    n->critic.act = act;
+    return B200RL_OK;
+}
+
 int b200rl_net_configure_optimizer(b200rl_net* n, float lr, float beta1, float beta2, float eps, float max_grad_norm) {
     REQUIRE(n, B200RL_ERR_INVALID, "null net");
     TRY(ctx_bind(n->ctx));

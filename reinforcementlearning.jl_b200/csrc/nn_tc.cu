@@ -33,7 +33,7 @@ constexpr float kScaleW = tcfwd::kScale;   // power-of-two operand scales (see t
 // K7 on tensor cores: PPO / A2C loss + backward for one minibatch, all four tile GEMMs on wgmma.
 //   GEMM1  H2pre[s][o] = sum_i H1[s][i]  W2[o][i]     A = H1 image (K-major), B = W2 image (K-major)
 //   GEMM2  dH1[s][i]   = sum_j dP2[s][j] W2[j][i]     A = dP2 image (K-major view of dP2^T), B = the W2 image read MN-major
-//   GEMM3  dW2[j][i]  += sum_s dP2[s][j] H1[s][i]     A = dP2^T, B = [H1^T | ones]: feature-major images (MN-major)
+//   GEMM3  dW2[j][i]  += sum_s dP2[s][j] H1[s][i]     A = dP2^T, B = H1^T (and the 1.0 column of x^T for db2): feature-major images (MN-major)
 //   GEMM4  dW1 | db1  += sum_s dP1[s][f] [x | 1][s]   A = dP1^T, B = [x | 1]^T (MN-major)
 // every product the 3-term fp16 split (hi*hi + hi*lo + lo*hi), FP32 accumulate.  GEMM3 / GEMM4 reduce over the tile's samples;
 // the MMA warpgroup adds their results into FP32 shared-memory accumulators (round-to-nearest adds, fixed owner per entry).
@@ -60,16 +60,18 @@ struct SmemBwd {
     alignas(128) uint8_t FP_lo[FIMG];
     alignas(128) uint8_t FH_lo[FIMG];      // H1^T lo
     alignas(128) uint8_t FH_full[FIMG];    // H1^T hi
-    alignas(16) uint8_t FH_ones[2 * GS_T]; // B operand of the db2 GEMM: feature 0 = 1.0 for every sample, the rest 0; written once
-    alignas(128) uint8_t FQ_full[FIMG];    // dP1^T hi | lo: A operand of GEMM4
+    alignas(128) uint8_t FQ_full[FIMG];    // dP1^T hi | lo: A operand of GEMM4, written by the MMA warpgroup from GEMM2's accumulators
     alignas(128) uint8_t FQ_lo[FIMG];
     alignas(128) uint8_t B1[WIMG_BYTES];   // rows 0..63: hi, 64..127: lo of (n = out o, k = in i)  = 64 W2[o + 64 i]
-    // B operand of GEMM4, double-buffered by tile parity (written at publish time, read by the GEMM4 of the same tile one
-    // phase later): features 0..3 = x_i hi, 4 = 1.0 (-> db1), 8..11 = x_i lo, the rest 0;  K = sample
+    // B operand of GEMM4, double-buffered by tile parity (written at publish time, read by the GEMM3 / GEMM4 of the same tile):
+    // features 0..3 = x_i hi, 4 = 1.0 (-> db1, and db2 in GEMM3), 8..11 = x_i lo, the rest 0;  K = sample
     alignas(128) uint8_t XT[2][2 * GS_T];
     alignas(128) uint8_t AH_full[FIMG];    // H1 hi | lo of the tile GEMM1 runs on (same layout as FH)
     alignas(128) uint8_t AH_lo[FIMG];
-    alignas(16) float D[TM * H];           // FP32 result of GEMM1 or GEMM2 for the workers (d_off layout)
+    alignas(16) float D[TM * H];           // FP32 result of GEMM1 for the workers (d_off layout)
+    // relu trunks: bit f = (H1[s][f] > 0) of sample s, by tile parity (written by layer1(), read by the GEMM2 epilogue: act'(H1));
+    // the sign is not recoverable from the fp16 image (hi > 0 and H1 > 0 differ for tiny positive H1)
+    uint64_t H1pos[2][TM];
     float W1[kInMax * H];
     float b1[H], b2[H];
     float W3[H * kNo];                     // [feature][head output]
@@ -79,7 +81,6 @@ struct SmemBwd {
     double RedD[16];
     float step_scale;
     alignas(8) uint64_t bar1;
-    alignas(8) uint64_t bar2;
     alignas(8) uint64_t bar3;
     alignas(8) uint64_t bar4;
     float AccW2[64 * 65 + 64];             // FP32 accumulators of GEMM3: dW2[j][i] at j * 65 + i, then db2[j] (all still operand-scaled)
@@ -158,12 +159,14 @@ __device__ int g_k7_watch = 0;   // watched worker thread (low 16 bits) of CTA (
 #endif
 // 16 worker warps + one MMA warpgroup (warps 16..19) that runs every wgmma: wgmma accumulators are registers of the warpgroup that
 // issues it, so the GEMMs sit on their own warpgroup and the workers never wait for the tensor core except where they need a result.
-// 640 threads leave 96 registers a thread; the MMA warpgroup holds at most one 64 x 64 accumulator (32 registers) at a time and
-// gives registers back (setmaxnreg.dec 64) so that the workers can take 104 (setmaxnreg.inc): 128 x 64 + 512 x 104 = 640 x 96.
+// 640 threads leave 96 registers a thread; the MMA warpgroup holds at most one 64 x 64 accumulator (32 registers) at a time plus
+// the GEMM2 epilogue's live state, and the workers take the rest (setmaxnreg): 128 x kRegsMma + 512 x kRegsWorker <= 640 x 96.
 constexpr int NT7_ALL = NT7 + 128;
 constexpr int kRegsMma = 64, kRegsWorker = 104;
 static_assert(128 * kRegsMma + NT7 * kRegsWorker <= NT7_ALL * 96, "setmaxnreg split must fit the CTA's register allocation");
-constexpr int kBarRdyA = 2, kBarRdyB = 3, kBarRdyC = 4;   // named barriers: workers arrive (bar.arrive), the MMA warpgroup waits (bar.sync)
+constexpr int kBarRdyA = 2, kBarRdyB = 3;   // named barriers: workers arrive (bar.arrive), the MMA warpgroup waits (bar.sync)
+constexpr int kBarMma = 4;                  // named barrier of the MMA warpgroup's 128 threads alone
+__device__ __forceinline__ void mma_sync() { asm volatile("bar.sync %0, 128;" ::"n"(kBarMma) : "memory"); }
 
 // ACT: the trunks' activation as a compile-time constant (B200RL_ACT_RELU / B200RL_ACT_TANH; -1 = read it from the descriptors, for
 // an actor and a critic with different activations).  With the activation known the relu build carries no tanhf expansions at
@@ -211,11 +214,8 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         if (tid < kNo) sm.b3[tid] = tid < d.nout ? p[head_b<false>(d, tid)] : 0.f;
         tcfwd::fill_w2_image<NT7_ALL>(sm.B1, W2);
     }
-    // constant B operand of the db2 GEMM: feature 0 = 1.0 (fp16 0x3C00) for every sample, the rest 0 (the XT buffers are written whole by publish())
-    for (int k = tid; k < 2 * TM; k += NT7_ALL)
-        *reinterpret_cast<uint4*>(sm.FH_ones + 16 * k) = make_uint4(k < TM ? 0x3C00u : 0u, 0u, 0u, 0u);
     if (tid == 32) {   // every thread of the MMA warpgroup arrives once per phase
-        wg::mbar_init(&sm.bar1, 128); wg::mbar_init(&sm.bar2, 128); wg::mbar_init(&sm.bar3, 128); wg::mbar_init(&sm.bar4, 128);
+        wg::mbar_init(&sm.bar1, 128); wg::mbar_init(&sm.bar3, 128); wg::mbar_init(&sm.bar4, 128);
     }
     wg::fence_proxy_async();
     __syncthreads();
@@ -239,9 +239,40 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         };
         auto gemm1 = [&](int h) { gemm_ts3<0>(dacc, sm.AH_full, sm.AH_lo, h, dB1k, 2 * G_F); };
         auto gemm2 = [&](int h) { gemm_ts3<1>(dacc, sm.FP_full, sm.FP_lo, h, dB1t, 2 * GW_S); };   // dH1 = dP2 x W2
+        // GEMM2 epilogue, samples 64h .. 64h+63: dP1 = D2 .* act'(H1) -> the dP1^T image (A operand of GEMM4).  Each thread
+        // writes its fragment's feature pairs as half2 words: a quad covers one 16-byte feature group of one sample and a warp
+        // 128 contiguous bytes (conflict-free).
+        auto store_dp1 = [&](int h, int pbuf) {
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                const int ss = 64 * h + row0 + 8 * hh;
+                const uint64_t pos = relu ? sm.H1pos[pbuf][ss] >> col0 : 0u;   // bit 8j (+1): feature 8j + col0 (+1)
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const uint32_t off = fimg_off(8 * j + col0, ss);
+                    // D2 carries scale_p * kScaleW; the dP1 operand wants scale_p: one exact power-of-two factor
+                    float v0 = dacc[4 * j + 2 * hh] * (1.0f / kScaleW), v1 = dacc[4 * j + 2 * hh + 1] * (1.0f / kScaleW);
+                    if (relu) {   // act'(H1) = (H1 > 0): the signs layer1() kept
+                        v0 = ((pos >> (8 * j)) & 1u) ? v0 : 0.f;
+                        v1 = ((pos >> (8 * j + 1)) & 1u) ? v1 : 0.f;
+                    } else {      // this tile's H1 = (hi + lo) / scale (the H1^T image is rewritten only after GEMM3 of this tile)
+                        const float inv_h = 1.0f / kScaleH;
+                        const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(sm.FH_full + off));
+                        const float2 lf = __half22float2(*reinterpret_cast<const __half2*>(sm.FH_lo + off));
+                        v0 *= dact_f(act, (hf.x + lf.x) * inv_h);
+                        v1 *= dact_f(act, (hf.y + lf.y) * inv_h);
+                    }
+                    uint32_t hi, lo;
+                    split2(v0, v1, hi, lo);
+                    *reinterpret_cast<uint32_t*>(sm.FQ_full + off) = hi;
+                    *reinterpret_cast<uint32_t*>(sm.FQ_lo + off) = lo;
+                }
+            }
+        };
         // GEMM3 (K = 128 samples, M = 64 features j): dP2^T hi x H1^T hi, lo x hi and hi x lo into one accumulator, then
-        // [dP2^T hi | lo] x ones = sum_s dP2 = db2 (column 0 of an N = 8 accumulator).  Added into AccW2 by the fragment's owner thread.
-        auto gemm3 = [&]() {
+        // [dP2^T hi | lo] x the x^T operand, whose feature 4 is 1.0 for every sample: sum_s dP2 = db2 lands in column 4 of an
+        // N = 8 accumulator.  Added into AccW2 by the fragment's owner thread.
+        auto gemm3 = [&](int buf) {
             const uint64_t dPh = wg::make_desc(wg::smem_u32(sm.FP_full), GF_T, GS_T), dPl = wg::make_desc(wg::smem_u32(sm.FP_lo), GF_T, GS_T);
             const uint64_t dHh = wg::make_desc(wg::smem_u32(sm.FH_full), GF_T, GS_T), dHl = wg::make_desc(wg::smem_u32(sm.FH_lo), GF_T, GS_T);
             wg::fence();
@@ -260,18 +291,18 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
                 for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
                     for (int e = 0; e < 2; ++e) sm.AccW2[(row0 + 8 * hh) * 65 + 8 * j + col0 + e] += dacc[4 * j + 2 * hh + e];
-            const uint64_t dOnes = wg::make_desc(wg::smem_u32(sm.FH_ones), GF_T, GS_T);
+            const uint64_t dX = wg::make_desc(wg::smem_u32(sm.XT[buf]), GF_T, GS_T);
             float d8[4] = {0.f, 0.f, 0.f, 0.f};
             wg::fence();
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
                 const uint32_t a = k * 2 * GF_T;
-                wg::mma_m64n8k16<1, 1>(d8, wg::desc_add(dPh, a), wg::desc_add(dOnes, a), k ? 1u : 0u);
-                wg::mma_m64n8k16<1, 1>(d8, wg::desc_add(dPl, a), wg::desc_add(dOnes, a), 1u);
+                wg::mma_m64n8k16<1, 1>(d8, wg::desc_add(dPh, a), wg::desc_add(dX, a), k ? 1u : 0u);
+                wg::mma_m64n8k16<1, 1>(d8, wg::desc_add(dPl, a), wg::desc_add(dX, a), 1u);
             }
             wg::commit();
             wg::wait_all();
-            if (col0 == 0) {
+            if (col0 == 4) {
                 sm.AccW2[64 * 65 + row0] += d8[0];
                 sm.AccW2[64 * 65 + row0 + 8] += d8[2];
             }
@@ -297,9 +328,9 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
                 for (int e = 0; e < 2; ++e)
                     if (col0 + e < 5) sm.AccD4[(row0 + 8 * hh) * 9 + col0 + e] += d4[2 * hh + e];
         };
-        // Per tile: G2(t) | G3(t) | G1(t+1), samples 0..63 (held in registers) | G1(t+1), samples 64..127 | G4(t).  D holds one
-        // result at a time: D2(t) is read by the workers' P7(t), so D1(t+1) is stored once they have handed over RdyC(t), which
-        // they do after P7(t).
+        // Per tile: G2(t) + epilogue (dP1^T image) | G1(t+1) | G3(t) | G4(t).  Only G2 -> G1 sits between the workers' hand-over
+        // of tile t (RdyA) and their P3 of tile t + 1 (bar1); G3(t) and G4(t) run under P3 / P45(t+1).  D holds D1 only: D1(t) is
+        // read in the workers' P3(t), before they hand over RdyA(t).
         if (cta < ntiles) {
             ready_wait(kBarRdyB);                      // H1 operand of the first tile
             for (int h = 0; h < 2; ++h) { gemm1(h); store_d(h); }
@@ -307,24 +338,18 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         }
         int buf = 0;
         for (int64_t tile = cta; tile < ntiles; tile += nctas, buf ^= 1) {
-            const bool has_next = tile + nctas < ntiles;
             ready_wait(kBarRdyA);                      // dP2 / H1^T images of this tile; the workers have read D1(t)
-            for (int h = 0; h < 2; ++h) { gemm2(h); store_d(h); }
-            wg::mbar_arrive(&sm.bar2);
-            gemm3();
-            wg::mbar_arrive(&sm.bar3);
-            if (has_next) {
+            for (int h = 0; h < 2; ++h) { gemm2(h); store_dp1(h, buf); }
+            wg::fence_proxy_async();                   // this thread's share of the dP1^T image -> visible to GEMM4 (after mma_sync)
+            if (tile + nctas < ntiles) {
                 ready_wait(kBarRdyB);                  // H1 operand of the next tile
-                gemm1(0);                              // GEMM1 of the next tile, first half
-            }
-            ready_wait(kBarRdyC);                      // dP1^T image of this tile (its x^T | 1 operand was written at publish time); D2 read
-            if (has_next) {
-                store_d(0);
-                gemm1(1);
-                store_d(1);
+                for (int h = 0; h < 2; ++h) { gemm1(h); store_d(h); }
                 wg::mbar_arrive(&sm.bar1);
             }
-            gemm4(buf);
+            gemm3(buf);
+            wg::mbar_arrive(&sm.bar3);
+            mma_sync();                                // every thread's share of the dP1^T image is in place
+            gemm4(buf);                                // (its x^T | 1 operand was written at publish time)
             wg::mbar_arrive(&sm.bar4);
         }
     } else {
@@ -338,9 +363,10 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
     float l0 = 0.f, l1 = 0.f;
     float mean = 0.f, inv_std = 1.f;
     if (hp.normalize_adv && b.norm2) { mean = b.norm2[0]; inv_std = b.norm2[1]; }
-    uint32_t ph1 = 0, ph2 = 0, ph3 = 0, ph4 = 0;
+    uint32_t ph1 = 0, ph3 = 0, ph4 = 0;
     bool gemm4_pending = false;
     int xbuf = 0;                     // XT buffer of the tile being published (tile parity within this CTA)
+    int pbuf = 0;                     // H1pos buffer of the tile layer1() runs on (tile parity within this CTA)
     // Random gather, per THREAD: each of the four feature-block threads of a sample loads the sample's whole 32-byte record
     // {state | action bits, logp_old, advantage, return} itself (two 16-byte loads from one sector; the three repeats hit L1), so
     // nothing is exchanged through shared memory and no barrier separates the gather from layer 1 or from the loss.  Software
@@ -386,10 +412,11 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
     for (int k = tid; k < 64 * 65 + 64; k += NT7) sm.AccW2[k] = 0.f;
     for (int k = tid; k < 64 * 9; k += NT7) sm.AccD4[k] = 0.f;
     // ---- software pipeline (one tile = 128 samples; tensor core and CUDA cores work on different tiles / phases) ----
-    //   workers        : ... P3(t) P45(t) | P0(t+1) P1(t+1) | P7(t) | P3(t+1) ...
-    //   MMA warpgroup  :              G2(t) G3(t) ..... G1(t+1) ........ G4(t) ...
-    // G2(t) / G3(t) run under P0/P1(t+1), G1(t+1) under P7(t), G4(t) under P3(t+1); the MMA warpgroup starts each GEMM as soon
-    // as the workers have handed its operands over (ready_arrive), so no worker waits for a GEMM whose result it does not need.
+    //   workers        : ... P3(t) P45(t) | P0(t+1) P1(t+1) | P3(t+1) P45(t+1) ...
+    //   MMA warpgroup  :              G2(t) + dP1(t) ..... G1(t+1) | G3(t) G4(t) ...
+    // G2(t) and its epilogue (dP1 = dH1 .* act'(H1) -> the GEMM4 operand) run under P0/P1(t+1), G3(t) / G4(t) under
+    // P3 / P45(t+1); the MMA warpgroup starts each GEMM as soon as the workers have handed its operands over (ready_arrive), so
+    // no worker waits for a GEMM whose result it does not need.
     // P0: the next tile's records leave the prefetch registers (x -> layer 1 and the x^T operand of GEMM4, scalars -> aux),
     // the records of the tile after it are requested, the index of the one after that computed / requested
     float xo[kInMax];
@@ -414,8 +441,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         gi_next = index_of(t + 2 * nctas);
         K7_T(17);
     };
-    uint32_t h1pos = 0, h1pos_tile = 0;   // relu: bit k = (H1[16c + k] > 0) of the tile layer1() ran on last / of the tile P7 works on
-    auto layer1 = [&]() {   // P1: H1 = act(W1 x + b1) -> A operand of GEMM1 (hi | lo fp16 images)
+    auto layer1 = [&]() {   // P1: H1 = act(W1 x + b1) -> A operand of GEMM1 (hi | lo fp16 images); relu: its signs -> H1pos
         uint32_t pos = 0;
         uint32_t hi8[8], lo8[8];
 #pragma unroll
@@ -438,7 +464,8 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             split2(h[0], h[1], hi8[2 * ch], lo8[2 * ch]);
             split2(h[2], h[3], hi8[2 * ch + 1], lo8[2 * ch + 1]);
         }
-        h1pos = pos;
+        if (relu) reinterpret_cast<uint16_t*>(&sm.H1pos[pbuf][s])[c] = (uint16_t)pos;   // bits 16c .. 16c+15 of the sample's word
+        pbuf ^= 1;
         store16_feat(sm.AH_full, 16 * c, s, hi8);
         store16_feat(sm.AH_lo, 16 * c, s, lo8);
     };
@@ -527,77 +554,29 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         }
         K7_T(5);
         wg::fence_proxy_async();
+        // The previous tile's GEMM4 must have consumed its XT buffer (the same parity as the next tile's, which publish() rewrites).
+        // Waited before this tile's hand-over: GEMM4(t) depends on it, so no bar4 phase can complete twice before it is waited for.
+        // (The MMA warpgroup runs GEMM4(t-1) before it waits for RdyA(t) anyway: the wait costs it nothing.)
+        if (gemm4_pending) {
+            wg::mbar_wait(&sm.bar4, ph4);
+            ph4 ^= 1u;
+        }
+        K7_T(6);
         ready_arrive(kBarRdyA);     // this thread's share of the GEMM2 / GEMM3 operands is in place
         gemm3_pending = true;       // (Zp is rewritten in P3 of the next tile, behind its wait for GEMM1, i.e. after every thread has passed
-                                    //  this point: no barrier needed here)
-        K7_T(6);
+        gemm4_pending = true;       //  this point: no barrier needed here)
         K7_T(7);
-        h1pos_tile = h1pos;         // this tile's H1 signs, before layer1() of the next tile replaces them
         if (has_next) {
-            if (gemm4_pending) {   // the previous tile's GEMM4 must have consumed its XT buffer (same parity as the next tile's) and the
-                wg::mbar_wait(&sm.bar4, ph4);     // dP1^T image before either is overwritten
-                ph4 ^= 1u;
-                gemm4_pending = false;
-            }
             publish(tile + nctas);
-            K7_T(8);
-            K7_T(9);
             layer1();
             wg::fence_proxy_async();
-            K7_T(10);
+            K7_T(8);
             ready_arrive(kBarRdyB);
-            K7_T(11);
+            K7_T(9);
         }
-        K7_T(12);
-        // ---- P7: dP1 = D2 .* act'(H1) -> dP1^T image (GEMM4 reduces it against [x | 1] into dW1 | db1) ----------
-        wg::mbar_wait(&sm.bar2, ph2);
-        ph2 ^= 1u;
-        K7_T(13);
-        {
-            float v[16];
-            d_ld16(sm.D, s, 16 * c, v);
-#pragma unroll
-            // D2 carries scale_p * kScaleW; the dP1 operand wants scale_p: one exact power-of-two factor (bit-identical to unscaling
-            // to dH1 and rescaling)
-            for (int k = 0; k < 16; ++k) v[k] *= 1.0f / kScaleW;
-            if (relu) {   // act'(H1) = (H1 > 0): the signs layer1() kept in a register
-#pragma unroll
-                for (int k = 0; k < 16; ++k) v[k] = ((h1pos_tile >> k) & 1u) ? v[k] : 0.f;
-            } else {
-                const float inv_h = 1.0f / kScaleH;
-#pragma unroll
-                for (int g8 = 0; g8 < 2; ++g8) {                               // this tile's H1 = (hi + lo) / scale (image still intact)
-                    const uint32_t off = fimg_off(16 * c + 8 * g8, s);
-                    const uint4 hv = *reinterpret_cast<const uint4*>(sm.FH_full + off), lv = *reinterpret_cast<const uint4*>(sm.FH_lo + off);
-                    const uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w}, lw[4] = {lv.x, lv.y, lv.z, lv.w};
-#pragma unroll
-                    for (int m = 0; m < 4; ++m) {
-                        const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hw[m])), lf = __half22float2(*reinterpret_cast<const __half2*>(&lw[m]));
-                        v[8 * g8 + 2 * m] *= dact_f(act, (hf.x + lf.x) * inv_h);
-                        v[8 * g8 + 2 * m + 1] *= dact_f(act, (hf.y + lf.y) * inv_h);
-                    }
-                }
-            }
-            if (gemm4_pending) {   // (last tile: no publish() waited for it)
-                wg::mbar_wait(&sm.bar4, ph4);
-                ph4 ^= 1u;
-                gemm4_pending = false;
-            }
-            {
-                uint32_t hi8[8], lo8[8];
-#pragma unroll
-                for (int m = 0; m < 8; ++m) split2(v[2 * m], v[2 * m + 1], hi8[m], lo8[m]);
-                store16_feat(sm.FQ_full, 16 * c, s, hi8);
-                store16_feat(sm.FQ_lo, 16 * c, s, lo8);
-            }
-            gemm4_pending = true;
-        }
-        K7_T(14);
 #ifdef B200RL_K7_TIMING
         if (tid == (g_k7_watch & 0xFFFF) && (int)blockIdx.x == (g_k7_watch >> 16)) g_k7_phase[15] += 1;
 #endif
-        wg::fence_proxy_async();
-        ready_arrive(kBarRdyC);
     }
     // ---- drain: last GEMM3 / GEMM4 (their sums are in AccW2 / AccD4), then the head gradients (fixed-order reductions) -------
     if (gemm3_pending) wg::mbar_wait(&sm.bar3, ph3);
