@@ -299,7 +299,9 @@ int b200rl_net_q_act(b200rl_net* net, const float* obs_dev, int64_t n, uint64_t*
 /* A value-based explorer applied to a batch the way BatchExplorer does (explorers/batch_explorer.jl:15-21): the inner explorer
  * is called once per column, column i draws from its own stream rng_dev[:, i] (the reference draws all columns from one
  * stream — not parallel; DESIGN.md §3), and for the kinds with a step column i is planned at step + i and the caller advances
- * `step` by n afterwards.  Per column, on Q = the column's Q-values (n_actions of them):
+ * `step` by n afterwards.  On a sharded ctx (rank r of a communicator of `world` ranks, b200rl_comm_rank_world) the n columns are
+ * columns r n .. r n + n - 1 of one BatchExplorer over the world n columns of all ranks: column i is planned at step + r n + i,
+ * and the caller advances `step` by world n (the same on every rank).  Per column, on Q = the column's Q-values (n_actions of them):
  *   kind 0 / 1  EpsilonGreedyExplorer{:linear | :exp, is_break_tie} (explorers/epsilon_greedy_explorer.jl:47-112): eps =
  *               get_eps(step + i) (Float64 schedule); u = rand(rng) is always drawn; u >= eps ? findmax(Q)[2] (or, is_break_tie,
  *               rand(rng, find_all_max(Q)[2])) : rand(rng, 1:n_actions)
@@ -346,7 +348,9 @@ int b200rl_evaluate(b200rl_net* net, b200rl_env* env, const b200rl_eval_config* 
  * N n_steps (as b200rl_replay_run).  The network (its update counter and target too) is only read.  Refused before any side effect:
  * B200RL_ERR_UNSUPPORTED for Float64, Acrobot and continuous-action envs; B200RL_ERR_INVALID for a network that is not a Q-network,
  * an input / head width that does not match the env, n_steps < 1, max_episodes < 0, an explorer without streams and a bad explorer
- * (see b200rl_explorer).  One fused launch for hidden = 64 on the tensor-core path. */
+ * (see b200rl_explorer).  One fused launch for hidden = 64 on the tensor-core path.  On a sharded ctx the columns are numbered
+ * over the ranks' union as in b200rl_net_q_explore: column i of rank r at window step k plans at ex->step + k world N + r N + i,
+ * and ex->step advances by world N n_steps. */
 int b200rl_evaluate_explore(b200rl_net* net, b200rl_env* env, int32_t n_steps, int32_t max_episodes, b200rl_explorer* ex,
                             uint64_t* explorer_rng_dev, float* returns_out, int32_t* lengths_out, int32_t* counts_out, int on_device);
 
@@ -432,12 +436,30 @@ typedef struct b200rl_replay b200rl_replay;
  * where rewards are not integers).  The explorer step, the update counter and the controller counters advance on the host by
  * arithmetic.  The trajectory keeps (min(2k + 1, capacity + 1), N) touched-leaf keys for the longest stretch k (prioritised).
  * create refuses, before any side effect: a network that is not a Q-network, a Float64 / continuous-action / Acrobot env,
- * trajectory lanes != N or a state width that does not match, a sharded ctx (world > 1), an n-step gamma != cfg->gamma (also
- * refused by run).  The trajectory needs a sampler; a change of its n-step setting between runs re-captures the graphs. */
+ * trajectory lanes != N or a state width that does not match, a sharded ctx with neither the peer exchange attached nor an NCCL
+ * communicator, an n-step gamma != cfg->gamma (also refused by run).  The trajectory needs a sampler; a change of its n-step
+ * setting between runs re-captures the graphs.
+ *
+ * Sharded (a ctx whose communicator has world G > 1; one process per GPU, DESIGN.md §3): G ranks of N envs each run what
+ * run(Agent(QBasedPolicy(DQNLearner, explorer), Trajectory), env, StopAfterNSteps(n)) runs over G N envs, in this sense:
+ *   1. Envs, rings, sum trees and sampler streams are per rank: rank r owns global envs [r N, (r + 1) N), its env and explorer
+ *      streams are keyed by the global env index, its trajectory holds only its own lanes.
+ *   2. Explorer columns are numbered globally: column i of rank r plans at explorer step s + r N + i, and a plan! advances the
+ *      step by G N — one BatchExplorer over the G N columns (see b200rl_net_q_explore).
+ *   3. Each update draws B per rank: the global batch is G B, the gradient their mean (1 / (B G)), one exchange per update.  PER
+ *      weights stay per rank, (N_r P_r(i))^-beta normalised over the rank's own batch — not one prioritised ring over the union.
+ *   4. Every rank runs the same InsertSampleRatioController schedule, hence the same updates per step and the target sync at the
+ *      same update: parameters, Adam state and target stay bit-identical on all ranks.
+ *   5. stats4: loss and grad_norm are global, mean |td| is the rank's own.
+ *   6. Each run starts with one small all-reduce in which the ranks compare N, B, n_steps, the controller (ratio, threshold,
+ *      counters), the explorer (kind, schedule, step), a digest of the DQN config and the n-step setting; if any differs — or a
+ *      rank refuses the run for a reason of its own — every rank returns B200RL_ERR_INVALID with nothing else touched.
+ * The update units are replayed as CUDA graphs when the peer exchange is attached and every rank owns its device
+ * (b200rl_comm_p2p_set_exclusive); with NCCL only, or ranks sharing a device, they launch eagerly. */
 int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl_traj* traj, const b200rl_dqn_config* cfg,
                          b200rl_replay** out);
 /* explorer_rng_dev: (4, N) DEVICE explorer streams (one per env, advanced).  ex: any b200rl_explorer kind (its step is advanced
- * by n_steps * N), NULL = GreedyExplorer (findmax, no draw).  ctl: counters advanced.  stats4 (may be NULL; synchronises):
+ * by n_steps * N * world), NULL = GreedyExplorer (findmax, no draw).  ctl: counters advanced.  stats4 (may be NULL; synchronises):
  * loss, grad_norm, mean |td|, n_updates of the last update in the window (untouched when the window ran none).  Refuses a bad
  * explorer schedule or controller values before any side effect.  A CUDA error part-way through returns with the device state
  * advanced and *ex / *ctl NOT advanced: the run cannot be continued from them. */
@@ -473,6 +495,9 @@ int b200rl_comm_p2p_attach(b200rl_ctx* ctx, void* const* regions);
 int b200rl_ctx_pci_bus_id(b200rl_ctx* ctx, char* out, int len);
 int b200rl_comm_p2p_set_exclusive(b200rl_ctx* ctx, int exclusive);
 int b200rl_comm_allreduce_f32(b200rl_ctx* ctx, float* dev_buf, int64_t n);
+/* rank and number of ranks of the ctx's communicator (0 and 1 without one): the column offset rank N and the explorer step
+ * stride world N of a sharded QBasedPolicy (b200rl_net_q_explore) */
+int b200rl_comm_rank_world(b200rl_ctx* ctx, int* rank, int* world);
 
 #ifdef __cplusplus
 }

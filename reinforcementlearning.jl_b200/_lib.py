@@ -189,6 +189,7 @@ SIGNATURES = {
     "b200rl_comm_p2p_attach": (_i32, [_vp, _vp]),
     "b200rl_ctx_pci_bus_id": (_i32, [_vp, _vp, _i32]),
     "b200rl_comm_p2p_set_exclusive": (_i32, [_vp, _i32]),
+    "b200rl_comm_rank_world": (_i32, [_vp, C.POINTER(_i32), C.POINTER(_i32)]),
 }
 
 _LIB = None
@@ -250,6 +251,12 @@ class Context:
 
     def sync(self):
         check(self.lib.b200rl_sync(self.h))
+
+    def rank_world(self):
+        """(rank, world) of the ctx's communicator; (0, 1) without one (b200rl_comm_rank_world)."""
+        r, w = C.c_int32(), C.c_int32()
+        check(self.lib.b200rl_comm_rank_world(self.h, C.byref(r), C.byref(w)))
+        return r.value, w.value
 
     def stream(self):
         s = C.c_void_p()

@@ -653,10 +653,11 @@ int b200rl_evaluate_explore(b200rl_net* n, b200rl_env* env, int32_t n_steps, int
     REQUIRE(n_steps >= 1, B200RL_ERR_INVALID, "n_steps must be >= 1");
     REQUIRE(max_episodes >= 0, B200RL_ERR_INVALID, "max_episodes must be >= 0");
     const int64_t N = b200rl_env_internal_n(env);
+    const int64_t NW = N * b200rl_comm_world(n->ctx);   // columns of one plan! over the ranks' union (DESIGN.md §3)
     if (ex) {
         REQUIRE(explorer_rng_dev, B200RL_ERR_INVALID, "an explorer other than GreedyExplorer needs the (4, N) device explorer streams");
         TRY(check_explorer(ex));
-        REQUIRE(n_steps <= ((1ll << 62) - (ex->step > 0 ? ex->step : 0)) / N, B200RL_ERR_INVALID, "explorer step would overflow");
+        REQUIRE(n_steps <= ((1ll << 62) - (ex->step > 0 ? ex->step : 0)) / NW, B200RL_ERR_INVALID, "explorer step would overflow");
     }
     TRY(ctx_bind(n->ctx));
     b200rl_ctx* ctx = n->ctx;
@@ -670,10 +671,10 @@ int b200rl_evaluate_explore(b200rl_net* n, b200rl_env* env, int32_t n_steps, int
         [&](int k, const EvalBufs& b, const void**) -> int {
             if (!ex) return nn_q_act(ctx, n->actor, n->params, obs, N, nullptr, 0.0f, (int32_t*)b.act, b.heads);   // GreedyExplorer
             b200rl_explorer e = *ex;
-            e.step = ex->step + (int64_t)k * N;     // BatchExplorer: the inner explorer's step moved N times per plan!
+            e.step = ex->step + (int64_t)k * NW;    // BatchExplorer: the inner explorer's step moved N · world times per plan!
             return nn_q_explore(ctx, n->actor, n->params, obs, N, xrng, e, (int32_t*)b.act, b.heads);
         }));
-    if (ex) ex->step += (int64_t)n_steps * N;
+    if (ex) ex->step += (int64_t)n_steps * NW;
     return B200RL_OK;
 }
 
@@ -1239,6 +1240,7 @@ namespace {
 __global__ void add_i64_kernel(long long* __restrict__ v, long long d) { *v += d; }
 }  // namespace
 
+constexpr int kAgree = 20;   // values of the agreement exchange of a sharded run (replay_agree)
 // what the captured launches bake in besides the handles: a change means re-capture
 struct ReplayKey {
     int tc, max_timeout, greedy, pad;
@@ -1256,12 +1258,13 @@ struct b200rl_replay {
     b200rl_dqn_config cfg;
     int64_t N, B;
     int32_t* action;              // (N) planned actions
-    long long* ex_step_dev;       // explorer step, advanced by N per step on the device
+    long long* ex_step_dev;       // explorer step, advanced by N · world per step on the device
     unsigned long long* upd_dev;  // optimiser steps of the Q-network (the target-sync phase), advanced per update on the device
     float* td_keep;               // TD errors of the last update
     int64_t* keys; float* vals;   // (stride, N) sum-tree leaves a fused collect window touched (prioritised ring)
     int stride_cap;               // rows of keys / vals allocated
     long long h_counters[2];
+    double* agree_dev;            // (world, 2 kAgree) table of the agreement exchange (sharded ctx)
     GraphUnit graphs;             // "1 step + m updates" units, by m
 };
 
@@ -1274,7 +1277,7 @@ static int replay_collect_step(b200rl_replay* r, uint64_t* rng, const b200rl_exp
     TRY(ctx_scratch(ctx, (size_t)r->N * n->actor.nout * 4 + 256, &s));
     if (ex) {
         TRY(nn_q_explore(ctx, n->actor, n->params, obs, r->N, (unsigned long long*)rng, *ex, r->action, (float*)s, r->ex_step_dev));
-        add_i64_kernel<<<1, 1, 0, ctx->stream>>>(r->ex_step_dev, (long long)r->N);
+        add_i64_kernel<<<1, 1, 0, ctx->stream>>>(r->ex_step_dev, (long long)r->N * b200rl_comm_world(ctx));
         LAUNCH_CHECK(ctx);
     } else {
         TRY(nn_q_act(ctx, n->actor, n->params, obs, r->N, nullptr, 0.0f, r->action, (float*)s));
@@ -1285,6 +1288,23 @@ static int replay_collect_step(b200rl_replay* r, uint64_t* rng, const b200rl_exp
 static int replay_stride(const b200rl_replay* r, int64_t k) {
     const int64_t F = b200rl_traj_internal_ring(r->traj).frames();
     return (int)(2 * k + 1 < F ? 2 * k + 1 : F);
+}
+// scratch every launch of the loop needs: the update's Q tables and TD errors, the staged collect's Q values
+static size_t replay_scratch_bytes(const b200rl_replay* r) {
+    const size_t q_bytes = (size_t)r->B * r->net->actor.nout * 4 * 2 + 256;
+    const size_t need_upd = q_bytes + (size_t)r->B * 4 + 256, need_q = (size_t)r->N * r->net->actor.nout * 4 + 256;
+    return need_upd > need_q ? need_upd : need_q;
+}
+// (stride, N) touched-leaf keys / vals for collect stretches up to `stride` rows (prioritised ring)
+static int replay_grow_keys(b200rl_replay* r, int stride) {
+    if (stride <= r->stride_cap) return B200RL_OK;
+    CUDA_TRY(cudaStreamSynchronize(r->ctx->stream));
+    cudaFree(r->keys); cudaFree(r->vals);
+    r->keys = nullptr; r->vals = nullptr; r->stride_cap = 0;
+    CUDA_TRY(cudaMalloc(&r->keys, (size_t)stride * r->N * 8));
+    CUDA_TRY(cudaMalloc(&r->vals, (size_t)stride * r->N * 4));
+    r->stride_cap = stride;
+    return B200RL_OK;
 }
 // k collect steps: one fused launch (H = 64 on the tensor-core path; + one sum-tree rebuild for a prioritised ring), otherwise k x
 // the staged launches
@@ -1298,7 +1318,7 @@ static int replay_collect(b200rl_replay* r, uint64_t* rng, const b200rl_explorer
                                       b200rl_traj_internal_default_priority(r->traj), prio ? 1 : 0, (int)k, r->keys, r->vals, stride);
         if (st == B200RL_OK) {
             if (ex) {
-                add_i64_kernel<<<1, 1, 0, ctx->stream>>>(r->ex_step_dev, (long long)r->N * k);
+                add_i64_kernel<<<1, 1, 0, ctx->stream>>>(r->ex_step_dev, (long long)r->N * b200rl_comm_world(ctx) * k);
                 LAUNCH_CHECK(ctx);
             }
             b200rl_traj_internal_add_pushed(r->traj, k);
@@ -1308,6 +1328,40 @@ static int replay_collect(b200rl_replay* r, uint64_t* rng, const b200rl_explorer
         if (st != B200RL_ERR_UNSUPPORTED) return st;
     }
     for (int64_t j = 0; j < k; ++j) TRY(replay_collect_step(r, rng, ex));
+    return B200RL_OK;
+}
+// The values the ranks of a sharded b200rl_replay_run must agree on (DESIGN.md §3): ranks that ran different numbers of updates
+// would wait for each other in the gradient exchange for ever.  Each 64-bit value travels as its two 32-bit halves (exact in
+// Float64) in the rank's own row of a (world, 2 kAgree) table; one sum all-reduce of the table hands every rank every row.
+static uint64_t f64_bits(double d) { uint64_t b; memcpy(&b, &d, 8); return b; }
+static int replay_agree(b200rl_replay* r, const b200rl_explorer* ex, const b200rl_insert_sample_ratio* ctl, int64_t n_steps, bool local_ok,
+                        bool* agree) {
+    b200rl_ctx* ctx = r->ctx;
+    const int world = b200rl_comm_world(ctx), rank = b200rl_comm_rank(ctx);
+    uint64_t cfg_digest = 1469598103934665603ull;   // FNV-1a of the DQN config's bytes (floats and int32s, no padding)
+    const unsigned char* cb = (const unsigned char*)&r->cfg;
+    for (size_t j = 0; j < sizeof r->cfg; ++j) cfg_digest = (cfg_digest ^ cb[j]) * 1099511628211ull;
+    int ns; float ng;
+    b200rl_traj_internal_nstep(r->traj, &ns, &ng);
+    const b200rl_explorer e = ex ? *ex : b200rl_explorer{};
+    const uint64_t v[kAgree] = {local_ok ? 1ull : 0ull, (uint64_t)r->N, (uint64_t)r->B, (uint64_t)n_steps,
+                                f64_bits(ctl->ratio), (uint64_t)ctl->threshold, (uint64_t)ctl->n_inserted, (uint64_t)ctl->n_sampled,
+                                ex ? 1ull : 0ull, (uint64_t)e.kind, f64_bits(e.eps_stable), f64_bits(e.eps_init), (uint64_t)e.warmup_steps,
+                                (uint64_t)e.decay_steps, (uint64_t)e.step, (uint64_t)e.is_break_tie, f64_bits(e.beta), cfg_digest,
+                                (uint64_t)ns, (uint64_t)f64_bits((double)ng)};
+    const int W = 2 * kAgree;
+    std::vector<double> tab((size_t)world * W, 0.0);
+    for (int j = 0; j < kAgree; ++j) {
+        tab[(size_t)rank * W + 2 * j] = (double)(uint32_t)(v[j] >> 32);
+        tab[(size_t)rank * W + 2 * j + 1] = (double)(uint32_t)v[j];
+    }
+    CUDA_TRY(cudaMemcpyAsync(r->agree_dev, tab.data(), tab.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    TRY(b200rl_comm_allreduce_internal(ctx, r->agree_dev, (int64_t)tab.size(), 1));
+    CUDA_TRY(cudaMemcpyAsync(tab.data(), r->agree_dev, tab.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    *agree = true;
+    for (int q = 0; q < world; ++q)
+        for (int j = 0; j < W; ++j) *agree = *agree && tab[(size_t)q * W + j] == tab[(size_t)rank * W + j];
     return B200RL_OK;
 }
 static int replay_unit(b200rl_replay* r, uint64_t* rng, const b200rl_explorer* ex, int64_t m) {
@@ -1323,6 +1377,7 @@ int b200rl_replay_destroy(b200rl_replay* r) {
     cudaSetDevice(r->ctx->device);
     cudaStreamSynchronize(r->ctx->stream);
     cudaFree(r->action); cudaFree(r->ex_step_dev); cudaFree(r->upd_dev); cudaFree(r->td_keep); cudaFree(r->keys); cudaFree(r->vals);
+    cudaFree(r->agree_dev);
     delete r;
     return B200RL_OK;
 }
@@ -1343,7 +1398,10 @@ int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl
     TrajBatchView b = b200rl_traj_internal_batch(traj);
     REQUIRE(b.B > 0, B200RL_ERR_INVALID, "the trajectory was created without a sampler (batch_size = 0)");
     REQUIRE(b.ns == q->actor.in, B200RL_ERR_INVALID, "trajectory state width != network input width");
-    REQUIRE(b200rl_comm_world(ctx) == 1, B200RL_ERR_UNSUPPORTED, "the replay agent loop runs on one GPU (communicator world > 1)");
+    const int world = b200rl_comm_world(ctx);
+    P2PTable peers;
+    REQUIRE(world == 1 || b200rl_comm_p2p_table(ctx, &peers) || b200rl_comm_has_nccl(ctx), B200RL_ERR_UNSUPPORTED,
+            "a sharded ctx needs the peer exchange attached or an NCCL communicator");
     TRY(check_nstep_gamma(traj, cfg));
     b200rl_replay* r = new b200rl_replay();   // (value-initialised: every pointer and counter starts at zero)
     r->ctx = ctx; r->net = q; r->env = env; r->traj = traj; r->cfg = *cfg; r->N = N; r->B = b.B;
@@ -1352,31 +1410,53 @@ int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl
     R_TRY(cudaMalloc(&r->ex_step_dev, sizeof(long long)));
     R_TRY(cudaMalloc(&r->upd_dev, sizeof(unsigned long long)));
     R_TRY(cudaMalloc(&r->td_keep, (size_t)b.B * 4));
+    if (world > 1) R_TRY(cudaMalloc(&r->agree_dev, (size_t)world * 2 * kAgree * sizeof(double)));
 #undef R_TRY
+    if (world > 1) {
+        // A sharded run allocates nothing: a device allocation serialises with the kernels running on the device, and the ranks of
+        // one process may share it — a rank allocating while a peer rank's kernel waits for it inside the exchange would never
+        // finish.  So the loop's scratch and the touched-leaf lists of the longest possible stretch are allocated here.
+        void* sc;
+        int st = ctx_scratch(ctx, replay_scratch_bytes(r), &sc);
+        if (st == B200RL_OK && b200rl_traj_internal_prioritized(traj)) st = replay_grow_keys(r, (int)b200rl_traj_internal_ring(traj).frames());
+        if (st != B200RL_OK) { b200rl_replay_destroy(r); return st; }
+    }
     *out = r;
     return B200RL_OK;
 }
 
 int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explorer* ex, b200rl_insert_sample_ratio* ctl, int64_t n_steps, float* stats4) {
     REQUIRE(r && ctl, B200RL_ERR_INVALID, "null argument");
-    REQUIRE(n_steps >= 0, B200RL_ERR_INVALID, "n_steps must be >= 0");
-    if (ex) {
-        REQUIRE(explorer_rng_dev, B200RL_ERR_INVALID, "an explorer other than GreedyExplorer needs the (4, N) device explorer streams");
-        TRY(check_explorer(ex));
-        REQUIRE(n_steps <= ((1ll << 62) - (ex->step > 0 ? ex->step : 0)) / r->N, B200RL_ERR_INVALID, "explorer step would overflow");
-    }
-    REQUIRE(replay::controller_ok(*ctl), B200RL_ERR_INVALID, "bad controller values (ratio finite in [0, 1e6], counters >= 0)");
-    REQUIRE(ctl->n_inserted + n_steps < (1ll << 52), B200RL_ERR_INVALID, "controller counters too large");
-    TRY(check_nstep_gamma(r->traj, &r->cfg));
+    const int world = b200rl_comm_world(r->ctx);
+    const int64_t NW = r->N * world;   // columns of one plan! over the ranks' union (DESIGN.md §3)
+    auto local_checks = [&]() -> int {
+        REQUIRE(n_steps >= 0, B200RL_ERR_INVALID, "n_steps must be >= 0");
+        if (ex) {
+            REQUIRE(explorer_rng_dev, B200RL_ERR_INVALID, "an explorer other than GreedyExplorer needs the (4, N) device explorer streams");
+            TRY(check_explorer(ex));
+            REQUIRE(n_steps <= ((1ll << 62) - (ex->step > 0 ? ex->step : 0)) / NW, B200RL_ERR_INVALID, "explorer step would overflow");
+        }
+        REQUIRE(replay::controller_ok(*ctl), B200RL_ERR_INVALID, "bad controller values (ratio finite in [0, 1e6], counters >= 0)");
+        REQUIRE(ctl->n_inserted + n_steps < (1ll << 52), B200RL_ERR_INVALID, "controller counters too large");
+        return check_nstep_gamma(r->traj, &r->cfg);
+    };
+    const int local = local_checks();
     TRY(ctx_bind(r->ctx));
     b200rl_ctx* ctx = r->ctx;
     b200rl_net* n = r->net;
+    if (world > 1) {   // every rank takes part in the exchange, a rank that refuses too, so that no rank waits for it
+        bool agree = false;
+        TRY(replay_agree(r, ex, ctl, n_steps, local == B200RL_OK, &agree));
+        if (local != B200RL_OK) return local;
+        REQUIRE(agree, B200RL_ERR_INVALID,
+                "the ranks of a sharded run disagree on N, batch size, n_steps, controller, explorer, DQN config or n-step setting "
+                "(or another rank refused the run)");
+    }
+    if (local != B200RL_OK) return local;
     if (n_steps == 0) return B200RL_OK;
     // every scratch user of the loop at its final size now, so that no captured launch sees the buffer move
     void* sc;
-    const size_t q_bytes = (size_t)r->B * n->actor.nout * 4 * 2 + 256;
-    const size_t need_upd = q_bytes + (size_t)r->B * 4 + 256, need_q = (size_t)r->N * n->actor.nout * 4 + 256;
-    TRY(ctx_scratch(ctx, need_upd > need_q ? need_upd : need_q, &sc));
+    TRY(ctx_scratch(ctx, replay_scratch_bytes(r), &sc));
     // the schedule of the window: m updates after each step; stretches of steps without an update become one collect launch
     b200rl_insert_sample_ratio c = *ctl;
     std::vector<int64_t> ms((size_t)n_steps);
@@ -1386,15 +1466,7 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
         run = ms[(size_t)j] == 0 ? run + 1 : 0;
         if (run > longest) longest = run;
     }
-    if (b200rl_traj_internal_prioritized(r->traj) && replay_stride(r, longest) > r->stride_cap) {   // touched-leaf lists of a window
-        const int stride = replay_stride(r, longest);
-        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-        cudaFree(r->keys); cudaFree(r->vals);
-        r->keys = nullptr; r->vals = nullptr; r->stride_cap = 0;
-        CUDA_TRY(cudaMalloc(&r->keys, (size_t)stride * r->N * 8));
-        CUDA_TRY(cudaMalloc(&r->vals, (size_t)stride * r->N * 4));
-        r->stride_cap = stride;
-    }
+    if (b200rl_traj_internal_prioritized(r->traj)) TRY(replay_grow_keys(r, replay_stride(r, longest)));   // touched-leaf lists of a window
     ReplayKey key;
     memset(&key, 0, sizeof key);
     key.tc = nn_tc_enabled() ? 1 : 0;
@@ -1412,6 +1484,11 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
     CUDA_TRY(cudaMemcpyAsync(r->ex_step_dev, &r->h_counters[0], sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemcpyAsync(r->upd_dev, &r->h_counters[1], sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
     const CounterSet counters{ctx, n, r->env, r->traj, nullptr};
+    // Captured when every rank owns its device.  Eager launches otherwise: NCCL collectives (no peer exchange) are not captured, and
+    // where ranks share a device, instantiating or uploading a graph may wait for the device's running kernels — one of them a peer's
+    // exchange waiting for this rank.
+    P2PTable peers;
+    const bool capturable = world == 1 || (b200rl_comm_p2p_table(ctx, &peers) && peers.exclusive);
     bool updated = false;
     for (int64_t j = 0; j < n_steps;) {
         const int64_t m = ms[(size_t)j];
@@ -1424,10 +1501,10 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
         }
         ++j;
         updated = true;
-        TRY(r->graphs.run(m, counters, true, [&] { return replay_unit(r, explorer_rng_dev, ex, m); }));
+        TRY(r->graphs.run(m, counters, capturable, [&] { return replay_unit(r, explorer_rng_dev, ex, m); }));
     }
     *ctl = c;
-    if (ex) ex->step += n_steps * r->N;
+    if (ex) ex->step += n_steps * NW;
     if (stats4 && updated) TRY(dqn_stats(n, r->td_keep, r->B, stats4));
     return B200RL_OK;
 }

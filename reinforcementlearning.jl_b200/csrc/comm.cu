@@ -105,6 +105,8 @@ void b200rl_comm_destroy_internal(b200rl_ctx* ctx) {
     }
 }
 int b200rl_comm_world(b200rl_ctx* ctx) { return ctx->comm ? ctx->comm->nranks : 1; }
+int b200rl_comm_rank(b200rl_ctx* ctx) { return ctx->comm ? ctx->comm->rank : 0; }
+bool b200rl_comm_has_nccl(b200rl_ctx* ctx) { return ctx->comm && ctx->comm->comm; }
 bool b200rl_comm_p2p_table(b200rl_ctx* ctx, P2PTable* out) {
     if (!ctx->comm || ctx->comm->tab.nranks <= 1) return false;
     *out = ctx->comm->tab;
@@ -227,6 +229,13 @@ int b200rl_ctx_pci_bus_id(b200rl_ctx* ctx, char* out, int len) {
 int b200rl_comm_p2p_set_exclusive(b200rl_ctx* ctx, int exclusive) {
     REQUIRE(ctx && ctx->comm && ctx->comm->tab.nranks > 1, B200RL_ERR_INVALID, "attach the peer exchange first");
     ctx->comm->tab.exclusive = exclusive ? 1 : 0;
+    return B200RL_OK;
+}
+/* rank and world of the ctx's communicator (0 and 1 without one) */
+int b200rl_comm_rank_world(b200rl_ctx* ctx, int* rank, int* world) {
+    REQUIRE(ctx && rank && world, B200RL_ERR_INVALID, "null argument");
+    *rank = b200rl_comm_rank(ctx);
+    *world = b200rl_comm_world(ctx);
     return B200RL_OK;
 }
 /* in-place sum all-reduce of a DEVICE fp32 buffer on the ctx stream */

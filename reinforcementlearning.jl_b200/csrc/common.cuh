@@ -111,6 +111,8 @@ struct P2PTable {   // nranks == 0: not attached
 };
 bool b200rl_comm_p2p_table(b200rl_ctx* ctx, P2PTable* out);   // false when no peer exchange is attached
 int b200rl_comm_world(b200rl_ctx* ctx);                        // ranks of the communicator (1 without one)
+int b200rl_comm_rank(b200rl_ctx* ctx);                         // this ctx's rank (0 without a communicator)
+bool b200rl_comm_has_nccl(b200rl_ctx* ctx);                    // the communicator has an NCCL communicator (not peer exchange only)
 // device-resident sequence numbers of the peer exchanges {gradient exchange, small all-reduce}: every exchange kernel reads
 // its counter, uses value + 1 and stores it back when it is done — no host-side state, so a captured CUDA graph can be replayed
 unsigned int* b200rl_comm_p2p_seq_dev(b200rl_ctx* ctx);

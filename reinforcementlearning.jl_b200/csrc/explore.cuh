@@ -5,7 +5,8 @@
 //   kind 2       EpsilonSpeedyExplorer(β) (RLFarm epsilon_speedy_explorer.jl:19-53): the same selection with ϵ = exp(-β·step)
 //   kind 3       WeightedSoftmaxExplorer (weighted_softmax_explorer.jl:20-21): sample(rng, Weights(softmax(Q), 1f0))
 //   kind 4       GumbelSoftmaxExplorer (gumbel_softmax_explorer.jl:12-16): argmax(logsoftmax(Q) .- log.(-log.(rand(rng, Float32, n))))
-// q_explore_kernel (b200rl_net_q_explore), the replay driver's staged collect and the fused collect run this code.
+// q_explore_kernel (b200rl_net_q_explore), the replay driver's staged collect and the fused collect run this code; on a sharded
+// ctx they number the columns globally (column_step).
 // Plain C++ once the CUDA qualifiers are defined away, so the CPU suite compiles this file for the host
 // (tests/hostdev/cuda_runtime.h, g++ -ffp-contract=off) and checks it against explorers.py, the oracle and a NumPy restatement.
 #pragma once
@@ -238,6 +239,14 @@ __host__ __device__ __forceinline__ int gumbel_softmax_select(const float* v, in
     for (int o = 0; o < kMaxActions; ++o)
         if (o < na) g[o] = fsub(fsub(d[o], lse), f32_log(-f32_log(xo_f32(st))));    // u = 0: log(0) = -Inf -> g = -Inf
     return greedy::findmax_index(g, na) + 1;
+}
+
+// The explorer step of local column i at plan k of a window that starts at explorer step `step`, for a batch sharded over the
+// ranks of a communicator (DESIGN.md §3): rank r of G owns N columns, numbered globally r·N + i, and every plan! of the whole
+// batch moves the step by G·N — what one BatchExplorer over the G·N columns does.  col0 = r·N, stride = G·N; on one GPU (col0 = 0,
+// stride = N) this is step + k·N + i.
+__host__ __device__ __forceinline__ long long column_step(long long step, long long col0, long long stride, long long k, long long i) {
+    return step + col0 + k * stride + i;
 }
 
 // The column planned at explorer step `step` on Q-values v[0 .. na), 1-based.  EXT = false compiles kinds 0 and 1 only (the

@@ -434,13 +434,15 @@ struct EvalArgs {
     int32_t* lengths;                   // (K, N), may be null
     int32_t* counts;                    // (N), may be null
 };
-// MODE 2: EvalArgs and the explorer of QBasedPolicy; column i at window step k plans at explorer step step0 + k N + i.  (A struct of
-// its own: the MODE 0 / 1 instantiations keep the kernel parameters, and the code, they had before MODE 2 existed.)
+// MODE 2: EvalArgs and the explorer of QBasedPolicy; column i at window step k plans at explorer step
+// explore::column_step(step0, col0, stride, k, i) = step0 + k N + i on one GPU.  (A struct of its own: the MODE 0 / 1
+// instantiations keep the kernel parameters, and the code, they had before MODE 2 existed.)
 struct EvalExploreArgs : EvalArgs {
     int greedy;                         // 1: GreedyExplorer (the first maximum under `>`, no draw)
     QExplorer ex;
     double beta;
     long long step0;
+    long long col0, stride;             // rank · N and world · N (0 and N on one GPU)
 };
 template <int MODE> using EvalArgsOf = typename std::conditional<MODE == 2, EvalExploreArgs, EvalArgs>::type;
 // the window reads and writes back a (4, N) stream per env: the policy streams (MODE 1) or the explorer streams (MODE 2, not greedy)
@@ -503,7 +505,8 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgsOf<MODE> g, 
                     if constexpr (MODE == 0) {
                         a_bits = greedy::greedy_action(g.actor, z);
                     } else if constexpr (MODE == 2) {
-                        a_bits = (uint32_t)plan_q_column<XEXT>(g.greedy, g.ex, g.beta, g.step0 + (long long)step * N + i, z, g.actor.nout, sl.prng, s);
+                        a_bits = (uint32_t)plan_q_column<XEXT>(g.greedy, g.ex, g.beta, explore::column_step(g.step0, g.col0, g.stride, step, i), z, g.actor.nout,
+                                                                sl.prng, s);
                     } else {
                         unsigned long long pr[4];
                         get_stream(sl.prng, s, pr);
@@ -571,6 +574,7 @@ struct ReplayArgs {
     int greedy;                            // 1: GreedyExplorer (findmax with `>`, no draw)
     QExplorer ex;                          // (beta: the kernel's last parameter)
     const long long* step_dev;             // explorer step before the window (device)
+    long long col0, xstride;               // explore::column_step: rank · N and world · N (0 and N on one GPU)
     unsigned long long* xrng;              // (4, N) explorer streams
     Ring ring;
     float default_priority;
@@ -643,7 +647,8 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
                     float z[kOutMax];
                     tile_heads(sm.net, sm.Zp, s, z);
                     if (DUEL) duel::combine(z, g.q.nout);
-                    const int a1 = plan_q_column<XEXT>(g.greedy, g.ex, beta, step0 + (long long)step * N + i, z, g.q.nout, sl.xrng, s);
+                    const int a1 = plan_q_column<XEXT>(g.greedy, g.ex, beta, explore::column_step(step0, g.col0, g.xstride, step, i), z, g.q.nout,
+                                                                sl.xrng, s);
                     const ActStep<float> res = slot_act(sl, s, p, ea.max_timeout, (typename Env::act_t)a1, sm.fin_cnt[s], sm.fin_ret[s], sm.fin_len[s]);
                     // push!(trajectory, (state = s', action = env.action, reward, terminal)) of lane i
                     float nobs[kInMax];
@@ -808,7 +813,7 @@ int nn_tc_evaluate(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const
     const b200rl_explorer e = ex ? *ex : b200rl_explorer{};
     const EvalArgs g{actor, params, hp, v.N, nsteps, K, policy_rng, returns, lengths, counts};
     const EvalExploreArgs gx{g, ex ? 0 : 1, QExplorer{e.eps_stable, e.eps_init, e.warmup_steps, e.decay_steps, e.step, e.kind, e.is_break_tie},
-                             e.beta, (long long)e.step};
+                             e.beta, (long long)e.step, (long long)b200rl_comm_rank(ctx) * v.N, (long long)b200rl_comm_world(ctx) * v.N};
     const int64_t groups = ((v.N + TM - 1) / TM + kSlots - 1) / kSlots;
     const int st = with_f32_env(v, [&](auto env_type, const auto& p) {
         using Env = typename decltype(env_type)::type;
@@ -832,7 +837,8 @@ int nn_tc_replay_collect(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& q, con
     if (!nn_tc_supported(q) || v.dtype != B200RL_F32 || v.continuous || ring.ns > kInMax) return B200RL_ERR_UNSUPPORTED;
     const b200rl_explorer e = ex ? *ex : b200rl_explorer{};
     const ReplayArgs g{q, params, v.N, nsteps, ex ? 0 : 1, QExplorer{e.eps_stable, e.eps_init, e.warmup_steps, e.decay_steps, e.step, e.kind, e.is_break_tie},
-                       step_dev, xrng, ring, default_priority, prioritized, keys, vals, stride};
+                       step_dev, (long long)b200rl_comm_rank(ctx) * v.N, (long long)b200rl_comm_world(ctx) * v.N, xrng, ring,
+                       default_priority, prioritized, keys, vals, stride};
     const int64_t groups = ((v.N + TM - 1) / TM + kSlots - 1) / kSlots;
     const int st = with_f32_env(v, [&](auto env_type, const auto& p) {
         using Env = typename decltype(env_type)::type;

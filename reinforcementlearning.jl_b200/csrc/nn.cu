@@ -786,23 +786,27 @@ __global__ void q_act_kernel(const float* __restrict__ qv, int na, int64_t N, un
 // BatchExplorer(EpsilonGreedyExplorer) over the columns of a (na, N) Q table (explorers/batch_explorer.jl:15-21,
 // epsilon_greedy_explorer.jl:102-112): column i is planned with get_ϵ(step + i) — the inner explorer's step advances once
 // per column — drawing from its own stream (explore.cuh).  step_dev (may be null): the step is read from device memory
-// instead of ex.step, so a captured launch can be replayed.
+// instead of ex.step, so a captured launch can be replayed.  col0: the global number of column 0 (rank · N on a sharded ctx).
 __global__ void q_explore_kernel(const float* __restrict__ qv, int na, int64_t N, unsigned long long* __restrict__ rng, b200rl_explorer ex,
-                                 const long long* __restrict__ step_dev, int32_t* __restrict__ action_out) {
+                                 const long long* __restrict__ step_dev, long long col0, int32_t* __restrict__ action_out) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
     const long long step = step_dev ? *step_dev : ex.step;
     unsigned long long st[4];
     explore::xo_load(rng, i, st);
-    const int action = explore::select(ex, step + i, qv + (int64_t)na * i, na, st);
+    const int action = explore::select(ex, explore::column_step(step, col0, N, 0, i), qv + (int64_t)na * i, na, st);
     explore::xo_store(rng, i, st);
     action_out[i] = action;
 }
 
 template <int H, bool BWD> constexpr size_t smem_bytes() { return sizeof(Smem<H, BWD>); }
 
-template <class K> int set_smem(K kernel, size_t bytes) {
-    CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+// raises `kernel`'s shared-memory limit on its first launch on a device: the attribute call may serialise with the kernels running on
+// the device, and with the ranks of a sharded run sharing one device, one of those may be a peer's exchange waiting for this rank
+template <auto kernel> int set_smem(b200rl_ctx* ctx, size_t bytes) {
+    static unsigned long long attr_devices = 0;
+    if (first_use_on_device(attr_devices, ctx->device))
+        CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     return B200RL_OK;
 }
 
@@ -826,7 +830,7 @@ template <int H>
 static int launch_forward(b200rl_ctx* ctx, int grid, const MlpDesc& actor, const MlpDesc& critic, const float* params, const AcHyper& hp,
                           int mode, const float* obs, int64_t N, unsigned long long* rng, void* action_out, float* logp_out,
                           float* value_out, float* head_out, float* state_copy) {
-    TRY(set_smem(forward_kernel<H>, smem_bytes<H, false>()));
+    TRY((set_smem<forward_kernel<H>>(ctx, smem_bytes<H, false>())));
     forward_kernel<H><<<grid, NT, smem_bytes<H, false>(), ctx->stream>>>(actor, critic, params, hp, mode, obs, N, rng, action_out, logp_out,
                                                                          value_out, head_out, state_copy);
     LAUNCH_CHECK(ctx);
@@ -835,7 +839,7 @@ static int launch_forward(b200rl_ctx* ctx, int grid, const MlpDesc& actor, const
 template <int H>
 static int launch_ac(b200rl_ctx* ctx, int grid, const MlpDesc& actor, const MlpDesc& critic, const float* params, const AcHyper& hp,
                      const AcBatch& b, float* partial, float* loss_partial, int64_t np) {
-    TRY(set_smem(ac_loss_grad_kernel<H>, smem_bytes<H, true>()));
+    TRY((set_smem<ac_loss_grad_kernel<H>>(ctx, smem_bytes<H, true>())));
     ac_loss_grad_kernel<H><<<grid, NT, smem_bytes<H, true>(), ctx->stream>>>(actor, critic, params, hp, b, partial, loss_partial, np);
     LAUNCH_CHECK(ctx);
     return B200RL_OK;
@@ -844,7 +848,7 @@ template <int H, bool DISC>
 static int launch_dqn(b200rl_ctx* ctx, int grid, const MlpDesc& q, const float* params, const float* s, const int32_t* a, const float* r,
                       const uint8_t* t, const float* qt, const float* qo, const float* w, int64_t B, float inv_B, float gamma, int huber,
                       float* partial, float* loss_partial, float* td_out, const float* disc) {
-    TRY(set_smem(dqn_loss_grad_kernel<H, DISC>, smem_bytes<H, true>()));
+    TRY((set_smem<dqn_loss_grad_kernel<H, DISC>>(ctx, smem_bytes<H, true>())));
     dqn_loss_grad_kernel<H, DISC><<<grid, NT, smem_bytes<H, true>(), ctx->stream>>>(q, params, s, a, r, t, qt, qo, w, B, inv_B, gamma, huber,
                                                                                    partial, loss_partial, td_out, disc);
     LAUNCH_CHECK(ctx);
@@ -1001,7 +1005,8 @@ int nn_dqn_max_partials(b200rl_ctx* ctx, int H) { return H == 64 ? 2 * ctx->sm_c
 int nn_q_explore(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float* obs, int64_t N, unsigned long long* rng,
                  const b200rl_explorer& ex, int32_t* action_out, float* q_out, const long long* step_dev) {
     TRY(nn_mlp_forward(ctx, q, params, obs, N, q_out));
-    q_explore_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(q_out, q.nout, N, rng, ex, step_dev, action_out);
+    const long long col0 = (long long)b200rl_comm_rank(ctx) * N;   // BatchExplorer over the union of the ranks' columns
+    q_explore_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(q_out, q.nout, N, rng, ex, step_dev, col0, action_out);
     LAUNCH_CHECK(ctx);
     return B200RL_OK;
 }

@@ -123,7 +123,8 @@ int nn_dqn_loss_grad(b200rl_ctx* ctx, const MlpDesc& q, const float* params, con
                      int double_dqn, float* partial, float* loss_partial, float* td_out, const float* disc);
 int nn_q_act(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float* obs, int64_t N, unsigned long long* rng, float epsilon,
              int32_t* action_out, float* q_out);
-// step_dev (may be null): explorer step read from device memory instead of ex.step
+// step_dev (may be null): explorer step read from device memory instead of ex.step.  On a sharded ctx column i is global column
+// rank · N + i (explore::column_step)
 int nn_q_explore(b200rl_ctx* ctx, const MlpDesc& q, const float* params, const float* obs, int64_t N, unsigned long long* rng,
                  const b200rl_explorer& ex, int32_t* action_out, float* q_out, const long long* step_dev = nullptr);
 

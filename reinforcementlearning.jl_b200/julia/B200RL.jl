@@ -586,7 +586,9 @@ set_step!(s::AbstractExplorer, step) = (s.step[] = step; nothing)      # Epsilon
 `EpsilonGreedyExplorer{kind, is_break_tie}`, `WeightedSoftmaxExplorer()`, `GumbelSoftmaxExplorer()`, ReinforcementLearningFarm's
 `EpsilonSpeedyExplorer(β)` or `GreedyExplorer()`: its fields are read on every `plan!` and its step (if it has one) is advanced
 by `n`, the way `BatchExplorer` calls the inner explorer once per column (batch_explorer.jl:15-21); the forward pass, the
-per-column schedule, the draws and the selection run in one device call.
+per-column schedule, the draws and the selection run in one device call.  On a sharded ctx (rank r of G, `comm_rank_world`) the
+`n` envs are global envs r n + 1 … (r + 1) n: the columns are numbered over all ranks and `plan!`, `replay!` and `evaluate` advance
+the step by G n per plan, as one `BatchExplorer` over the G n envs would.
 """
 mutable struct B200QBasedPolicy{E<:AbstractExplorer} <: AbstractPolicy
     ctx::B200Context
@@ -613,11 +615,17 @@ function B200QBasedPolicy(ctx::B200Context, learner::B200DQNLearner, explorer::A
         ccall((:b200rl_free, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), x.ctx.h, x.d_action)
     end
 end
+"""`(rank, world)` of the ctx's communicator; `(0, 1)` without one (b200rl_comm_rank_world)."""
+function comm_rank_world(ctx::B200Context)
+    r, w = Ref{Cint}(0), Ref{Cint}(1)
+    check(ccall((:b200rl_comm_rank_world, LIB), Cint, (Ptr{Cvoid}, Ref{Cint}, Ref{Cint}), ctx.h, r, w))
+    (Int(r[]), Int(w[]))
+end
 function RLBase.plan!(p::B200QBasedPolicy, env::B200VecEnv)
     ex = ExplorerC(p.explorer)
     check(ccall((:b200rl_net_q_explore, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Ptr{Cvoid}, Ref{ExplorerC}, Ptr{Cvoid}),
                 p.learner.net.h, device_ptr(env, OBS), p.n, p.d_rng, Ref(ex), p.d_action))
-    set_step!(p.explorer, ex.step + p.n)
+    set_step!(p.explorer, ex.step + p.n * comm_rank_world(p.ctx)[2])   # BatchExplorer over every rank's columns (DESIGN.md §3)
     DeviceActions(p.d_action)
 end
 function RLBase.plan!(p::B200QBasedPolicy{GreedyExplorer}, env::B200VecEnv)
@@ -775,7 +783,7 @@ function replay!(a::B200Agent, env::B200VecEnv, n_steps::Integer)
         h = Ref{Ptr{Cvoid}}(C_NULL)
         st = ccall((:b200rl_replay_create, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ref{DQNConfigC}, Ref{Ptr{Cvoid}}),
                    p.ctx.h, p.learner.net.h, env.h, t.h, Ref(p.learner.cfg), h)
-        st in (-1, -3) && return false              # B200RL_ERR_INVALID / _UNSUPPORTED (e.g. a sharded ctx): the stage loop runs it
+        st in (-1, -3) && return false              # B200RL_ERR_INVALID / _UNSUPPORTED (e.g. a sharded ctx without an exchange): the stage loop runs it
         check(st)
         a.replay, a.replay_env = h[], env.h
     end

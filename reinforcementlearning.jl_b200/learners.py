@@ -433,7 +433,11 @@ class QBasedPolicy(AbstractPolicy):
     """QBasedPolicy(learner = DQNLearner(...), explorer = EpsilonGreedyExplorer(...)) (q_based_policy.jl:13-49) on a batched
     env: ``plan`` = BatchExplorer over Q(state(env), .) — forward pass, schedule, draws and arg-max in one device call.
 
-    ``explorer_rng``: (N, 4) uint64 raw Xoshiro states, one explorer stream per env."""
+    ``explorer_rng``: (N, 4) uint64 raw Xoshiro states, one explorer stream per env.
+
+    On a sharded ctx (rank r of G, ``ctx.rank_world()``) the N envs are global envs r N .. r N + N - 1: column i plans at explorer
+    step ``step + r N + i`` and every plan advances the explorer by G N, as one BatchExplorer over the G N envs of all ranks would
+    (DESIGN.md §3).  Every rank's explorer therefore holds the same step."""
 
     def __init__(self, ctx, learner, explorer, explorer_rng, n_envs):
         self.ctx, self.lib, self.learner, self.explorer, self.n = ctx, ctx.lib, learner, explorer, int(n_envs)
@@ -462,7 +466,7 @@ class QBasedPolicy(AbstractPolicy):
         if hasattr(ex, "as_struct"):
             st = ex.as_struct()
             L.check(self.lib.b200rl_net_q_explore(net.h, obs, self.n, C.c_void_p(self._d_rng), C.byref(st), C.c_void_p(self._d_action)))
-            ex.advance(self.n)
+            ex.advance(self.n * self.ctx.rank_world()[1])
         else:   # GreedyExplorer: findmax, no draw
             L.check(self.lib.b200rl_net_q_act(net.h, obs, self.n, None, 0.0, C.c_void_p(self._d_action)))
         return self._d_action
@@ -569,7 +573,7 @@ def evaluate(net, env, n_steps, max_episodes=1, mode="greedy", rng=None):
 
     ``net`` may also be a :class:`QBasedPolicy` (b200rl_evaluate_explore): its Q-network planned by its explorer on its explorer
     streams, exactly as ``run(policy, env, StopAfterNSteps(n_steps))`` would — the streams and the explorer's step advance
-    (``explorer.advance(N * n_steps)``); ``mode`` and ``rng`` do not apply.  To evaluate without touching a training policy, build a
+    (``explorer.advance(N * n_steps)``, ``N * G * n_steps`` on a sharded ctx of G ranks); ``mode`` and ``rng`` do not apply.  To evaluate without touching a training policy, build a
     second QBasedPolicy over the same learner with its own explorer and streams."""
     if isinstance(net, QBasedPolicy):
         return _evaluate_q_based(net, env, n_steps, max_episodes)
@@ -613,7 +617,7 @@ def _evaluate_q_based(policy, env, n_steps, max_episodes):
     L.check(lib.b200rl_evaluate_explore(policy.learner.net.h, env.h, int(n_steps), K, None if st is None else C.byref(st),
                                         C.c_void_p(policy._d_rng), L.ptr(returns), L.ptr(lengths), L.ptr(counts), 0))
     if st is not None:
-        ex.advance(n * int(n_steps))
+        ex.advance(n * policy.ctx.rank_world()[1] * int(n_steps))   # (= st.step - ex.step: BatchExplorer over every rank's columns)
     return dict(returns=returns, lengths=lengths, counts=counts)
 
 
@@ -659,7 +663,8 @@ class Agent(AbstractPolicy):
     # ---- device agent loop ----------------------------------------------------------------------
     def replay_supported(self, env):
         """The env side of the device loop: in-kernel auto-reset, Float32, a discrete action space, <= 4 observations, and
-        the trajectory's controller is an InsertSampleRatioController; the ctx must not be sharded (refused by create)."""
+        the trajectory's controller is an InsertSampleRatioController.  A sharded ctx needs the peer exchange attached or an NCCL
+        communicator (refused by create otherwise)."""
         t, lr = self.trajectory, self.policy.learner
         return (self.fusable and env.auto_reset and env.T is np.float32 and not env.continuous and env.kind != L.ENV_ACROBOT
                 and type(t.controller) is InsertSampleRatioController and t.batch_size > 0 and t.lanes == env.n and t.ns == lr.net.n_in
@@ -674,7 +679,7 @@ class Agent(AbstractPolicy):
         h = C.c_void_p()
         st = pol.lib.b200rl_replay_create(pol.ctx.h, lr.net.h, env.h, self.trajectory.h, C.byref(lr.cfg), C.byref(h))
         if st in (L.ERR_UNSUPPORTED, L.ERR_INVALID):
-            return None            # e.g. a sharded ctx: the stage loop keeps running the agent (and raises its own errors)
+            return None            # e.g. a sharded ctx without an exchange: the stage loop keeps running the agent (and raises its own errors)
         L.check(st)
         self._replay, self._replay_key = h, key
         return h
@@ -682,7 +687,8 @@ class Agent(AbstractPolicy):
     def run_replay(self, env, n_steps, want_stats=False):
         """n_steps x {plan!, act!, push!, optimise!} of the stage protocol on the device (b200rl_replay_run): the same
         transitions, updates, streams and counters.  Returns the last update's {loss, grad_norm, mean_abs_td, n_updates}
-        (want_stats, synchronises) or None."""
+        (want_stats, synchronises) or None.  On a sharded ctx every rank calls it with the same n_steps, controller and explorer
+        (the explorer advances by N * world per step); loss and grad_norm are global, mean_abs_td is the rank's own."""
         pol, c = self.policy, self.trajectory.controller
         h = self._handle(env)
         ex = pol.explorer.as_struct() if type(pol.explorer) in DEVICE_EXPLORERS else None

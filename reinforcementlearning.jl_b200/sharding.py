@@ -2,7 +2,8 @@
 rank r of G owns [r*N/G, (r+1)*N/G); RNG streams are keyed by the GLOBAL env index so a sharded
 run owns exactly the streams the single-GPU run would; gradients are local sums scaled by
 1/(B_local * G) and summed across ranks (one all-reduce per optimiser step); the advantage
-normalisation uses globally reduced sums.  No compute here — index arithmetic only."""
+normalisation uses globally reduced sums.  No compute here — index arithmetic, seeding, and the
+constructor of one rank's DQN agent (dqn_rank_agent)."""
 import numpy as np
 
 
@@ -63,6 +64,35 @@ def glorot_actor_critic(seed, n_in, hidden, n_out):
     parts = dense(hidden, n_in) + dense(hidden, hidden) + dense(n_out, hidden)
     parts += dense(hidden, n_in) + dense(hidden, hidden) + dense(1, hidden)
     return np.concatenate(parts)
+
+
+def dqn_rank_agent(ctx, env_kind, n_total, seed, q_params, hidden, n_out, cfg, explorer, capacity, batch_size, act=0, kind=None,
+                   prioritized=False, n_step=1, ratio=1.0, threshold=1, env_params=None):
+    """One rank's share of a sharded DQN replay run (DESIGN.md §3): ``Agent(QBasedPolicy(DQNLearner, explorer), Trajectory)`` over
+    the global envs [r N, (r + 1) N) of ``n_total`` (rank and world from ``ctx.rank_world()``).
+
+    Env streams are ``splitmix_states(seed, lo, hi)``, explorer streams ``splitmix_states(seed + 1, lo, hi)`` — keyed by the global
+    env index, so the union of the ranks owns exactly the streams of one run over all envs — and the ring's sampler streams
+    ``splitmix_states(seed + 2 + r, 0, batch_size)`` (each rank samples its own batch).  ``q_params`` seeds the Q-network and its
+    target, identical on every rank; ``explorer`` is this rank's copy of the (identical) explorer, its step the global one.  The
+    trajectory holds this rank's N lanes only.  Returns dict(env, net, traj, learner, policy, agent)."""
+    from . import envs, learners
+    rank, world = ctx.rank_world()
+    lo, hi = shard_range(n_total, rank, world)
+    n = hi - lo
+    kw = {} if env_params is None else dict(params=env_params)
+    env = envs.B200VecEnv(ctx, env_kind, n, splitmix_states(seed, lo, hi), auto_reset=True, **kw)
+    n_in = envs._NOBS[env.kind]
+    q_params = np.ascontiguousarray(q_params, np.float32)
+    net = learners.Network(ctx, n_in, hidden, n_out, q_params.copy(), act=act, kind=learners.KIND_Q if kind is None else kind)
+    net.set(learners.NET_TARGET, q_params.copy())   # (the target starts as the parameters on every rank)
+    traj = learners.Trajectory(ctx, n_in, capacity, lanes=n, batch_size=batch_size,
+                               sampler_rng=splitmix_states(seed + 2 + rank, 0, batch_size), prioritized=prioritized,
+                               n_step=n_step, gamma=cfg.gamma)
+    traj.controller = learners.InsertSampleRatioController(ratio=ratio, threshold=threshold)
+    learner = learners.DQNLearner(ctx, net, traj, cfg)
+    policy = learners.QBasedPolicy(ctx, learner, explorer, splitmix_states(seed + 1, lo, hi), n)
+    return dict(env=env, net=net, traj=traj, learner=learner, policy=policy, agent=learners.Agent(policy, traj))
 
 
 def attach_peer_exchange(ctx, rank, world, all_gather_bytes):
