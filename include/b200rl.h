@@ -97,7 +97,11 @@ typedef enum {
     B200RL_FIELD_FLAGS = 6,     /* (N,) uint8     bit0 terminal, bit1 already auto-reset         */
     B200RL_FIELD_ACTION = 7,    /* (N,) int32 | T last action                                    */
     B200RL_FIELD_EPISODE_RETURN = 8,  /* (N,) float32  running return of the episode in progress (device-side hooks)  */
-    B200RL_FIELD_EPISODE_STATS = 9    /* (4,) float64  the counters b200rl_env_episode_stats reads (checkpoints)      */
+    B200RL_FIELD_EPISODE_STATS = 9,   /* (4,) float64  the counters b200rl_env_episode_stats reads (checkpoints)      */
+    B200RL_FIELD_OBS_F32 = 10         /* (NOBS, N) float32  Float32.(state(env)), round to nearest (what the learners read):
+                                         FIELD_OBS itself for a Float32 env, a mirror kept by every env kernel for a Float64
+                                         one wrapped by b200rl_env_set_state_f32 (unknown field without the wrapper);
+                                         read-only, it follows env_set of STATE / OBS */
 } b200rl_field;
 
 /* Final field values of the reference's params structs (already rounded to T by the
@@ -129,7 +133,8 @@ typedef struct {   /* AcrobotEnvParams{T} + book_or_nips: 3rd_party/AcrobotEnv.j
  * env (Julia side: `Xoshiro(seed_i)` fields s0..s3).  Like the reference constructors it
  * performs one reset!() per env.  Supported: CartPole f32|f64 discrete, f32 continuous; Pendulum f32|f64
  * continuous|discrete; MountainCar f32|f64 discrete|continuous (T = Float64 is the reference constructors' default,
- * PendulumEnv.jl:42, MountainCarEnv.jl:67; the learners / trajectory take Float32 envs). */
+ * PendulumEnv.jl:42, MountainCarEnv.jl:67; the learners / trajectory take Float32 envs and Float64 envs wrapped by
+ * b200rl_env_set_state_f32). */
 int b200rl_env_create(b200rl_ctx* ctx, int kind, int dtype, int64_t n_envs, const void* params,
                       const uint64_t* rng_state, b200rl_env** out);
 int b200rl_env_destroy(b200rl_env* env);
@@ -137,6 +142,13 @@ int b200rl_env_destroy(b200rl_env* env);
  * also when the wrapper's current_t (= env.t + 1) exceeds max_t; reward(env) still forwards to the wrapped
  * env.  max_t = 0 removes the wrapper. */
 int b200rl_env_set_max_timeout(b200rl_env* env, int64_t max_t);
+/* StateTransformedEnv(env; state_mapping = s -> Float32.(s)) (RLEnvs/src/environments/wrappers/StateTransformedEnv.jl:15-19):
+ * on != 0 lets the learners, the trajectory push and the evaluation take a Float64 env.  The dynamics are untouched (state, RNG
+ * streams, t, flags, rewards, episode statistics and FIELD_OBS stay bit for bit the unwrapped env's); the networks read
+ * FIELD_OBS_F32, rewards enter a rollout or replay ring as Float32(reward), and a continuous Float32 action reaches the env as
+ * Float64(clamp(a, lo, hi)).  On a Float32 env it is the identity (accepted, changes nothing); on Acrobot B200RL_ERR_UNSUPPORTED.
+ * on = 0 removes the wrapper. */
+int b200rl_env_set_state_f32(b200rl_env* env, int on);
 /* Base.copy(env) (RLBase/src/interface.jl:443): deep copy incl. RNG streams */
 int b200rl_env_copy(b200rl_env* env, b200rl_env** out);
 /* Random.seed!(env, seed) (CartPoleEnv.jl:83): replace the raw RNG states */
@@ -229,7 +241,8 @@ int b200rl_traj_push_episode_start(b200rl_traj* traj, const float* obs, int on_d
  * written by the same call. */
 int b200rl_traj_push(b200rl_traj* traj, const int32_t* action, const float* reward, const uint8_t* terminal, const float* next_obs,
                      int on_device);
-/* the same, reading the env's device fields directly (no host round trip) */
+/* the same, reading the env's device fields directly (no host round trip).  A Float64 env wrapped by b200rl_env_set_state_f32 is
+ * accepted: FIELD_OBS_F32 and Float32(reward) are pushed. */
 int b200rl_traj_push_env(b200rl_traj* traj, b200rl_env* env, int first_state_only);
 /* checkpoint of the ring: field 0 state (ns, lanes, cap+1) f32 | 1 action i32 | 2 reward f32 | 3 flag u8 (bit0 terminal, bit1
  * sampleable) | 4 head (lanes) i32 | 5 count (lanes) i32 | 6 pending (lanes) u8 | 7 n_sampleable i64 | 8 sum tree (2L) f32 |
@@ -335,7 +348,8 @@ int b200rl_net_act_greedy(b200rl_net* net, const float* obs, int64_t n, void* ac
  *       Float32 sum of their rewards in step order and env.t at termination; slots no episode reaches are left untouched
  *   counts (N) i32                         : episodes each env finished in the window (may exceed K)
  * The env ends where the stage protocol leaves it (every field, its streams and episode statistics); the network and every
- * other handle are only read.  Float32 envs with <= 4 observations.  on_device = 0: host outputs (synchronises), 1: device
+ * other handle are only read.  Float32 envs with <= 4 observations, or Float64 ones wrapped by b200rl_env_set_state_f32 (the
+ * network reads FIELD_OBS_F32; a record is the Float32 sum of Float32(reward), as the env's EPISODE_RETURN).  on_device = 0: host outputs (synchronises), 1: device
  * outputs (asynchronous on the ctx stream). */
 typedef struct { int32_t mode, n_steps, max_episodes; } b200rl_eval_config;   /* mode 0 greedy, 1 sample */
 int b200rl_evaluate(b200rl_net* net, b200rl_env* env, const b200rl_eval_config* cfg, uint64_t* policy_rng_dev,
@@ -346,7 +360,7 @@ int b200rl_evaluate(b200rl_net* net, b200rl_env* env, const b200rl_eval_config* 
  * GreedyExplorer (the first maximum under `>`, b200rl_net_q_act with epsilon = 0; no draw, no streams needed).  Outputs, env side
  * effects and on_device as b200rl_evaluate; the (4, N) DEVICE explorer streams are advanced in place and, on success, ex->step by
  * N n_steps (as b200rl_replay_run).  The network (its update counter and target too) is only read.  Refused before any side effect:
- * B200RL_ERR_UNSUPPORTED for Float64, Acrobot and continuous-action envs; B200RL_ERR_INVALID for a network that is not a Q-network,
+ * B200RL_ERR_UNSUPPORTED for Float64 envs without b200rl_env_set_state_f32, Acrobot and continuous-action envs; B200RL_ERR_INVALID for a network that is not a Q-network,
  * an input / head width that does not match the env, n_steps < 1, max_episodes < 0, an explorer without streams and a bad explorer
  * (see b200rl_explorer).  One fused launch for hidden = 64 on the tensor-core path.  On a sharded ctx the columns are numbered
  * over the ranks' union as in b200rl_net_q_explore: column i of rank r at window step k plans at ex->step + k world N + r N + i,
@@ -371,7 +385,9 @@ typedef struct b200rl_onpolicy b200rl_onpolicy;
 int b200rl_net_ac_step(b200rl_net* net, const b200rl_onpolicy_config* cfg, const float* states, const void* actions,
                        const float* logp_old, const float* adv, const float* ret, int64_t total, const int32_t* idx, int64_t batch,
                        float adv_mean, float adv_inv_std, int apply_update, float* losses_out);
-/* Agent(PPOPolicy | A2CPolicy, PPOTrajectory): rollout tensors (N, T) on the device */
+/* Agent(PPOPolicy | A2CPolicy, PPOTrajectory): rollout tensors (N, T) on the device.  A Float64 env wrapped by
+ * b200rl_env_set_state_f32 is accepted: the rollout states are FIELD_OBS_F32, its rewards Float32(reward), and a continuous
+ * action reaches the env as Float64(clamp(a, lo, hi)) while the rollout keeps the unclamped Float32 sample. */
 int b200rl_onpolicy_create(b200rl_ctx* ctx, b200rl_net* net, b200rl_env* env, const b200rl_onpolicy_config* cfg,
                            const uint64_t* policy_rng, b200rl_onpolicy** out);
 int b200rl_onpolicy_destroy(b200rl_onpolicy* agent);
@@ -456,6 +472,9 @@ typedef struct b200rl_replay b200rl_replay;
  *      rank refuses the run for a reason of its own — every rank returns B200RL_ERR_INVALID with nothing else touched.
  * The update units are replayed as CUDA graphs when the peer exchange is attached and every rank owns its device
  * (b200rl_comm_p2p_set_exclusive); with NCCL only, or ranks sharing a device, they launch eagerly. */
+/* A Float64 env wrapped by b200rl_env_set_state_f32 is accepted (the ring stores FIELD_OBS_F32 and Float32(reward)); whether the
+ * wrapper is in effect (a wrapped Float64 env; on a Float32 env it changes nothing) takes part in the graph key and, on a sharded
+ * ctx, in the agreement of point 6. */
 int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl_traj* traj, const b200rl_dqn_config* cfg,
                          b200rl_replay** out);
 /* explorer_rng_dev: (4, N) DEVICE explorer streams (one per env, advanced).  ex: any b200rl_explorer kind (its step is advanced

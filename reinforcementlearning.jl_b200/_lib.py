@@ -17,6 +17,7 @@ ERR_INVALID, ERR_CUDA, ERR_UNSUPPORTED, ERR_ACTION, ERR_NCCL, ERR_OOM = -1, -2, 
 ENV_CARTPOLE, ENV_PENDULUM, ENV_MOUNTAINCAR, ENV_CARTPOLE_CONTINUOUS, ENV_MOUNTAINCAR_CONTINUOUS, ENV_ACROBOT = 0, 1, 2, 3, 4, 5
 F32, F64 = 0, 1
 FIELD_STATE, FIELD_OBS, FIELD_REWARD, FIELD_TERMINAL, FIELD_T, FIELD_RNG, FIELD_FLAGS, FIELD_ACTION, FIELD_EPISODE_RETURN, FIELD_EPISODE_STATS = range(10)
+FIELD_OBS_F32 = 10
 
 
 class B200RLError(RuntimeError):
@@ -106,6 +107,7 @@ SIGNATURES = {
     "b200rl_env_create": (_i32, [_vp, _i32, _i32, _i64, _vp, _vp, _pp]),
     "b200rl_env_destroy": (_i32, [_vp]),
     "b200rl_env_set_max_timeout": (_i32, [_vp, _i64]),
+    "b200rl_env_set_state_f32": (_i32, [_vp, _i32]),
     "b200rl_env_copy": (_i32, [_vp, _pp]),
     "b200rl_env_seed": (_i32, [_vp, _vp]),
     "b200rl_env_reset": (_i32, [_vp, _i32]),

@@ -18,11 +18,21 @@
 #include "ring.cuh"
 
 static void* env_field(b200rl_env* e, int f) { void* p = nullptr; b200rl_env_ptr(e, f, &p); return p; }
+// the observation the networks read; refuses a Float64 env that is not wrapped by b200rl_env_set_state_f32 (and Acrobot)
+static int learner_obs(b200rl_env* e, const float** obs) {
+    *obs = b200rl_env_internal_obs_f32(e);
+    REQUIRE(*obs, B200RL_ERR_UNSUPPORTED,
+            "the networks read Float32 observations: construct the env with T = Float32 or wrap it in StateTransformedEnv(env, Float32) "
+            "(b200rl_env_set_state_f32)");
+    return B200RL_OK;
+}
 
 namespace {
-__global__ void clamp_copy_kernel(float* __restrict__ dst, const float* __restrict__ src, int64_t n, float lo, float hi) {
+// D = double: the action a Float64 env receives, Float64(clamp(a, lo, hi))
+template <class D>
+__global__ void clamp_copy_kernel(D* __restrict__ dst, const float* __restrict__ src, int64_t n, float lo, float hi) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) dst[i] = fminf(fmaxf(src[i], lo), hi);
+    if (i < n) dst[i] = (D)fminf(fmaxf(src[i], lo), hi);
 }
 // plan!(greedy policy) on the (nout, N) head outputs: raw action bits (greedy.cuh); clamp != 0: a continuous action is
 // handed to the env as clamp(mu, lo, hi)
@@ -111,6 +121,18 @@ __global__ void finalize_norm2_kernel(const double* __restrict__ sums2, double c
     }
 }
 }  // namespace
+
+// a continuous action as the env receives it: clamp(a, lo, hi) of its action space, in the env's T (dst holds N of them)
+static int env_action_clamped(b200rl_env* env, const float* a, int64_t N, void* dst) {
+    b200rl_ctx* ctx = b200rl_env_internal_ctx(env);
+    const float bound = b200rl_env_internal_action_bound(env);
+    if (b200rl_env_internal_dtype(env) == B200RL_F64)
+        clamp_copy_kernel<double><<<grid_for(N, 256), 256, 0, ctx->stream>>>((double*)dst, a, N, -bound, bound);
+    else
+        clamp_copy_kernel<float><<<grid_for(N, 256), 256, 0, ctx->stream>>>((float*)dst, a, N, -bound, bound);
+    LAUNCH_CHECK(ctx);
+    return B200RL_OK;
+}
 
 // ------------------------------------------------------------------ network handle ---------
 struct b200rl_net {
@@ -266,7 +288,7 @@ struct EvalBufs {
     float* acc_ret;
     int32_t* acc_len;
     uint32_t* act;
-    float* act_clamped;
+    void* act_clamped;            // (N) T: the clamped continuous action the env receives
     float* heads;                 // (nout, N)
 };
 
@@ -287,7 +309,7 @@ static int eval_window(b200rl_ctx* ctx, b200rl_env* env, int nout, int nsteps, i
     const size_t o_len = off; off += on_device ? 0 : round256(rec_bytes);
     const size_t o_cnt = off; off += round256((size_t)N * 4);
     const size_t o_acc = off; off += round256((size_t)N * 4) * 2;
-    const size_t o_act = off; off += round256((size_t)N * 4) * 2;
+    const size_t o_act = off; off += round256((size_t)N * 4) + round256((size_t)N * 8);
     const size_t o_heads = off; off += round256((size_t)N * nout * 4);
     void* sc;
     TRY(ctx_scratch(ctx, off, &sc));
@@ -299,7 +321,7 @@ static int eval_window(b200rl_ctx* ctx, b200rl_env* env, int nout, int nsteps, i
     b.acc_ret = (float*)(base + o_acc);
     b.acc_len = (int32_t*)(base + o_acc + round256((size_t)N * 4));
     b.act = (uint32_t*)(base + o_act);
-    b.act_clamped = (float*)(base + o_act + round256((size_t)N * 4));
+    b.act_clamped = base + o_act + round256((size_t)N * 4);
     b.heads = (float*)(base + o_heads);
     if (!on_device) {   // record slots the window does not fill keep the caller's values
         if (b.ret && rec_bytes) CUDA_TRY(cudaMemcpyAsync(b.ret, returns_out, rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
@@ -310,12 +332,13 @@ static int eval_window(b200rl_ctx* ctx, b200rl_env* env, int nout, int nsteps, i
     if (st == B200RL_ERR_UNSUPPORTED) {   // staged: plan! -> act! (auto-reset) -> record, n_steps times, no host sync
         CUDA_TRY(cudaMemsetAsync(b.cnt, 0, (size_t)N * 4, ctx->stream));
         CUDA_TRY(cudaMemsetAsync(b.acc_ret, 0, round256((size_t)N * 4) * 2, ctx->stream));
-        const float* rew = (const float*)env_field(env, B200RL_FIELD_REWARD);
         const uint8_t* flags = (const uint8_t*)env_field(env, B200RL_FIELD_FLAGS);
         for (int k = 0; k < nsteps; ++k) {
             const void* a_env = b.act;
             TRY(plan(k, b, &a_env));
             TRY(b200rl_env_step(env, a_env, 1, 1));
+            const float* rew;   // (a Float64 env: Float32(reward), as its EPISODE_RETURN adds it)
+            TRY(b200rl_env_internal_reward_f32(env, &rew));
             eval_record_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(rew, flags, N, K, b.acc_ret, b.acc_len, b.cnt, b.ret, b.len);
             LAUNCH_CHECK(ctx);
         }
@@ -599,7 +622,8 @@ int b200rl_evaluate(b200rl_net* n, b200rl_env* env, const b200rl_eval_config* cf
                     int32_t* lengths_out, int32_t* counts_out, int on_device) {
     REQUIRE(n && env && cfg, B200RL_ERR_INVALID, "null argument");
     REQUIRE(b200rl_env_internal_ctx(env) == n->ctx, B200RL_ERR_INVALID, "net/env belong to another ctx");
-    REQUIRE(b200rl_env_internal_dtype(env) == B200RL_F32, B200RL_ERR_UNSUPPORTED, "the networks read Float32 observations: construct the env with T = Float32");
+    const float* obs;
+    TRY(learner_obs(env, &obs));
     REQUIRE(b200rl_env_internal_kind(env) != B200RL_ENV_ACROBOT, B200RL_ERR_UNSUPPORTED, "AcrobotEnv has 6 observations (networks take at most 4)");
     REQUIRE(cfg->mode == 0 || cfg->mode == 1, B200RL_ERR_INVALID, "mode must be 0 (greedy) or 1 (sample)");
     REQUIRE(!(cfg->mode == 1 && is_q_kind(n->kind)), B200RL_ERR_UNSUPPORTED, "mode 1 samples a policy head: evaluate a Q-network with mode 0 or QBasedPolicy");
@@ -616,8 +640,8 @@ int b200rl_evaluate(b200rl_net* n, b200rl_env* env, const b200rl_eval_config* cf
     const int K = cfg->max_episodes, mode = cfg->mode, nsteps = cfg->n_steps;
     const AcHyper& hp = kSamplerHyper;
     unsigned long long* prng = (unsigned long long*)policy_rng_dev;
-    const float* obs = (const float*)env_field(env, B200RL_FIELD_OBS);
     const float bound = b200rl_env_internal_action_bound(env);
+    const bool f64 = b200rl_env_internal_dtype(env) == B200RL_F64;
     return eval_window(
         ctx, env, n->actor.nout, nsteps, K, returns_out, lengths_out, counts_out, on_device,
         [&](const EvalBufs& b) -> int { return nn_tc_evaluate(ctx, env, n->actor, n->params, hp, mode, nsteps, K, prng, b.ret, b.len, b.cnt); },
@@ -626,11 +650,14 @@ int b200rl_evaluate(b200rl_net* n, b200rl_env* env, const b200rl_eval_config* cf
                 TRY(nn_mlp_forward(ctx, n->actor, n->params, obs, N, b.heads));
                 greedy_select_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(b.heads, n->actor, N, cont ? 1 : 0, -bound, bound, b.act);
                 LAUNCH_CHECK(ctx);
+                if (cont && f64) {   // Float64 of the clamped mu
+                    TRY(env_action_clamped(env, (const float*)b.act, N, b.act_clamped));
+                    *a_env = b.act_clamped;
+                }
             } else {
                 TRY(nn_policy_act(ctx, n->actor, n->critic, n->params, hp, obs, N, prng, b.act, nullptr, nullptr, nullptr, nullptr));
                 if (cont) {
-                    clamp_copy_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(b.act_clamped, (const float*)b.act, N, -bound, bound);
-                    LAUNCH_CHECK(ctx);
+                    TRY(env_action_clamped(env, (const float*)b.act, N, b.act_clamped));
                     *a_env = b.act_clamped;
                 }
             }
@@ -644,7 +671,8 @@ int b200rl_evaluate_explore(b200rl_net* n, b200rl_env* env, int32_t n_steps, int
                             uint64_t* explorer_rng_dev, float* returns_out, int32_t* lengths_out, int32_t* counts_out, int on_device) {
     REQUIRE(n && env, B200RL_ERR_INVALID, "null argument");
     REQUIRE(b200rl_env_internal_ctx(env) == n->ctx, B200RL_ERR_INVALID, "net/env belong to another ctx");
-    REQUIRE(b200rl_env_internal_dtype(env) == B200RL_F32, B200RL_ERR_UNSUPPORTED, "the Q-network reads Float32 observations: construct the env with T = Float32");
+    const float* obs;
+    TRY(learner_obs(env, &obs));
     REQUIRE(b200rl_env_internal_kind(env) != B200RL_ENV_ACROBOT, B200RL_ERR_UNSUPPORTED, "AcrobotEnv has 6 observations (networks take at most 4)");
     REQUIRE(!b200rl_env_internal_continuous(env), B200RL_ERR_UNSUPPORTED, "QBasedPolicy needs a discrete action space");
     REQUIRE(is_q_kind(n->kind), B200RL_ERR_INVALID, "needs a Q-network (kind 2 or 3)");
@@ -662,7 +690,6 @@ int b200rl_evaluate_explore(b200rl_net* n, b200rl_env* env, int32_t n_steps, int
     TRY(ctx_bind(n->ctx));
     b200rl_ctx* ctx = n->ctx;
     unsigned long long* xrng = (unsigned long long*)explorer_rng_dev;
-    const float* obs = (const float*)env_field(env, B200RL_FIELD_OBS);
     TRY(eval_window(
         ctx, env, n->actor.nout, n_steps, max_episodes, returns_out, lengths_out, counts_out, on_device,
         [&](const EvalBufs& b) -> int {
@@ -746,7 +773,7 @@ struct b200rl_onpolicy {
     bool bootstrap_done;   // column T of states / values already written by the fused rollout
     unsigned long long* rng;
     float* states; void* actions; float* logp; float* rewards; uint8_t* terminals; float* values; float* adv; float* ret;
-    float* act_clamped;
+    void* act_clamped;           // (N) T: the clamped continuous action the env receives
     double* norm_partials; double* norm_sums; float* norm2;
     int32_t* perm_dev;
     float* stats_dev; int stats_rows;
@@ -808,7 +835,8 @@ int b200rl_onpolicy_create(b200rl_ctx* ctx, b200rl_net* net, b200rl_env* env, co
     REQUIRE(net && env && cfg && policy_rng && out, B200RL_ERR_INVALID, "null argument");
     REQUIRE(!is_q_kind(net->kind), B200RL_ERR_INVALID, "needs an actor-critic network");
     REQUIRE(net->ctx == ctx && b200rl_env_internal_ctx(env) == ctx, B200RL_ERR_INVALID, "net/env belong to another ctx");
-    REQUIRE(b200rl_env_internal_dtype(env) == B200RL_F32, B200RL_ERR_UNSUPPORTED, "the learners read Float32 observations: construct the env with T = Float32");
+    const float* obs;
+    TRY(learner_obs(env, &obs));
     REQUIRE(cfg->update_freq >= 1 && cfg->n_epochs >= 1 && cfg->n_microbatches >= 1, B200RL_ERR_INVALID, "bad config");
     int nobs = b200rl_env_internal_nobs(env);
     REQUIRE(nobs == net->actor.in, B200RL_ERR_INVALID, "network input width != observation width");
@@ -826,7 +854,7 @@ int b200rl_onpolicy_create(b200rl_ctx* ctx, b200rl_net* net, b200rl_env* env, co
     A_TRY(cudaMalloc(&a->actions, NT_ * 4)); A_TRY(cudaMalloc(&a->logp, NT_ * 4)); A_TRY(cudaMalloc(&a->rewards, NT_ * 4));
     A_TRY(cudaMalloc(&a->terminals, NT_)); A_TRY(cudaMalloc(&a->values, (size_t)N * (a->T + 1) * 4));
     A_TRY(cudaMalloc(&a->adv, NT_ * 4)); A_TRY(cudaMalloc(&a->ret, NT_ * 4));
-    A_TRY(cudaMalloc(&a->act_clamped, (size_t)N * 4));
+    A_TRY(cudaMalloc(&a->act_clamped, (size_t)N * 8));   // (N) T
     A_TRY(cudaMalloc(&a->norm_partials, (size_t)b200rl_gae_fused_partials_count(N) * sizeof(double)));
     A_TRY(cudaMalloc(&a->norm_sums, 2 * sizeof(double))); A_TRY(cudaMalloc(&a->norm2, 2 * sizeof(float)));
     a->stats_rows = cfg->n_epochs * cfg->n_microbatches;
@@ -855,7 +883,8 @@ int b200rl_onpolicy_plan(b200rl_onpolicy* a, void* actions_host) {
     TRY(ctx_bind(a->ctx));
     a->bootstrap_done = false;
     int64_t N = a->N;
-    const float* obs = (const float*)env_field(a->env, B200RL_FIELD_OBS);
+    const float* obs;
+    TRY(learner_obs(a->env, &obs));
     char* act_col = (char*)a->actions + (size_t)N * a->t * 4;
     TRY(nn_policy_act(a->ctx, a->net->actor, a->net->critic, a->net->params, ac_hyper(a->cfg), obs, N, a->rng, act_col, a->logp + (size_t)N * a->t,
                       a->values + (size_t)N * a->t, nullptr, a->states + (size_t)N * a->ns * a->t));
@@ -872,9 +901,7 @@ int b200rl_onpolicy_act(b200rl_onpolicy* a) {
     TRY(ctx_bind(a->ctx));
     char* act_col = (char*)a->actions + (size_t)a->N * a->t * 4;
     if (a->continuous) {  // the env asserts a in its action space; the stored (unclamped) action keeps its log-prob
-        const float bound = b200rl_env_internal_action_bound(a->env);
-        clamp_copy_kernel<<<grid_for(a->N, 256), 256, 0, a->ctx->stream>>>(a->act_clamped, (const float*)act_col, a->N, -bound, bound);
-        LAUNCH_CHECK(a->ctx);
+        TRY(env_action_clamped(a->env, (const float*)act_col, a->N, a->act_clamped));
         return b200rl_env_step(a->env, a->act_clamped, 1, 1);
     }
     return b200rl_env_step(a->env, act_col, 1, 1);
@@ -892,6 +919,8 @@ int b200rl_onpolicy_collect(b200rl_onpolicy* a, int n_steps) {
     REQUIRE(a && n_steps >= 0, B200RL_ERR_INVALID, "bad argument");
     if (n_steps > 0 && nn_tc_enabled()) {   // one launch for the whole stretch (fwd_tc.cu)
         REQUIRE(a->t + n_steps <= a->T, B200RL_ERR_INVALID, "rollout is full: call b200rl_onpolicy_update first");
+        const float* obs;
+        TRY(learner_obs(a->env, &obs));   // (the wrapper may have been removed since create)
         TRY(ctx_bind(a->ctx));
         const int fin = a->t + n_steps == a->T ? 1 : 0;
         int st = nn_tc_rollout(a->ctx, a->env, a->net->actor, a->net->critic, a->net->params, ac_hyper(a->cfg), a->rng, a->t, n_steps, a->T, fin, a->states,
@@ -938,7 +967,8 @@ int b200rl_onpolicy_update(b200rl_onpolicy* a, const int32_t* perm_host, float* 
     auto phase = [&](int k) -> int { return pb >= 0 ? b200rl_timer_record(ctx, pb + k) : B200RL_OK; };
     TRY(phase(0));
     // bootstrap value of the state after the last step
-    const float* obs = (const float*)env_field(a->env, B200RL_FIELD_OBS);
+    const float* obs;
+    TRY(learner_obs(a->env, &obs));
     // (a copy kernel, not cudaMemcpyAsync D2D: device-to-device copies are on CUDA's implicit-synchronisation list)
     if (!a->bootstrap_done) {   // (the fused rollout has already written column T of states / values)
         copy_f32_kernel<<<grid_for(N * a->ns, 256), 256, 0, ctx->stream>>>(a->states + (size_t)N * a->ns * T, obs, N * a->ns);
@@ -1018,11 +1048,14 @@ int b200rl_onpolicy_update(b200rl_onpolicy* a, const int32_t* perm_host, float* 
 int b200rl_onpolicy_iterate(b200rl_onpolicy* a, int n_iters, float* stats_host) {
     REQUIRE(a && n_iters >= 0, B200RL_ERR_INVALID, "bad argument");
     REQUIRE(a->t == 0, B200RL_ERR_INVALID, "iterate needs an empty rollout (t = 0)");
+    const float* obs;
+    TRY(learner_obs(a->env, &obs));
     TRY(ctx_bind(a->ctx));
     b200rl_ctx* ctx = a->ctx;
     P2PTable peers;
     const bool capturable = b200rl_comm_world(ctx) == 1 || b200rl_comm_p2p_table(ctx, &peers);
-    const int key[2] = {nn_tc_enabled() ? 1 : 0, b200rl_env_internal_max_timeout(a->env)};   // launch arguments the graph bakes in
+    // launch arguments the graph bakes in
+    const int key[3] = {nn_tc_enabled() ? 1 : 0, b200rl_env_internal_max_timeout(a->env), b200rl_env_internal_state_f32(a->env) ? 1 : 0};
     a->graph.rekey(key, sizeof key);
     const CounterSet counters{ctx, a->net, a->env, nullptr, &a->n_updates};
     for (int it = 0; it < n_iters; ++it) {
@@ -1098,7 +1131,8 @@ int b200rl_onpolicy_time_kernel(b200rl_onpolicy* a, int which, int reps, float* 
     const b200rl_onpolicy_config& c = a->cfg;
     int64_t N = a->N, T = a->T, NT_ = N * T, B = NT_ / c.n_microbatches;
     const AcHyper hp = ac_hyper(c);
-    const float* obs = (const float*)env_field(a->env, B200RL_FIELD_OBS);
+    const float* obs;
+    TRY(learner_obs(a->env, &obs));
     int ctas = (nn_tc_enabled() && nn_tc_bwd_supported(n->actor, n->critic)) ? nn_tc_partial_rows(2 * (ctx->sm_count / 2), n->actor, hp, B) : nn_grid_ctas(ctx, n->actor.H);
     void* rng_copy = nullptr;
     if (which == 1) {
@@ -1147,12 +1181,13 @@ int b200rl_onpolicy_time_kernel(b200rl_onpolicy* a, int which, int reps, float* 
 int b200rl_traj_push_env(b200rl_traj* t, b200rl_env* env, int first_state_only) {
     REQUIRE(t && env, B200RL_ERR_INVALID, "null argument");
     REQUIRE(b200rl_traj_internal_lanes(t) == b200rl_env_internal_n(env), B200RL_ERR_INVALID, "trajectory lanes != number of envs");
-    REQUIRE(b200rl_env_internal_dtype(env) == B200RL_F32, B200RL_ERR_UNSUPPORTED, "the trajectory stores Float32 states: construct the env with T = Float32");
-    const float* obs = (const float*)env_field(env, B200RL_FIELD_OBS);
+    const float* obs;   // (the trajectory stores Float32 states)
+    TRY(learner_obs(env, &obs));
     if (first_state_only == 2) return b200rl_traj_push_episode_start(t, obs, 1, 1);   // only the lanes whose episode has ended (soft reset)
     if (first_state_only) return b200rl_traj_push_state(t, obs, 1);
-    return b200rl_traj_push(t, (const int32_t*)env_field(env, B200RL_FIELD_ACTION), (const float*)env_field(env, B200RL_FIELD_REWARD),
-                            (const uint8_t*)env_field(env, B200RL_FIELD_FLAGS), obs, 1);
+    const float* rew;
+    TRY(b200rl_env_internal_reward_f32(env, &rew));
+    return b200rl_traj_push(t, (const int32_t*)env_field(env, B200RL_FIELD_ACTION), rew, (const uint8_t*)env_field(env, B200RL_FIELD_FLAGS), obs, 1);
 }
 
 /* optimise!(DQNLearner / PrioritizedDQNLearner, batch): sample + gather (K4), TD loss + backward
@@ -1240,10 +1275,10 @@ namespace {
 __global__ void add_i64_kernel(long long* __restrict__ v, long long d) { *v += d; }
 }  // namespace
 
-constexpr int kAgree = 20;   // values of the agreement exchange of a sharded run (replay_agree)
+constexpr int kAgree = 21;   // values of the agreement exchange of a sharded run (replay_agree)
 // what the captured launches bake in besides the handles: a change means re-capture
 struct ReplayKey {
-    int tc, max_timeout, greedy, pad;
+    int tc, max_timeout, greedy, state_f32;
     int nstep_n; float nstep_gamma;  // the sampler's n-step setting (picks the sample kernel and its window arguments)
     b200rl_explorer ex;          // step zeroed (it lives in device memory)
     const void* rng;
@@ -1272,7 +1307,8 @@ struct b200rl_replay {
 static int replay_collect_step(b200rl_replay* r, uint64_t* rng, const b200rl_explorer* ex) {
     b200rl_ctx* ctx = r->ctx;
     b200rl_net* n = r->net;
-    const float* obs = (const float*)env_field(r->env, B200RL_FIELD_OBS);
+    const float* obs;
+    TRY(learner_obs(r->env, &obs));
     void* s;
     TRY(ctx_scratch(ctx, (size_t)r->N * n->actor.nout * 4 + 256, &s));
     if (ex) {
@@ -1348,7 +1384,7 @@ static int replay_agree(b200rl_replay* r, const b200rl_explorer* ex, const b200r
                                 f64_bits(ctl->ratio), (uint64_t)ctl->threshold, (uint64_t)ctl->n_inserted, (uint64_t)ctl->n_sampled,
                                 ex ? 1ull : 0ull, (uint64_t)e.kind, f64_bits(e.eps_stable), f64_bits(e.eps_init), (uint64_t)e.warmup_steps,
                                 (uint64_t)e.decay_steps, (uint64_t)e.step, (uint64_t)e.is_break_tie, f64_bits(e.beta), cfg_digest,
-                                (uint64_t)ns, (uint64_t)f64_bits((double)ng)};
+                                (uint64_t)ns, (uint64_t)f64_bits((double)ng), b200rl_env_internal_state_f32(r->env) ? 1ull : 0ull};
     const int W = 2 * kAgree;
     std::vector<double> tab((size_t)world * W, 0.0);
     for (int j = 0; j < kAgree; ++j) {
@@ -1388,7 +1424,8 @@ int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl
     REQUIRE(is_q_kind(q->kind), B200RL_ERR_INVALID, "needs a Q-network (kind 2 or 3)");
     REQUIRE(q->ctx == ctx && b200rl_env_internal_ctx(env) == ctx && b200rl_traj_internal_ctx(traj) == ctx, B200RL_ERR_INVALID,
             "net/env/trajectory belong to another ctx");
-    REQUIRE(b200rl_env_internal_dtype(env) == B200RL_F32, B200RL_ERR_UNSUPPORTED, "the Q-network reads Float32 observations: construct the env with T = Float32");
+    const float* obs;
+    TRY(learner_obs(env, &obs));
     REQUIRE(b200rl_env_internal_kind(env) != B200RL_ENV_ACROBOT, B200RL_ERR_UNSUPPORTED, "AcrobotEnv has 6 observations (networks take at most 4)");
     REQUIRE(!b200rl_env_internal_continuous(env), B200RL_ERR_UNSUPPORTED, "QBasedPolicy needs a discrete action space");
     REQUIRE(b200rl_env_internal_nobs(env) == q->actor.in, B200RL_ERR_INVALID, "network input width != observation width");
@@ -1438,6 +1475,8 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
         }
         REQUIRE(replay::controller_ok(*ctl), B200RL_ERR_INVALID, "bad controller values (ratio finite in [0, 1e6], counters >= 0)");
         REQUIRE(ctl->n_inserted + n_steps < (1ll << 52), B200RL_ERR_INVALID, "controller counters too large");
+        const float* obs;
+        TRY(learner_obs(r->env, &obs));   // (the wrapper may have been removed since create)
         return check_nstep_gamma(r->traj, &r->cfg);
     };
     const int local = local_checks();
@@ -1449,7 +1488,8 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
         TRY(replay_agree(r, ex, ctl, n_steps, local == B200RL_OK, &agree));
         if (local != B200RL_OK) return local;
         REQUIRE(agree, B200RL_ERR_INVALID,
-                "the ranks of a sharded run disagree on N, batch size, n_steps, controller, explorer, DQN config or n-step setting "
+                "the ranks of a sharded run disagree on N, batch size, n_steps, controller, explorer, DQN config, n-step setting or the "
+                "StateTransformedEnv(env, Float32) wrapper "
                 "(or another rank refused the run)");
     }
     if (local != B200RL_OK) return local;
@@ -1472,6 +1512,7 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
     key.tc = nn_tc_enabled() ? 1 : 0;
     key.max_timeout = b200rl_env_internal_max_timeout(r->env);
     key.greedy = ex ? 0 : 1;
+    key.state_f32 = b200rl_env_internal_state_f32(r->env) ? 1 : 0;
     b200rl_traj_internal_nstep(r->traj, &key.nstep_n, &key.nstep_gamma);
     if (ex) { key.ex = *ex; key.ex.step = 0; }
     key.rng = explorer_rng_dev;

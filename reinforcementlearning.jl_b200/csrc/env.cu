@@ -57,12 +57,13 @@ __global__ void __launch_bounds__(kBlock) env_step_kernel(typename Env::P p, Env
             });
             Env::store(a.state, i, s);
             if (!Env::kObsIsState) Env::write_obs(a.obs, i, N, s);
+            store_obs_f32<Env>(a, i, N, s);
             a.t[i] = t;
             a.flags[i] = (uint8_t)f;
             reinterpret_cast<T*>(a.reward)[i] = r.rew;
             reinterpret_cast<act_t*>(a.action)[i] = act;
             a.ep_ret[i] = ret;
-            if (a.traj_reward) reinterpret_cast<T*>(a.traj_reward)[i] = r.rew;
+            if (a.traj_reward) reinterpret_cast<float*>(a.traj_reward)[i] = (float)r.rew;   // the rollout's Float32 reward
             if (a.traj_terminal) a.traj_terminal[i] = r.done ? 1 : 0;
         }
         if (have_rng) store_rng(a.rng, i, g);
@@ -88,12 +89,19 @@ __global__ void __launch_bounds__(kBlock) env_reset_kernel(typename Env::P p, En
         store_rng(a.rng, i, g);
         Env::store(a.state, i, s);
         if (!Env::kObsIsState) Env::write_obs(a.obs, i, N, s);
+        store_obs_f32<Env>(a, i, N, s);
         a.t[i] = 0;
         reinterpret_cast<act_t*>(a.action)[i] = act;
         a.ep_ret[i] = 0.f;
         if (ResetReward<Env>::set) reinterpret_cast<typename Env::real*>(a.reward)[i] = (typename Env::real)ResetReward<Env>::value();
     }
     a.flags[i] = 0;
+}
+
+// Float32(x) of n doubles: the observation mirror after env_set, the Float32 reward a trajectory push reads
+__global__ void narrow_f64_kernel(float* __restrict__ dst, const double* __restrict__ src, int64_t n) {
+    int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+    if (i < n) dst[i] = (float)src[i];
 }
 
 }  // namespace
@@ -116,6 +124,8 @@ struct b200rl_env {
         AcrobotP acro;
     } p;
     size_t asize;   // bytes per stored action (8 for a Float64 continuous action space, else 4)
+    bool state_f32;   // StateTransformedEnv(env; state_mapping = s -> Float32.(s)): the learners read the Float32 mirror
+    float* rew_f32;   // (N) Float32(reward) for the trajectory pushes of a Float64 env (null for the others)
     EnvArrays a;
     uint64_t steps_launched;
 };
@@ -198,9 +208,16 @@ static int dispatch_reset(b200rl_env* e, int force) {
     return B200RL_ERR_INVALID;
 }
 
+// a Float64 env other than Acrobot keeps the (NOBS, N) float mirror of its observation behind the observation (env_device.cuh)
+static bool has_obs_f32(const b200rl_env* e) { return e->dtype == B200RL_F64 && e->kind != B200RL_ENV_ACROBOT; }
+static float* obs_f32_ptr(const b200rl_env* e) {
+    return has_obs_f32(e) ? reinterpret_cast<float*>(reinterpret_cast<double*>(e->a.obs) + (size_t)e->N * e->nobs) : (float*)e->a.obs;
+}
+
 static size_t field_bytes(const b200rl_env* e, int field) {
     size_t N = (size_t)e->N;
     switch (field) {
+        case B200RL_FIELD_OBS_F32: return b200rl_env_internal_obs_f32(e) ? N * e->nobs * 4 : 0;
         case B200RL_FIELD_STATE: return N * e->ns * e->tsize;
         case B200RL_FIELD_OBS: return N * e->nobs * e->tsize;
         case B200RL_FIELD_REWARD: return N * e->tsize;
@@ -224,15 +241,22 @@ static void* field_ptr(const b200rl_env* e, int field) {
         case B200RL_FIELD_ACTION: return e->a.action;
         case B200RL_FIELD_EPISODE_RETURN: return e->a.ep_ret;
         case B200RL_FIELD_EPISODE_STATS: return e->a.stats;
+        case B200RL_FIELD_OBS_F32: return (void*)b200rl_env_internal_obs_f32(e);
     }
     return nullptr;
 }
 
 static int env_alloc(b200rl_env* e) {
     size_t N = (size_t)e->N;
-    CUDA_TRY(cudaMalloc(&e->a.state, N * e->ns * e->tsize));
-    if (e->kind == B200RL_ENV_PENDULUM || e->kind == B200RL_ENV_ACROBOT) CUDA_TRY(cudaMalloc(&e->a.obs, N * e->nobs * e->tsize));
+    const size_t mirror = has_obs_f32(e) ? N * e->nobs * 4 : 0;   // the Float32 mirror behind the observation
+    const bool own_obs = e->kind == B200RL_ENV_PENDULUM || e->kind == B200RL_ENV_ACROBOT;
+    CUDA_TRY(cudaMalloc(&e->a.state, N * e->ns * e->tsize + (own_obs ? 0 : mirror)));
+    if (own_obs) CUDA_TRY(cudaMalloc(&e->a.obs, N * e->nobs * e->tsize + mirror));
     else e->a.obs = e->a.state;
+    if (mirror) {
+        CUDA_TRY(cudaMalloc(&e->rew_f32, N * 4));
+        CUDA_TRY(cudaMemsetAsync(obs_f32_ptr(e), 0, mirror, e->ctx->stream));
+    }
     CUDA_TRY(cudaMalloc(&e->a.reward, N * e->tsize));
     CUDA_TRY(cudaMalloc(&e->a.flags, N));
     CUDA_TRY(cudaMalloc(&e->a.t, N * 4));
@@ -271,6 +295,7 @@ int b200rl_env_create(b200rl_ctx* ctx, int kind, int dtype, int64_t n_envs, cons
     if (kind == B200RL_ENV_CARTPOLE_CONTINUOUS) kind = B200RL_ENV_CARTPOLE;
     if (kind == B200RL_ENV_MOUNTAINCAR_CONTINUOUS) kind = B200RL_ENV_MOUNTAINCAR;
     e->ctx = ctx; e->kind = kind; e->dtype = dtype; e->N = n_envs; e->continuous = cont_kind;
+    e->state_f32 = false; e->rew_f32 = nullptr;
     e->tsize = dtype == B200RL_F64 ? 8 : 4;
     e->steps_launched = 0;
     if (kind == B200RL_ENV_CARTPOLE) {
@@ -347,7 +372,7 @@ int b200rl_env_destroy(b200rl_env* e) {
     cudaFree(e->a.state);
     if (e->a.obs != e->a.state) cudaFree(e->a.obs);
     cudaFree(e->a.reward); cudaFree(e->a.flags); cudaFree(e->a.t); cudaFree(e->a.rng); cudaFree(e->a.action);
-    cudaFree(e->a.ep_ret); cudaFree(e->a.stats); cudaFree(e->a.err);
+    cudaFree(e->a.ep_ret); cudaFree(e->a.stats); cudaFree(e->a.err); cudaFree(e->rew_f32);
     delete e;
     return B200RL_OK;
 }
@@ -357,6 +382,7 @@ int b200rl_env_copy(b200rl_env* src, b200rl_env** out) {
     TRY(ctx_bind(src->ctx));
     b200rl_env* e = new b200rl_env(*src);
     memset(&e->a, 0, sizeof e->a);
+    e->rew_f32 = nullptr;
     e->a.max_timeout = src->a.max_timeout;
     int s = env_alloc(e);
     if (s != B200RL_OK) { b200rl_env_destroy(e); return s; }
@@ -365,6 +391,8 @@ int b200rl_env_copy(b200rl_env* src, b200rl_env** out) {
         CUDA_TRY(cudaMemcpyAsync(field_ptr(e, f), field_ptr(src, f), field_bytes(src, f), cudaMemcpyDeviceToDevice, st));
     if (e->a.obs != e->a.state)
         CUDA_TRY(cudaMemcpyAsync(e->a.obs, src->a.obs, field_bytes(src, B200RL_FIELD_OBS), cudaMemcpyDeviceToDevice, st));
+    if (has_obs_f32(e))
+        CUDA_TRY(cudaMemcpyAsync(obs_f32_ptr(e), obs_f32_ptr(src), (size_t)e->N * e->nobs * 4, cudaMemcpyDeviceToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(e->a.ep_ret, src->a.ep_ret, (size_t)src->N * 4, cudaMemcpyDeviceToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(e->a.stats, src->a.stats, 4 * sizeof(double), cudaMemcpyDeviceToDevice, st));
     *out = e;
@@ -408,6 +436,13 @@ int b200rl_env_set_max_timeout(b200rl_env* e, int64_t max_t) {
     return B200RL_OK;
 }
 
+int b200rl_env_set_state_f32(b200rl_env* e, int on) {
+    REQUIRE(e, B200RL_ERR_INVALID, "null env");
+    REQUIRE(e->kind != B200RL_ENV_ACROBOT, B200RL_ERR_UNSUPPORTED, "AcrobotEnv has 6 observations: no learner reads them");
+    e->state_f32 = on != 0;   // (the env kernels keep a Float64 env's mirror current: turning the wrapper on needs no fill)
+    return B200RL_OK;
+}
+
 int b200rl_env_step_random(b200rl_env* e, int auto_reset) {
     REQUIRE(e, B200RL_ERR_INVALID, "null env");
     REQUIRE(!e->continuous, B200RL_ERR_UNSUPPORTED,
@@ -438,8 +473,14 @@ int b200rl_env_set(b200rl_env* e, int field, const void* host_src, size_t bytes)
     TRY(ctx_bind(e->ctx));
     size_t need = field_bytes(e, field);
     REQUIRE(need != 0 && field != B200RL_FIELD_TERMINAL, B200RL_ERR_INVALID, "field not settable (TERMINAL is bit 0 of FLAGS)");
+    REQUIRE(field != B200RL_FIELD_OBS_F32, B200RL_ERR_INVALID, "OBS_F32 follows the observation: set STATE / OBS");
     REQUIRE(bytes >= need, B200RL_ERR_INVALID, "source too small");
     CUDA_TRY(cudaMemcpyAsync(field_ptr(e, field), host_src, need, cudaMemcpyHostToDevice, e->ctx->stream));
+    if (has_obs_f32(e) && (field == B200RL_FIELD_STATE || field == B200RL_FIELD_OBS)) {   // the mirror follows the observation
+        const int64_t n = e->N * e->nobs;
+        narrow_f64_kernel<<<grid_for(n, kBlock), kBlock, 0, e->ctx->stream>>>(obs_f32_ptr(e), (const double*)e->a.obs, n);
+        LAUNCH_CHECK(e->ctx);
+    }
     CUDA_TRY(cudaStreamSynchronize(e->ctx->stream));
     if (field == B200RL_FIELD_EPISODE_STATS) e->steps_launched = (uint64_t)(((const double*)host_src)[3] / (double)e->N + 0.5);
     return B200RL_OK;
@@ -498,6 +539,19 @@ int b200rl_env_internal_view(b200rl_env* e, envdev::EnvView* out) {
 void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n) { e->steps_launched += n; }
 uint64_t b200rl_env_internal_steps(const b200rl_env* e) { return e->steps_launched; }
 int b200rl_env_internal_max_timeout(const b200rl_env* e) { return e->a.max_timeout; }
+bool b200rl_env_internal_state_f32(const b200rl_env* e) { return e->dtype == B200RL_F64 && e->state_f32; }   // (the identity on Float32)
+const float* b200rl_env_internal_obs_f32(const b200rl_env* e) {
+    if (e->dtype == B200RL_F32) return (const float*)e->a.obs;
+    return e->state_f32 ? obs_f32_ptr(e) : nullptr;
+}
+int b200rl_env_internal_reward_f32(b200rl_env* e, const float** out) {   // (a launch on the ctx stream for a Float64 env)
+    if (e->dtype == B200RL_F32) { *out = (const float*)e->a.reward; return B200RL_OK; }
+    REQUIRE(e->rew_f32, B200RL_ERR_UNSUPPORTED, "AcrobotEnv has no Float32 view");
+    narrow_f64_kernel<<<grid_for(e->N, kBlock), kBlock, 0, e->ctx->stream>>>(e->rew_f32, (const double*)e->a.reward, e->N);
+    LAUNCH_CHECK(e->ctx);
+    *out = e->rew_f32;
+    return B200RL_OK;
+}
 int b200rl_env_internal_dtype(const b200rl_env* e) { return e->dtype; }
 int64_t b200rl_env_internal_n(const b200rl_env* e) { return e->N; }
 int b200rl_env_internal_kind(const b200rl_env* e) { return e->kind; }

@@ -15,7 +15,7 @@ using jld::Xo;
 
 struct EnvArrays {
     void* state;      // (NS, N) T
-    void* obs;        // (NOBS, N) T   (== state when the observation is the state)
+    void* obs;        // (NOBS, N) T   (== state when the observation is the state); a Float64 env's Float32 mirror follows it (obs_f32)
     void* reward;     // (N) T
     uint8_t* flags;   // (N)  bit0 terminal, bit1 already auto-reset
     int32_t* t;       // (N)
@@ -333,6 +333,27 @@ struct AcrobotD {
         o[0] = jld::jcos(s.th1); o[1] = jld::jsin(s.th1); o[2] = jld::jcos(s.th2); o[3] = jld::jsin(s.th2); o[4] = s.dth1; o[5] = s.dth2;
     }
 };
+
+// StateTransformedEnv(env; state_mapping = s -> Float32.(s)) of a Float64 env: a (NOBS, N) float mirror of the observation, each
+// entry the round-to-nearest of the Float64 observation (observe()).  It sits right behind the (NOBS, N) double observation in the
+// same allocation, so no kernel takes a new parameter and the Float32 instantiations stay what they were.  Acrobot (6
+// observations, no learner reads them) has none.
+template <class Env> struct HasObsF32 {
+    static constexpr bool value = std::is_same<typename Env::real, double>::value && Env::NOBS <= 4;
+};
+template <class Env> __device__ __forceinline__ float* obs_f32(const EnvArrays& a, int64_t N) {
+    return reinterpret_cast<float*>(reinterpret_cast<double*>(a.obs) + (size_t)N * Env::NOBS);
+}
+// writes the mirror entry of env i (a no-op for the envs without a mirror)
+template <class Env> __device__ __forceinline__ void store_obs_f32(const EnvArrays& a, int64_t i, int64_t N, const typename Env::S& s) {
+    if constexpr (HasObsF32<Env>::value) {
+        float o[4];
+        Env::observe(s, o);
+        float* m = obs_f32<Env>(a, N) + (size_t)Env::NOBS * i;
+#pragma unroll
+        for (int j = 0; j < Env::NOBS; ++j) m[j] = o[j];
+    }
+}
 
 // What one act! step reports besides the env it updated
 template <class T> struct ActStep {

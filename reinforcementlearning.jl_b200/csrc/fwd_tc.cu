@@ -151,12 +151,13 @@ __device__ __forceinline__ void put_stream(unsigned long long* w, int s, const u
 
 template <class E> struct EnvSlot {   // the env part of a slot; each kernel's slot type adds its own fields
     using Env = E;
+    using act_bits = typename std::conditional<sizeof(typename Env::act_t) == 8, unsigned long long, uint32_t>::type;
     typename Env::S st[TM];
     int t[TM];
     int flags[TM];
     float ep_ret[TM];
-    float last_rew[TM];
-    uint32_t last_act[TM];                 // env.action after the last act! (a reset may have redrawn it), raw bits
+    typename Env::real last_rew[TM];
+    act_bits last_act[TM];                 // env.action after the last act! (a reset may have redrawn it), raw bits
     unsigned long long erng[4 * TM];       // env stream
 };
 
@@ -195,6 +196,7 @@ __device__ __forceinline__ void store_group(const Slot* slot, int nslots, int64_
             const Slot& sl = slot[k];
             Env::store(ea.state, i, sl.st[s]);
             if (!Env::kObsIsState) Env::write_obs(ea.obs, i, N, sl.st[s]);
+            store_obs_f32<Env>(ea, i, N, sl.st[s]);
             ea.t[i] = sl.t[s];
             ea.flags[i] = (uint8_t)sl.flags[s];
             ea.ep_ret[i] = sl.ep_ret[s];
@@ -202,8 +204,8 @@ __device__ __forceinline__ void store_group(const Slot* slot, int nslots, int64_
             get_stream(sl.erng, s, e);
             explore::xo_store(ea.rng, i, e);
             if (stepped) {
-                reinterpret_cast<float*>(ea.reward)[i] = sl.last_rew[s];
-                reinterpret_cast<uint32_t*>(ea.action)[i] = sl.last_act[s];
+                reinterpret_cast<typename Env::real*>(ea.reward)[i] = sl.last_rew[s];
+                reinterpret_cast<typename Slot::act_bits*>(ea.action)[i] = sl.last_act[s];
             }
             more(sl, i);
         }
@@ -211,20 +213,22 @@ __device__ __forceinline__ void store_group(const Slot* slot, int nslots, int64_
 }
 
 // the action the env receives for the head's raw action bits: the 1-based index, or the continuous action clamped to the action space
+// (a Float64 env: Float64 of the clamped Float32 action; the bounds are exact in Float32, so this is the clamp in Float64)
 template <class Env> __device__ __forceinline__ typename Env::act_t env_action(uint32_t a_bits) {
     using act_t = typename Env::act_t;
-    if (std::is_same<act_t, float>::value) return (act_t)fminf(fmaxf(__uint_as_float(a_bits), -Env::kActionBound), Env::kActionBound);
+    if (std::is_floating_point<act_t>::value) return (act_t)fminf(fmaxf(__uint_as_float(a_bits), -Env::kActionBound), Env::kActionBound);
     return (act_t)(int32_t)a_bits;
 }
 // act!(env, a) of owner thread s's env in its slot: the act! step of env_step_kernel<Env, false, true>, the fused auto-reset drawing
-// from the slot's env stream, a finished episode added to the thread's tally
+// from the slot's env stream, a finished episode added to the thread's tally.  The reward it returns is Float32(reward), what a
+// rollout or the replay ring stores; the slot keeps the env's own.
 template <class Env>
 __device__ __forceinline__ ActStep<float> slot_act(EnvSlot<Env>& sl, int s, const typename Env::P& p, int max_timeout, typename Env::act_t act,
                                                    int& fin_cnt, float& fin_ret, int& fin_len) {
     typename Env::S st = sl.st[s];
     int t = sl.t[s], f = sl.flags[s];
     float ret = sl.ep_ret[s];
-    const ActStep<float> r = act_step<Env, true>(p, max_timeout, st, t, f, ret, act, fin_cnt, fin_ret, fin_len, [&](auto&& reset) {
+    const ActStep<typename Env::real> r = act_step<Env, true>(p, max_timeout, st, t, f, ret, act, fin_cnt, fin_ret, fin_len, [&](auto&& reset) {
         unsigned long long w[4];
         get_stream(sl.erng, s, w);
         Xo e{w[0], w[1], w[2], w[3]};
@@ -234,10 +238,10 @@ __device__ __forceinline__ ActStep<float> slot_act(EnvSlot<Env>& sl, int s, cons
     });
     sl.st[s] = st; sl.t[s] = t; sl.flags[s] = f; sl.ep_ret[s] = ret;
     sl.last_rew[s] = r.rew;
-    uint32_t bits;
-    memcpy(&bits, &act, 4);
+    typename EnvSlot<Env>::act_bits bits;
+    memcpy(&bits, &act, sizeof bits);
     sl.last_act[s] = bits;
-    return r;
+    return ActStep<float>{(float)r.rew, r.done, r.ret, r.len};
 }
 
 // b200rl_explorer without its trailing beta, which the kernels that plan with it take separately: the parameters the ϵ-greedy
@@ -703,9 +707,21 @@ template <auto kernel, class Smem, class... Args> int launch_fused(b200rl_ctx* c
 }
 
 template <class Env> struct EnvTag { using type = Env; };
-// Calls f(EnvTag<Env>{}, params) with the Float32 device env type of the handle and its parameters (a continuous variant reads the
-// parameter block of its discrete kind, which has the same layout).  The caller has checked v.dtype == B200RL_F32.
-template <class F> int with_f32_env(const EnvView& v, F&& f) {
+// Calls f(EnvTag<Env>{}, params) with the device env type of the handle and its parameters (a continuous variant reads the
+// parameter block of its discrete kind, which has the same layout).  The caller has checked that the networks can read the env
+// (b200rl_env_internal_obs_f32): a Float32 env, or a Float64 one behind StateTransformedEnv(env, Float32).
+template <class F> int with_learner_env(const EnvView& v, F&& f) {
+    if (v.dtype == B200RL_F64) {
+        switch (v.kind) {
+            case B200RL_ENV_CARTPOLE:   // (CartPoleEnv(continuous = true) is Float32 only)
+                return f(EnvTag<CartPoleD<double, false>>{}, v.p.cp64);
+            case B200RL_ENV_PENDULUM:
+                return v.continuous ? f(EnvTag<PendulumD<true, double>>{}, v.p.pend64) : f(EnvTag<PendulumD<false, double>>{}, v.p.pend64);
+            case B200RL_ENV_MOUNTAINCAR:
+                return v.continuous ? f(EnvTag<MountainCarD<true, double>>{}, v.p.mc64) : f(EnvTag<MountainCarD<false, double>>{}, v.p.mc64);
+        }
+        return B200RL_ERR_UNSUPPORTED;
+    }
     switch (v.kind) {
         case B200RL_ENV_CARTPOLE: {
             if (!v.continuous) return f(EnvTag<CartPoleD<float, false>>{}, v.p.cp32);
@@ -785,14 +801,14 @@ int nn_tc_rollout(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const 
                   float* values, float* rewards, uint8_t* terminals) {
     EnvView v;
     TRY(b200rl_env_internal_view(env, &v));
-    if (!(nn_tc_supported(actor) && nn_tc_supported(critic)) || critic.nout != 1 || v.dtype != B200RL_F32) return B200RL_ERR_UNSUPPORTED;
+    if (!(nn_tc_supported(actor) && nn_tc_supported(critic)) || critic.nout != 1 || !b200rl_env_internal_obs_f32(env)) return B200RL_ERR_UNSUPPORTED;
     if (actor.act != critic.act) return B200RL_ERR_UNSUPPORTED;   // the fused kernel is compiled per activation (staged launches handle a mixed pair)
     const int64_t ntiles = (v.N + TM - 1) / TM;
     if (ntiles > (int64_t)kSlots * 2 * ctx->sm_count) return B200RL_ERR_UNSUPPORTED;
     if ((actor.heads2 != 0) != (v.continuous != 0)) return B200RL_ERR_UNSUPPORTED;   // Gaussian head <-> continuous action space
     if (!v.continuous && actor.nout != b200rl_env_internal_n_actions(env)) return B200RL_ERR_UNSUPPORTED;
     const RollArgs g{actor, critic, params, hp, v.N, t0, nsteps, T, final_bootstrap, policy_rng, states, actions, logp, values, rewards, terminals};
-    const int st = with_f32_env(v, [&](auto env_type, const auto& p) {
+    const int st = with_learner_env(v, [&](auto env_type, const auto& p) {
         using Env = typename decltype(env_type)::type;
         // the activation is a template parameter (both trunks share it, checked above)
         return actor.act == B200RL_ACT_RELU ? launch_fused<rollout_tc_kernel<Env, B200RL_ACT_RELU>, SmemRoll<Env>>(ctx, ntiles, g, p, v.a)
@@ -809,13 +825,13 @@ int nn_tc_evaluate(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const
                    int K, unsigned long long* policy_rng, float* returns, int32_t* lengths, int32_t* counts, const b200rl_explorer* ex) {
     EnvView v;
     TRY(b200rl_env_internal_view(env, &v));
-    if (!nn_tc_supported(actor) || v.dtype != B200RL_F32 || (mode == 2 && v.continuous)) return B200RL_ERR_UNSUPPORTED;
+    if (!nn_tc_supported(actor) || !b200rl_env_internal_obs_f32(env) || (mode == 2 && v.continuous)) return B200RL_ERR_UNSUPPORTED;
     const b200rl_explorer e = ex ? *ex : b200rl_explorer{};
     const EvalArgs g{actor, params, hp, v.N, nsteps, K, policy_rng, returns, lengths, counts};
     const EvalExploreArgs gx{g, ex ? 0 : 1, QExplorer{e.eps_stable, e.eps_init, e.warmup_steps, e.decay_steps, e.step, e.kind, e.is_break_tie},
                              e.beta, (long long)e.step, (long long)b200rl_comm_rank(ctx) * v.N, (long long)b200rl_comm_world(ctx) * v.N};
     const int64_t groups = ((v.N + TM - 1) / TM + kSlots - 1) / kSlots;
-    const int st = with_f32_env(v, [&](auto env_type, const auto& p) {
+    const int st = with_learner_env(v, [&](auto env_type, const auto& p) {
         using Env = typename decltype(env_type)::type;
         if (mode == 0) return launch_evaluate<Env, 0>(ctx, groups, g, p, v.a);
         if (mode == 1) return launch_evaluate<Env, 1>(ctx, groups, g, p, v.a);
@@ -834,13 +850,13 @@ int nn_tc_replay_collect(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& q, con
                          int nsteps, int64_t* keys, float* vals, int stride) {
     EnvView v;
     TRY(b200rl_env_internal_view(env, &v));
-    if (!nn_tc_supported(q) || v.dtype != B200RL_F32 || v.continuous || ring.ns > kInMax) return B200RL_ERR_UNSUPPORTED;
+    if (!nn_tc_supported(q) || !b200rl_env_internal_obs_f32(env) || v.continuous || ring.ns > kInMax) return B200RL_ERR_UNSUPPORTED;
     const b200rl_explorer e = ex ? *ex : b200rl_explorer{};
     const ReplayArgs g{q, params, v.N, nsteps, ex ? 0 : 1, QExplorer{e.eps_stable, e.eps_init, e.warmup_steps, e.decay_steps, e.step, e.kind, e.is_break_tie},
                        step_dev, (long long)b200rl_comm_rank(ctx) * v.N, (long long)b200rl_comm_world(ctx) * v.N, xrng, ring,
                        default_priority, prioritized, keys, vals, stride};
     const int64_t groups = ((v.N + TM - 1) / TM + kSlots - 1) / kSlots;
-    const int st = with_f32_env(v, [&](auto env_type, const auto& p) {
+    const int st = with_learner_env(v, [&](auto env_type, const auto& p) {
         using Env = typename decltype(env_type)::type;
         if constexpr (std::is_floating_point<typename Env::act_t>::value) return (int)B200RL_ERR_UNSUPPORTED;   // (rejected above)
         else if (!g.greedy && g.ex.kind >= 2) return launch_replay_collect<Env, true>(ctx, groups, g, p, v.a, e.beta);

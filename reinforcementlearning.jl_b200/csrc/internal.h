@@ -13,6 +13,13 @@ int b200rl_env_internal_view(b200rl_env* e, envdev::EnvView* out);
 void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n);
 uint64_t b200rl_env_internal_steps(const b200rl_env* e);
 int b200rl_env_internal_max_timeout(const b200rl_env* e);
+// StateTransformedEnv(env, Float32) in effect: a Float64 env with the wrapper (on a Float32 env the wrapper changes nothing)
+bool b200rl_env_internal_state_f32(const b200rl_env* e);
+// the Float32 observation (NOBS, N) the networks read: FIELD_OBS of a Float32 env, the mirror of a Float64 env wrapped by
+// b200rl_env_set_state_f32; null for a Float64 env without the wrapper
+const float* b200rl_env_internal_obs_f32(const b200rl_env* e);
+// Float32(reward(env)) (N): FIELD_REWARD of a Float32 env, a converted copy (launched on the ctx stream) of a Float64 env's
+int b200rl_env_internal_reward_f32(b200rl_env* e, const float** out);
 int b200rl_env_internal_dtype(const b200rl_env* e);
 int64_t b200rl_env_internal_n(const b200rl_env* e);
 int b200rl_env_internal_kind(const b200rl_env* e);

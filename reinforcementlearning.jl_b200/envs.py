@@ -61,6 +61,7 @@ class B200VecEnv:
         self.n = int(n_envs)
         self.T = np.dtype(T).type
         self.auto_reset = bool(auto_reset)
+        self.state_f32 = False
         if params is None:
             if self.kind == L.ENV_CARTPOLE:
                 params = cartpole_params(T=self.T, **kwargs)
@@ -126,6 +127,18 @@ class B200VecEnv:
         """MaxTimeoutEnv(env, max_t) (wrappers/MaxTimeoutEnv.jl:17-28); 0 removes the wrapper."""
         L.check(self.lib.b200rl_env_set_max_timeout(self.h, int(max_t)))
 
+    def set_state_float32(self, on=True):
+        """StateTransformedEnv(env; state_mapping = s -> Float32.(s)) (wrappers/StateTransformedEnv.jl:15-19) as a flag: state()
+        returns Float32 (round to nearest of the Float64 observation) and the learners, trajectories and evaluate() take a Float64
+        env.  The dynamics are untouched: every other field stays the unwrapped env's, bit for bit.  ``on=False`` removes the
+        wrapper.  The identity on a Float32 env; refused on Acrobot."""
+        L.check(self.lib.b200rl_env_set_state_f32(self.h, int(bool(on))))
+        self.state_f32 = bool(on)
+
+    def obs_device_ptr(self):
+        """device pointer of the Float32 (NOBS, N) observation the networks read (refused for an unwrapped Float64 env)"""
+        return self.device_ptr(L.FIELD_OBS_F32)
+
     def act_random_(self):
         """plan!(RandomPolicy(), env) + act!(env, a) fused: each env draws from its own stream."""
         L.check(self.lib.b200rl_env_step_random(self.h, int(self.auto_reset)))
@@ -136,7 +149,9 @@ class B200VecEnv:
         return out
 
     def state(self):
-        """state(env): (NOBS, N) observation batch."""
+        """state(env): (NOBS, N) observation batch (Float32 behind set_state_float32)."""
+        if self.state_f32:
+            return self._get(L.FIELD_OBS_F32, (_NOBS[self.kind], self.n), np.float32)
         return self._get(L.FIELD_OBS, (_NOBS[self.kind], self.n), self.T)
 
     def internal_state(self):

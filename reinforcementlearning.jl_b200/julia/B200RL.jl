@@ -90,7 +90,7 @@ AcrobotParamsC(p::RLEnvs.AcrobotEnvParams; book_or_nips::AbstractString = "book"
 const KINDS = Dict(:CartPole => 0, :Pendulum => 1, :MountainCar => 2, :ContinuousCartPole => 3, :ContinuousMountainCar => 4, :Acrobot => 5)
 const NS = Dict(0 => 4, 1 => 2, 2 => 2, 3 => 4, 4 => 2, 5 => 4)
 const NOBS = Dict(0 => 4, 1 => 3, 2 => 2, 3 => 4, 4 => 2, 5 => 6)
-@enum Field STATE = 0 OBS = 1 REWARD = 2 TERMINAL = 3 TSTEP = 4 RNG = 5 FLAGS = 6 ACTION = 7
+@enum Field STATE = 0 OBS = 1 REWARD = 2 TERMINAL = 3 TSTEP = 4 RNG = 5 FLAGS = 6 ACTION = 7 OBS_F32 = 10
 
 """
     B200VecEnv(ctx, kind, N; T = Float32, seeds, auto_reset = true, params = nothing)
@@ -110,6 +110,8 @@ mutable struct B200VecEnv{T} <: AbstractEnv
     obs::Matrix{T}
     rewards::Vector{T}
     terminals::Vector{UInt8}
+    state_f32::Bool        # StateTransformedEnv(env, Float32): state(env) is the Float32 mirror
+    obs32::Matrix{Float32}
 end
 
 function B200VecEnv(ctx::B200Context, kind::Symbol, n::Integer; T = Float32, seeds::AbstractVector{Xoshiro},
@@ -125,7 +127,8 @@ function B200VecEnv(ctx::B200Context, kind::Symbol, n::Integer; T = Float32, see
     GC.@preserve st pref check(ccall((:b200rl_env_create, LIB), Cint,
         (Ptr{Cvoid}, Cint, Cint, Int64, Ptr{Cvoid}, Ptr{UInt64}, Ref{Ptr{Cvoid}}),
         ctx.h, k, T === Float64 ? 1 : 0, n, pptr, st, out))
-    env = B200VecEnv{T}(ctx, out[], k, n, auto_reset, continuous, n_actions, zeros(T, NOBS[k], n), zeros(T, n), zeros(UInt8, n))
+    env = B200VecEnv{T}(ctx, out[], k, n, auto_reset, continuous, n_actions, zeros(T, NOBS[k], n), zeros(T, n), zeros(UInt8, n),
+                          false, zeros(Float32, NOBS[k], n))
     finalizer(e -> (e.h == C_NULL || ccall((:b200rl_env_destroy, LIB), Cint, (Ptr{Cvoid},), e.h); e.h = C_NULL), env)
 end
 
@@ -137,6 +140,19 @@ episode has taken `max_t` interactions; `reward` still forwards to the wrapped e
 """
 function RLEnvs.MaxTimeoutEnv(env::B200VecEnv, max_t::Integer)
     check(ccall((:b200rl_env_set_max_timeout, LIB), Cint, (Ptr{Cvoid}, Int64), env.h, max_t))
+    env
+end
+
+"""
+    StateTransformedEnv(env::B200VecEnv, Float32)
+
+`StateTransformedEnv(env; state_mapping = s -> Float32.(s))` (wrappers/StateTransformedEnv.jl:15-19) as a flag on a Float64 batched
+env: `state(env)` is the Float32 observation mirror (the round to nearest of the Float64 observation), which the learners,
+trajectories and the policies' `plan!` read; the dynamics stay the Float64 env's.  Returns `env`.
+"""
+function RLEnvs.StateTransformedEnv(env::B200VecEnv, ::Type{Float32})
+    check(ccall((:b200rl_env_set_state_f32, LIB), Cint, (Ptr{Cvoid}, Cint), env.h, 1))
+    env.state_f32 = true
     env
 end
 
@@ -162,8 +178,8 @@ struct FusedRandomAction end                                  # plan!(B200Random
 RLBase.act!(env::B200VecEnv, ::FusedRandomAction) =
     check(ccall((:b200rl_env_step_random, LIB), Cint, (Ptr{Cvoid}, Cint), env.h, env.auto_reset))
 
-RLBase.state(env::B200VecEnv, ::Observation, ::DefaultPlayer) = fetch!(env, OBS, env.obs)
-RLBase.state(env::B200VecEnv) = fetch!(env, OBS, env.obs)
+RLBase.state(env::B200VecEnv, ::Observation, ::DefaultPlayer) = RLBase.state(env)
+RLBase.state(env::B200VecEnv) = env.state_f32 ? fetch!(env, OBS_F32, env.obs32) : fetch!(env, OBS, env.obs)
 RLBase.reward(env::B200VecEnv) = fetch!(env, REWARD, env.rewards)
 RLBase.is_terminated(env::B200VecEnv) = (fetch!(env, TERMINAL, env.terminals); env.terminals .!= 0)
 # CartPoleEnv.jl:95-96, PendulumEnv.jl:73-74, MountainCarEnv.jl:85-86 (one sub-env's space; every sub-env has the same)
@@ -188,7 +204,8 @@ end
 function Base.copy(env::B200VecEnv{T}) where {T}
     out = Ref{Ptr{Cvoid}}(C_NULL)
     check(ccall((:b200rl_env_copy, LIB), Cint, (Ptr{Cvoid}, Ref{Ptr{Cvoid}}), env.h, out))
-    e = B200VecEnv{T}(env.ctx, out[], env.kind, env.n, env.auto_reset, env.continuous, env.n_actions, copy(env.obs), copy(env.rewards), copy(env.terminals))
+    e = B200VecEnv{T}(env.ctx, out[], env.kind, env.n, env.auto_reset, env.continuous, env.n_actions, copy(env.obs), copy(env.rewards), copy(env.terminals),
+                          env.state_f32, copy(env.obs32))
     finalizer(x -> (x.h == C_NULL || ccall((:b200rl_env_destroy, LIB), Cint, (Ptr{Cvoid},), x.h); x.h = C_NULL), e)
 end
 "Zero-copy device pointer of an env field for fused consumers (b200rl_env_ptr)."
@@ -624,13 +641,13 @@ end
 function RLBase.plan!(p::B200QBasedPolicy, env::B200VecEnv)
     ex = ExplorerC(p.explorer)
     check(ccall((:b200rl_net_q_explore, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Ptr{Cvoid}, Ref{ExplorerC}, Ptr{Cvoid}),
-                p.learner.net.h, device_ptr(env, OBS), p.n, p.d_rng, Ref(ex), p.d_action))
+                p.learner.net.h, device_ptr(env, OBS_F32), p.n, p.d_rng, Ref(ex), p.d_action))
     set_step!(p.explorer, ex.step + p.n * comm_rank_world(p.ctx)[2])   # BatchExplorer over every rank's columns (DESIGN.md §3)
     DeviceActions(p.d_action)
 end
 function RLBase.plan!(p::B200QBasedPolicy{GreedyExplorer}, env::B200VecEnv)
     check(ccall((:b200rl_net_q_act, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Ptr{Cvoid}, Cfloat, Ptr{Cvoid}),
-                p.learner.net.h, device_ptr(env, OBS), p.n, C_NULL, 0f0, p.d_action))
+                p.learner.net.h, device_ptr(env, OBS_F32), p.n, C_NULL, 0f0, p.d_action))
     DeviceActions(p.d_action)
 end
 
@@ -655,7 +672,7 @@ end
 function RLBase.plan!(p::B200GreedyPolicy, env::B200VecEnv)
     env.continuous && throw(ArgumentError("B200GreedyPolicy plans discrete actions; evaluate a Gaussian policy with `evaluate`"))
     check(ccall((:b200rl_net_act_greedy, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Ptr{Cvoid}, Cint),
-                p.net.h, device_ptr(env, OBS), p.n, p.d_action, 1))
+                p.net.h, device_ptr(env, OBS_F32), p.n, p.d_action, 1))
     DeviceActions(p.d_action)
 end
 

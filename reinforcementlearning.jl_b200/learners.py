@@ -187,7 +187,8 @@ class OnPolicyAgent(AbstractPolicy):
             L.check(self.lib.b200rl_onpolicy_plan(self.h, L.ptr(self._act_buf)))
             if self.continuous:
                 lo, hi = env.action_space()               # the env asserts a in -2.0..2.0 (Pendulum) | -1.0..1.0
-                return np.clip(self._act_buf, lo, hi)
+                # a Float64 env receives Float64 of the clamped Float32 sample (exact bounds: the clamp in Float64)
+                return np.clip(self._act_buf, np.float32(lo), np.float32(hi)).astype(env.act_dtype)
             return self._act_buf
         L.check(self.lib.b200rl_onpolicy_plan(self.h, None))
         return FusedAction("policy")
@@ -462,7 +463,7 @@ class QBasedPolicy(AbstractPolicy):
     def plan_device(self, env):
         """plan!(policy, env) leaving the actions on the device; returns the device pointer of the (N,) int32 actions."""
         net, ex = self.learner.net, self.explorer
-        obs = C.c_void_p(env.device_ptr(L.FIELD_OBS))
+        obs = C.c_void_p(env.obs_device_ptr())
         if hasattr(ex, "as_struct"):
             st = ex.as_struct()
             L.check(self.lib.b200rl_net_q_explore(net.h, obs, self.n, C.c_void_p(self._d_rng), C.byref(st), C.c_void_p(self._d_action)))
@@ -535,7 +536,7 @@ class EvaluationPolicy(AbstractPolicy):
 
     def plan_device(self, env):
         """plan!(policy, env) leaving the raw actions (int32 | float) on the device; returns their device pointer."""
-        obs = C.c_void_p(env.device_ptr(L.FIELD_OBS))
+        obs = C.c_void_p(env.obs_device_ptr())
         if self.mode == "greedy":
             L.check(self.lib.b200rl_net_act_greedy(self.net.h, obs, self.n, C.c_void_p(self._d_action), 1))
         else:
@@ -549,7 +550,7 @@ class EvaluationPolicy(AbstractPolicy):
             if self._host_act is None:
                 self._host_act = np.empty(self.n, np.float32)
             lo, hi = env.action_space()
-            return np.clip(self.ctx.d2h(self._host_act, d), np.float32(lo), np.float32(hi))
+            return np.clip(self.ctx.d2h(self._host_act, d), np.float32(lo), np.float32(hi)).astype(env.act_dtype)
         return FusedAction("policy")
 
     def act_fused(self, env):
@@ -662,11 +663,12 @@ class Agent(AbstractPolicy):
 
     # ---- device agent loop ----------------------------------------------------------------------
     def replay_supported(self, env):
-        """The env side of the device loop: in-kernel auto-reset, Float32, a discrete action space, <= 4 observations, and
+        """The env side of the device loop: in-kernel auto-reset, Float32 observations (a Float32 env, or a Float64 one behind
+        set_state_float32), a discrete action space, <= 4 observations, and
         the trajectory's controller is an InsertSampleRatioController.  A sharded ctx needs the peer exchange attached or an NCCL
         communicator (refused by create otherwise)."""
         t, lr = self.trajectory, self.policy.learner
-        return (self.fusable and env.auto_reset and env.T is np.float32 and not env.continuous and env.kind != L.ENV_ACROBOT
+        return (self.fusable and env.auto_reset and (env.T is np.float32 or env.state_f32) and not env.continuous and env.kind != L.ENV_ACROBOT
                 and type(t.controller) is InsertSampleRatioController and t.batch_size > 0 and t.lanes == env.n and t.ns == lr.net.n_in
                 and lr.net.n_in == _NOBS.get(env.kind) and self._handle(env) is not None)
 
