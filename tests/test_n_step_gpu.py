@@ -8,6 +8,7 @@ import pytest
 
 import nstep_ref as N
 import oracle_lib as O
+import q_ref as Q
 
 pytestmark = pytest.mark.gpu
 
@@ -163,20 +164,6 @@ def _fill_both(pkg, ctx, ns, lanes, cap, frames, prioritized, B, seed, n=1, gamm
     return tr, ref, slots
 
 
-def _oracle_nstep_loss_grad(desc, p, pt, b, w, huber, double_dqn):
-    """the oracle's DQN loss with R = G + discount·(1-t)·q': one oracle call per window length (one discount each)"""
-    B = b["reward"].size
-    grad, loss, td = np.zeros(O.q_nparams(desc)), 0.0, np.empty(B, np.float32)
-    for m in np.unique(b["horizon"]):
-        i = np.flatnonzero(b["horizon"] == m)
-        d = b["discount"][i[0]]
-        assert np.all(b["discount"][i] == d)
-        g, l, t = O.dqn_loss_grad(desc, p, pt, b["state"][:, i], b["action"][i], b["reward"][i], b["terminal"][i], b["next_state"][:, i],
-                                  None if w is None else w[i], float(d), huber, double_dqn)
-        grad += g * (i.size / B); loss += l * i.size / B; td[i] = t
-    return grad, loss, td
-
-
 UPDATE_CASES = [(128, True, False, True), (64, False, False, False), (128, True, True, True), (64, True, True, True), (128, False, False, False)]
 
 
@@ -202,7 +189,7 @@ def test_dqn_update_parity_n3(pkg, ctx, hidden, huber, double_dqn, prioritized):
         _check_against_restatement(tr, b, n, gamma)
         assert (b["horizon"] < n).any() and (b["horizon"] == n).any()
         w = b["weight"] if prioritized else None
-        g, loss, td = _oracle_nstep_loss_grad(desc, p, pt, b, w, huber, double_dqn)
+        g, loss, td = Q.oracle_dqn_loss_grad(desc, p, pt, b, w, huber, double_dqn)
         gc, gn = O.clip_by_global_norm(g.astype(np.float32), 10.0)
         O.adam_step(p, gc, m, v, bt)
         tol = 2e-5 * (1 + it)

@@ -9,28 +9,10 @@ import pytest
 import torch
 
 import oracle_lib as O
+import q_ref as Q
+from q_ref import unpack_mlp
 
 torch.set_num_threads(2)
-
-
-def unpack_mlp(p, n_in, H, heads, act):
-    """flat Flux-order params -> torch forward function"""
-    o = 0
-    def take(n):
-        nonlocal o
-        v = p[o:o + n]; o += n
-        return v
-    W1 = take(H * n_in).reshape(n_in, H).T; b1 = take(H)
-    W2 = take(H * H).reshape(H, H).T; b2 = take(H)
-    hs = []
-    for d in heads:
-        W = take(d * H).reshape(H, d).T; b = take(d)
-        hs.append((W, b))
-    f = torch.relu if act == O.ACT_RELU else torch.tanh
-    def fwd(x):  # x (B, n_in)
-        h = f(x @ W1.T + b1); h = f(h @ W2.T + b2)
-        return torch.cat([h @ W.T + b for W, b in hs], dim=1)
-    return fwd, o
 
 
 def make_batch(ns, total, rng, gaussian):
@@ -90,36 +72,48 @@ def test_actor_critic_grad_matches_autograd(algo, act):
     assert np.linalg.norm(grad - g_t) <= 2e-5 * np.linalg.norm(g_t)
 
 
-@pytest.mark.parametrize("huber,double_dqn,weighted", [(True, False, True), (False, False, False), (True, True, False)])
-def test_dqn_grad_matches_autograd(huber, double_dqn, weighted):
-    ns, H, na, B = 4, 128, 2, 400
-    desc = O.ac_desc(ns, H, na)
+R_, T_ = O.ACT_RELU, O.ACT_TANH
+# (ns, H, na, act, huber, double_dqn, weighted, tie): every observation width 1..4, head width 1..4, both hidden widths and both
+# activations the TD loss + backward kernel accepts
+DQN_GRAD_CASES = [
+    pytest.param(4, 128, 2, R_, True, False, True, False, id="True-False-True"),
+    pytest.param(4, 128, 2, R_, False, False, False, False, id="False-False-False"),
+    pytest.param(4, 128, 2, R_, True, True, False, False, id="True-True-False"),
+    pytest.param(1, 64, 4, R_, True, False, True, False, id="ns1-H64-na4-relu"),
+    pytest.param(2, 128, 3, T_, True, True, False, False, id="ns2-H128-na3-tanh-double"),
+    pytest.param(3, 64, 1, T_, False, False, False, False, id="ns3-H64-na1-tanh"),
+    pytest.param(4, 128, 4, R_, False, False, True, False, id="ns4-H128-na4-relu"),
+    pytest.param(4, 64, 2, T_, True, False, False, False, id="ns4-H64-na2-tanh"),
+    pytest.param(1, 128, 3, T_, False, True, True, False, id="ns1-H128-na3-tanh-double"),
+    pytest.param(3, 128, 4, R_, True, True, False, False, id="ns3-H128-na4-relu-double"),
+    pytest.param(2, 64, 1, R_, True, False, False, False, id="ns2-H64-na1-relu"),
+    # the online net's Q(s') of actions 2 and 3 tie exactly; the target net's differ: "first maximum wins" decides R
+    pytest.param(2, 64, 3, R_, True, True, False, True, id="ns2-H64-na3-relu-double-tie"),
+]
+
+
+@pytest.mark.parametrize("ns,H,na,act,huber,double_dqn,weighted,tie", DQN_GRAD_CASES)
+def test_dqn_grad_matches_autograd(ns, H, na, act, huber, double_dqn, weighted, tie):
+    B = 400
+    desc = O.ac_desc(ns, H, na, act)
     rng = np.random.default_rng(4)
     p = O.glorot_params(desc, 2, q_net=True); pt = O.glorot_params(desc, 3, q_net=True)
+    if tie:
+        p = Q.tie_actions(p, ns, H, na, 2, 3)
     s = rng.standard_normal((ns, B)).astype(np.float32); s2 = rng.standard_normal((ns, B)).astype(np.float32)
     a = rng.integers(1, na + 1, B).astype(np.int32); r = (3 * rng.standard_normal(B)).astype(np.float32)
     t = (rng.random(B) < 0.2).astype(np.uint8); w = rng.random(B).astype(np.float32) if weighted else None
     grad, loss, td = O.dqn_loss_grad(desc, p, pt, s, a, r, t, s2, w, 0.99, huber, double_dqn)
-    P = torch.tensor(p, dtype=torch.float64, requires_grad=True)
-    q, _ = unpack_mlp(P, ns, H, [na], O.ACT_RELU)
-    qt, _ = unpack_mlp(torch.tensor(pt, dtype=torch.float64), ns, H, [na], O.ACT_RELU)
-    with torch.no_grad():
-        qn = qt(torch.tensor(s2.T, dtype=torch.float64))
-        if double_dqn:
-            best = q(torch.tensor(s2.T, dtype=torch.float64)).argmax(1)
-            qnext = qn[torch.arange(B), best]
-        else:
-            qnext = qn.max(1).values
-        R = torch.tensor(r, dtype=torch.float64) + float(np.float32(0.99)) * (1 - torch.tensor(t, dtype=torch.float64)) * qnext
-    qv = q(torch.tensor(s.T, dtype=torch.float64))[torch.arange(B), torch.tensor(a - 1, dtype=torch.long)]
-    e = R - qv
-    l = torch.where(e.abs() < 1, 0.5 * e * e, e.abs() - 0.5) if huber else e * e
-    W = torch.tensor(w, dtype=torch.float64) if weighted else torch.ones(B, dtype=torch.float64)
-    L = (W * l).mean()
-    L.backward()
-    assert loss == pytest.approx(L.item(), rel=2e-5)
-    np.testing.assert_allclose(td, e.detach().numpy(), rtol=1e-4, atol=1e-5)
-    assert np.linalg.norm(grad - P.grad.numpy()) <= 2e-5 * np.linalg.norm(P.grad.numpy())
+    g64, L64, e64 = Q.dqn_loss_grad(p, pt, ns, H, na, act, s, a, r, t, s2, w, 0.99, huber, double_dqn)
+    assert loss == pytest.approx(L64, rel=2e-5)
+    np.testing.assert_allclose(td, e64, rtol=1e-4, atol=1e-5)
+    assert np.linalg.norm(grad - g64) <= 2e-5 * np.linalg.norm(g64)
+    if tie:
+        qo, qt = Q.q_values(p, ns, H, na, act, s2), Q.q_values(pt, ns, H, na, act, s2)
+        assert np.array_equal(qo[:, 1], qo[:, 2]) and np.array_equal(*O.q_values(desc, p, s2)[1:])    # float64 and the oracle's float32
+        # on these samples action 3's target value would move the TD error by far more than the tolerance: the rule is observable
+        moved = (qo.argmax(1) == 1) & (t == 0) & (np.abs(qt[:, 2] - qt[:, 1]) > 1e-2)
+        assert moved.mean() > 0.1
 
 
 def test_adam_matches_torch_optim():
