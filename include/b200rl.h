@@ -37,7 +37,8 @@ typedef enum {
     B200RL_ERR_UNSUPPORTED = -3,    /* configuration outside the hot-path scope */
     B200RL_ERR_ACTION = -4,         /* an action outside action_space(env) was seen (replaces `@assert a in action_space(env)`) */
     B200RL_ERR_NCCL = -5,
-    B200RL_ERR_OOM = -6
+    B200RL_ERR_OOM = -6,
+    B200RL_ERR_OVERFLOW = -7        /* an episode log lost records: more than K episodes of one env between two flushes */
 } b200rl_status;
 
 typedef struct b200rl_ctx b200rl_ctx;
@@ -184,6 +185,31 @@ int b200rl_env_check(b200rl_env* env);
  * out[0] = finished episodes, out[1] = sum of their returns, out[2] = sum of their lengths,
  * out[3] = total env-steps taken.  reset_after != 0 zeroes the counters. */
 int b200rl_env_episode_stats(b200rl_env* env, double* out4, int reset_after);
+/* device episode log: the per-env lists of TotalRewardPerEpisode / BatchStepsPerEpisode (RLCore/src/core/hooks.jl:146-231)
+ * without a host copy per step.  b200rl_env_episode_log attaches a ring of K records per env (K = 0 detaches it, and
+ * attaching again starts empty; with the same K it keeps the same ring, so captured agent loops are not re-captured).  The
+ * kernels that write it run as instantiations of their own; an env without a log runs the code it ran before the log existed.
+ * Every act! that ends an episode (the finished-episode rule of b200rl_env_episode_stats:
+ * the MaxTimeoutEnv cut counts, a terminal env stepped again without a reset does not) writes {return, length} to the env's
+ * next slot: the return is the Float32 step-order sum of the episode's rewards (FIELD_EPISODE_RETURN), the length env.t.
+ * b200rl_env_step / _step_random, the fused rollout, b200rl_onpolicy_iterate and b200rl_replay_run write it;
+ * b200rl_evaluate / b200rl_evaluate_explore do not (an evaluation is a run of its own).  b200rl_env_copy does not copy it. */
+int b200rl_env_episode_log(b200rl_env* env, int32_t K);
+/* one record of a flushed list: env = rank * N + i on a sharded ctx (rank of b200rl_comm_rank_world), else i */
+typedef struct {
+    int64_t env;
+    float ret;
+    int32_t len;
+} b200rl_episode_record;
+/* Starts (asynchronously, on the ctx stream) the hand-over of every record logged since the previous flush: host_buf is
+ * PINNED host memory (b200rl_host_alloc) of 16 + 16 * capacity bytes, which receives int64 n, int64 overflowing envs, then n
+ * b200rl_episode_record ordered by (env, episode).  The caller leaves host_buf alone until b200rl_env_episode_log_read of it
+ * returns; a flush every K env steps or less cannot overflow (an episode lasts at least one step). */
+int b200rl_env_episode_log_flush(b200rl_env* env, void* host_buf, int64_t capacity);
+/* waits for the last flush into host_buf and sets *n_out to its list length.  B200RL_ERR_OVERFLOW when an env finished more
+ * than K episodes between the two flushes (its oldest records were overwritten; the message names how many envs) or the list
+ * is longer than capacity. */
+int b200rl_env_episode_log_read(b200rl_env* env, const void* host_buf, int64_t* n_out);
 
 /* ---------------------------------------------------------------- returns ---------- */
 /* generalized_advantage_estimation / discount_rewards / discount_rewards_reduced

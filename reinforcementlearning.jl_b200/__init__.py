@@ -4,7 +4,7 @@ run(policy, env, stop, hook) surface.  Python host mirror of the Julia glue
 there is no CPU fallback."""
 from . import _lib
 from ._lib import B200RLError, Context, load
-from .core import (AbstractHook, AbstractPolicy, BatchStepsPerEpisode, ComposedHook, DeviceEpisodeStats, DoEveryNSteps, DoOnExit, EmptyHook, Experiment, ResetAfterNSteps, ResetIfEnvTerminated,
+from .core import (AbstractHook, AbstractPolicy, BatchStepsPerEpisode, ComposedHook, DeviceEpisodeLog, DeviceEpisodeStats, DoEveryNSteps, DoOnExit, EmptyHook, Experiment, ResetAfterNSteps, ResetIfEnvTerminated,
                    RandomPolicy, StopAfterNEpisodes, StopAfterNoImprovement, StopAfterNSeconds, StopAfterNSteps, StopIfAll, StopIfAny,
                    StopSignal, TimePerStep, TotalBatchRewardPerEpisode, run)
 from .envs import B200VecEnv, cartpole_params, mountaincar_params, pendulum_params

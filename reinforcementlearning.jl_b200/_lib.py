@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.environ.get("B200RL_LIB") or os.path.join(HERE, "libb200rl.so")
 
 OK = 0
-ERR_INVALID, ERR_CUDA, ERR_UNSUPPORTED, ERR_ACTION, ERR_NCCL, ERR_OOM = -1, -2, -3, -4, -5, -6
+ERR_INVALID, ERR_CUDA, ERR_UNSUPPORTED, ERR_ACTION, ERR_NCCL, ERR_OOM, ERR_OVERFLOW = -1, -2, -3, -4, -5, -6, -7
 
 ENV_CARTPOLE, ENV_PENDULUM, ENV_MOUNTAINCAR, ENV_CARTPOLE_CONTINUOUS, ENV_MOUNTAINCAR_CONTINUOUS, ENV_ACROBOT = 0, 1, 2, 3, 4, 5
 F32, F64 = 0, 1
@@ -118,6 +118,9 @@ SIGNATURES = {
     "b200rl_env_ptr": (_i32, [_vp, _i32, _pp]),
     "b200rl_env_check": (_i32, [_vp]),
     "b200rl_env_episode_stats": (_i32, [_vp, _vp, _i32]),
+    "b200rl_env_episode_log": (_i32, [_vp, C.c_int32]),
+    "b200rl_env_episode_log_flush": (_i32, [_vp, _vp, _i64]),
+    "b200rl_env_episode_log_read": (_i32, [_vp, _vp, C.POINTER(_i64)]),
     "b200rl_gae_f32": (_i32, [_vp, _vp, _vp, _vp, _vp, _f32, _f32, _i64, _i64, _i32, _i32]),
     "b200rl_gae_f64": (_i32, [_vp, _vp, _vp, _vp, _vp, _f64, _f64, _i64, _i64, _i32, _i32]),
     "b200rl_discount_rewards_f32": (_i32, [_vp, _vp, _vp, _vp, _vp, _f32, _i64, _i64, _i32, _i32]),

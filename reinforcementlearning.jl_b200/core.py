@@ -130,6 +130,157 @@ class DeviceEpisodeStats(AbstractHook):
             self.stats = env.episode_stats()
 
 
+class DeviceEpisodeLog(AbstractHook):
+    """TotalBatchRewardPerEpisode + BatchStepsPerEpisode kept on the device (b200rl_env_episode_log): ``rewards`` and ``steps`` are
+    per-env lists with the meaning of those two hooks' fields, but no step copies anything to the host, so run() keeps its fused
+    paths.  Each env logs into a ring of ``capacity`` records; run() splits the fused loop into windows of at most ``capacity``
+    env steps and flushes after each (an episode lasts at least one step, so no ring can overflow), the stage loop flushes every
+    ``capacity`` PostActStage pushes.  A flush is read one flush later (or at PostExperimentStage), so the host never waits inside
+    a window; the records are kept as arrays and turned into the lists when ``rewards`` / ``steps`` are read.  The returns are the
+    env's Float32 step-order sums (FIELD_EPISODE_RETURN); evaluate() is not logged.  On a sharded ctx the records carry the
+    global env index rank * N + i; the lists are indexed by the local env i.
+
+    The ring stays attached to the env after the run and the two pinned host buffers stay with the hook, so the next run of the
+    same hook (or of another DeviceEpisodeLog of the same size on that env, which takes them over) allocates nothing and keeps the
+    captured graphs; attaching again empties the ring.  ``close()`` detaches the ring and frees the buffers.  One env is recorded by
+    one hook at a time: a second hook that starts while the first is inside a run is refused."""
+    per_step = False
+
+    def __init__(self, batchsize, capacity=64):
+        if capacity < 1:
+            raise ValueError("capacity must be >= 1")
+        self._lists = ([[] for _ in range(batchsize)], [[] for _ in range(batchsize)])
+        self.capacity = int(capacity)
+        self._env = None
+        self._bufs = []
+        self._chunks = []        # record arrays read from the device, in flush order
+        self._pending = None     # index of the buffer whose flush has not been read yet
+        self._acts = 0           # PostActStage pushes since the last flush (stage loop)
+        self._running = False
+
+    @property
+    def rewards(self):
+        return self._materialize()[0]
+
+    @property
+    def steps(self):
+        return self._materialize()[1]
+
+    def __getitem__(self, _):    # getindex of TotalRewardPerEpisode and BatchStepsPerEpisode (hooks.jl:160, 207)
+        return self._materialize()
+
+    def push(self, stage, policy, env):
+        if stage == PreExperimentStage:
+            self._attach(env)
+        elif stage == PostActStage:
+            self._acts += 1
+            if self._acts >= self.capacity:
+                self.flush()
+        elif stage == PostExperimentStage:
+            try:
+                self.flush()
+                self._read()
+            finally:
+                self._running = False
+
+    def _attach(self, env):
+        owner = getattr(env, "_episode_log_hook", None)
+        if owner is not None and owner is not self:
+            if owner._running:
+                raise RuntimeError("another DeviceEpisodeLog is recording this env")
+            owner._hand_over(self, env)
+        elif self._env is not None and self._env is not env:
+            self.close()
+        records = env.n * self.capacity
+        if self._bufs and self._records != records:
+            self._free_buffers()
+        env.episode_log(self.capacity)          # (the same K again: the same ring, emptied)
+        env._episode_log_hook = self
+        self._env, self._records = env, records
+        self._base = env.ctx.rank_world()[0] * env.n
+        if not self._bufs:
+            self._bufs, self._bufs_ctx = [env.episode_log_buffer(records) for _ in range(2)], env.ctx
+        self._next, self._pending, self._acts, self._running = 0, None, 0, True
+
+    def _hand_over(self, other, env):
+        """an idle hook lets `other` record `env`: its buffers go along when they have the right size"""
+        if self._bufs and self._records == env.n * other.capacity and not other._bufs:
+            other._bufs, other._records, other._bufs_ctx, self._bufs = self._bufs, self._records, self._bufs_ctx, []
+        self._free_buffers()
+        self._env = None
+
+    def _free_buffers(self):
+        for _, addr in self._bufs:
+            self._bufs_ctx.host_free(addr)
+        self._bufs = []
+
+    def close(self):
+        """detach the ring from the env and free the pinned buffers"""
+        env, self._env, self._running = self._env, None, False
+        if env is not None and getattr(env, "_episode_log_hook", None) is self:
+            env._episode_log_hook = None
+            if env.h:
+                env.episode_log(0)
+        self._free_buffers()
+
+    def __del__(self):
+        try:
+            if self._bufs and self._bufs_ctx.h:
+                self.close()
+        except Exception:
+            pass
+
+    def flush(self):
+        """Hand the records of the window that just ended to the host buffer not being read, then read the previous flush."""
+        if self._env is None:
+            return
+        try:
+            _, addr = self._bufs[self._next]
+            self._env.episode_log_flush(addr, self._records)
+            self._read()
+        except BaseException:
+            self._pending, self._running = None, False
+            raise
+        self._pending, self._next, self._acts = self._next, 1 - self._next, 0
+
+    def _read(self):
+        if self._pending is None:
+            return
+        arr, addr = self._bufs[self._pending]
+        self._pending = None
+        rec = self._env.episode_log_read(arr, addr)
+        if len(rec):
+            self._chunks.append(rec)
+
+    def _materialize(self):
+        if self._chunks:
+            rec = np.concatenate(self._chunks)
+            self._chunks = []
+            env = rec["env"] - self._base
+            rec = rec[np.argsort(env, kind="stable")]   # by env; the flushes are in time order, so episodes stay in order
+            ends = np.cumsum(np.bincount(env, minlength=len(self._lists[0])))
+            rets, lens = rec["ret"].tolist(), rec["len"].tolist()
+            start = 0
+            for i, end in enumerate(ends.tolist()):
+                if end > start:
+                    self._lists[0][i].extend(rets[start:end])
+                    self._lists[1][i].extend(lens[start:end])
+                start = end
+        return self._lists
+
+
+def _episode_log_window(hook):
+    """(the DeviceEpisodeLog hooks of `hook`, the longest window in env steps they allow or None)"""
+    hooks = hook.hooks if isinstance(hook, ComposedHook) else (hook,)
+    logs = [h for h in hooks if isinstance(h, DeviceEpisodeLog)]
+    return logs, (min(h.capacity for h in logs) if logs else None)
+
+
+def _flush(logs):
+    for h in logs:
+        h.flush()
+
+
 class TimePerStep(AbstractHook):
     """hooks.jl:243-262 (wall-clock per loop iteration)."""
 
@@ -340,22 +491,33 @@ def run(policy, env=None, stop_condition=None, hook=None, reset_condition=None):
     # {plan!, act!, push!}) — the same transitions, parameters and statistics as stepping through the stages.
     if (getattr(policy, "fusable", False) and env.auto_reset and not getattr(hook, "per_step", True)
             and isinstance(stop_condition, StopAfterNSteps) and isinstance(reset_condition, ResetIfEnvTerminated)):
+        # a DeviceEpisodeLog of capacity K: windows of at most K env steps, each followed by a flush of the log
+        logs, window = _episode_log_window(hook)
         if hasattr(policy, "run_replay"):
             # replay Agent: the whole stretch as device launches (b200rl_replay_run), updates replayed as CUDA graphs
             if policy.replay_supported(env):
                 n = stop_condition.remaining()
-                policy.run_replay(env, n)
+                for j in range(0, n, window or n):
+                    policy.run_replay(env, min(n - j, window or n))
+                    _flush(logs)
                 is_stop = stop_condition.advance(n)
         else:
             while not is_stop:
-                if policy._t == 0 and stop_condition.remaining() >= policy.T and hasattr(policy, "iterate"):
+                if (policy._t == 0 and stop_condition.remaining() >= policy.T and hasattr(policy, "iterate")
+                        and (window is None or policy.T <= window)):
                     # whole iterations (rollout + update) as one CUDA-graph launch each (b200rl_onpolicy_iterate)
                     k = stop_condition.remaining() // policy.T if not policy.fetch_stats else 1
+                    if window is not None:
+                        k = min(k, window // policy.T)
                     policy.iterate(k, want_stats=policy.fetch_stats)
+                    _flush(logs)
                     is_stop = stop_condition.advance(k * policy.T)
                     continue
                 n = min(policy.T - policy._t, stop_condition.remaining())
+                if window is not None:
+                    n = min(n, window)
                 policy.collect(n)
+                _flush(logs)
                 if policy._t == policy.T:
                     policy._t = 0
                     policy.update(want_stats=policy.fetch_stats)

@@ -330,6 +330,12 @@ static int eval_window(b200rl_ctx* ctx, b200rl_env* env, int nout, int nsteps, i
     TRY(b200rl_env_reset(env, 1));   // reset!(env; is_force = true), run.jl:46
     int st = nn_tc_enabled() ? fused(b) : B200RL_ERR_UNSUPPORTED;
     if (st == B200RL_ERR_UNSUPPORTED) {   // staged: plan! -> act! (auto-reset) -> record, n_steps times, no host sync
+        // (an evaluation is a run of its own: its K1 steps do not write the env's episode log)
+        struct LogHold {
+            b200rl_env* e;
+            ~LogHold() { b200rl_env_internal_log_hold(e, false); }
+        } hold{env};
+        b200rl_env_internal_log_hold(env, true);
         CUDA_TRY(cudaMemsetAsync(b.cnt, 0, (size_t)N * 4, ctx->stream));
         CUDA_TRY(cudaMemsetAsync(b.acc_ret, 0, round256((size_t)N * 4) * 2, ctx->stream));
         const uint8_t* flags = (const uint8_t*)env_field(env, B200RL_FIELD_FLAGS);
@@ -1055,8 +1061,10 @@ int b200rl_onpolicy_iterate(b200rl_onpolicy* a, int n_iters, float* stats_host) 
     P2PTable peers;
     const bool capturable = b200rl_comm_world(ctx) == 1 || b200rl_comm_p2p_table(ctx, &peers);
     // launch arguments the graph bakes in
-    const int key[3] = {nn_tc_enabled() ? 1 : 0, b200rl_env_internal_max_timeout(a->env), b200rl_env_internal_state_f32(a->env) ? 1 : 0};
-    a->graph.rekey(key, sizeof key);
+    struct { int tc, max_timeout, state_f32, pad; uint64_t log[4]; } key = {nn_tc_enabled() ? 1 : 0, b200rl_env_internal_max_timeout(a->env),
+                                                                             b200rl_env_internal_state_f32(a->env) ? 1 : 0, 0, {}};
+    b200rl_env_internal_log_key(a->env, key.log);
+    a->graph.rekey(&key, sizeof key);
     const CounterSet counters{ctx, a->net, a->env, nullptr, &a->n_updates};
     for (int it = 0; it < n_iters; ++it) {
         TRY(a->graph.run(0, counters, capturable, [&]() -> int {
@@ -1284,6 +1292,7 @@ struct ReplayKey {
     const void* rng;
     const void* scratch;
     const void* keys;
+    uint64_t log[4];             // the env's episode log
 };
 struct b200rl_replay {
     b200rl_ctx* ctx;
@@ -1518,6 +1527,7 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
     key.rng = explorer_rng_dev;
     key.scratch = ctx->scratch;
     key.keys = r->keys;
+    b200rl_env_internal_log_key(r->env, key.log);
     r->graphs.rekey(&key, sizeof key);
     // device copies of the counters the launches read
     r->h_counters[0] = ex ? (long long)ex->step : 0;

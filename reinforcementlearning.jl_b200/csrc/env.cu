@@ -10,6 +10,7 @@
 //   RLEnvs/src/environments/examples/MountainCarEnv.jl:99-135
 // Compiled with -fmad=false (no contraction; Julia never contracts) and IEEE div.
 #include <type_traits>
+#include <vector>
 
 #include "common.cuh"
 #include "env_device.cuh"
@@ -23,8 +24,9 @@ namespace {
 constexpr int kBlock = 256;
 
 // ------------------------------------------------------------------ kernels -----------
-template <class Env, bool RANDOM, bool AUTO>
-__global__ void __launch_bounds__(kBlock) env_step_kernel(typename Env::P p, EnvArrays a, int64_t N, const void* actions_v) {
+// LOG: a finished episode is also written to the env's episode log (EnvArraysLog)
+template <class Env, bool RANDOM, bool AUTO, bool LOG>
+__global__ void __launch_bounds__(kBlock) env_step_kernel(typename Env::P p, EnvArgs<LOG> a, int64_t N, const void* actions_v) {
     using T = typename Env::real;
     using act_t = typename Env::act_t;
     __shared__ StatsScratch<kBlock / 32> red;
@@ -51,10 +53,10 @@ __global__ void __launch_bounds__(kBlock) env_step_kernel(typename Env::P p, Env
         }
         if (ok) {
             float ret = a.ep_ret[i];
-            const ActStep<T> r = act_step<Env, AUTO>(p, a.max_timeout, s, t, f, ret, act, fin_cnt, fin_ret, fin_len, [&](auto&& reset) {
+            const ActStep<T> r = act_step<Env, AUTO, LOG>(p, a.max_timeout, s, t, f, ret, act, fin_cnt, fin_ret, fin_len, [&](auto&& reset) {
                 if (!have_rng) { g = load_rng(a.rng, i); have_rng = true; }
                 reset(g);
-            });
+            }, episode_log_of(a), i);
             Env::store(a.state, i, s);
             if (!Env::kObsIsState) Env::write_obs(a.obs, i, N, s);
             store_obs_f32<Env>(a, i, N, s);
@@ -104,6 +106,86 @@ __global__ void narrow_f64_kernel(float* __restrict__ dst, const double* __restr
     if (i < n) dst[i] = (float)src[i];
 }
 
+// ------------------------------------------------------------------ episode log flush --
+// One flush turns the records every env logged since the previous flush into one list ordered by (env, episode): the pending
+// counts of each CTA (log_count_kernel), an exclusive scan of the CTA totals (log_offsets_kernel), and each env's records written at
+// its offset (log_scatter_kernel), which recomputes the in-CTA prefix.  The list goes straight to the caller's pinned host buffer.
+
+// pending records of env i (0 past N); an env with more than K counts as overflowing (overflow != null) and contributes K
+__device__ __forceinline__ uint32_t flush_pending(const EpisodeLog& log, const uint32_t* cursor, int64_t i, int64_t N,
+                                                  unsigned long long* overflow) {
+    if (i >= N) return 0;
+    uint32_t n = log_pending(log, cursor, i);
+    if (n > (uint32_t)log.K) {
+        if (overflow) atomicAdd(overflow, 1ull);
+        n = (uint32_t)log.K;
+    }
+    return n;
+}
+// exclusive prefix of v over the CTA: a warp-shuffle scan, then the warp totals; *total is the CTA's sum.  Every thread calls it.
+__device__ __forceinline__ long long cta_exclusive_scan(long long v, long long (&warp_tot)[kBlock / 32], long long* total) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    long long x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const long long y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) warp_tot[w] = x;
+    __syncthreads();
+    long long before = 0, all = 0;
+#pragma unroll
+    for (int k = 0; k < kBlock / 32; ++k) {
+        if (k < w) before += warp_tot[k];
+        all += warp_tot[k];
+    }
+    __syncthreads();   // (warp_tot may be rewritten by the caller's next scan)
+    *total = all;
+    return before + x - v;
+}
+
+__global__ void __launch_bounds__(kBlock) log_count_kernel(EpisodeLog log, const uint32_t* __restrict__ cursor, int64_t N,
+                                                           long long* __restrict__ cta_tot, unsigned long long* overflow) {
+    __shared__ long long warp_tot[kBlock / 32];
+    const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+    long long total;
+    cta_exclusive_scan(flush_pending(log, cursor, i, N, overflow), warp_tot, &total);
+    if (threadIdx.x == 0) cta_tot[blockIdx.x] = total;
+}
+
+// one CTA: cta_tot[0 .. nb) -> exclusive offsets in place; hdr = {list length, overflowing envs}; the overflow counter is cleared
+__global__ void __launch_bounds__(kBlock) log_offsets_kernel(long long* __restrict__ cta_tot, int64_t nb, unsigned long long* overflow,
+                                                             long long* hdr) {
+    __shared__ long long warp_tot[kBlock / 32];
+    long long carry = 0;
+    for (int64_t b0 = 0; b0 < nb; b0 += kBlock) {
+        const int64_t b = b0 + threadIdx.x;
+        long long total;
+        const long long ex = cta_exclusive_scan(b < nb ? cta_tot[b] : 0, warp_tot, &total);
+        if (b < nb) cta_tot[b] = carry + ex;
+        carry += total;
+    }
+    if (threadIdx.x == 0) {
+        hdr[0] = carry;
+        hdr[1] = (long long)*overflow;
+        *overflow = 0;
+    }
+}
+
+__global__ void __launch_bounds__(kBlock) log_scatter_kernel(EpisodeLog log, uint32_t* __restrict__ cursor, int64_t N,
+                                                             const long long* __restrict__ cta_off, int64_t global0, EpisodeRecord* out,
+                                                             int64_t capacity) {
+    __shared__ long long warp_tot[kBlock / 32];
+    const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
+    const uint32_t n = flush_pending(log, cursor, i, N, nullptr);
+    long long total;
+    const long long off = cta_off[blockIdx.x] + cta_exclusive_scan(n, warp_tot, &total);
+    if (i < N) {
+        if (n) log_emit(log, cursor, i, n, global0 + i, out + off, capacity - off);
+        cursor[i] = log.count[i];
+    }
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------ handle ------------
@@ -128,17 +210,45 @@ struct b200rl_env {
     float* rew_f32;   // (N) Float32(reward) for the trajectory pushes of a Float64 env (null for the others)
     EnvArrays a;
     uint64_t steps_launched;
+    // episode log (b200rl_env_episode_log): the device ring (written by the env's steps unless a staged evaluation holds it off);
+    // the flush keeps each env's read position, its scan scratch (CTA totals, then the overflow counter) and the last flush into
+    // each buffer
+    EpisodeLog log_ring;
+    bool log_held;
+    uint32_t* log_cursor;
+    long long* log_scratch;
+    struct LogFlush { const void* buf; int64_t capacity; cudaEvent_t done; };
+    std::vector<LogFlush> log_flushes;
 };
 
-template <class Env> static int launch_step(b200rl_env* e, const typename Env::P& p, const void* actions, bool random, bool auto_reset) {
-    unsigned grid = grid_for(e->N, kBlock);
+static void log_free(b200rl_env* e) {
+    if (e->log_ring.count) cudaStreamSynchronize(e->ctx->stream);
+    cudaFree(e->log_ring.ret); cudaFree(e->log_ring.len); cudaFree(e->log_ring.count);
+    cudaFree(e->log_cursor); cudaFree(e->log_scratch);
+    for (auto& f : e->log_flushes) cudaEventDestroy(f.done);
+    e->log_flushes.clear();
+    e->log_ring = EpisodeLog{};
+    e->log_cursor = nullptr;
+    e->log_scratch = nullptr;
+}
+
+// the episode log the env's steps write: none while a staged evaluation holds it off
+static EpisodeLog active_log(const b200rl_env* e) { return e->log_held ? EpisodeLog{} : e->log_ring; }
+
+template <class Env, bool RANDOM, bool AUTO> static void launch_step_as(b200rl_env* e, const typename Env::P& p, const void* actions) {
+    const unsigned grid = grid_for(e->N, kBlock);
     cudaStream_t st = e->ctx->stream;
+    const EpisodeLog log = active_log(e);
+    if (log.count) env_step_kernel<Env, RANDOM, AUTO, true><<<grid, kBlock, 0, st>>>(p, EnvArraysLog{e->a, log}, e->N, actions);
+    else env_step_kernel<Env, RANDOM, AUTO, false><<<grid, kBlock, 0, st>>>(p, e->a, e->N, actions);
+}
+template <class Env> static int launch_step(b200rl_env* e, const typename Env::P& p, const void* actions, bool random, bool auto_reset) {
     if (random) {
-        if (auto_reset) env_step_kernel<Env, true, true><<<grid, kBlock, 0, st>>>(p, e->a, e->N, nullptr);
-        else env_step_kernel<Env, true, false><<<grid, kBlock, 0, st>>>(p, e->a, e->N, nullptr);
+        if (auto_reset) launch_step_as<Env, true, true>(e, p, nullptr);
+        else launch_step_as<Env, true, false>(e, p, nullptr);
     } else {
-        if (auto_reset) env_step_kernel<Env, false, true><<<grid, kBlock, 0, st>>>(p, e->a, e->N, actions);
-        else env_step_kernel<Env, false, false><<<grid, kBlock, 0, st>>>(p, e->a, e->N, actions);
+        if (auto_reset) launch_step_as<Env, false, true>(e, p, actions);
+        else launch_step_as<Env, false, false>(e, p, actions);
     }
     LAUNCH_CHECK(e->ctx);
     return B200RL_OK;
@@ -373,6 +483,7 @@ int b200rl_env_destroy(b200rl_env* e) {
     if (e->a.obs != e->a.state) cudaFree(e->a.obs);
     cudaFree(e->a.reward); cudaFree(e->a.flags); cudaFree(e->a.t); cudaFree(e->a.rng); cudaFree(e->a.action);
     cudaFree(e->a.ep_ret); cudaFree(e->a.stats); cudaFree(e->a.err); cudaFree(e->rew_f32);
+    log_free(e);
     delete e;
     return B200RL_OK;
 }
@@ -383,6 +494,8 @@ int b200rl_env_copy(b200rl_env* src, b200rl_env** out) {
     b200rl_env* e = new b200rl_env(*src);
     memset(&e->a, 0, sizeof e->a);
     e->rew_f32 = nullptr;
+    e->log_ring = EpisodeLog{}; e->log_held = false; e->log_cursor = nullptr; e->log_scratch = nullptr;   // (hook data, not env state)
+    e->log_flushes.clear();
     e->a.max_timeout = src->a.max_timeout;
     int s = env_alloc(e);
     if (s != B200RL_OK) { b200rl_env_destroy(e); return s; }
@@ -521,9 +634,108 @@ int b200rl_env_episode_stats(b200rl_env* e, double* out4, int reset_after) {
     return B200RL_OK;
 }
 
+int b200rl_env_episode_log(b200rl_env* e, int32_t K) {
+    REQUIRE(e, B200RL_ERR_INVALID, "null env");
+    REQUIRE(K >= 0 && K <= (1 << 20), B200RL_ERR_INVALID, "K must be in 0 .. 2^20");
+    TRY(ctx_bind(e->ctx));
+    const size_t N = (size_t)e->N, nb = grid_for(e->N, kBlock);
+    cudaStream_t st = e->ctx->stream;
+    if (K > 0 && K == e->log_ring.K) {   // the same ring, emptied: the captured launches that write it stay valid
+        CUDA_TRY(cudaMemsetAsync(e->log_ring.count, 0, N * 4, st));
+        CUDA_TRY(cudaMemsetAsync(e->log_cursor, 0, N * 4, st));
+        CUDA_TRY(cudaMemsetAsync(e->log_scratch, 0, (nb + 1) * sizeof(long long), st));
+        for (auto& f : e->log_flushes) f.buf = nullptr;   // (every buffer starts without a flush)
+        CUDA_TRY(cudaStreamSynchronize(st));
+        return B200RL_OK;
+    }
+    log_free(e);
+    if (K == 0) return B200RL_OK;
+    EpisodeLog& l = e->log_ring;
+    CUDA_TRY_OR(cudaMalloc(&l.ret, N * K * 4), log_free(e));
+    CUDA_TRY_OR(cudaMalloc(&l.len, N * K * 4), log_free(e));
+    CUDA_TRY_OR(cudaMalloc(&l.count, N * 4), log_free(e));
+    CUDA_TRY_OR(cudaMalloc(&e->log_cursor, N * 4), log_free(e));
+    CUDA_TRY_OR(cudaMalloc(&e->log_scratch, (nb + 1) * sizeof(long long)), log_free(e));
+    CUDA_TRY_OR(cudaMemsetAsync(l.count, 0, N * 4, st), log_free(e));
+    CUDA_TRY_OR(cudaMemsetAsync(e->log_cursor, 0, N * 4, st), log_free(e));
+    CUDA_TRY_OR(cudaMemsetAsync(e->log_scratch, 0, (nb + 1) * sizeof(long long), st), log_free(e));
+    // the events of the flushes into two host buffers (what DeviceEpisodeLog uses) are created now: creating one may wait for the
+    // device, and ranks sharing a device must not do that while a peer's kernel waits for them inside an exchange
+    for (int j = 0; j < 2; ++j) {
+        cudaEvent_t ev;
+        CUDA_TRY_OR(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming), log_free(e));
+        e->log_flushes.push_back(b200rl_env::LogFlush{nullptr, 0, ev});
+    }
+    CUDA_TRY_OR(cudaStreamSynchronize(st), log_free(e));
+    l.K = K;
+    return B200RL_OK;
+}
+
+int b200rl_env_episode_log_flush(b200rl_env* e, void* host_buf, int64_t capacity) {
+    REQUIRE(e && host_buf, B200RL_ERR_INVALID, "null argument");
+    REQUIRE(e->log_ring.count, B200RL_ERR_INVALID, "no episode log attached (b200rl_env_episode_log)");
+    REQUIRE(capacity >= 0, B200RL_ERR_INVALID, "capacity must be >= 0");
+    TRY(ctx_bind(e->ctx));
+    cudaPointerAttributes at;
+    CUDA_TRY(cudaPointerGetAttributes(&at, host_buf));
+    REQUIRE(at.type == cudaMemoryTypeHost && at.devicePointer, B200RL_ERR_INVALID, "host_buf must be pinned host memory (b200rl_host_alloc)");
+    b200rl_env::LogFlush* f = nullptr;
+    for (auto& x : e->log_flushes) if (x.buf == host_buf) f = &x;
+    for (auto& x : e->log_flushes) if (!f && !x.buf) { f = &x; f->buf = host_buf; }   // a spare event
+    if (!f) {
+        cudaEvent_t ev;
+        CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        e->log_flushes.push_back(b200rl_env::LogFlush{host_buf, 0, ev});
+        f = &e->log_flushes.back();
+    }
+    f->capacity = capacity;
+    const unsigned nb = grid_for(e->N, kBlock);
+    long long* hdr = (long long*)at.devicePointer;
+    unsigned long long* overflow = (unsigned long long*)(e->log_scratch + nb);
+    cudaStream_t st = e->ctx->stream;
+    log_count_kernel<<<nb, kBlock, 0, st>>>(e->log_ring, e->log_cursor, e->N, e->log_scratch, overflow);
+    LAUNCH_CHECK(e->ctx);
+    log_offsets_kernel<<<1, kBlock, 0, st>>>(e->log_scratch, nb, overflow, hdr);
+    LAUNCH_CHECK(e->ctx);
+    log_scatter_kernel<<<nb, kBlock, 0, st>>>(e->log_ring, e->log_cursor, e->N, e->log_scratch, (int64_t)b200rl_comm_rank(e->ctx) * e->N,
+                                              reinterpret_cast<EpisodeRecord*>(hdr + 2), capacity);
+    LAUNCH_CHECK(e->ctx);
+    CUDA_TRY(cudaEventRecord(f->done, st));
+    return B200RL_OK;
+}
+
+int b200rl_env_episode_log_read(b200rl_env* e, const void* host_buf, int64_t* n_out) {
+    REQUIRE(e && host_buf && n_out, B200RL_ERR_INVALID, "null argument");
+    const b200rl_env::LogFlush* f = nullptr;
+    for (const auto& x : e->log_flushes) if (host_buf && x.buf == host_buf) f = &x;
+    REQUIRE(f, B200RL_ERR_INVALID, "no flush into this buffer since the log was attached");
+    TRY(ctx_bind(e->ctx));
+    CUDA_TRY(cudaEventSynchronize(f->done));
+    const long long* hdr = (const long long*)host_buf;
+    *n_out = hdr[0];
+    if (hdr[1]) {
+        b200rl_set_error("b200rl_env_episode_log_read: %lld of the %lld envs finished more than K = %d episodes between two flushes "
+                         "(records were overwritten before they were read): flush at least every K env steps",
+                         (long long)hdr[1], (long long)e->N, e->log_ring.K);
+        return B200RL_ERR_OVERFLOW;
+    }
+    if (hdr[0] > f->capacity) {
+        b200rl_set_error("b200rl_env_episode_log_read: the flush found %lld records, the buffer holds %lld", (long long)hdr[0],
+                         (long long)f->capacity);
+        return B200RL_ERR_OVERFLOW;
+    }
+    return B200RL_OK;
+}
+
 }  // extern "C"
 
 // internal hooks for other translation units (fused consumers; internal.h)
+void b200rl_env_internal_log_hold(b200rl_env* e, bool hold) { e->log_held = hold; }
+void b200rl_env_internal_log_key(const b200rl_env* e, uint64_t key[4]) {
+    const EpisodeLog l = active_log(e);
+    key[0] = (uint64_t)(uintptr_t)l.ret; key[1] = (uint64_t)(uintptr_t)l.len;
+    key[2] = (uint64_t)(uintptr_t)l.count; key[3] = (uint64_t)l.K;
+}
 int b200rl_env_internal_set_traj_targets(b200rl_env* e, void* reward_col, uint8_t* terminal_col) {
     e->a.traj_reward = reward_col;
     e->a.traj_terminal = terminal_col;
@@ -532,6 +744,7 @@ int b200rl_env_internal_set_traj_targets(b200rl_env* e, void* reward_col, uint8_
 int b200rl_env_internal_view(b200rl_env* e, envdev::EnvView* out) {
     REQUIRE(e && out, B200RL_ERR_INVALID, "null argument");
     out->kind = e->kind; out->dtype = e->dtype; out->continuous = e->continuous ? 1 : 0; out->N = e->N; out->a = e->a;
+    out->log = active_log(e);
     static_assert(sizeof(out->p) == sizeof(e->p), "params union");
     memcpy(&out->p, &e->p, sizeof out->p);
     return B200RL_OK;

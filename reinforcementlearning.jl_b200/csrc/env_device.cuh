@@ -13,6 +13,36 @@
 namespace envdev {
 using jld::Xo;
 
+// b200rl_env_episode_log: a ring of K records per env, (K, N) column-major like the evaluation records, and the number of
+// episodes logged so far; count == null: no log.  Record c of env i sits in slot c % K.
+struct EpisodeLog {
+    float* ret;        // (K, N) the episode's Float32 step-order return (the accumulator of FIELD_EPISODE_RETURN)
+    int32_t* len;      // (K, N) env.t at the end of the episode
+    uint32_t* count;   // (N)
+    int K;
+};
+__device__ __forceinline__ void log_episode(const EpisodeLog& log, int64_t i, float ret, int len) {
+    const uint32_t c = log.count[i];
+    const size_t j = (size_t)log.K * (size_t)i + c % (uint32_t)log.K;
+    log.ret[j] = ret;
+    log.len[j] = len;
+    log.count[i] = c + 1;
+}
+
+// A flush (env.cu) hands over the records logged since the previous one, env by env in episode order: env i has
+// count - cursor of them (the uint32 counters wrap together); more than K means the ring overwrote records nobody read.
+struct EpisodeRecord { int64_t env; float ret; int32_t len; };   // b200rl_episode_record
+__device__ __forceinline__ uint32_t log_pending(const EpisodeLog& log, const uint32_t* cursor, int64_t i) { return log.count[i] - cursor[i]; }
+// env i's n pending records (n <= K) to out[0 .. min(n, room)), tagged with the env's global index
+__device__ __forceinline__ void log_emit(const EpisodeLog& log, const uint32_t* cursor, int64_t i, uint32_t n, int64_t global, EpisodeRecord* out,
+                                         int64_t room) {
+    const uint32_t c0 = cursor[i];
+    for (uint32_t e = 0; e < n && (int64_t)e < room; ++e) {
+        const size_t j = (size_t)log.K * (size_t)i + (c0 + e) % (uint32_t)log.K;
+        out[e] = EpisodeRecord{global, log.ret[j], log.len[j]};
+    }
+}
+
 struct EnvArrays {
     void* state;      // (NS, N) T
     void* obs;        // (NOBS, N) T   (== state when the observation is the state); a Float64 env's Float32 mirror follows it (obs_f32)
@@ -29,6 +59,14 @@ struct EnvArrays {
     uint8_t* traj_terminal;
     int max_timeout;  // MaxTimeoutEnv(env, max_t) (wrappers/MaxTimeoutEnv.jl:17-28); 0 = not wrapped
 };
+// The kernels that write the episode log take it behind their EnvArrays under a template flag LOG: the instantiations without
+// it take EnvArrays alone, the parameters (and so the code) they had before the log existed.
+struct EnvArraysLog : EnvArrays {
+    EpisodeLog log;
+};
+template <bool LOG> using EnvArgs = typename std::conditional<LOG, EnvArraysLog, EnvArrays>::type;
+__device__ __forceinline__ EpisodeLog episode_log_of(const EnvArrays&) { return EpisodeLog{}; }
+__device__ __forceinline__ EpisodeLog episode_log_of(const EnvArraysLog& a) { return a.log; }
 
 __device__ __forceinline__ Xo load_rng(const unsigned long long* rng, int64_t i) {
     const ulonglong2* p = reinterpret_cast<const ulonglong2*>(rng + 4 * i);
@@ -368,16 +406,22 @@ template <class T> struct ActStep {
 // that finishes here — done, and not the terminal state of an env that was not reset since — is added to the caller's tally
 // (fin_cnt, fin_ret, fin_len).  AUTO: a terminating step is followed by MultiThreadEnv's soft reset (reset!(env; is_force = false)):
 // with_rng(f) calls f(Xo&) on the env's stream, which the caller may fetch only then; the reset may redraw `act` (env.action).
-template <class Env, bool AUTO, class WithRng>
+// LOG: the same finished episode is also written to env i's episode log `log` (without it the step is the code it was before
+// the log existed).
+template <class Env, bool AUTO, bool LOG = false, class WithRng>
 __device__ __forceinline__ ActStep<typename Env::real> act_step(const typename Env::P& p, int max_timeout, typename Env::S& s, int& t,
                                                                 int& flags, float& ep_ret, typename Env::act_t& act, int& fin_cnt,
-                                                                float& fin_ret, int& fin_len, WithRng&& with_rng) {
+                                                                float& fin_ret, int& fin_len, WithRng&& with_rng,
+                                                                EpisodeLog log = EpisodeLog{}, int64_t i = 0) {
     ActStep<typename Env::real> r;
     Env::step(p, s, t, act, r.done, r.rew);
     if (max_timeout > 0 && t + 1 > max_timeout) r.done = true;
     r.ret = ep_ret + (float)r.rew;
     r.len = t;
-    if (r.done && !((flags & 1) && !(flags & 2))) { fin_cnt += 1; fin_ret += r.ret; fin_len += t; }
+    if (r.done && !((flags & 1) && !(flags & 2))) {
+        fin_cnt += 1; fin_ret += r.ret; fin_len += t;
+        if constexpr (LOG) log_episode(log, i, r.ret, t);
+    }
     ep_ret = r.done ? 0.f : r.ret;
     flags = r.done ? 1 : 0;
     if (AUTO && r.done) {
@@ -428,6 +472,7 @@ struct EnvView {
     int kind, dtype, continuous;
     int64_t N;
     EnvArrays a;
+    EpisodeLog log;   // the episode log the env's steps write (count == null: none)
     union {
         CartPoleD<float>::P cp32;
         CartPoleD<double>::P cp64;

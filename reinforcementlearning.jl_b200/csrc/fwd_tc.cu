@@ -220,22 +220,22 @@ template <class Env> __device__ __forceinline__ typename Env::act_t env_action(u
     return (act_t)(int32_t)a_bits;
 }
 // act!(env, a) of owner thread s's env in its slot: the act! step of env_step_kernel<Env, false, true>, the fused auto-reset drawing
-// from the slot's env stream, a finished episode added to the thread's tally.  The reward it returns is Float32(reward), what a
-// rollout or the replay ring stores; the slot keeps the env's own.
-template <class Env>
+// from the slot's env stream, a finished episode added to the thread's tally (and to env i's episode log when the caller passes
+// one).  The reward it returns is Float32(reward), what a rollout or the replay ring stores; the slot keeps the env's own.
+template <class Env, bool LOG = false>
 __device__ __forceinline__ ActStep<float> slot_act(EnvSlot<Env>& sl, int s, const typename Env::P& p, int max_timeout, typename Env::act_t act,
-                                                   int& fin_cnt, float& fin_ret, int& fin_len) {
+                                                   int& fin_cnt, float& fin_ret, int& fin_len, EpisodeLog log = EpisodeLog{}, int64_t i = 0) {
     typename Env::S st = sl.st[s];
     int t = sl.t[s], f = sl.flags[s];
     float ret = sl.ep_ret[s];
-    const ActStep<typename Env::real> r = act_step<Env, true>(p, max_timeout, st, t, f, ret, act, fin_cnt, fin_ret, fin_len, [&](auto&& reset) {
+    const ActStep<typename Env::real> r = act_step<Env, true, LOG>(p, max_timeout, st, t, f, ret, act, fin_cnt, fin_ret, fin_len, [&](auto&& reset) {
         unsigned long long w[4];
         get_stream(sl.erng, s, w);
         Xo e{w[0], w[1], w[2], w[3]};
         reset(e);
         const unsigned long long o[4] = {e.s0, e.s1, e.s2, e.s3};
         put_stream(sl.erng, s, o);
-    });
+    }, log, i);
     sl.st[s] = st; sl.t[s] = t; sl.flags[s] = f; sl.ep_ret[s] = ret;
     sl.last_rew[s] = r.rew;
     typename EnvSlot<Env>::act_bits bits;
@@ -306,9 +306,10 @@ struct RollArgs {
     uint8_t* terminals;         // (N, T)
 };
 
-// A CTA owns one group of up to kSlots tiles for the whole launch (the caller bounds N by it).
-template <class Env, int ACT>
-__global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename Env::P p, EnvArrays ea) {
+// A CTA owns one group of up to kSlots tiles for the whole launch (the caller bounds N by it).  LOG: finished episodes are also
+// written to the env's episode log.
+template <class Env, int ACT, bool LOG>
+__global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename Env::P p, EnvArgs<LOG> ea) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     SmemRoll<Env>& sm = *reinterpret_cast<SmemRoll<Env>*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -382,7 +383,7 @@ __global__ void __launch_bounds__(NT, 2) rollout_tc_kernel(RollArgs g, typename 
                 put_stream(sl.prng, s, pr);
                 reinterpret_cast<uint32_t*>(g.actions)[(size_t)N * t + i] = a_bits;
                 g.logp[(size_t)N * t + i] = lp;
-                const ActStep<float> r = slot_act(sl, s, p, ea.max_timeout, env_action<Env>(a_bits), fin_cnt, fin_ret, fin_len);
+                const ActStep<float> r = slot_act<Env, LOG>(sl, s, p, ea.max_timeout, env_action<Env>(a_bits), fin_cnt, fin_ret, fin_len, episode_log_of(ea), i);
                 g.rewards[(size_t)N * t + i] = r.rew;
                 g.terminals[(size_t)N * t + i] = r.done ? 1 : 0;
             }
@@ -518,6 +519,7 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgsOf<MODE> g, 
                         a_bits = policy::sample_head(g.actor.heads2, g.actor.nout, g.hp, z, pr, lp);
                         put_stream(sl.prng, s, pr);
                     }
+                    // (no episode log: an evaluation is a run of its own, whose episodes the training hook does not see)
                     const ActStep<float> r = slot_act(sl, s, p, ea.max_timeout, env_action<Env>(a_bits), sm.fin_cnt[s], sm.fin_ret[s], sm.fin_len[s]);
                     if (r.done) {
                         const int e = sl.cnt[s];   // record of the episode that ends: its return and env.t
@@ -590,9 +592,9 @@ struct ReplayArgs {
 
 // DUEL: a dueling Q-network, its head rows combined into Q (duel.cuh) before the selection (the instantiations without it are the
 // code of a plain Q-network).  XEXT: the explorer kinds 2-4 (speedy, weighted / Gumbel softmax; explore::select<true>) — the
-// instantiations without it compile the ϵ-greedy kinds 0 / 1 only.
-template <class Env, int ACT, bool DUEL = false, bool XEXT = false>
-__global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, typename Env::P p, EnvArrays ea, double beta) {
+// instantiations without it compile the ϵ-greedy kinds 0 / 1 only.  LOG: finished episodes are also written to the env's episode log.
+template <class Env, int ACT, bool DUEL, bool XEXT, bool LOG>
+__global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, typename Env::P p, EnvArgs<LOG> ea, double beta) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     SmemReplay<Env>& sm = *reinterpret_cast<SmemReplay<Env>*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -653,7 +655,7 @@ __global__ void __launch_bounds__(NT, 2) replay_collect_tc_kernel(ReplayArgs g, 
                     if (DUEL) duel::combine(z, g.q.nout);
                     const int a1 = plan_q_column<XEXT>(g.greedy, g.ex, beta, explore::column_step(step0, g.col0, g.xstride, step, i), z, g.q.nout,
                                                                 sl.xrng, s);
-                    const ActStep<float> res = slot_act(sl, s, p, ea.max_timeout, (typename Env::act_t)a1, sm.fin_cnt[s], sm.fin_ret[s], sm.fin_len[s]);
+                    const ActStep<float> res = slot_act<Env, LOG>(sl, s, p, ea.max_timeout, (typename Env::act_t)a1, sm.fin_cnt[s], sm.fin_ret[s], sm.fin_len[s], episode_log_of(ea), i);
                     // push!(trajectory, (state = s', action = env.action, reward, terminal)) of lane i
                     float nobs[kInMax];
                     Env::observe(sl.st[s], nobs);
@@ -757,15 +759,26 @@ int launch_evaluate(b200rl_ctx* ctx, int64_t groups, const EvalArgsOf<MODE>& g, 
                 : launch_fused<evaluate_tc_kernel<Env, TANH, MODE, false, XEXT>, SmemEval<Env>>(ctx, groups, g, p, ea);
 }
 
-template <class Env, bool XEXT>
-int launch_replay_collect(b200rl_ctx* ctx, int64_t groups, const ReplayArgs& g, const typename Env::P& p, const EnvArrays& ea, double beta) {
+template <class Env, bool XEXT, bool LOG>
+int launch_replay_collect(b200rl_ctx* ctx, int64_t groups, const ReplayArgs& g, const typename Env::P& p, const EnvArgs<LOG>& ea, double beta) {
     constexpr int RELU = B200RL_ACT_RELU, TANH = B200RL_ACT_TANH;
     const bool relu = g.q.act == RELU;
     if (g.q.duel)
-        return relu ? launch_fused<replay_collect_tc_kernel<Env, RELU, true, XEXT>, SmemReplay<Env>>(ctx, groups, g, p, ea, beta)
-                    : launch_fused<replay_collect_tc_kernel<Env, TANH, true, XEXT>, SmemReplay<Env>>(ctx, groups, g, p, ea, beta);
-    return relu ? launch_fused<replay_collect_tc_kernel<Env, RELU, false, XEXT>, SmemReplay<Env>>(ctx, groups, g, p, ea, beta)
-                : launch_fused<replay_collect_tc_kernel<Env, TANH, false, XEXT>, SmemReplay<Env>>(ctx, groups, g, p, ea, beta);
+        return relu ? launch_fused<replay_collect_tc_kernel<Env, RELU, true, XEXT, LOG>, SmemReplay<Env>>(ctx, groups, g, p, ea, beta)
+                    : launch_fused<replay_collect_tc_kernel<Env, TANH, true, XEXT, LOG>, SmemReplay<Env>>(ctx, groups, g, p, ea, beta);
+    return relu ? launch_fused<replay_collect_tc_kernel<Env, RELU, false, XEXT, LOG>, SmemReplay<Env>>(ctx, groups, g, p, ea, beta)
+                : launch_fused<replay_collect_tc_kernel<Env, TANH, false, XEXT, LOG>, SmemReplay<Env>>(ctx, groups, g, p, ea, beta);
+}
+// the instantiation with the episode log when the env has one attached, the one without it otherwise
+template <class Env, bool XEXT>
+int launch_replay_collect(b200rl_ctx* ctx, int64_t groups, const ReplayArgs& g, const typename Env::P& p, const EnvView& v, double beta) {
+    if (v.log.count) return launch_replay_collect<Env, XEXT, true>(ctx, groups, g, p, EnvArraysLog{v.a, v.log}, beta);
+    return launch_replay_collect<Env, XEXT, false>(ctx, groups, g, p, v.a, beta);
+}
+template <class Env, int ACT>
+int launch_rollout(b200rl_ctx* ctx, int64_t ntiles, const RollArgs& g, const typename Env::P& p, const EnvView& v) {
+    if (v.log.count) return launch_fused<rollout_tc_kernel<Env, ACT, true>, SmemRoll<Env>>(ctx, ntiles, g, p, EnvArraysLog{v.a, v.log});
+    return launch_fused<rollout_tc_kernel<Env, ACT, false>, SmemRoll<Env>>(ctx, ntiles, g, p, v.a);
 }
 
 }  // namespace
@@ -811,8 +824,8 @@ int nn_tc_rollout(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const 
     const int st = with_learner_env(v, [&](auto env_type, const auto& p) {
         using Env = typename decltype(env_type)::type;
         // the activation is a template parameter (both trunks share it, checked above)
-        return actor.act == B200RL_ACT_RELU ? launch_fused<rollout_tc_kernel<Env, B200RL_ACT_RELU>, SmemRoll<Env>>(ctx, ntiles, g, p, v.a)
-                                            : launch_fused<rollout_tc_kernel<Env, B200RL_ACT_TANH>, SmemRoll<Env>>(ctx, ntiles, g, p, v.a);
+        return actor.act == B200RL_ACT_RELU ? launch_rollout<Env, B200RL_ACT_RELU>(ctx, ntiles, g, p, v)
+                                            : launch_rollout<Env, B200RL_ACT_TANH>(ctx, ntiles, g, p, v);
     });
     if (st == B200RL_OK) b200rl_env_internal_add_steps(env, (uint64_t)nsteps);
     return st;
@@ -859,8 +872,8 @@ int nn_tc_replay_collect(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& q, con
     const int st = with_learner_env(v, [&](auto env_type, const auto& p) {
         using Env = typename decltype(env_type)::type;
         if constexpr (std::is_floating_point<typename Env::act_t>::value) return (int)B200RL_ERR_UNSUPPORTED;   // (rejected above)
-        else if (!g.greedy && g.ex.kind >= 2) return launch_replay_collect<Env, true>(ctx, groups, g, p, v.a, e.beta);
-        else return launch_replay_collect<Env, false>(ctx, groups, g, p, v.a, 0.0);
+        else if (!g.greedy && g.ex.kind >= 2) return launch_replay_collect<Env, true>(ctx, groups, g, p, v, e.beta);
+        else return launch_replay_collect<Env, false>(ctx, groups, g, p, v, 0.0);
     });
     if (st == B200RL_OK) b200rl_env_internal_add_steps(env, (uint64_t)nsteps);
     return st;

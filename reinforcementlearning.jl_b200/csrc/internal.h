@@ -13,6 +13,10 @@ int b200rl_env_internal_view(b200rl_env* e, envdev::EnvView* out);
 void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n);
 uint64_t b200rl_env_internal_steps(const b200rl_env* e);
 int b200rl_env_internal_max_timeout(const b200rl_env* e);
+// hold = true: the env's kernels stop writing its episode log (a staged evaluation is not logged); false: they write it again
+void b200rl_env_internal_log_hold(b200rl_env* e, bool hold);
+// the episode log the env's kernels write (all zero: none) as {ret, len, count, K} — captured launches bake it in
+void b200rl_env_internal_log_key(const b200rl_env* e, uint64_t key[4]);
 // StateTransformedEnv(env, Float32) in effect: a Float64 env with the wrapper (on a Float32 env the wrapper changes nothing)
 bool b200rl_env_internal_state_f32(const b200rl_env* e);
 // the Float32 observation (NOBS, N) the networks read: FIELD_OBS of a Float32 env, the mirror of a Float64 env wrapped by

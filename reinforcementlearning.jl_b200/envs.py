@@ -204,6 +204,28 @@ class B200VecEnv:
         L.check(self.lib.b200rl_env_episode_stats(self.h, L.ptr(out), int(reset)))
         return {"episodes": int(out[0]), "return_sum": out[1], "length_sum": out[2], "env_steps": int(out[3])}
 
+    # ---- device episode log (b200rl_env_episode_log) -----------------------------------
+    EPISODE_RECORD = np.dtype([("env", "<i8"), ("ret", "<f4"), ("len", "<i4")])   # b200rl_episode_record
+
+    def episode_log(self, K):
+        """Attach a ring of K {return, length} records per env, written by every step that ends an episode (K = 0 detaches)."""
+        L.check(self.lib.b200rl_env_episode_log(self.h, int(K)))
+
+    def episode_log_buffer(self, capacity):
+        """Pinned host buffer for flushes of up to ``capacity`` records: (array view, address); free with ctx.host_free."""
+        return self.ctx.host_alloc((16 + 16 * int(capacity),), np.uint8)
+
+    def episode_log_flush(self, buf, capacity):
+        """Start handing the records logged since the previous flush to the pinned buffer ``buf`` (an address); no sync."""
+        L.check(self.lib.b200rl_env_episode_log_flush(self.h, C.c_void_p(buf), int(capacity)))
+
+    def episode_log_read(self, buf_arr, buf):
+        """Wait for the last flush into ``buf`` and return its records (EPISODE_RECORD, ordered by env then episode; a copy).
+        Raises (ERR_OVERFLOW) when an env finished more than K episodes between two flushes."""
+        n = C.c_int64()
+        L.check(self.lib.b200rl_env_episode_log_read(self.h, C.c_void_p(buf), C.byref(n)))
+        return buf_arr[16:16 + 16 * n.value].view(self.EPISODE_RECORD).copy()
+
     # ---- spaces (shape information only) ---------------------------------------------
     def action_space(self):
         if self.kind == L.ENV_CARTPOLE:

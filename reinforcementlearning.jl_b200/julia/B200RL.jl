@@ -29,7 +29,7 @@ using ReinforcementLearningCore: AbstractStage, PreExperimentStage, PostExperime
     EpsilonGreedyExplorer, GreedyExplorer, AbstractExplorer, WeightedSoftmaxExplorer, GumbelSoftmaxExplorer
 
 export B200Context, B200VecEnv, B200Network, B200OnPolicyAgent, B200RandomPolicy, B200Trajectory, B200DQNLearner, B200QBasedPolicy,
-    B200Agent, B200EpisodeStats, InsertSampleRatio, B200GreedyPolicy, evaluate, replay!, set_nstep!
+    B200Agent, B200EpisodeStats, B200EpisodeLog, InsertSampleRatio, B200GreedyPolicy, evaluate, replay!, set_nstep!
 
 const LIB = get(ENV, "B200RL_LIB", joinpath(@__DIR__, "..", "libb200rl.so"))
 
@@ -238,6 +238,77 @@ end
 Base.push!(h::B200EpisodeStats, ::PreExperimentStage, ::AbstractPolicy, env::B200VecEnv) = (episode_stats(env; reset = true); nothing)
 Base.push!(h::B200EpisodeStats, ::PostExperimentStage, ::AbstractPolicy, env::B200VecEnv) = (h.stats = episode_stats(env); nothing)
 
+"""
+    B200EpisodeLog(batchsize; capacity = 64)
+
+`TotalRewardPerEpisode` + `BatchStepsPerEpisode` (hooks.jl:146-231) kept on the device (b200rl_env_episode_log): `rewards` and
+`steps` are per-env vectors, filled from a ring of `capacity` records per env without a host copy per step.  `_run` splits its
+fused loops into windows of at most `capacity` env steps and flushes after each; the stage loop flushes every `capacity`
+`PostActStage` pushes.  A flush is read one flush later (or at `PostExperimentStage`).  Returns are the env's Float32 step-order
+sums; `evaluate` is not logged; on a sharded ctx the records carry `rank * N + i` and the vectors are indexed by the local env.
+`hook[]` = (rewards, steps).
+"""
+mutable struct B200EpisodeLog <: AbstractHook
+    rewards::Vector{Vector{Float32}}
+    steps::Vector{Vector{Int}}
+    capacity::Int
+    env::Union{Nothing,B200VecEnv}
+    bufs::Vector{Ptr{Cvoid}}     # two pinned buffers of 16 + 16 * N * capacity bytes
+    next::Int
+    pending::Int                 # buffer whose flush is not read yet (0: none)
+    acts::Int
+    base::Int                    # rank * N
+    B200EpisodeLog(batchsize::Integer; capacity::Integer = 64) =
+        new([Float32[] for _ in 1:batchsize], [Int[] for _ in 1:batchsize], capacity, nothing, Ptr{Cvoid}[], 1, 0, 0, 0)
+end
+Base.getindex(h::B200EpisodeLog) = (h.rewards, h.steps)
+log_records(h::B200EpisodeLog) = h.env.n * h.capacity
+function log_detach!(h::B200EpisodeLog)
+    h.env === nothing && return
+    check(ccall((:b200rl_env_episode_log, LIB), Cint, (Ptr{Cvoid}, Int32), h.env.h, 0))
+    foreach(b -> check(ccall((:b200rl_host_free, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}), h.env.ctx.h, b)), h.bufs)
+    h.env, h.bufs = nothing, Ptr{Cvoid}[]
+end
+function log_read!(h::B200EpisodeLog)
+    h.pending == 0 && return
+    buf, n = h.bufs[h.pending], Ref{Int64}(0)
+    h.pending = 0
+    check(ccall((:b200rl_env_episode_log_read, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ref{Int64}), h.env.h, buf, n))
+    for k in 0:n[]-1                                      # b200rl_episode_record: int64 env, float32 ret, int32 len
+        rec = buf + 16 + 16k
+        i = unsafe_load(Ptr{Int64}(rec)) - h.base + 1
+        push!(h.rewards[i], unsafe_load(Ptr{Float32}(rec + 8)))
+        push!(h.steps[i], Int(unsafe_load(Ptr{Int32}(rec + 12))))
+    end
+end
+function log_flush!(h::B200EpisodeLog)
+    h.env === nothing && return
+    check(ccall((:b200rl_env_episode_log_flush, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Int64), h.env.h, h.bufs[h.next], log_records(h)))
+    log_read!(h)
+    h.pending, h.next, h.acts = h.next, 3 - h.next, 0
+end
+function Base.push!(h::B200EpisodeLog, ::PreExperimentStage, ::AbstractPolicy, env::B200VecEnv)
+    log_detach!(h)
+    check(ccall((:b200rl_env_episode_log, LIB), Cint, (Ptr{Cvoid}, Int32), env.h, h.capacity))
+    h.env = env
+    rank, world = Ref{Cint}(0), Ref{Cint}(1)
+    check(ccall((:b200rl_comm_rank_world, LIB), Cint, (Ptr{Cvoid}, Ref{Cint}, Ref{Cint}), env.ctx.h, rank, world))
+    h.base = rank[] * env.n
+    h.bufs = map(1:2) do _
+        p = Ref{Ptr{Cvoid}}(C_NULL)
+        check(ccall((:b200rl_host_alloc, LIB), Cint, (Ptr{Cvoid}, Csize_t, Ref{Ptr{Cvoid}}), env.ctx.h, 16 + 16 * log_records(h), p))
+        p[]
+    end
+    h.next, h.pending, h.acts = 1, 0, 0
+    nothing
+end
+function Base.push!(h::B200EpisodeLog, ::PostActStage, ::AbstractPolicy, ::B200VecEnv)
+    h.acts += 1
+    h.acts >= h.capacity && log_flush!(h)
+    nothing
+end
+Base.push!(h::B200EpisodeLog, ::PostExperimentStage, ::AbstractPolicy, ::B200VecEnv) = (log_flush!(h); log_read!(h); log_detach!(h); nothing)
+
 # ---- run-loop impedance (SURVEY §7 "Run-loop impedance") --------------------------------------
 # the kernel resets finished sub-envs itself; the scalar reset condition must never fire
 RLCore.check!(::ResetIfEnvTerminated, ::AbstractPolicy, ::B200VecEnv) = false
@@ -262,11 +333,14 @@ function RLCore._run(policy::AbstractPolicy, env::B200VecEnv, stop_condition::Ab
     # Fused fast path (the Python mirror's run(), core.py): a device-resident on-policy agent, a hook with nothing to do per
     # step and a step-count stop condition let whole stretches of the loop run as ONE kernel launch (b200rl_onpolicy_collect:
     # n x {plan!, act!, push!}) — the same transitions, parameters and statistics as stepping through the stages.
-    if policy isa B200OnPolicyAgent && policy.fused && env.auto_reset && hook isa Union{B200EpisodeStats,RLCore.EmptyHook} &&
+    # A B200EpisodeLog of capacity K: windows of at most K env steps, each followed by a flush of the log.
+    window = hook isa B200EpisodeLog ? hook.capacity : typemax(Int)
+    if policy isa B200OnPolicyAgent && policy.fused && env.auto_reset && hook isa Union{B200EpisodeStats,B200EpisodeLog,RLCore.EmptyHook} &&
        stop_condition isa StopAfterNSteps && reset_condition isa ResetIfEnvTerminated
         while true                                                  # StopAfterNSteps: check! is true once cur >= step, then cur += 1
-            n = min(policy.T - policy.t, max(1, stop_condition.step - stop_condition.cur + 1))
+            n = min(policy.T - policy.t, max(1, stop_condition.step - stop_condition.cur + 1), window)
             collect!(policy, n)
+            hook isa B200EpisodeLog && log_flush!(hook)
             RLBase.optimise!(policy, PostActStage())
             stop_condition.cur += n
             stop_condition.progress === nothing || RLCore.ProgressMeter.update!(stop_condition.progress, min(stop_condition.cur, stop_condition.step))
@@ -278,9 +352,18 @@ function RLCore._run(policy::AbstractPolicy, env::B200VecEnv, stop_condition::Ab
         return hook
     end
     # the replay agent's device loop (Python: Agent.run_replay): the whole window in one replay! call
-    if policy isa B200Agent && hook isa Union{B200EpisodeStats,RLCore.EmptyHook} && stop_condition isa StopAfterNSteps &&
-       reset_condition isa ResetIfEnvTerminated && replay!(policy, env, max(1, stop_condition.step - stop_condition.cur + 1))
-        stop_condition.cur += max(1, stop_condition.step - stop_condition.cur + 1)
+    n_replay = max(1, stop_condition isa StopAfterNSteps ? stop_condition.step - stop_condition.cur + 1 : 1)
+    if policy isa B200Agent && hook isa Union{B200EpisodeStats,B200EpisodeLog,RLCore.EmptyHook} && stop_condition isa StopAfterNSteps &&
+       reset_condition isa ResetIfEnvTerminated && replay!(policy, env, min(n_replay, window))
+        if hook isa B200EpisodeLog
+            log_flush!(hook)
+            for j in window+1:window:n_replay                      # the remaining windows of the log
+                replay!(policy, env, min(window, n_replay - j + 1)) ||
+                    error("replay!: a window after the first was refused (the env or trajectory changed during the run)")
+                log_flush!(hook)
+            end
+        end
+        stop_condition.cur += n_replay
         push!(policy, PostExperimentStage(), env)
         push!(hook, PostExperimentStage(), policy, env)
         check(ccall((:b200rl_env_check, LIB), Cint, (Ptr{Cvoid},), env.h))
