@@ -434,6 +434,22 @@ int b200rl_onpolicy_update(b200rl_onpolicy* agent, const int32_t* perm_host, flo
  * update_freq steps) when no host-side hook needs per-step data. */
 int b200rl_onpolicy_iterate(b200rl_onpolicy* agent, int n_iters, float* stats_host);
 int b200rl_onpolicy_graph_active(b200rl_onpolicy* agent, int* out);   /* 1: iterate replays a captured graph */
+/* run(agent, env, StopAfterNEpisodes(k)) (RLCore/src/core/stop_conditions.jl:82-118, batched: every lane whose is_terminated is
+ * true after a step counts one episode, a MaxTimeoutEnv cut included) on the fused path, for at most max_steps env steps.
+ * budget = k - cur.  The loop runs steps 1 .. s*, s* = the first step after which the episodes counted reach budget (a budget
+ * <= 0: exactly one step, as the stage loop checks only after a step), or max_steps steps when the budget is not reached.
+ * *steps_done = steps run, *episodes_done = episodes those steps ended (>= budget when the budget was reached; may overshoot it).
+ * The result equals the stage loop's (plan!, act!, push!, optimise!, check per step) bit for bit: a rollout completed by step s*
+ * is updated; one that s* falls inside stays part-filled (b200rl_onpolicy_fill), and the next call continues it.
+ * How: each stretch (the rest of the rollout) that could reach the budget (N · steps >= budget - episodes so far) first copies the
+ * env arrays, policy streams and rollout columns to a shadow (allocated by the agent's first call, then kept:
+ * about the rollout's size again); a counting kernel reduces the stretch's terminal
+ * columns per step and finds the crossing; a crossing before the stretch's last step restores the shadow and runs collect(s*).
+ * One synchronisation per stretch; whole rollouts that cannot reach the budget run as b200rl_onpolicy_iterate.  max_steps: the
+ * longest window between two flushes of an episode log.  stats_host: as b200rl_onpolicy_iterate, rows of the last update run
+ * (untouched when none ran).  A sharded ctx (world > 1) is refused with B200RL_ERR_UNSUPPORTED before any side effect. */
+int b200rl_onpolicy_run_episodes(b200rl_onpolicy* agent, int64_t max_steps, int64_t budget, float* stats_host, int64_t* steps_done,
+                                 int64_t* episodes_done);
 /* field: 0 state (ns,N,T+1) | 1 action | 2 logp | 3 reward | 4 terminal u8 | 5 value (N,T+1) |
  * 6 advantage | 7 return | 8 policy rng (4,N) u64 | 9 {adv mean, inv std} */
 int b200rl_onpolicy_get(b200rl_onpolicy* agent, int field, void* host_dst, size_t bytes);
@@ -510,6 +526,18 @@ int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl
  * advanced and *ex / *ctl NOT advanced: the run cannot be continued from them. */
 int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explorer* ex, b200rl_insert_sample_ratio* ctl,
                       int64_t n_steps, float* stats4);
+/* run(Agent(QBasedPolicy(DQNLearner, explorer), Trajectory), env, StopAfterNEpisodes(k)) on the device, for at most max_steps env
+ * steps: steps, budget (= k - cur), *steps_done and *episodes_done as b200rl_onpolicy_run_episodes.  Step s* runs with its updates,
+ * target sync and controller / explorer counters: what b200rl_replay_run(s*) does.  Chunks of at most min(capacity / 2, 2048)
+ * steps (the ring then still holds every frame a chunk pushed) run as b200rl_replay_run; a chunk that could reach the budget first
+ * copies the env arrays, the ring (frames, heads, counts, sum tree, sampler streams), the explorer streams and the Q-network
+ * (parameters, Adam moments, beta^t, target, last loss / TD) to a shadow allocated by the handle's first call and kept
+ * (about the ring's size again: a configuration near the device's memory can fail here with B200RL_ERR_OOM).  A counting kernel reduces the
+ * terminal flags the chunk pushed per step; a crossing before the chunk's last step restores the shadow and the host counters
+ * (*ex, *ctl, update and step counters) and runs b200rl_replay_run(s*).  stats4: as b200rl_replay_run, for the last update run.
+ * A sharded ctx (world > 1) is refused with B200RL_ERR_UNSUPPORTED before any side effect. */
+int b200rl_replay_run_episodes(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explorer* ex, b200rl_insert_sample_ratio* ctl,
+                               int64_t max_steps, int64_t budget, float* stats4, int64_t* steps_done, int64_t* episodes_done);
 int b200rl_replay_graph_active(b200rl_replay* r, int* out);   /* 1: a "1 step + m updates" unit has been captured and replayed */
 int b200rl_replay_destroy(b200rl_replay* r);
 

@@ -173,6 +173,7 @@ SIGNATURES = {
     "b200rl_onpolicy_update": (_i32, [_vp, _vp, _vp]),
     "b200rl_onpolicy_iterate": (_i32, [_vp, _i32, _vp]),
     "b200rl_onpolicy_graph_active": (_i32, [_vp, C.POINTER(_i32)]),
+    "b200rl_onpolicy_run_episodes": (_i32, [_vp, _i64, _i64, _vp, C.POINTER(_i64), C.POINTER(_i64)]),
     "b200rl_onpolicy_get": (_i32, [_vp, _i32, _vp, _sz]),
     "b200rl_onpolicy_set": (_i32, [_vp, _i32, _vp, _sz]),
     "b200rl_onpolicy_export_state": (_i32, [_vp, _vp]),
@@ -182,6 +183,7 @@ SIGNATURES = {
     "b200rl_dqn_last_td": (_i32, [_vp, _vp, _vp, _i64]),
     "b200rl_replay_create": (_i32, [_vp, _vp, _vp, _vp, _vp, _pp]),
     "b200rl_replay_run": (_i32, [_vp, _vp, _vp, _vp, _i64, _vp]),
+    "b200rl_replay_run_episodes": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _vp, C.POINTER(_i64), C.POINTER(_i64)]),
     "b200rl_replay_graph_active": (_i32, [_vp, C.POINTER(_i32)]),
     "b200rl_replay_destroy": (_i32, [_vp]),
     "b200rl_set_tensor_cores": (_i32, [_i32]),

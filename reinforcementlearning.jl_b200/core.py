@@ -281,6 +281,29 @@ def _flush(logs):
         h.flush()
 
 
+def _run_episodes_fused(policy, env, stop_condition, hook):
+    """StopAfterNEpisodes on the fused paths: windows of at most the episode log's capacity, each one library call that stops
+    at the crossing of the remaining budget, followed by a flush.  Returns False (nothing run) where the stage loop keeps the
+    run: a sharded ctx (the stop would count the episodes of every rank), a replay agent the device loop does not take."""
+    if env.ctx.rank_world()[1] > 1:
+        return False
+    if hasattr(policy, "run_replay"):
+        if not policy.replay_supported(env):
+            return False
+        step = lambda n, budget: policy.run_replay_episodes(env, n, budget)
+    elif hasattr(policy, "run_episodes"):
+        step = policy.run_episodes
+    else:
+        return False
+    logs, window = _episode_log_window(hook)
+    while True:
+        _, episodes = step(window or (1 << 62), stop_condition.episode - stop_condition.cur)
+        stop_condition.cur += episodes
+        _flush(logs)
+        if stop_condition.cur >= stop_condition.episode:
+            return True
+
+
 class TimePerStep(AbstractHook):
     """hooks.jl:243-262 (wall-clock per loop iteration)."""
 
@@ -522,6 +545,11 @@ def run(policy, env=None, stop_condition=None, hook=None, reset_condition=None):
                     policy._t = 0
                     policy.update(want_stats=policy.fetch_stats)
                 is_stop = stop_condition.advance(n)
+    # The same fused paths for an episode-count stop condition: the loop runs ahead stretch by stretch, counts the episodes on the
+    # device and stops after exactly the step the stage loop would stop after (b200rl_*_run_episodes), with the same state.
+    if (getattr(policy, "fusable", False) and env.auto_reset and not getattr(hook, "per_step", True)
+            and isinstance(stop_condition, StopAfterNEpisodes) and isinstance(reset_condition, ResetIfEnvTerminated)):
+        is_stop = _run_episodes_fused(policy, env, stop_condition, hook)
     def act(action):
         if isinstance(action, FusedAction):
             if action.kind == "random":

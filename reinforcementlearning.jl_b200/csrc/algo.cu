@@ -16,6 +16,7 @@
 #include "nn.cuh"
 #include "replay_schedule.h"
 #include "ring.cuh"
+#include "stop_episodes.cuh"
 
 static void* env_field(b200rl_env* e, int f) { void* p = nullptr; b200rl_env_ptr(e, f, &p); return p; }
 // the observation the networks read; refuses a Float64 env that is not wrapped by b200rl_env_set_state_f32 (and Acrobot)
@@ -261,6 +262,66 @@ public:
         return B200RL_OK;
     }
 };
+
+// ------------------------------------------------------------------ StopAfterNEpisodes ------
+// b200rl_onpolicy_run_episodes / b200rl_replay_run_episodes run a stretch of steps ahead and roll it back when the episode budget
+// is reached inside it (stop_episodes.cuh).  Shadow: the device state such a stretch changes, copied aside before it (mark) and
+// copied back (restore) in one launch each.  Its buffer is allocated by the handle's first run_episodes call (stop_buffers).
+static size_t round256(size_t b) { return (b + 255) / 256 * 256; }
+struct Shadow {
+    char* buf = nullptr;
+    size_t cap = 0, used = 0;
+    stop::Regions g{};
+    void clear() { g.n = 0; used = 0; }
+    int add(void* p, size_t bytes) {
+        REQUIRE(g.n < stop::kMaxRegions && used + round256(bytes) <= cap, B200RL_ERR_INVALID, "shadow buffer too small");
+        g.state[g.n] = (char*)p; g.shadow[g.n] = buf + used; g.bytes[g.n] = bytes;
+        ++g.n; used += round256(bytes);
+        return B200RL_OK;
+    }
+    int add_regions(const DevRegion* r, int n) {
+        for (int k = 0; k < n; ++k) TRY(add(r[k].p, r[k].bytes));
+        return B200RL_OK;
+    }
+    int copy(b200rl_ctx* ctx, bool to_shadow) const {
+        size_t most = 0;
+        for (int k = 0; k < g.n; ++k) most = g.bytes[k] > most ? g.bytes[k] : most;
+        if (!g.n || !most) return B200RL_OK;
+        const unsigned cap_x = (unsigned)(4 * (ctx->sm_count > 0 ? ctx->sm_count : 132));
+        unsigned x = grid_for((int64_t)((most + 15) / 16), 256);
+        stop::copy_regions_kernel<<<dim3(x < cap_x ? x : cap_x, (unsigned)g.n), 256, 0, ctx->stream>>>(g, to_shadow ? 1 : 0);
+        LAUNCH_CHECK(ctx);
+        return B200RL_OK;
+    }
+};
+// Per-step counts of one stretch and its crossing: `counts` (s + 2 entries; the last two receive {s*, episodes}) is zeroed, `count`
+// launches the counting kernel, the crossing is read back through the pinned pair `host` (synchronises: once per stretch).
+template <class Count>
+static int stop_crossing(b200rl_ctx* ctx, unsigned long long* counts, int64_t s, int64_t remaining, long long* host, Count&& count,
+                         StopCrossing* out) {
+    CUDA_TRY(cudaMemsetAsync(counts, 0, (size_t)s * sizeof(unsigned long long), ctx->stream));
+    TRY(count());
+    long long* dev_out = (long long*)(counts + s);
+    stop::crossing_kernel<<<1, 1, 0, ctx->stream>>>(counts, s, remaining, dev_out);
+    LAUNCH_CHECK(ctx);
+    CUDA_TRY(cudaMemcpyAsync(host, dev_out, 2 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    *out = StopCrossing{host[0], host[1]};
+    return B200RL_OK;
+}
+
+// The buffers of b200rl_*_run_episodes, allocated by the first call and kept with the handle (an agent that never stops on an episode
+// count holds none; later calls allocate nothing): the shadow (`shadow_bytes`), `n_counts` per-step counts + {s*, episodes}, the
+// pinned pair.
+static int stop_buffers(b200rl_ctx* ctx, Shadow& sh, size_t shadow_bytes, unsigned long long** counts, int64_t n_counts, long long** host) {
+    if (sh.buf) return B200RL_OK;
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    CUDA_TRY(cudaMalloc(counts, (size_t)(n_counts + 2) * sizeof(unsigned long long)));
+    CUDA_TRY(cudaHostAlloc(host, 2 * sizeof(long long), cudaHostAllocDefault));
+    CUDA_TRY(cudaMalloc(&sh.buf, shadow_bytes));
+    sh.cap = shadow_bytes;
+    return B200RL_OK;
+}
 
 // kinds 2 and 3 are Q-networks (one flat vector, a target network, the DQN entry points); 0 and 1 actor-critic pairs
 static bool is_q_kind(int kind) { return kind == 2 || kind == 3; }
@@ -787,6 +848,9 @@ struct b200rl_onpolicy {
     unsigned int* upd_dev;       // device copy of n_updates: keys the minibatch permutation, ticked by the last optimiser step of an update
     uint64_t n_updates;
     GraphUnit graph;             // one whole iteration (collect(T) + update) for b200rl_onpolicy_iterate
+    Shadow shadow;               // b200rl_onpolicy_run_episodes (allocated by its first call): env arrays, policy streams and rollout columns
+    unsigned long long* stop_counts;   // (T + 2) per-step terminal counts of a stretch, then {s*, episodes}
+    long long* stop_host;        // pinned {s*, episodes}
 };
 
 // the (n_epochs * n_microbatches, 6) stats rows of the last update (synchronises)
@@ -828,6 +892,7 @@ int b200rl_onpolicy_destroy(b200rl_onpolicy* a) {
     cudaFree(a->rng); cudaFree(a->states); cudaFree(a->actions); cudaFree(a->logp); cudaFree(a->rewards); cudaFree(a->terminals);
     cudaFree(a->values); cudaFree(a->adv); cudaFree(a->ret); cudaFree(a->act_clamped); cudaFree(a->norm_partials); cudaFree(a->norm_sums);
     cudaFree(a->norm2); cudaFree(a->perm_dev); cudaFree(a->stats_dev); cudaFree(a->rec); cudaFree(a->upd_dev);
+    cudaFree(a->shadow.buf); cudaFree(a->stop_counts); cudaFreeHost(a->stop_host);
     delete a;
     return B200RL_OK;
 }
@@ -1076,6 +1141,88 @@ int b200rl_onpolicy_iterate(b200rl_onpolicy* a, int n_iters, float* stats_host) 
     if (stats_host && n_iters > 0) TRY(read_stats(a, stats_host));
     return B200RL_OK;
 }
+/* run(agent, env, StopAfterNEpisodes(k)) for at most max_steps env steps (include/b200rl.h).  One stretch = the rest of the
+ * rollout (collect(T - t), capped by max_steps).  A stretch that could reach the budget (N · s >= budget - episodes so far) is
+ * marked first; the terminal columns it wrote are counted; if the budget is reached before its last step, the mark is restored
+ * and collect(s*) runs instead.  A full rollout is updated, as optimise! at the PostActStage of its last step would; the update
+ * of a stretch that could reach the budget runs only after the count, so the network never needs a shadow. */
+int b200rl_onpolicy_run_episodes(b200rl_onpolicy* a, int64_t max_steps, int64_t budget, float* stats_host, int64_t* steps_done,
+                                 int64_t* episodes_done) {
+    REQUIRE(a && steps_done && episodes_done && max_steps >= 1, B200RL_ERR_INVALID, "bad argument");
+    REQUIRE(b200rl_comm_world(a->ctx) == 1, B200RL_ERR_UNSUPPORTED,
+            "StopAfterNEpisodes counts the episodes of every rank: a sharded ctx keeps the stage loop");
+    const float* obs;
+    TRY(learner_obs(a->env, &obs));
+    TRY(ctx_bind(a->ctx));
+    b200rl_ctx* ctx = a->ctx;
+    {
+        size_t bytes = b200rl_env_internal_step_bytes_max(a->env) + round256((size_t)a->N * 32);
+        for (int f = 0; f <= 5; ++f) {
+            void* p; size_t b;
+            TRY(rollout_field(a, f, &p, &b));
+            bytes += round256(b);
+        }
+        TRY(stop_buffers(ctx, a->shadow, bytes, &a->stop_counts, a->T, &a->stop_host));
+    }
+    int64_t done = 0, episodes = 0;
+    bool updated = false;
+    while (done < max_steps) {
+        const int64_t left = max_steps - done;
+        const int s = (int)(a->T - a->t < left ? a->T - a->t : left);
+        const int64_t remaining = budget - episodes;
+        const int t0 = a->t;
+        const bool boot0 = a->bootstrap_done;
+        const uint64_t env_steps0 = b200rl_env_internal_steps(a->env);
+        const bool may_stop = remaining <= a->N * (int64_t)s;   // (a lane ends at most one episode per step)
+        if (may_stop) {
+            a->shadow.clear();
+            DevRegion er[kEnvStepRegionsMax];
+            TRY(a->shadow.add_regions(er, b200rl_env_internal_step_regions(a->env, er)));
+            TRY(a->shadow.add(a->rng, (size_t)a->N * 32));
+            for (int f = 0; f <= 5; ++f) {
+                void* p; size_t bytes;
+                TRY(rollout_field(a, f, &p, &bytes));
+                TRY(a->shadow.add(p, bytes));
+            }
+            TRY(a->shadow.copy(ctx, true));
+        }
+        // a whole rollout that cannot reach the budget: collect + update as one graph launch (b200rl_onpolicy_iterate); the update
+        // leaves the terminal columns as they are
+        const bool whole = !may_stop && t0 == 0 && s == a->T;
+        if (whole) {
+            TRY(b200rl_onpolicy_iterate(a, 1, nullptr));
+            updated = true;
+        } else {
+            TRY(b200rl_onpolicy_collect(a, s));
+        }
+        StopCrossing c;
+        TRY(stop_crossing(ctx, a->stop_counts, s, remaining, a->stop_host, [&]() -> int {
+            stop::count_columns_kernel<<<dim3(grid_for(a->N, stop::kCountBlock), (unsigned)(s < 65535 ? s : 65535)), stop::kCountBlock, 0,
+                                          ctx->stream>>>(a->terminals, a->N, t0, s, a->stop_counts);
+            LAUNCH_CHECK(ctx);
+            return B200RL_OK;
+        }, &c));
+        if (c.step != 0 && c.step < s) {   // the stage loop stops after step s* of the stretch: roll back, collect(s*)
+            TRY(a->shadow.copy(ctx, false));
+            a->t = t0;
+            a->bootstrap_done = boot0;
+            b200rl_env_internal_add_steps(a->env, env_steps0 - b200rl_env_internal_steps(a->env));
+            TRY(b200rl_onpolicy_collect(a, (int)c.step));
+        }
+        done += c.step ? c.step : s;
+        episodes += c.episodes;
+        if (!whole && a->t == a->T) {
+            TRY(b200rl_onpolicy_update(a, nullptr, nullptr));
+            updated = true;
+        }
+        if (c.step) break;
+    }
+    *steps_done = done;
+    *episodes_done = episodes;
+    if (stats_host && updated) TRY(read_stats(a, stats_host));
+    return B200RL_OK;
+}
+
 /* 1 when b200rl_onpolicy_iterate replays a captured graph, 0 when it launches eagerly (diagnostic for tests / bench) */
 int b200rl_onpolicy_graph_active(b200rl_onpolicy* a, int* out) {
     REQUIRE(a && out, B200RL_ERR_INVALID, "null argument");
@@ -1283,6 +1430,7 @@ namespace {
 __global__ void add_i64_kernel(long long* __restrict__ v, long long d) { *v += d; }
 }  // namespace
 
+constexpr int64_t kStopChunkMax = 2048;   // steps per chunk of b200rl_replay_run_episodes (its counts sit in shared memory)
 constexpr int kAgree = 21;   // values of the agreement exchange of a sharded run (replay_agree)
 // what the captured launches bake in besides the handles: a change means re-capture
 struct ReplayKey {
@@ -1310,6 +1458,10 @@ struct b200rl_replay {
     long long h_counters[2];
     double* agree_dev;            // (world, 2 kAgree) table of the agreement exchange (sharded ctx)
     GraphUnit graphs;             // "1 step + m updates" units, by m
+    Shadow shadow;                // b200rl_replay_run_episodes (allocated by its first call): env arrays, ring, explorer streams, Q-network
+    int64_t stop_chunk;           // longest chunk whose pushes the ring still holds: 2 s + 1 <= cap + 1 frames
+    unsigned long long* stop_counts;   // (stop_chunk + 2) per-step terminal counts of a chunk, then {s*, episodes}
+    long long* stop_host;         // pinned {s*, episodes}
 };
 
 // plan! -> act! -> push!(trajectory): the launches of the stage protocol (QBasedPolicy.plan_device, env.act_, Agent.push)
@@ -1423,6 +1575,7 @@ int b200rl_replay_destroy(b200rl_replay* r) {
     cudaStreamSynchronize(r->ctx->stream);
     cudaFree(r->action); cudaFree(r->ex_step_dev); cudaFree(r->upd_dev); cudaFree(r->td_keep); cudaFree(r->keys); cudaFree(r->vals);
     cudaFree(r->agree_dev);
+    cudaFree(r->shadow.buf); cudaFree(r->stop_counts); cudaFreeHost(r->stop_host);
     delete r;
     return B200RL_OK;
 }
@@ -1457,6 +1610,10 @@ int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl
     R_TRY(cudaMalloc(&r->upd_dev, sizeof(unsigned long long)));
     R_TRY(cudaMalloc(&r->td_keep, (size_t)b.B * 4));
     if (world > 1) R_TRY(cudaMalloc(&r->agree_dev, (size_t)world * 2 * kAgree * sizeof(double)));
+    {   // StopAfterNEpisodes (b200rl_replay_run_episodes): the chunk length; its buffers are allocated by the first call
+        const int64_t cap = b200rl_traj_internal_ring(traj).cap;
+        r->stop_chunk = cap / 2 < kStopChunkMax ? cap / 2 : kStopChunkMax;
+    }
 #undef R_TRY
     if (world > 1) {
         // A sharded run allocates nothing: a device allocation serialises with the kernels running on the device, and the ranks of
@@ -1557,6 +1714,76 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
     *ctl = c;
     if (ex) ex->step += n_steps * NW;
     if (stats4 && updated) TRY(dqn_stats(n, r->td_keep, r->B, stats4));
+    return B200RL_OK;
+}
+
+/* run(agent, env, StopAfterNEpisodes(k)) for at most max_steps env steps (include/b200rl.h): b200rl_replay_run in chunks of at most
+ * stop_chunk steps.  A chunk that could reach the budget (N · s >= budget - episodes so far) is marked first; the terminal flags it
+ * pushed into the ring are counted; if the budget is reached before its last step, the mark and the host counters are restored
+ * and b200rl_replay_run(s*) runs instead: step s* with its updates, target sync and counters. */
+int b200rl_replay_run_episodes(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explorer* ex, b200rl_insert_sample_ratio* ctl,
+                               int64_t max_steps, int64_t budget, float* stats4, int64_t* steps_done, int64_t* episodes_done) {
+    REQUIRE(r && ctl && steps_done && episodes_done && max_steps >= 1, B200RL_ERR_INVALID, "bad argument");
+    REQUIRE(b200rl_comm_world(r->ctx) == 1, B200RL_ERR_UNSUPPORTED,
+            "StopAfterNEpisodes counts the episodes of every rank: a sharded ctx keeps the stage loop");
+    TRY(ctx_bind(r->ctx));
+    b200rl_ctx* ctx = r->ctx;
+    b200rl_net* n = r->net;
+    {
+        DevRegion tr[kTrajStateRegionsMax];
+        const int nt = b200rl_traj_internal_state_regions(r->traj, tr);
+        size_t bytes = b200rl_env_internal_step_bytes_max(r->env) + round256((size_t)r->N * 32) + 4 * round256((size_t)n->np * 4) +
+                       3 * 256 + round256((size_t)r->B * 4);
+        for (int k = 0; k < nt; ++k) bytes += round256(tr[k].bytes);
+        TRY(stop_buffers(ctx, r->shadow, bytes, &r->stop_counts, r->stop_chunk, &r->stop_host));
+    }
+    const uint64_t updates0 = n->n_updates;
+    int64_t done = 0, episodes = 0;
+    while (done < max_steps) {
+        const int64_t s = r->stop_chunk < max_steps - done ? r->stop_chunk : max_steps - done;
+        const int64_t remaining = budget - episodes;
+        const b200rl_explorer ex0 = ex ? *ex : b200rl_explorer{};
+        const b200rl_insert_sample_ratio ctl0 = *ctl;
+        const uint64_t env_steps0 = b200rl_env_internal_steps(r->env), net_updates0 = n->n_updates;
+        const int64_t pushed0 = b200rl_traj_internal_pushed(r->traj);
+        const bool may_stop = remaining <= r->N * s;   // (a lane ends at most one episode per step)
+        if (may_stop) {
+            Shadow& sh = r->shadow;
+            sh.clear();
+            DevRegion rg[kEnvStepRegionsMax > kTrajStateRegionsMax ? kEnvStepRegionsMax : kTrajStateRegionsMax];
+            TRY(sh.add_regions(rg, b200rl_env_internal_step_regions(r->env, rg)));
+            TRY(sh.add_regions(rg, b200rl_traj_internal_state_regions(r->traj, rg)));
+            if (ex && explorer_rng_dev) TRY(sh.add(explorer_rng_dev, (size_t)r->N * 32));
+            const size_t pb = (size_t)n->np * 4;
+            TRY(sh.add(n->params, pb)); TRY(sh.add(n->m, pb)); TRY(sh.add(n->v, pb)); TRY(sh.add(n->target, pb));
+            TRY(sh.add(n->beta_t, 2 * 4)); TRY(sh.add(n->loss4, 4 * 4)); TRY(sh.add(n->gnorm, 4));
+            TRY(sh.add(r->td_keep, (size_t)r->B * 4));
+            TRY(sh.copy(ctx, true));
+        }
+        TRY(b200rl_replay_run(r, explorer_rng_dev, ex, ctl, s, nullptr));
+        StopCrossing c;
+        TRY(stop_crossing(ctx, r->stop_counts, s, remaining, r->stop_host, [&]() -> int {
+            stop::count_ring_kernel<<<grid_for(r->N, stop::kCountBlock), stop::kCountBlock, (size_t)s * sizeof(int), ctx->stream>>>(
+                b200rl_traj_internal_ring(r->traj), (int)s, r->stop_counts);
+            LAUNCH_CHECK(ctx);
+            return B200RL_OK;
+        }, &c));
+        if (c.step != 0 && c.step < s) {   // the stage loop stops after step s* of the chunk: roll back, b200rl_replay_run(s*)
+            TRY(r->shadow.copy(ctx, false));
+            if (ex) *ex = ex0;
+            *ctl = ctl0;
+            b200rl_env_internal_add_steps(r->env, env_steps0 - b200rl_env_internal_steps(r->env));
+            b200rl_traj_internal_add_pushed(r->traj, pushed0 - b200rl_traj_internal_pushed(r->traj));
+            n->n_updates = net_updates0;
+            TRY(b200rl_replay_run(r, explorer_rng_dev, ex, ctl, c.step, nullptr));
+        }
+        done += c.step ? c.step : s;
+        episodes += c.episodes;
+        if (c.step) break;
+    }
+    *steps_done = done;
+    *episodes_done = episodes;
+    if (stats4 && n->n_updates != updates0) TRY(dqn_stats(n, r->td_keep, r->B, stats4));
     return B200RL_OK;
 }
 

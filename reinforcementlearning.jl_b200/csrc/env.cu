@@ -749,6 +749,33 @@ int b200rl_env_internal_view(b200rl_env* e, envdev::EnvView* out) {
     memcpy(&out->p, &e->p, sizeof out->p);
     return B200RL_OK;
 }
+int b200rl_env_internal_step_regions(const b200rl_env* e, DevRegion* out) {
+    const size_t N = (size_t)e->N, mirror = has_obs_f32(e) ? N * e->nobs * 4 : 0;
+    int n = 0;
+    if (e->a.obs == e->a.state) {
+        out[n++] = {e->a.state, N * e->ns * e->tsize + mirror};
+    } else {
+        out[n++] = {e->a.state, N * e->ns * e->tsize};
+        out[n++] = {e->a.obs, N * e->nobs * e->tsize + mirror};
+    }
+    out[n++] = {e->a.reward, N * e->tsize};
+    if (e->rew_f32) out[n++] = {e->rew_f32, N * 4};
+    out[n++] = {e->a.flags, N};
+    out[n++] = {e->a.t, N * 4};
+    out[n++] = {e->a.rng, N * 32};
+    out[n++] = {e->a.action, N * e->asize};
+    out[n++] = {e->a.ep_ret, N * 4};
+    out[n++] = {e->a.stats, 4 * sizeof(double)};
+    if (e->log_ring.count) out[n++] = {e->log_ring.count, N * 4};
+    return n;
+}
+size_t b200rl_env_internal_step_bytes_max(const b200rl_env* e) {
+    DevRegion r[kEnvStepRegionsMax];
+    const int n = b200rl_env_internal_step_regions(e, r);
+    size_t total = e->log_ring.count ? 0 : (size_t)e->N * 4 + 256;   // (room for the write counts of an episode log attached later)
+    for (int k = 0; k < n; ++k) total += (r[k].bytes + 255) / 256 * 256;
+    return total;
+}
 void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n) { e->steps_launched += n; }
 uint64_t b200rl_env_internal_steps(const b200rl_env* e) { return e->steps_launched; }
 int b200rl_env_internal_max_timeout(const b200rl_env* e) { return e->a.max_timeout; }

@@ -7,7 +7,16 @@
 struct Ring;                              // ring.cuh
 namespace envdev { struct EnvView; }     // env_device.cuh
 
+// a device array {pointer, bytes}: the state a stretch of the fused loops changes (b200rl_*_run_episodes shadow it)
+struct DevRegion { void* p; size_t bytes; };
+
 // ---- env.cu
+// the device arrays an env step writes (state, observation and its Float32 mirror, reward, flags, t, streams, action, episode
+// return and statistics, the episode log's write counts) -> out[0 .. n), n <= kEnvStepRegionsMax
+constexpr int kEnvStepRegionsMax = 11;
+int b200rl_env_internal_step_regions(const b200rl_env* e, DevRegion* out);
+// their bytes, each rounded up to 256, with room for the write counts of an episode log attached later
+size_t b200rl_env_internal_step_bytes_max(const b200rl_env* e);
 int b200rl_env_internal_set_traj_targets(b200rl_env* e, void* reward_col, uint8_t* terminal_col);
 int b200rl_env_internal_view(b200rl_env* e, envdev::EnvView* out);
 void b200rl_env_internal_add_steps(b200rl_env* e, uint64_t n);
@@ -40,6 +49,10 @@ bool b200rl_traj_internal_prioritized(b200rl_traj* t);
 b200rl_ctx* b200rl_traj_internal_ctx(b200rl_traj* t);
 int64_t b200rl_traj_internal_lanes(b200rl_traj* t);
 void b200rl_traj_internal_add_pushed(b200rl_traj* t, int64_t n);
+// the ring's checkpoint fields (b200rl_traj_get 0 .. 9: frames, head, count, pending, n_sampleable, sum tree, sampler streams)
+// -> out[0 .. n), n <= kTrajStateRegionsMax
+constexpr int kTrajStateRegionsMax = 10;
+int b200rl_traj_internal_state_regions(b200rl_traj* t, DevRegion* out);
 int64_t b200rl_traj_internal_pushed(b200rl_traj* t);
 Ring b200rl_traj_internal_ring(b200rl_traj* t);
 float b200rl_traj_internal_default_priority(b200rl_traj* t);

@@ -519,6 +519,16 @@ bool b200rl_traj_internal_prioritized(b200rl_traj* t) { return t->prioritized; }
 b200rl_ctx* b200rl_traj_internal_ctx(b200rl_traj* t) { return t->ctx; }
 int64_t b200rl_traj_internal_lanes(b200rl_traj* t) { return t->r.lanes; }
 void b200rl_traj_internal_add_pushed(b200rl_traj* t, int64_t n) { t->pushed += n; }
+int b200rl_traj_internal_state_regions(b200rl_traj* t, DevRegion* out) {
+    int n = 0;
+    for (int f = 0; f < kTrajStateRegionsMax; ++f) {
+        if ((f == 8 && !t->prioritized) || (f == 9 && t->B == 0)) continue;
+        void* p; size_t bytes;
+        traj_field(t, f, &p, &bytes);
+        out[n++] = {p, bytes};
+    }
+    return n;
+}
 int64_t b200rl_traj_internal_pushed(b200rl_traj* t) { return t->pushed; }
 Ring b200rl_traj_internal_ring(b200rl_traj* t) { return t->r; }
 float b200rl_traj_internal_default_priority(b200rl_traj* t) { return t->default_priority; }

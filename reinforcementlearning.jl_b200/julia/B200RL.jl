@@ -369,6 +369,19 @@ function RLCore._run(policy::AbstractPolicy, env::B200VecEnv, stop_condition::Ab
         check(ccall((:b200rl_env_check, LIB), Cint, (Ptr{Cvoid},), env.h))
         return hook
     end
+    # StopAfterNEpisodes on the same fused paths (Python: run() through OnPolicyAgent.run_episodes / Agent.run_replay_episodes): each
+    # window is one library call that runs ahead, counts the episodes on the device and stops after exactly the step the stage loop
+    # stops after (b200rl_onpolicy_run_episodes / b200rl_replay_run_episodes); the progress meter is updated after every window.
+    # A sharded ctx is refused by the first call with nothing run, and the stage loop below takes the run.
+    if stop_condition isa StopAfterNEpisodes && hook isa Union{B200EpisodeStats,B200EpisodeLog,RLCore.EmptyHook} &&
+       reset_condition isa ResetIfEnvTerminated && env.auto_reset && ctx_world(env) == 1 &&
+       ((policy isa B200OnPolicyAgent && policy.fused) || (policy isa B200Agent && replay!(policy, env, 0))) &&
+       run_episodes!(policy, env, stop_condition, hook, window)
+        push!(policy, PostExperimentStage(), env)
+        push!(hook, PostExperimentStage(), policy, env)
+        check(ccall((:b200rl_env_check, LIB), Cint, (Ptr{Cvoid},), env.h))
+        return hook
+    end
     timer = RLCore.timer                                       # same labels as run.jl:46-72
     while true
         did_reset = false
@@ -899,6 +912,68 @@ function replay!(a::B200Agent, env::B200VecEnv, n_steps::Integer)
     end
     c.n_inserted, c.n_sampled = Int(ctl[].n_inserted), Int(ctl[].n_sampled)
     true
+end
+
+"""
+    episodes!(agent, env, max_steps, budget) -> (steps, episodes) | nothing
+
+At most `max_steps` env steps of `run(agent, env, StopAfterNEpisodes(k))` on the device, budget = k - cur: the loop stops after the
+step at which the episodes counted reach the budget, with the stage loop's state (b200rl_onpolicy_run_episodes /
+b200rl_replay_run_episodes).  `nothing` (nothing run) on a sharded ctx, whose stop would count the episodes of every rank.
+"""
+function episodes!(a::B200OnPolicyAgent, ::B200VecEnv, max_steps::Integer, budget::Integer)
+    steps, eps = Ref{Int64}(0), Ref{Int64}(0)
+    st = GC.@preserve a ccall((:b200rl_onpolicy_run_episodes, LIB), Cint, (Ptr{Cvoid}, Int64, Int64, Ptr{Float32}, Ref{Int64}, Ref{Int64}),
+                              a.h, max_steps, budget, a.stats, steps, eps)
+    st == -3 && return nothing                                      # B200RL_ERR_UNSUPPORTED: a sharded ctx
+    check(st)
+    t, T = Ref{Cint}(0), Ref{Cint}(0)
+    check(ccall((:b200rl_onpolicy_fill, LIB), Cint, (Ptr{Cvoid}, Ref{Cint}, Ref{Cint}), a.h, t, T))
+    a.t = Int(t[])                                                  # a stop inside a rollout leaves it part-filled
+    steps[], eps[]
+end
+function episodes!(a::B200Agent, ::B200VecEnv, max_steps::Integer, budget::Integer)   # (replay!(a, env, 0) made the handle)
+    p, c = a.policy, a.trajectory.controller
+    ctl = Ref(InsertSampleRatioC(c.ratio, c.threshold, c.n_inserted, c.n_sampled))
+    steps, eps = Ref{Int64}(0), Ref{Int64}(0)
+    if device_explorer(p.explorer)
+        ex = Ref(ExplorerC(p.explorer))
+        st = ccall((:b200rl_replay_run_episodes, LIB), Cint,
+                   (Ptr{Cvoid}, Ptr{Cvoid}, Ref{ExplorerC}, Ref{InsertSampleRatioC}, Int64, Int64, Ptr{Cfloat}, Ref{Int64}, Ref{Int64}),
+                   a.replay, p.d_rng, ex, ctl, max_steps, budget, C_NULL, steps, eps)
+        st == -3 && return nothing
+        check(st)
+        set_step!(p.explorer, ex[].step)
+    else                                                            # GreedyExplorer: findmax, no draw
+        st = ccall((:b200rl_replay_run_episodes, LIB), Cint,
+                   (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ref{InsertSampleRatioC}, Int64, Int64, Ptr{Cfloat}, Ref{Int64}, Ref{Int64}),
+                   a.replay, p.d_rng, C_NULL, ctl, max_steps, budget, C_NULL, steps, eps)
+        st == -3 && return nothing
+        check(st)
+    end
+    c.n_inserted, c.n_sampled = Int(ctl[].n_inserted), Int(ctl[].n_sampled)
+    steps[], eps[]
+end
+function ctx_world(env::B200VecEnv)
+    rank, world = Ref{Cint}(0), Ref{Cint}(1)
+    check(ccall((:b200rl_comm_rank_world, LIB), Cint, (Ptr{Cvoid}, Ref{Cint}, Ref{Cint}), env.ctx.h, rank, world))
+    Int(world[])
+end
+# the windows of a StopAfterNEpisodes run on the fused path: false (nothing run) when the first call refuses the ctx
+function run_episodes!(policy, env::B200VecEnv, s::StopAfterNEpisodes, hook, window::Integer)
+    first = true
+    while true
+        r = episodes!(policy, env, window, s.episode - s.cur)
+        if r === nothing
+            first && return false
+            error("b200rl_*_run_episodes: a window after the first was refused (the ctx changed during the run)")
+        end
+        first = false
+        s.cur += r[2]
+        hook isa B200EpisodeLog && log_flush!(hook)
+        s.progress === nothing || RLCore.ProgressMeter.update!(s.progress, min(s.cur, s.episode))
+        s.cur >= s.episode && return true
+    end
 end
 
 # ---- pure-function drop-ins (utils/basic.jl:138-417) --------------------------------------------

@@ -239,6 +239,23 @@ class OnPolicyAgent(AbstractPolicy):
         self.last_stats = stats
         return stats
 
+    def run_episodes(self, max_steps, budget):
+        """run(agent, env, StopAfterNEpisodes(k)) for at most max_steps env steps on the fused path, budget = k - cur
+        (b200rl_onpolicy_run_episodes): stops after the step at which the episodes counted reach the budget, as the stage loop
+        does.  Returns (steps run, episodes they ended)."""
+        rows = self.cfg.n_epochs * self.cfg.n_microbatches
+        stats = np.zeros((rows, 6), np.float32) if self.fetch_stats else None
+        c0, c1 = np.zeros(3, np.int64), np.zeros(3, np.int64)
+        steps, episodes = C.c_int64(), C.c_int64()
+        L.check(self.lib.b200rl_onpolicy_export_state(self.h, L.ptr(c0)))
+        L.check(self.lib.b200rl_onpolicy_run_episodes(self.h, int(max_steps), int(budget), L.ptr(stats), C.byref(steps), C.byref(episodes)))
+        L.check(self.lib.b200rl_onpolicy_export_state(self.h, L.ptr(c1)))
+        self._t = int(c1[0])
+        if c1[1] != c0[1]:
+            self.n_updates += int(c1[1] - c0[1])
+            self.last_stats = stats
+        return steps.value, episodes.value
+
     def graph_active(self):
         v = C.c_int()
         L.check(self.lib.b200rl_onpolicy_graph_active(self.h, C.byref(v)))
@@ -704,6 +721,26 @@ class Agent(AbstractPolicy):
         if stats is None or np.isnan(stats[3]):
             return None
         return dict(loss=stats[0], grad_norm=stats[1], mean_abs_td=stats[2], n_updates=int(stats[3]))
+
+    def run_replay_episodes(self, env, max_steps, budget, want_stats=False):
+        """run(agent, env, StopAfterNEpisodes(k)) for at most max_steps env steps on the device, budget = k - cur
+        (b200rl_replay_run_episodes): the steps, updates, streams and counters of the stage loop up to the step at which the
+        episodes counted reach the budget.  Returns (steps run, episodes they ended[, last update's stats or None])."""
+        pol, c = self.policy, self.trajectory.controller
+        h = self._handle(env)
+        ex = pol.explorer.as_struct() if type(pol.explorer) in DEVICE_EXPLORERS else None
+        ctl = L.InsertSampleRatio(c.ratio, c.threshold, c.n_inserted, c.n_sampled)
+        stats = np.full(4, np.nan, np.float32) if want_stats else None
+        steps, episodes = C.c_int64(), C.c_int64()
+        L.check(pol.lib.b200rl_replay_run_episodes(h, C.c_void_p(pol._d_rng), None if ex is None else C.byref(ex), C.byref(ctl),
+                                                   int(max_steps), int(budget), L.ptr(stats), C.byref(steps), C.byref(episodes)))
+        if ex is not None and hasattr(pol.explorer, "step"):
+            pol.explorer.step = ex.step
+        c.n_inserted, c.n_sampled = ctl.n_inserted, ctl.n_sampled
+        if not want_stats:
+            return steps.value, episodes.value
+        st = None if np.isnan(stats[3]) else dict(loss=stats[0], grad_norm=stats[1], mean_abs_td=stats[2], n_updates=int(stats[3]))
+        return steps.value, episodes.value, st
 
     def graph_active(self):
         v = C.c_int()
