@@ -8,6 +8,8 @@
 // with a power-of-two scale S per operand (exact; undone on the FP32 accumulator), accumulated in FP32.  fp16 covers K = 16 per
 // instruction at the same 2^-22 product accuracy as a tf32 split at K = 8.  fp16 has 5 exponent bits: activations
 // must stay below 65504 in magnitude (scale 1), weights below 1023 (scale 64); gradients are scaled by ~1/(4 inv_B) at launch.
+// The forward's relu H1 is an operand at scale 64: from H1 = 1023.75 on it rounds to inf, and every head output of that sample
+// comes out NaN (tc_fwd.cuh act2_f), not finite and wrong.
 // Below 6e-5 the lo part is subnormal: absolute error <= 2^-25 per element, far inside the 1e-5 bar.  Layer 1 (K <= 4) and the
 // heads (N <= 2) stay on FFMA.  The forward-only kernels (policy inference, fused rollout) live in fwd_tc.cu (same split).
 #include "nn.cuh"

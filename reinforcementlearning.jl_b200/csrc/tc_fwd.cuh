@@ -153,6 +153,15 @@ __device__ __forceinline__ void gemm_block(uint8_t* blk, const NetSm& w, int wgi
             *reinterpret_cast<float2*>(blk + dacc_off(row0 + 8 * h, 8 * j + col0)) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
 }
 
+// the layer-2 activation of the epilogue.  Relu is max.NaN: an H1 operand past fp16's range (relu H1 >= 1023.75, 64 H1 rounds to
+// inf) makes hi*hi + lo*hi = inf - inf, a NaN accumulator for the sample, and fmaxf(NaN, 0) = 0 would turn that into finite head
+// outputs (b3).  With max.NaN the NaN reaches every head output of the sample: past the envelope the forward is loud, not wrong.
+__device__ __forceinline__ float act2_f(int act, float z) {
+    if (act != B200RL_ACT_RELU) return tanhf(z);
+    float r;
+    asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(z));
+    return r;
+}
 // epilogue of this thread's sample: H2[32c .. 32c+32) = act(D + b2), partial head sums over these 32 features (UNROLL: as above)
 template <int ACT, int UNROLL = (ACT == B200RL_ACT_RELU ? 2 : 1)>
 __device__ __forceinline__ void head_partials(const NetSm& w, int act_rt, int c, int s, const uint8_t* tile, float (&zp)[kOutMax]) {
@@ -172,7 +181,7 @@ __device__ __forceinline__ void head_partials(const NetSm& w, int act_rt, int c,
 #pragma unroll
         for (int k = 0; k < 16; ++k) {
             const int f = 32 * c + 16 * grp + k;
-            float h2 = act_f(act, fmaf(v[k], 1.0f / (kScale * kScale), w.b2[f]));   // operand scales undone (exact power of two)
+            float h2 = act2_f(act, fmaf(v[k], 1.0f / (kScale * kScale), w.b2[f]));   // operand scales undone (exact power of two)
             float4 ww = *reinterpret_cast<const float4*>(w.W3 + f * kOutMax);
             zp[0] = fmaf(ww.x, h2, zp[0]); zp[1] = fmaf(ww.y, h2, zp[1]); zp[2] = fmaf(ww.z, h2, zp[2]); zp[3] = fmaf(ww.w, h2, zp[3]);
         }
