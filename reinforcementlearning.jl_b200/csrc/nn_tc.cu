@@ -649,6 +649,10 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         float* lp = loss_partial + (int64_t)blockIdx.x * 4;
         lp[0] = role ? 0.f : a0; lp[1] = role ? 0.f : a1; lp[2] = role ? a0 : 0.f; lp[3] = 0.f;
     }
+    // the separate reduction reads 2 * nrows loss rows (nn_ac_loss_grad's row count, the FFMA kernel's layout); the ones past
+    // this grid's own are zero, not whatever an earlier launch (an FFMA one on the same network) left there
+    if (blockIdx.x == 0)
+        for (int k = tid; k < 4 * (2 * nrows - (int)gridDim.x); k += NT7) loss_partial[4 * (int64_t)gridDim.x + k] = 0.f;
     // ---- fused optimiser step (K8 inside K7's tail): K8's arithmetic (optim.cuh) and its CTA-order gradient and loss sums; the
     //      gradient-norm total is summed per lane, then by a butterfly, so it may round differently from K8's --------------------
     if (st.params) {
