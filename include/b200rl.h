@@ -434,20 +434,24 @@ int b200rl_onpolicy_update(b200rl_onpolicy* agent, const int32_t* perm_host, flo
  * update_freq steps) when no host-side hook needs per-step data. */
 int b200rl_onpolicy_iterate(b200rl_onpolicy* agent, int n_iters, float* stats_host);
 int b200rl_onpolicy_graph_active(b200rl_onpolicy* agent, int* out);   /* 1: iterate replays a captured graph */
-/* run(agent, env, StopAfterNEpisodes(k)) (RLCore/src/core/stop_conditions.jl:82-118, batched: every lane whose is_terminated is
- * true after a step counts one episode, a MaxTimeoutEnv cut included) on the fused path, for at most max_steps env steps.
- * budget = k - cur.  The loop runs steps 1 .. s*, s* = the first step after which the episodes counted reach budget (a budget
- * <= 0: exactly one step, as the stage loop checks only after a step), or max_steps steps when the budget is not reached.
- * *steps_done = steps run, *episodes_done = episodes those steps ended (>= budget when the budget was reached; may overshoot it).
- * The result equals the stage loop's (plan!, act!, push!, optimise!, check per step) bit for bit: a rollout completed by step s*
- * is updated; one that s* falls inside stays part-filled (b200rl_onpolicy_fill), and the next call continues it.
- * How: each stretch (the rest of the rollout) that could reach the budget (N · steps >= budget - episodes so far) first copies the
- * env arrays, policy streams and rollout columns to a shadow (allocated by the agent's first call, then kept:
- * about the rollout's size again); a counting kernel reduces the stretch's terminal
- * columns per step and finds the crossing; a crossing before the stretch's last step restores the shadow and runs collect(s*).
- * One synchronisation per stretch; whole rollouts that cannot reach the budget run as b200rl_onpolicy_iterate.  max_steps: the
- * longest window between two flushes of an episode log.  stats_host: as b200rl_onpolicy_iterate, rows of the last update run
- * (untouched when none ran).  A sharded ctx (world > 1) is refused with B200RL_ERR_UNSUPPORTED before any side effect. */
+/* run(agent, env, StopAfterNSteps | StopAfterNEpisodes(k)) on the fused path, for at most max_steps env steps; max_steps: the
+ * longest window between two flushes of an episode log.  The result equals the stage loop's (plan!, act!, push!, optimise!, check
+ * per step) bit for bit: a rollout completed inside the run is updated, a part-filled one stays so (b200rl_onpolicy_fill) and the
+ * next call continues it.  Each stretch is the rest of the rollout; whole rollouts that cannot reach a budget run as
+ * b200rl_onpolicy_iterate, one graph launch each.  stats_host: as b200rl_onpolicy_iterate, rows of the last update run (untouched
+ * when none ran).
+ * budget < 0 (StopAfterNSteps): no episodes are counted (*episodes_done = 0), nothing is allocated and nothing synchronises per
+ * stretch; the run returns at the last rollout boundary inside max_steps if there is one (*steps_done = the steps up to it), so that
+ * a caller's window never splits a whole-rollout graph launch, and otherwise runs max_steps steps.  A sharded ctx is accepted.
+ * budget >= 0 (StopAfterNEpisodes(k), budget = max(0, k - cur); RLCore/src/core/stop_conditions.jl:82-118, batched: every lane
+ * whose is_terminated is true after a step counts one episode, a MaxTimeoutEnv cut included): the loop runs steps 1 .. s*, s* =
+ * the first step after which the episodes counted reach budget (budget 0: exactly one step, as the stage loop checks only after a
+ * step), or max_steps steps when the budget is not reached.  *steps_done = steps run, *episodes_done = episodes those steps ended
+ * (>= budget when the budget was reached; may overshoot it).  Each stretch that could reach the budget (N · steps >= budget -
+ * episodes so far) first copies the env arrays, policy streams and rollout columns to a shadow (allocated by the agent's first call
+ * with a budget, then kept: about the rollout's size again); a counting kernel reduces the stretch's terminal columns per step and
+ * finds the crossing; a crossing before the stretch's last step restores the shadow and runs collect(s*).  One synchronisation per
+ * stretch.  A sharded ctx (world > 1) is refused with B200RL_ERR_UNSUPPORTED before any side effect. */
 int b200rl_onpolicy_run_episodes(b200rl_onpolicy* agent, int64_t max_steps, int64_t budget, float* stats_host, int64_t* steps_done,
                                  int64_t* episodes_done);
 /* field: 0 state (ns,N,T+1) | 1 action | 2 logp | 3 reward | 4 terminal u8 | 5 value (N,T+1) |
@@ -526,16 +530,17 @@ int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl
  * advanced and *ex / *ctl NOT advanced: the run cannot be continued from them. */
 int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explorer* ex, b200rl_insert_sample_ratio* ctl,
                       int64_t n_steps, float* stats4);
-/* run(Agent(QBasedPolicy(DQNLearner, explorer), Trajectory), env, StopAfterNEpisodes(k)) on the device, for at most max_steps env
- * steps: steps, budget (= k - cur), *steps_done and *episodes_done as b200rl_onpolicy_run_episodes.  Step s* runs with its updates,
- * target sync and controller / explorer counters: what b200rl_replay_run(s*) does.  Chunks of at most min(capacity / 2, 2048)
- * steps (the ring then still holds every frame a chunk pushed) run as b200rl_replay_run; a chunk that could reach the budget first
- * copies the env arrays, the ring (frames, heads, counts, sum tree, sampler streams), the explorer streams and the Q-network
- * (parameters, Adam moments, beta^t, target, last loss / TD) to a shadow allocated by the handle's first call and kept
- * (about the ring's size again: a configuration near the device's memory can fail here with B200RL_ERR_OOM).  A counting kernel reduces the
- * terminal flags the chunk pushed per step; a crossing before the chunk's last step restores the shadow and the host counters
- * (*ex, *ctl, update and step counters) and runs b200rl_replay_run(s*).  stats4: as b200rl_replay_run, for the last update run.
- * A sharded ctx (world > 1) is refused with B200RL_ERR_UNSUPPORTED before any side effect. */
+/* run(Agent(QBasedPolicy(DQNLearner, explorer), Trajectory), env, StopAfterNSteps | StopAfterNEpisodes(k)) on the device, for at
+ * most max_steps env steps: budget, *steps_done and *episodes_done as b200rl_onpolicy_run_episodes.  budget < 0: b200rl_replay_run
+ * (max_steps) (a sharded ctx is accepted).  budget >= 0: step s* runs with its updates, target sync and controller / explorer
+ * counters: what b200rl_replay_run(s*) does.  Chunks of at most min(capacity / 2, 2048) steps (the ring then still holds every frame
+ * a chunk pushed) run as b200rl_replay_run; a chunk that could reach the budget first copies the env arrays, the ring (frames,
+ * heads, counts, sum tree, sampler streams), the explorer streams and the Q-network (parameters, Adam moments, beta^t, target, last
+ * loss / TD) to a shadow allocated by the handle's first call with a budget and kept (about the ring's size again: a configuration
+ * near the device's memory can fail here with B200RL_ERR_OOM).  A counting kernel reduces the terminal flags the chunk pushed per
+ * step; a crossing before the chunk's last step restores the shadow and the host counters (*ex, *ctl, update and step counters) and
+ * runs b200rl_replay_run(s*).  stats4: as b200rl_replay_run, for the last update run.  With a budget, a sharded ctx (world > 1) is
+ * refused with B200RL_ERR_UNSUPPORTED before any side effect. */
 int b200rl_replay_run_episodes(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explorer* ex, b200rl_insert_sample_ratio* ctl,
                                int64_t max_steps, int64_t budget, float* stats4, int64_t* steps_done, int64_t* episodes_done);
 int b200rl_replay_graph_active(b200rl_replay* r, int* out);   /* 1: a "1 step + m updates" unit has been captured and replayed */

@@ -281,26 +281,33 @@ def _flush(logs):
         h.flush()
 
 
-def _run_episodes_fused(policy, env, stop_condition, hook):
-    """StopAfterNEpisodes on the fused paths: windows of at most the episode log's capacity, each one library call that stops
-    at the crossing of the remaining budget, followed by a flush.  Returns False (nothing run) where the stage loop keeps the
-    run: a sharded ctx (the stop would count the episodes of every rank), a replay agent the device loop does not take."""
-    if env.ctx.rank_world()[1] > 1:
+def _run_fused(policy, env, stop_condition, hook):
+    """StopAfterNSteps or StopAfterNEpisodes on the fused paths: windows of at most the episode log's capacity, each one library call
+    (b200rl_*_run_episodes) followed by a flush.  The library cuts a window into stretches; a StopAfterNEpisodes window stops at the
+    crossing of the remaining budget, a StopAfterNSteps one (no budget) may end early at the end of a rollout.  Returns False
+    (nothing run) where the stage loop keeps the run: an episode count on a sharded ctx (the stop would count the episodes of every
+    rank), a replay agent the device loop does not take."""
+    episodes = isinstance(stop_condition, StopAfterNEpisodes)
+    if episodes and env.ctx.rank_world()[1] > 1:
         return False
     if hasattr(policy, "run_replay"):
         if not policy.replay_supported(env):
             return False
         step = lambda n, budget: policy.run_replay_episodes(env, n, budget)
-    elif hasattr(policy, "run_episodes"):
-        step = policy.run_episodes
     else:
-        return False
+        step = policy.run_episodes
     logs, window = _episode_log_window(hook)
+    window = window or (1 << 62)
     while True:
-        _, episodes = step(window or (1 << 62), stop_condition.episode - stop_condition.cur)
-        stop_condition.cur += episodes
+        if episodes:
+            _, n = step(window, stop_condition.episode - stop_condition.cur)
+            stop_condition.cur += n
+            is_stop = stop_condition.cur >= stop_condition.episode
+        else:
+            steps, _ = step(min(window, stop_condition.remaining()), None)
+            is_stop = stop_condition.advance(steps)
         _flush(logs)
-        if stop_condition.cur >= stop_condition.episode:
+        if is_stop:
             return True
 
 
@@ -508,48 +515,13 @@ def run(policy, env=None, stop_condition=None, hook=None, reset_condition=None):
     policy.push(PreExperimentStage, env)
     env.reset_(is_force=True)  # run.jl:46
     policy.push(PreEpisodeStage, env)   # run.jl:47-49: every lane starts an episode (there is no per-lane episode stage in the batched loop)
-    is_stop = False
-    # Fused fast path: a device-resident agent (actions never visit the host), a hook that does nothing per step and a
-    # step-count stop condition let whole stretches of the loop below run as ONE kernel launch (agent.collect(n): n x
-    # {plan!, act!, push!}) — the same transitions, parameters and statistics as stepping through the stages.
-    if (getattr(policy, "fusable", False) and env.auto_reset and not getattr(hook, "per_step", True)
-            and isinstance(stop_condition, StopAfterNSteps) and isinstance(reset_condition, ResetIfEnvTerminated)):
-        # a DeviceEpisodeLog of capacity K: windows of at most K env steps, each followed by a flush of the log
-        logs, window = _episode_log_window(hook)
-        if hasattr(policy, "run_replay"):
-            # replay Agent: the whole stretch as device launches (b200rl_replay_run), updates replayed as CUDA graphs
-            if policy.replay_supported(env):
-                n = stop_condition.remaining()
-                for j in range(0, n, window or n):
-                    policy.run_replay(env, min(n - j, window or n))
-                    _flush(logs)
-                is_stop = stop_condition.advance(n)
-        else:
-            while not is_stop:
-                if (policy._t == 0 and stop_condition.remaining() >= policy.T and hasattr(policy, "iterate")
-                        and (window is None or policy.T <= window)):
-                    # whole iterations (rollout + update) as one CUDA-graph launch each (b200rl_onpolicy_iterate)
-                    k = stop_condition.remaining() // policy.T if not policy.fetch_stats else 1
-                    if window is not None:
-                        k = min(k, window // policy.T)
-                    policy.iterate(k, want_stats=policy.fetch_stats)
-                    _flush(logs)
-                    is_stop = stop_condition.advance(k * policy.T)
-                    continue
-                n = min(policy.T - policy._t, stop_condition.remaining())
-                if window is not None:
-                    n = min(n, window)
-                policy.collect(n)
-                _flush(logs)
-                if policy._t == policy.T:
-                    policy._t = 0
-                    policy.update(want_stats=policy.fetch_stats)
-                is_stop = stop_condition.advance(n)
-    # The same fused paths for an episode-count stop condition: the loop runs ahead stretch by stretch, counts the episodes on the
-    # device and stops after exactly the step the stage loop would stop after (b200rl_*_run_episodes), with the same state.
-    if (getattr(policy, "fusable", False) and env.auto_reset and not getattr(hook, "per_step", True)
-            and isinstance(stop_condition, StopAfterNEpisodes) and isinstance(reset_condition, ResetIfEnvTerminated)):
-        is_stop = _run_episodes_fused(policy, env, stop_condition, hook)
+    # Fused path: a device-resident agent (actions never visit the host), a hook that does nothing per step and a stop condition
+    # that counts steps or episodes let whole stretches of the loop below run on the device, with the transitions, parameters,
+    # statistics and stop step of stepping through the stages.
+    is_stop = (getattr(policy, "fusable", False) and env.auto_reset and not getattr(hook, "per_step", True)
+               and isinstance(stop_condition, (StopAfterNSteps, StopAfterNEpisodes)) and isinstance(reset_condition, ResetIfEnvTerminated)
+               and _run_fused(policy, env, stop_condition, hook))
+
     def act(action):
         if isinstance(action, FusedAction):
             if action.kind == "random":

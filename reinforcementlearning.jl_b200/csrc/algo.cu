@@ -263,10 +263,11 @@ public:
     }
 };
 
-// ------------------------------------------------------------------ StopAfterNEpisodes ------
-// b200rl_onpolicy_run_episodes / b200rl_replay_run_episodes run a stretch of steps ahead and roll it back when the episode budget
-// is reached inside it (stop_episodes.cuh).  Shadow: the device state such a stretch changes, copied aside before it (mark) and
-// copied back (restore) in one launch each.  Its buffer is allocated by the handle's first run_episodes call (stop_buffers).
+// ------------------------------------------------------------------ fused runs ---------------
+// b200rl_onpolicy_run_episodes / b200rl_replay_run_episodes (run_stretches below) run a stretch of steps ahead and roll it back when
+// the episode budget is reached inside it (stop_episodes.cuh).  Shadow: the device state such a stretch changes, copied aside
+// before it (mark) and copied back (restore) in one launch each.  Its buffer is allocated by the handle's first call with an
+// episode budget (stop_buffers).
 static size_t round256(size_t b) { return (b + 255) / 256 * 256; }
 struct Shadow {
     char* buf = nullptr;
@@ -310,16 +311,68 @@ static int stop_crossing(b200rl_ctx* ctx, unsigned long long* counts, int64_t s,
     return B200RL_OK;
 }
 
-// The buffers of b200rl_*_run_episodes, allocated by the first call and kept with the handle (an agent that never stops on an episode
-// count holds none; later calls allocate nothing): the shadow (`shadow_bytes`), `n_counts` per-step counts + {s*, episodes}, the
+// The buffers of a run with an episode budget, allocated by the handle's first such run and kept (an agent that never stops on an
+// episode count holds none; later runs allocate nothing): the shadow, per-step counts of the longest stretch + {s*, episodes}, the
 // pinned pair.
-static int stop_buffers(b200rl_ctx* ctx, Shadow& sh, size_t shadow_bytes, unsigned long long** counts, int64_t n_counts, long long** host) {
-    if (sh.buf) return B200RL_OK;
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    CUDA_TRY(cudaMalloc(counts, (size_t)(n_counts + 2) * sizeof(unsigned long long)));
-    CUDA_TRY(cudaHostAlloc(host, 2 * sizeof(long long), cudaHostAllocDefault));
-    CUDA_TRY(cudaMalloc(&sh.buf, shadow_bytes));
-    sh.cap = shadow_bytes;
+struct StopBuffers {
+    Shadow shadow;
+    unsigned long long* counts = nullptr;
+    long long* host = nullptr;
+    int alloc(b200rl_ctx* ctx, size_t shadow_bytes, int64_t longest) {
+        if (shadow.buf) return B200RL_OK;
+        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+        CUDA_TRY(cudaMalloc(&counts, (size_t)(longest + 2) * sizeof(unsigned long long)));
+        CUDA_TRY(cudaHostAlloc(&host, 2 * sizeof(long long), cudaHostAllocDefault));
+        CUDA_TRY(cudaMalloc(&shadow.buf, shadow_bytes));
+        shadow.cap = shadow_bytes;
+        return B200RL_OK;
+    }
+    void release() { cudaFree(shadow.buf); cudaFree(counts); cudaFreeHost(host); }
+};
+
+/* The one loop of a fused run: at most max_steps env steps of run(agent, env, StopAfterNSteps | StopAfterNEpisodes), cut into
+ * stretches by the agent (`ops`: OnPolicyStretches, ReplayStretches).  budget >= 0: a stretch that could reach the budget
+ * (N · s >= budget - episodes so far) is marked first; the terminal flags it wrote are counted; if the budget is reached before its
+ * last step, the mark and the host counters are restored and its first s* steps run instead.  budget < 0: nothing is marked or
+ * counted — no allocation and no synchronisation per stretch, so a sharded ctx may run it — and the run returns at the agent's
+ * last boundary (the end of a rollout) inside max_steps, if there is one: a window of the caller never splits a rollout that
+ * would otherwise run as one graph launch.
+ * Ops: Saved save() / restore(Saved) of the host counters; shadow_bytes() and longest() (stretch) of the buffers; mark() the
+ * device state into the shadow; stretch(left, counting) -> s; run(s, may_stop); count(s, Saved) launches the counting kernel;
+ * end_stretch() after the count; at_boundary(left). */
+template <class Ops>
+static int run_stretches(b200rl_ctx* ctx, StopBuffers& sb, int64_t N, Ops& ops, int64_t max_steps, int64_t budget, int64_t* steps_done,
+                         int64_t* episodes_done) {
+    const bool counting = budget >= 0;
+    if (counting) TRY(sb.alloc(ctx, ops.shadow_bytes(), ops.longest()));
+    int64_t done = 0, episodes = 0;
+    while (done < max_steps) {
+        const int64_t s = ops.stretch(max_steps - done, counting);
+        const int64_t remaining = budget - episodes;
+        const typename Ops::Saved saved = ops.save();
+        const bool may_stop = counting && remaining <= N * s;   // (a lane ends at most one episode per step)
+        if (may_stop) {
+            sb.shadow.clear();
+            TRY(ops.mark(sb.shadow));
+            TRY(sb.shadow.copy(ctx, true));
+        }
+        TRY(ops.run(s, may_stop));
+        StopCrossing c{0, 0};
+        if (counting) {
+            TRY(stop_crossing(ctx, sb.counts, s, remaining, sb.host, [&] { return ops.count(s, saved, sb.counts); }, &c));
+            if (c.step != 0 && c.step < s) {   // the stage loop stops after step s* of the stretch: roll back, run s* steps
+                TRY(sb.shadow.copy(ctx, false));
+                ops.restore(saved);
+                TRY(ops.run(c.step, true));
+            }
+        }
+        done += c.step ? c.step : s;
+        episodes += c.episodes;
+        TRY(ops.end_stretch());
+        if (c.step || (!counting && ops.at_boundary(max_steps - done))) break;
+    }
+    *steps_done = done;
+    *episodes_done = episodes;
     return B200RL_OK;
 }
 
@@ -848,9 +901,7 @@ struct b200rl_onpolicy {
     unsigned int* upd_dev;       // device copy of n_updates: keys the minibatch permutation, ticked by the last optimiser step of an update
     uint64_t n_updates;
     GraphUnit graph;             // one whole iteration (collect(T) + update) for b200rl_onpolicy_iterate
-    Shadow shadow;               // b200rl_onpolicy_run_episodes (allocated by its first call): env arrays, policy streams and rollout columns
-    unsigned long long* stop_counts;   // (T + 2) per-step terminal counts of a stretch, then {s*, episodes}
-    long long* stop_host;        // pinned {s*, episodes}
+    StopBuffers stop;            // b200rl_onpolicy_run_episodes with a budget: env arrays, policy streams and rollout columns
 };
 
 // the (n_epochs * n_microbatches, 6) stats rows of the last update (synchronises)
@@ -892,7 +943,7 @@ int b200rl_onpolicy_destroy(b200rl_onpolicy* a) {
     cudaFree(a->rng); cudaFree(a->states); cudaFree(a->actions); cudaFree(a->logp); cudaFree(a->rewards); cudaFree(a->terminals);
     cudaFree(a->values); cudaFree(a->adv); cudaFree(a->ret); cudaFree(a->act_clamped); cudaFree(a->norm_partials); cudaFree(a->norm_sums);
     cudaFree(a->norm2); cudaFree(a->perm_dev); cudaFree(a->stats_dev); cudaFree(a->rec); cudaFree(a->upd_dev);
-    cudaFree(a->shadow.buf); cudaFree(a->stop_counts); cudaFreeHost(a->stop_host);
+    a->stop.release();
     delete a;
     return B200RL_OK;
 }
@@ -1141,85 +1192,75 @@ int b200rl_onpolicy_iterate(b200rl_onpolicy* a, int n_iters, float* stats_host) 
     if (stats_host && n_iters > 0) TRY(read_stats(a, stats_host));
     return B200RL_OK;
 }
-/* run(agent, env, StopAfterNEpisodes(k)) for at most max_steps env steps (include/b200rl.h).  One stretch = the rest of the
- * rollout (collect(T - t), capped by max_steps).  A stretch that could reach the budget (N · s >= budget - episodes so far) is
- * marked first; the terminal columns it wrote are counted; if the budget is reached before its last step, the mark is restored
- * and collect(s*) runs instead.  A full rollout is updated, as optimise! at the PostActStage of its last step would; the update
- * of a stretch that could reach the budget runs only after the count, so the network never needs a shadow. */
+/* The on-policy agent's part of run_stretches.  A stretch is the rest of the rollout (collect(T - t), capped by max_steps); a whole
+ * rollout that cannot reach the budget runs as one graph launch (b200rl_onpolicy_iterate), whose update leaves the terminal columns as
+ * they are.  A full rollout is updated, as optimise! at the PostActStage of its last step would; the update of a stretch that could
+ * reach the budget runs only after the count, so the network never needs a shadow. */
+struct OnPolicyStretches {
+    b200rl_onpolicy* a;
+    bool whole = false, updated = false;
+    struct Saved { int t; bool bootstrap_done; uint64_t env_steps; };
+    Saved save() const { return {a->t, a->bootstrap_done, b200rl_env_internal_steps(a->env)}; }
+    void restore(const Saved& s0) const {
+        a->t = s0.t;
+        a->bootstrap_done = s0.bootstrap_done;
+        b200rl_env_internal_add_steps(a->env, s0.env_steps - b200rl_env_internal_steps(a->env));
+    }
+    size_t shadow_bytes() const {
+        size_t bytes = b200rl_env_internal_step_bytes_max(a->env) + round256((size_t)a->N * 32);
+        for (int f = 0; f <= 5; ++f) {
+            void* p; size_t b;
+            rollout_field(a, f, &p, &b);
+            bytes += round256(b);
+        }
+        return bytes;
+    }
+    int64_t longest() const { return a->T; }
+    int mark(Shadow& sh) const {
+        DevRegion er[kEnvStepRegionsMax];
+        TRY(sh.add_regions(er, b200rl_env_internal_step_regions(a->env, er)));
+        TRY(sh.add(a->rng, (size_t)a->N * 32));
+        for (int f = 0; f <= 5; ++f) {
+            void* p; size_t bytes;
+            TRY(rollout_field(a, f, &p, &bytes));
+            TRY(sh.add(p, bytes));
+        }
+        return B200RL_OK;
+    }
+    int64_t stretch(int64_t left, bool) const { return a->T - a->t < left ? a->T - a->t : left; }
+    int run(int64_t s, bool may_stop) {
+        whole = !may_stop && a->t == 0 && s == a->T;
+        if (!whole) return b200rl_onpolicy_collect(a, (int)s);
+        updated = true;
+        return b200rl_onpolicy_iterate(a, 1, nullptr);
+    }
+    int count(int64_t s, const Saved& s0, unsigned long long* counts) const {
+        b200rl_ctx* ctx = a->ctx;
+        stop::count_columns_kernel<<<dim3(grid_for(a->N, stop::kCountBlock), (unsigned)(s < 65535 ? s : 65535)), stop::kCountBlock, 0,
+                                      ctx->stream>>>(a->terminals, a->N, s0.t, (int)s, counts);
+        LAUNCH_CHECK(ctx);
+        return B200RL_OK;
+    }
+    int end_stretch() {
+        if (whole || a->t != a->T) return B200RL_OK;
+        updated = true;
+        return b200rl_onpolicy_update(a, nullptr, nullptr);
+    }
+    bool at_boundary(int64_t left) const { return a->t == 0 && left < a->T; }
+};
+
+/* run(agent, env, StopAfterNSteps | StopAfterNEpisodes(k)) for at most max_steps env steps (include/b200rl.h): run_stretches */
 int b200rl_onpolicy_run_episodes(b200rl_onpolicy* a, int64_t max_steps, int64_t budget, float* stats_host, int64_t* steps_done,
                                  int64_t* episodes_done) {
     REQUIRE(a && steps_done && episodes_done && max_steps >= 1, B200RL_ERR_INVALID, "bad argument");
-    REQUIRE(b200rl_comm_world(a->ctx) == 1, B200RL_ERR_UNSUPPORTED,
+    REQUIRE(budget < 0 || b200rl_comm_world(a->ctx) == 1, B200RL_ERR_UNSUPPORTED,
             "StopAfterNEpisodes counts the episodes of every rank: a sharded ctx keeps the stage loop");
     const float* obs;
     TRY(learner_obs(a->env, &obs));
     TRY(ctx_bind(a->ctx));
-    b200rl_ctx* ctx = a->ctx;
-    {
-        size_t bytes = b200rl_env_internal_step_bytes_max(a->env) + round256((size_t)a->N * 32);
-        for (int f = 0; f <= 5; ++f) {
-            void* p; size_t b;
-            TRY(rollout_field(a, f, &p, &b));
-            bytes += round256(b);
-        }
-        TRY(stop_buffers(ctx, a->shadow, bytes, &a->stop_counts, a->T, &a->stop_host));
-    }
-    int64_t done = 0, episodes = 0;
-    bool updated = false;
-    while (done < max_steps) {
-        const int64_t left = max_steps - done;
-        const int s = (int)(a->T - a->t < left ? a->T - a->t : left);
-        const int64_t remaining = budget - episodes;
-        const int t0 = a->t;
-        const bool boot0 = a->bootstrap_done;
-        const uint64_t env_steps0 = b200rl_env_internal_steps(a->env);
-        const bool may_stop = remaining <= a->N * (int64_t)s;   // (a lane ends at most one episode per step)
-        if (may_stop) {
-            a->shadow.clear();
-            DevRegion er[kEnvStepRegionsMax];
-            TRY(a->shadow.add_regions(er, b200rl_env_internal_step_regions(a->env, er)));
-            TRY(a->shadow.add(a->rng, (size_t)a->N * 32));
-            for (int f = 0; f <= 5; ++f) {
-                void* p; size_t bytes;
-                TRY(rollout_field(a, f, &p, &bytes));
-                TRY(a->shadow.add(p, bytes));
-            }
-            TRY(a->shadow.copy(ctx, true));
-        }
-        // a whole rollout that cannot reach the budget: collect + update as one graph launch (b200rl_onpolicy_iterate); the update
-        // leaves the terminal columns as they are
-        const bool whole = !may_stop && t0 == 0 && s == a->T;
-        if (whole) {
-            TRY(b200rl_onpolicy_iterate(a, 1, nullptr));
-            updated = true;
-        } else {
-            TRY(b200rl_onpolicy_collect(a, s));
-        }
-        StopCrossing c;
-        TRY(stop_crossing(ctx, a->stop_counts, s, remaining, a->stop_host, [&]() -> int {
-            stop::count_columns_kernel<<<dim3(grid_for(a->N, stop::kCountBlock), (unsigned)(s < 65535 ? s : 65535)), stop::kCountBlock, 0,
-                                          ctx->stream>>>(a->terminals, a->N, t0, s, a->stop_counts);
-            LAUNCH_CHECK(ctx);
-            return B200RL_OK;
-        }, &c));
-        if (c.step != 0 && c.step < s) {   // the stage loop stops after step s* of the stretch: roll back, collect(s*)
-            TRY(a->shadow.copy(ctx, false));
-            a->t = t0;
-            a->bootstrap_done = boot0;
-            b200rl_env_internal_add_steps(a->env, env_steps0 - b200rl_env_internal_steps(a->env));
-            TRY(b200rl_onpolicy_collect(a, (int)c.step));
-        }
-        done += c.step ? c.step : s;
-        episodes += c.episodes;
-        if (!whole && a->t == a->T) {
-            TRY(b200rl_onpolicy_update(a, nullptr, nullptr));
-            updated = true;
-        }
-        if (c.step) break;
-    }
-    *steps_done = done;
-    *episodes_done = episodes;
-    if (stats_host && updated) TRY(read_stats(a, stats_host));
+    OnPolicyStretches ops{a};
+    TRY(run_stretches(a->ctx, a->stop, a->N, ops, max_steps, budget, steps_done, episodes_done));
+    if (stats_host && ops.updated) TRY(read_stats(a, stats_host));
     return B200RL_OK;
 }
 
@@ -1458,10 +1499,8 @@ struct b200rl_replay {
     long long h_counters[2];
     double* agree_dev;            // (world, 2 kAgree) table of the agreement exchange (sharded ctx)
     GraphUnit graphs;             // "1 step + m updates" units, by m
-    Shadow shadow;                // b200rl_replay_run_episodes (allocated by its first call): env arrays, ring, explorer streams, Q-network
+    StopBuffers stop;             // b200rl_replay_run_episodes with a budget: env arrays, ring, explorer streams, Q-network
     int64_t stop_chunk;           // longest chunk whose pushes the ring still holds: 2 s + 1 <= cap + 1 frames
-    unsigned long long* stop_counts;   // (stop_chunk + 2) per-step terminal counts of a chunk, then {s*, episodes}
-    long long* stop_host;         // pinned {s*, episodes}
 };
 
 // plan! -> act! -> push!(trajectory): the launches of the stage protocol (QBasedPolicy.plan_device, env.act_, Agent.push)
@@ -1567,6 +1606,58 @@ static int replay_unit(b200rl_replay* r, uint64_t* rng, const b200rl_explorer* e
     return B200RL_OK;
 }
 
+/* The replay agent's part of run_stretches: b200rl_replay_run per stretch — with a budget chunks of at most stop_chunk steps (the
+ * ring then still holds every frame a chunk pushed, which count_ring_kernel reads), without one the whole window.  A rollback
+ * restores the host counters b200rl_replay_run advanced: *ex, *ctl, env steps, pushed frames, optimiser steps. */
+struct ReplayStretches {
+    b200rl_replay* r;
+    uint64_t* rng;
+    b200rl_explorer* ex;
+    b200rl_insert_sample_ratio* ctl;
+    struct Saved { b200rl_explorer ex; b200rl_insert_sample_ratio ctl; uint64_t env_steps, net_updates; int64_t pushed; };
+    Saved save() const {
+        return {ex ? *ex : b200rl_explorer{}, *ctl, b200rl_env_internal_steps(r->env), r->net->n_updates, b200rl_traj_internal_pushed(r->traj)};
+    }
+    void restore(const Saved& s0) const {
+        if (ex) *ex = s0.ex;
+        *ctl = s0.ctl;
+        b200rl_env_internal_add_steps(r->env, s0.env_steps - b200rl_env_internal_steps(r->env));
+        b200rl_traj_internal_add_pushed(r->traj, s0.pushed - b200rl_traj_internal_pushed(r->traj));
+        r->net->n_updates = s0.net_updates;
+    }
+    size_t shadow_bytes() const {
+        DevRegion tr[kTrajStateRegionsMax];
+        const int nt = b200rl_traj_internal_state_regions(r->traj, tr);
+        size_t bytes = b200rl_env_internal_step_bytes_max(r->env) + round256((size_t)r->N * 32) + 4 * round256((size_t)r->net->np * 4) +
+                       3 * 256 + round256((size_t)r->B * 4);
+        for (int k = 0; k < nt; ++k) bytes += round256(tr[k].bytes);
+        return bytes;
+    }
+    int64_t longest() const { return r->stop_chunk; }
+    int mark(Shadow& sh) const {
+        b200rl_net* n = r->net;
+        DevRegion rg[kEnvStepRegionsMax > kTrajStateRegionsMax ? kEnvStepRegionsMax : kTrajStateRegionsMax];
+        TRY(sh.add_regions(rg, b200rl_env_internal_step_regions(r->env, rg)));
+        TRY(sh.add_regions(rg, b200rl_traj_internal_state_regions(r->traj, rg)));
+        if (ex && rng) TRY(sh.add(rng, (size_t)r->N * 32));
+        const size_t pb = (size_t)n->np * 4;
+        TRY(sh.add(n->params, pb)); TRY(sh.add(n->m, pb)); TRY(sh.add(n->v, pb)); TRY(sh.add(n->target, pb));
+        TRY(sh.add(n->beta_t, 2 * 4)); TRY(sh.add(n->loss4, 4 * 4)); TRY(sh.add(n->gnorm, 4));
+        return sh.add(r->td_keep, (size_t)r->B * 4);
+    }
+    int64_t stretch(int64_t left, bool counting) const { return counting && r->stop_chunk < left ? r->stop_chunk : left; }
+    int run(int64_t s, bool) const { return b200rl_replay_run(r, rng, ex, ctl, s, nullptr); }
+    int count(int64_t s, const Saved&, unsigned long long* counts) const {
+        b200rl_ctx* ctx = r->ctx;
+        stop::count_ring_kernel<<<grid_for(r->N, stop::kCountBlock), stop::kCountBlock, (size_t)s * sizeof(int), ctx->stream>>>(
+            b200rl_traj_internal_ring(r->traj), (int)s, counts);
+        LAUNCH_CHECK(ctx);
+        return B200RL_OK;
+    }
+    int end_stretch() const { return B200RL_OK; }
+    bool at_boundary(int64_t) const { return false; }
+};
+
 extern "C" {
 
 int b200rl_replay_destroy(b200rl_replay* r) {
@@ -1575,7 +1666,7 @@ int b200rl_replay_destroy(b200rl_replay* r) {
     cudaStreamSynchronize(r->ctx->stream);
     cudaFree(r->action); cudaFree(r->ex_step_dev); cudaFree(r->upd_dev); cudaFree(r->td_keep); cudaFree(r->keys); cudaFree(r->vals);
     cudaFree(r->agree_dev);
-    cudaFree(r->shadow.buf); cudaFree(r->stop_counts); cudaFreeHost(r->stop_host);
+    r->stop.release();
     delete r;
     return B200RL_OK;
 }
@@ -1610,7 +1701,7 @@ int b200rl_replay_create(b200rl_ctx* ctx, b200rl_net* q, b200rl_env* env, b200rl
     R_TRY(cudaMalloc(&r->upd_dev, sizeof(unsigned long long)));
     R_TRY(cudaMalloc(&r->td_keep, (size_t)b.B * 4));
     if (world > 1) R_TRY(cudaMalloc(&r->agree_dev, (size_t)world * 2 * kAgree * sizeof(double)));
-    {   // StopAfterNEpisodes (b200rl_replay_run_episodes): the chunk length; its buffers are allocated by the first call
+    {   // StopAfterNEpisodes (b200rl_replay_run_episodes): the chunk length; its buffers are allocated by the first run with a budget
         const int64_t cap = b200rl_traj_internal_ring(traj).cap;
         r->stop_chunk = cap / 2 < kStopChunkMax ? cap / 2 : kStopChunkMax;
     }
@@ -1717,73 +1808,17 @@ int b200rl_replay_run(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explo
     return B200RL_OK;
 }
 
-/* run(agent, env, StopAfterNEpisodes(k)) for at most max_steps env steps (include/b200rl.h): b200rl_replay_run in chunks of at most
- * stop_chunk steps.  A chunk that could reach the budget (N · s >= budget - episodes so far) is marked first; the terminal flags it
- * pushed into the ring are counted; if the budget is reached before its last step, the mark and the host counters are restored
- * and b200rl_replay_run(s*) runs instead: step s* with its updates, target sync and counters. */
+/* run(agent, env, StopAfterNSteps | StopAfterNEpisodes(k)) for at most max_steps env steps (include/b200rl.h): run_stretches */
 int b200rl_replay_run_episodes(b200rl_replay* r, uint64_t* explorer_rng_dev, b200rl_explorer* ex, b200rl_insert_sample_ratio* ctl,
                                int64_t max_steps, int64_t budget, float* stats4, int64_t* steps_done, int64_t* episodes_done) {
     REQUIRE(r && ctl && steps_done && episodes_done && max_steps >= 1, B200RL_ERR_INVALID, "bad argument");
-    REQUIRE(b200rl_comm_world(r->ctx) == 1, B200RL_ERR_UNSUPPORTED,
+    REQUIRE(budget < 0 || b200rl_comm_world(r->ctx) == 1, B200RL_ERR_UNSUPPORTED,
             "StopAfterNEpisodes counts the episodes of every rank: a sharded ctx keeps the stage loop");
     TRY(ctx_bind(r->ctx));
-    b200rl_ctx* ctx = r->ctx;
-    b200rl_net* n = r->net;
-    {
-        DevRegion tr[kTrajStateRegionsMax];
-        const int nt = b200rl_traj_internal_state_regions(r->traj, tr);
-        size_t bytes = b200rl_env_internal_step_bytes_max(r->env) + round256((size_t)r->N * 32) + 4 * round256((size_t)n->np * 4) +
-                       3 * 256 + round256((size_t)r->B * 4);
-        for (int k = 0; k < nt; ++k) bytes += round256(tr[k].bytes);
-        TRY(stop_buffers(ctx, r->shadow, bytes, &r->stop_counts, r->stop_chunk, &r->stop_host));
-    }
-    const uint64_t updates0 = n->n_updates;
-    int64_t done = 0, episodes = 0;
-    while (done < max_steps) {
-        const int64_t s = r->stop_chunk < max_steps - done ? r->stop_chunk : max_steps - done;
-        const int64_t remaining = budget - episodes;
-        const b200rl_explorer ex0 = ex ? *ex : b200rl_explorer{};
-        const b200rl_insert_sample_ratio ctl0 = *ctl;
-        const uint64_t env_steps0 = b200rl_env_internal_steps(r->env), net_updates0 = n->n_updates;
-        const int64_t pushed0 = b200rl_traj_internal_pushed(r->traj);
-        const bool may_stop = remaining <= r->N * s;   // (a lane ends at most one episode per step)
-        if (may_stop) {
-            Shadow& sh = r->shadow;
-            sh.clear();
-            DevRegion rg[kEnvStepRegionsMax > kTrajStateRegionsMax ? kEnvStepRegionsMax : kTrajStateRegionsMax];
-            TRY(sh.add_regions(rg, b200rl_env_internal_step_regions(r->env, rg)));
-            TRY(sh.add_regions(rg, b200rl_traj_internal_state_regions(r->traj, rg)));
-            if (ex && explorer_rng_dev) TRY(sh.add(explorer_rng_dev, (size_t)r->N * 32));
-            const size_t pb = (size_t)n->np * 4;
-            TRY(sh.add(n->params, pb)); TRY(sh.add(n->m, pb)); TRY(sh.add(n->v, pb)); TRY(sh.add(n->target, pb));
-            TRY(sh.add(n->beta_t, 2 * 4)); TRY(sh.add(n->loss4, 4 * 4)); TRY(sh.add(n->gnorm, 4));
-            TRY(sh.add(r->td_keep, (size_t)r->B * 4));
-            TRY(sh.copy(ctx, true));
-        }
-        TRY(b200rl_replay_run(r, explorer_rng_dev, ex, ctl, s, nullptr));
-        StopCrossing c;
-        TRY(stop_crossing(ctx, r->stop_counts, s, remaining, r->stop_host, [&]() -> int {
-            stop::count_ring_kernel<<<grid_for(r->N, stop::kCountBlock), stop::kCountBlock, (size_t)s * sizeof(int), ctx->stream>>>(
-                b200rl_traj_internal_ring(r->traj), (int)s, r->stop_counts);
-            LAUNCH_CHECK(ctx);
-            return B200RL_OK;
-        }, &c));
-        if (c.step != 0 && c.step < s) {   // the stage loop stops after step s* of the chunk: roll back, b200rl_replay_run(s*)
-            TRY(r->shadow.copy(ctx, false));
-            if (ex) *ex = ex0;
-            *ctl = ctl0;
-            b200rl_env_internal_add_steps(r->env, env_steps0 - b200rl_env_internal_steps(r->env));
-            b200rl_traj_internal_add_pushed(r->traj, pushed0 - b200rl_traj_internal_pushed(r->traj));
-            n->n_updates = net_updates0;
-            TRY(b200rl_replay_run(r, explorer_rng_dev, ex, ctl, c.step, nullptr));
-        }
-        done += c.step ? c.step : s;
-        episodes += c.episodes;
-        if (c.step) break;
-    }
-    *steps_done = done;
-    *episodes_done = episodes;
-    if (stats4 && n->n_updates != updates0) TRY(dqn_stats(n, r->td_keep, r->B, stats4));
+    const uint64_t updates0 = r->net->n_updates;
+    ReplayStretches ops{r, explorer_rng_dev, ex, ctl};
+    TRY(run_stretches(r->ctx, r->stop, r->N, ops, max_steps, budget, steps_done, episodes_done));
+    if (stats4 && r->net->n_updates != updates0) TRY(dqn_stats(r->net, r->td_keep, r->B, stats4));
     return B200RL_OK;
 }
 

@@ -330,53 +330,29 @@ function RLCore._run(policy::AbstractPolicy, env::B200VecEnv, stop_condition::Ab
     push!(policy, PreExperimentStage(), env)
     RLBase.reset!(env; is_force = true)
     push!(policy, PreEpisodeStage(), env)                      # run.jl:47-49: every lane starts an episode
-    # Fused fast path (the Python mirror's run(), core.py): a device-resident on-policy agent, a hook with nothing to do per
-    # step and a step-count stop condition let whole stretches of the loop run as ONE kernel launch (b200rl_onpolicy_collect:
-    # n x {plan!, act!, push!}) — the same transitions, parameters and statistics as stepping through the stages.
-    # A B200EpisodeLog of capacity K: windows of at most K env steps, each followed by a flush of the log.
+    # Fused path (the Python mirror's run(), core.py): a device-resident agent, a hook with nothing to do per step and a stop
+    # condition that counts steps or episodes let whole stretches of the loop run on the device, with the stage loop's results.
+    # Windows of at most a B200EpisodeLog's capacity, each one library call (episodes!) followed by a flush of the log; the library
+    # cuts a window into stretches.  A StopAfterNEpisodes window stops at the crossing of the remaining budget (an episode count on
+    # a sharded ctx keeps the stage loop), a StopAfterNSteps one (budget -1) may end early at the end of a rollout.
     window = hook isa B200EpisodeLog ? hook.capacity : typemax(Int)
-    if policy isa B200OnPolicyAgent && policy.fused && env.auto_reset && hook isa Union{B200EpisodeStats,B200EpisodeLog,RLCore.EmptyHook} &&
-       stop_condition isa StopAfterNSteps && reset_condition isa ResetIfEnvTerminated
-        while true                                                  # StopAfterNSteps: check! is true once cur >= step, then cur += 1
-            n = min(policy.T - policy.t, max(1, stop_condition.step - stop_condition.cur + 1), window)
-            collect!(policy, n)
-            hook isa B200EpisodeLog && log_flush!(hook)
-            RLBase.optimise!(policy, PostActStage())
-            stop_condition.cur += n
-            stop_condition.progress === nothing || RLCore.ProgressMeter.update!(stop_condition.progress, min(stop_condition.cur, stop_condition.step))
-            stop_condition.cur > stop_condition.step && break
-        end
-        push!(policy, PostExperimentStage(), env)
-        push!(hook, PostExperimentStage(), policy, env)
-        check(ccall((:b200rl_env_check, LIB), Cint, (Ptr{Cvoid},), env.h))
-        return hook
-    end
-    # the replay agent's device loop (Python: Agent.run_replay): the whole window in one replay! call
-    n_replay = max(1, stop_condition isa StopAfterNSteps ? stop_condition.step - stop_condition.cur + 1 : 1)
-    if policy isa B200Agent && hook isa Union{B200EpisodeStats,B200EpisodeLog,RLCore.EmptyHook} && stop_condition isa StopAfterNSteps &&
-       reset_condition isa ResetIfEnvTerminated && replay!(policy, env, min(n_replay, window))
-        if hook isa B200EpisodeLog
-            log_flush!(hook)
-            for j in window+1:window:n_replay                      # the remaining windows of the log
-                replay!(policy, env, min(window, n_replay - j + 1)) ||
-                    error("replay!: a window after the first was refused (the env or trajectory changed during the run)")
-                log_flush!(hook)
+    if hook isa Union{B200EpisodeStats,B200EpisodeLog,RLCore.EmptyHook} && reset_condition isa ResetIfEnvTerminated && env.auto_reset &&
+       (stop_condition isa StopAfterNSteps || (stop_condition isa StopAfterNEpisodes && ctx_world(env) == 1)) &&
+       ((policy isa B200OnPolicyAgent && policy.fused) || (policy isa B200Agent && replay!(policy, env, 0)))
+        while true
+            if stop_condition isa StopAfterNSteps                  # check! is true once cur >= step, then cur += 1
+                steps, _ = episodes!(policy, env, min(window, max(1, stop_condition.step - stop_condition.cur + 1)), -1)
+                stop_condition.cur += steps
+                done, progress = stop_condition.cur > stop_condition.step, min(stop_condition.cur, stop_condition.step)
+            else
+                _, n = episodes!(policy, env, window, max(0, stop_condition.episode - stop_condition.cur))   # (0: one step)
+                stop_condition.cur += n
+                done, progress = stop_condition.cur >= stop_condition.episode, min(stop_condition.cur, stop_condition.episode)
             end
+            hook isa B200EpisodeLog && log_flush!(hook)
+            stop_condition.progress === nothing || RLCore.ProgressMeter.update!(stop_condition.progress, progress)
+            done && break
         end
-        stop_condition.cur += n_replay
-        push!(policy, PostExperimentStage(), env)
-        push!(hook, PostExperimentStage(), policy, env)
-        check(ccall((:b200rl_env_check, LIB), Cint, (Ptr{Cvoid},), env.h))
-        return hook
-    end
-    # StopAfterNEpisodes on the same fused paths (Python: run() through OnPolicyAgent.run_episodes / Agent.run_replay_episodes): each
-    # window is one library call that runs ahead, counts the episodes on the device and stops after exactly the step the stage loop
-    # stops after (b200rl_onpolicy_run_episodes / b200rl_replay_run_episodes); the progress meter is updated after every window.
-    # A sharded ctx is refused by the first call with nothing run, and the stage loop below takes the run.
-    if stop_condition isa StopAfterNEpisodes && hook isa Union{B200EpisodeStats,B200EpisodeLog,RLCore.EmptyHook} &&
-       reset_condition isa ResetIfEnvTerminated && env.auto_reset && ctx_world(env) == 1 &&
-       ((policy isa B200OnPolicyAgent && policy.fused) || (policy isa B200Agent && replay!(policy, env, 0))) &&
-       run_episodes!(policy, env, stop_condition, hook, window)
         push!(policy, PostExperimentStage(), env)
         push!(hook, PostExperimentStage(), policy, env)
         check(ccall((:b200rl_env_check, LIB), Cint, (Ptr{Cvoid},), env.h))
@@ -915,18 +891,17 @@ function replay!(a::B200Agent, env::B200VecEnv, n_steps::Integer)
 end
 
 """
-    episodes!(agent, env, max_steps, budget) -> (steps, episodes) | nothing
+    episodes!(agent, env, max_steps, budget) -> (steps, episodes)
 
-At most `max_steps` env steps of `run(agent, env, StopAfterNEpisodes(k))` on the device, budget = k - cur: the loop stops after the
-step at which the episodes counted reach the budget, with the stage loop's state (b200rl_onpolicy_run_episodes /
-b200rl_replay_run_episodes).  `nothing` (nothing run) on a sharded ctx, whose stop would count the episodes of every rank.
+At most `max_steps` env steps of `run(agent, env, stop)` on the device (b200rl_onpolicy_run_episodes / b200rl_replay_run_episodes),
+with the stage loop's state.  budget = k - cur for `StopAfterNEpisodes(k)`: the loop stops after the step at which the episodes
+counted reach it (refused on a sharded ctx, whose stop would count the episodes of every rank).  budget < 0 for `StopAfterNSteps`:
+`max_steps` steps, or fewer when the last rollout they complete ends earlier; no episodes are counted.
 """
 function episodes!(a::B200OnPolicyAgent, ::B200VecEnv, max_steps::Integer, budget::Integer)
     steps, eps = Ref{Int64}(0), Ref{Int64}(0)
-    st = GC.@preserve a ccall((:b200rl_onpolicy_run_episodes, LIB), Cint, (Ptr{Cvoid}, Int64, Int64, Ptr{Float32}, Ref{Int64}, Ref{Int64}),
-                              a.h, max_steps, budget, a.stats, steps, eps)
-    st == -3 && return nothing                                      # B200RL_ERR_UNSUPPORTED: a sharded ctx
-    check(st)
+    GC.@preserve a check(ccall((:b200rl_onpolicy_run_episodes, LIB), Cint, (Ptr{Cvoid}, Int64, Int64, Ptr{Float32}, Ref{Int64}, Ref{Int64}),
+                               a.h, max_steps, budget, a.stats, steps, eps))
     t, T = Ref{Cint}(0), Ref{Cint}(0)
     check(ccall((:b200rl_onpolicy_fill, LIB), Cint, (Ptr{Cvoid}, Ref{Cint}, Ref{Cint}), a.h, t, T))
     a.t = Int(t[])                                                  # a stop inside a rollout leaves it part-filled
@@ -938,18 +913,14 @@ function episodes!(a::B200Agent, ::B200VecEnv, max_steps::Integer, budget::Integ
     steps, eps = Ref{Int64}(0), Ref{Int64}(0)
     if device_explorer(p.explorer)
         ex = Ref(ExplorerC(p.explorer))
-        st = ccall((:b200rl_replay_run_episodes, LIB), Cint,
-                   (Ptr{Cvoid}, Ptr{Cvoid}, Ref{ExplorerC}, Ref{InsertSampleRatioC}, Int64, Int64, Ptr{Cfloat}, Ref{Int64}, Ref{Int64}),
-                   a.replay, p.d_rng, ex, ctl, max_steps, budget, C_NULL, steps, eps)
-        st == -3 && return nothing
-        check(st)
+        check(ccall((:b200rl_replay_run_episodes, LIB), Cint,
+                    (Ptr{Cvoid}, Ptr{Cvoid}, Ref{ExplorerC}, Ref{InsertSampleRatioC}, Int64, Int64, Ptr{Cfloat}, Ref{Int64}, Ref{Int64}),
+                    a.replay, p.d_rng, ex, ctl, max_steps, budget, C_NULL, steps, eps))
         set_step!(p.explorer, ex[].step)
     else                                                            # GreedyExplorer: findmax, no draw
-        st = ccall((:b200rl_replay_run_episodes, LIB), Cint,
-                   (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ref{InsertSampleRatioC}, Int64, Int64, Ptr{Cfloat}, Ref{Int64}, Ref{Int64}),
-                   a.replay, p.d_rng, C_NULL, ctl, max_steps, budget, C_NULL, steps, eps)
-        st == -3 && return nothing
-        check(st)
+        check(ccall((:b200rl_replay_run_episodes, LIB), Cint,
+                    (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ref{InsertSampleRatioC}, Int64, Int64, Ptr{Cfloat}, Ref{Int64}, Ref{Int64}),
+                    a.replay, p.d_rng, C_NULL, ctl, max_steps, budget, C_NULL, steps, eps))
     end
     c.n_inserted, c.n_sampled = Int(ctl[].n_inserted), Int(ctl[].n_sampled)
     steps[], eps[]
@@ -958,22 +929,6 @@ function ctx_world(env::B200VecEnv)
     rank, world = Ref{Cint}(0), Ref{Cint}(1)
     check(ccall((:b200rl_comm_rank_world, LIB), Cint, (Ptr{Cvoid}, Ref{Cint}, Ref{Cint}), env.ctx.h, rank, world))
     Int(world[])
-end
-# the windows of a StopAfterNEpisodes run on the fused path: false (nothing run) when the first call refuses the ctx
-function run_episodes!(policy, env::B200VecEnv, s::StopAfterNEpisodes, hook, window::Integer)
-    first = true
-    while true
-        r = episodes!(policy, env, window, s.episode - s.cur)
-        if r === nothing
-            first && return false
-            error("b200rl_*_run_episodes: a window after the first was refused (the ctx changed during the run)")
-        end
-        first = false
-        s.cur += r[2]
-        hook isa B200EpisodeLog && log_flush!(hook)
-        s.progress === nothing || RLCore.ProgressMeter.update!(s.progress, min(s.cur, s.episode))
-        s.cur >= s.episode && return true
-    end
 end
 
 # ---- pure-function drop-ins (utils/basic.jl:138-417) --------------------------------------------

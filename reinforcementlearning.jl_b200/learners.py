@@ -135,6 +135,12 @@ class Network:
         return dict(actor_loss=losses[0], critic_loss=losses[1], entropy=losses[2], loss=losses[3], grad_norm=losses[4])
 
 
+def _library_budget(budget):
+    """the budget argument of b200rl_*_run_episodes: -1 (none) for StopAfterNSteps; an episode budget already spent is 0 (one
+    step, as the stage loop checks only after a step), never negative"""
+    return -1 if budget is None else max(0, int(budget))
+
+
 ROLL_STATE, ROLL_ACTION, ROLL_LOGP, ROLL_REWARD, ROLL_TERMINAL, ROLL_VALUE, ROLL_ADV, ROLL_RET, ROLL_RNG, ROLL_NORM = range(10)
 
 
@@ -149,7 +155,7 @@ class OnPolicyAgent(AbstractPolicy):
         self.ctx, self.lib, self.net, self.env, self.cfg = ctx, ctx.lib, net, env, cfg
         self.n, self.T = env.n, cfg.update_freq
         self.host_actions = host_actions
-        self.fusable = not host_actions     # run() may hand whole stretches of env steps to collect()
+        self.fusable = not host_actions     # run() may hand whole stretches of env steps to run_episodes()
         policy_rng = np.ascontiguousarray(policy_rng, np.uint64).reshape(self.n, 4)
         h = C.c_void_p()
         L.check(self.lib.b200rl_onpolicy_create(ctx.h, net.h, env.h, C.byref(cfg), L.ptr(policy_rng), C.byref(h)))
@@ -240,15 +246,17 @@ class OnPolicyAgent(AbstractPolicy):
         return stats
 
     def run_episodes(self, max_steps, budget):
-        """run(agent, env, StopAfterNEpisodes(k)) for at most max_steps env steps on the fused path, budget = k - cur
-        (b200rl_onpolicy_run_episodes): stops after the step at which the episodes counted reach the budget, as the stage loop
-        does.  Returns (steps run, episodes they ended)."""
+        """At most max_steps env steps of run(agent, env, stop) on the fused path (b200rl_onpolicy_run_episodes).  budget = k - cur
+        for StopAfterNEpisodes(k): stops after the step at which the episodes counted reach it, as the stage loop does (a budget
+        <= 0: one step).  budget None for StopAfterNSteps: runs max_steps steps, or stops earlier at the end of the last rollout
+        they complete.  Returns (steps run, episodes they ended; 0 without a budget)."""
         rows = self.cfg.n_epochs * self.cfg.n_microbatches
         stats = np.zeros((rows, 6), np.float32) if self.fetch_stats else None
         c0, c1 = np.zeros(3, np.int64), np.zeros(3, np.int64)
         steps, episodes = C.c_int64(), C.c_int64()
         L.check(self.lib.b200rl_onpolicy_export_state(self.h, L.ptr(c0)))
-        L.check(self.lib.b200rl_onpolicy_run_episodes(self.h, int(max_steps), int(budget), L.ptr(stats), C.byref(steps), C.byref(episodes)))
+        L.check(self.lib.b200rl_onpolicy_run_episodes(self.h, int(max_steps), _library_budget(budget), L.ptr(stats), C.byref(steps),
+                                                      C.byref(episodes)))
         L.check(self.lib.b200rl_onpolicy_export_state(self.h, L.ptr(c1)))
         self._t = int(c1[0])
         if c1[1] != c0[1]:
@@ -660,8 +668,8 @@ class Agent(AbstractPolicy):
         if not hasattr(trajectory, "controller"):
             trajectory.controller = InsertSampleRatioController()
         self._host_act = None
-        # run() may hand whole stretches of the loop to run_replay (b200rl_replay_run): a DQN learner behind one of the device
-        # explorers (epsilon-greedy, speedy, weighted / Gumbel softmax, greedy) whose actions stay on the device.  The env's side is
+        # run() may hand whole stretches of the loop to run_replay_episodes (b200rl_replay_run_episodes): a DQN learner behind one of
+        # the device explorers (epsilon-greedy, speedy, weighted / Gumbel softmax, greedy) whose actions stay on the device.  The env's side is
         # checked per run (replay_supported).
         self.fusable = (not host_actions and isinstance(policy, QBasedPolicy) and isinstance(policy.learner, DQNLearner)
                         and type(policy.explorer) in DEVICE_EXPLORERS + (GreedyExplorer,))
@@ -723,9 +731,10 @@ class Agent(AbstractPolicy):
         return dict(loss=stats[0], grad_norm=stats[1], mean_abs_td=stats[2], n_updates=int(stats[3]))
 
     def run_replay_episodes(self, env, max_steps, budget, want_stats=False):
-        """run(agent, env, StopAfterNEpisodes(k)) for at most max_steps env steps on the device, budget = k - cur
-        (b200rl_replay_run_episodes): the steps, updates, streams and counters of the stage loop up to the step at which the
-        episodes counted reach the budget.  Returns (steps run, episodes they ended[, last update's stats or None])."""
+        """At most max_steps env steps of run(agent, env, stop) on the device (b200rl_replay_run_episodes): the steps, updates,
+        streams and counters of the stage loop.  budget = k - cur for StopAfterNEpisodes(k): stops after the step at which the
+        episodes counted reach it (a budget <= 0: one step).  budget None for StopAfterNSteps: runs max_steps steps, as run_replay
+        does.  Returns (steps run, episodes they ended[, last update's stats or None])."""
         pol, c = self.policy, self.trajectory.controller
         h = self._handle(env)
         ex = pol.explorer.as_struct() if type(pol.explorer) in DEVICE_EXPLORERS else None
@@ -733,7 +742,8 @@ class Agent(AbstractPolicy):
         stats = np.full(4, np.nan, np.float32) if want_stats else None
         steps, episodes = C.c_int64(), C.c_int64()
         L.check(pol.lib.b200rl_replay_run_episodes(h, C.c_void_p(pol._d_rng), None if ex is None else C.byref(ex), C.byref(ctl),
-                                                   int(max_steps), int(budget), L.ptr(stats), C.byref(steps), C.byref(episodes)))
+                                                   int(max_steps), _library_budget(budget), L.ptr(stats), C.byref(steps),
+                                                   C.byref(episodes)))
         if ex is not None and hasattr(pol.explorer, "step"):
             pol.explorer.step = ex.step
         c.n_inserted, c.n_sampled = ctl.n_inserted, ctl.n_sampled

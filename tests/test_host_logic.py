@@ -355,23 +355,26 @@ def test_reset_conditions_and_experiment(pkg):
 
 
 class StubFusedAgent:
-    """The surface run() uses of a device-resident OnPolicyAgent: collect(n) / update() bookkeeping only."""
-    fusable, fetch_stats = True, False
+    """The surface run() uses of a device-resident OnPolicyAgent: run_episodes(n, budget) bookkeeping only.  As the library does
+    without an episode budget, a call returns at the end of the last rollout its n steps complete, if there is one."""
+    fusable = True
 
     def __init__(self, T):
         self.T, self._t, self.calls, self.pushed = T, 0, [], []
 
     def push(self, stage, env, action=None):
         self.pushed.append(stage)
+        self.env = env
 
-    def collect(self, n):
-        assert 1 <= n <= self.T - self._t
-        self.calls.append(("collect", n))
-        self._t += n
-
-    def update(self, want_stats=False):
-        assert self._t == 0                      # run() clears the fill level before the update, like OnPolicyAgent.update does
-        self.calls.append(("update",))
+    def run_episodes(self, max_steps, budget):
+        assert budget is None and max_steps >= 1
+        first = self.T - self._t                 # steps to the end of the rollout being filled
+        steps = max_steps if max_steps < first else max_steps - (max_steps - first) % self.T
+        self.calls.append(("run_episodes", max_steps, steps))
+        for _ in range(steps):
+            self.env._step()
+        self._t = (self._t + steps) % self.T
+        return steps, 0
 
     def plan(self, env):
         from_stage = pkg_core.FusedAction("policy")
@@ -386,20 +389,21 @@ class StubFusedAgent:
         pass
 
 
-def test_fused_fast_path_hands_whole_stretches_to_collect(pkg):
-    """run() with a fusable agent + a hook that does nothing per step + StopAfterNSteps: stretches of min(T - t, remaining) steps, an
-    update whenever the rollout is full, exactly n env steps in total — and the stage loop otherwise."""
+def test_fused_fast_path_hands_whole_stretches_to_run_episodes(pkg):
+    """run() with a fusable agent + a hook that does nothing per step + StopAfterNSteps: calls of the remaining steps (no
+    episode budget) until exactly n env steps ran — a call that ends at a rollout boundary is followed by one for the rest — and the
+    stage loop otherwise."""
     global pkg_core
     pkg_core = pkg.core
     agent = StubFusedAgent(T=8)
     env = StubVecEnv([5, 7])
     pkg.run(agent, env, pkg.StopAfterNSteps(21), pkg.DeviceEpisodeStats())   # per_step = False: nothing happens at the act stages
-    assert agent.calls == [("collect", 8), ("update",), ("collect", 8), ("update",), ("collect", 5)]
+    assert agent.calls == [("run_episodes", 21, 16), ("run_episodes", 5, 5)]
     assert agent._t == 5 and env.log[0] == ("reset", True) and env.log[-1] == ("check",)
     assert agent.pushed == ["PreExperimentStage", "PreEpisodeStage", "PostExperimentStage"]   # run.jl:47: the forced reset starts an episode
     # a second run continues filling the same rollout: 3 more steps complete it
     pkg.run(agent, env, pkg.StopAfterNSteps(4), pkg.EmptyHook())
-    assert agent.calls[-3:] == [("collect", 3), ("update",), ("collect", 1)]
+    assert agent.calls[-2:] == [("run_episodes", 4, 3), ("run_episodes", 1, 1)]
     # a per-step hook (or a reset condition) falls back to the stage protocol: plan! -> act_fused per step
     agent2 = StubFusedAgent(T=8)
     pkg.run(agent2, StubVecEnv([5, 7]), pkg.StopAfterNSteps(3), pkg.BatchStepsPerEpisode(2))

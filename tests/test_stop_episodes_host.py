@@ -2,7 +2,8 @@
 
 csrc/stop_episodes.cuh's crossing arithmetic (the first step at which the per-step episode counts reach the remaining budget)
 compiled for the host and compared with a NumPy restatement; run()'s dispatch of StopAfterNEpisodes to the fused library calls
-(b200rl_*_run_episodes) on stub envs and agents, and to the stage loop where the fused path does not apply."""
+(b200rl_*_run_episodes) on stub envs and agents, and to the stage loop where the fused path does not apply; the same dispatch for
+StopAfterNSteps (no episode budget)."""
 import ctypes as C
 import os
 import subprocess
@@ -162,7 +163,8 @@ class StubEnv:
 
 
 class StubAgent:
-    """a device agent stand-in: the stage protocol steps the env through act_; run_episodes steps it up to the crossing"""
+    """a device agent stand-in: the stage protocol steps the env through act_; run_episodes steps it up to the crossing, or
+    max_steps steps without a budget"""
 
     def __init__(self, fusable=True, host_actions=False):
         self.fusable, self.host_actions = fusable, host_actions
@@ -184,6 +186,8 @@ class StubAgent:
         while steps < max_steps:
             self.env.step()
             steps += 1
+            if budget is None:
+                continue
             episodes += int(self.env.term.sum())
             if episodes >= budget:
                 break
@@ -225,6 +229,33 @@ def test_dispatch_fused(pkg, which, k, cur):
         assert len(agent.calls) == -(-env.steps // window)
         assert env.flushes >= len(agent.calls)
     assert agent.calls[0][1] == k - cur
+
+
+def stage_reference_steps(pkg, n, cur):
+    """steps and stop.cur of the stage loop for StopAfterNSteps(n, cur) with a per-step hook"""
+    env, agent = StubEnv(PERIODS), StubAgent(fusable=False)
+    stop = pkg.StopAfterNSteps(n, cur)
+    pkg.run(agent, env, stop, pkg.BatchStepsPerEpisode(env.n))
+    assert not agent.calls
+    return env.steps, stop.cur
+
+
+@pytest.mark.parametrize("which", ["empty", "log", "composed"])
+@pytest.mark.parametrize("n,cur", [(1, 1), (12, 1), (13, 1), (13, 4), (7, 9)])
+def test_dispatch_fused_steps(pkg, which, n, cur):
+    """StopAfterNSteps through the same call, without an episode budget: windows of none, 4 and 3 steps"""
+    env, agent = StubEnv(PERIODS), StubAgent()
+    stop = pkg.StopAfterNSteps(n, cur)
+    pkg.run(agent, env, stop, make_hook(pkg, which, env.n), pkg.ResetIfEnvTerminated())
+    assert agent.calls, "the fused call was not taken"
+    assert all(budget is None for _, budget in agent.calls)
+    assert (env.steps, stop.cur) == stage_reference_steps(pkg, n, cur)
+    window = {"empty": None, "log": 4, "composed": 3}[which]
+    if window is None:
+        assert agent.calls == [(env.steps, None)]
+    else:
+        assert [m for m, _ in agent.calls] == [min(window, env.steps - j) for j in range(0, env.steps, window)]
+        assert env.flushes >= len(agent.calls)
 
 
 def test_dispatch_stage_loop(pkg):
