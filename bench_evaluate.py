@@ -98,6 +98,7 @@ def main():
 
     # ---- stage protocol: run(EvaluationPolicy) with device-side episode statistics -----------------------------------------
     policy = pkg.EvaluationPolicy(net, n)
+    policy.fusable = False      # the stage loop itself (run() would take the fused evaluation kernel: bench_evaluate_run.py)
     hook = pkg.DeviceEpisodeStats()
     stage = lambda: pkg.run(policy, env, pkg.StopAfterNSteps(args.stage_steps), hook)
     stage()

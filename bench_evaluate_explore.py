@@ -93,6 +93,7 @@ def main():
 
     # ---- context: the stage protocol, q_explore + act! launches per step ------------------------------------------------------
     policy = pkg.QBasedPolicy(ctx, types.SimpleNamespace(net=net), explorers["epsilon_greedy"](), xseeds, n)
+    policy.fusable = False      # the stage loop itself (run() would take the fused evaluation kernel: bench_evaluate_run.py)
     hook = pkg.DeviceEpisodeStats()
     stage = []
     for rep in range(args.reps + 1):

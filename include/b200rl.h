@@ -192,8 +192,8 @@ int b200rl_env_episode_stats(b200rl_env* env, double* out4, int reset_after);
  * Every act! that ends an episode (the finished-episode rule of b200rl_env_episode_stats:
  * the MaxTimeoutEnv cut counts, a terminal env stepped again without a reset does not) writes {return, length} to the env's
  * next slot: the return is the Float32 step-order sum of the episode's rewards (FIELD_EPISODE_RETURN), the length env.t.
- * b200rl_env_step / _step_random, the fused rollout, b200rl_onpolicy_iterate and b200rl_replay_run write it;
- * b200rl_evaluate / b200rl_evaluate_explore do not (an evaluation is a run of its own).  b200rl_env_copy does not copy it. */
+ * b200rl_env_step / _step_random, the fused rollout, b200rl_onpolicy_iterate, b200rl_replay_run and b200rl_eval_run_episodes write
+ * it; b200rl_evaluate / b200rl_evaluate_explore do not (an evaluation is a run of its own).  b200rl_env_copy does not copy it. */
 int b200rl_env_episode_log(b200rl_env* env, int32_t K);
 /* one record of a flushed list: env = rank * N + i on a sharded ctx (rank of b200rl_comm_rank_world), else i */
 typedef struct {
@@ -393,6 +393,31 @@ int b200rl_evaluate(b200rl_net* net, b200rl_env* env, const b200rl_eval_config* 
  * and ex->step advances by world N n_steps. */
 int b200rl_evaluate_explore(b200rl_net* net, b200rl_env* env, int32_t n_steps, int32_t max_episodes, b200rl_explorer* ex,
                             uint64_t* explorer_rng_dev, float* returns_out, int32_t* lengths_out, int32_t* counts_out, int on_device);
+/* run(policy, env, StopAfterNSteps | StopAfterNEpisodes(k), hook) for a policy that does not train: the network's greedy (mode 0)
+ * or sampling (mode 1, kinds 0 / 1) policy, or QBasedPolicy (mode 2, kinds 2 / 3).  Unlike b200rl_evaluate it continues from the
+ * env's current state (run() has force-reset it once), writes no records but the env's episode log when one is attached, and stops
+ * on an episode count.  The handle holds the buffers of the episode count across calls; create refuses what b200rl_evaluate[_explore]
+ * refuse, with their statuses (a Float64 env without b200rl_env_set_state_f32, Acrobot, mode 1 on a Q-network, a Q-network on a
+ * continuous env, an input / head width that does not match).  The net and env must outlive the handle. */
+typedef struct b200rl_eval b200rl_eval;
+int b200rl_eval_create(b200rl_net* net, b200rl_env* env, int32_t mode, b200rl_eval** out);
+int b200rl_eval_destroy(b200rl_eval* h);
+/* At most max_steps (>= 1) steps of the stage loop's {plan!, act! with the in-kernel auto-reset, check!}: plan! is mode 0's
+ * b200rl_net_act_greedy, mode 1's b200rl_net_act sampler on the (4, N) DEVICE policy streams rng_dev, mode 2's b200rl_net_q_explore
+ * (ex; column numbering and ex->step as b200rl_evaluate_explore, on the explorer streams rng_dev) or, ex = NULL, GreedyExplorer.
+ * Every env field (streams, statistics and the episode log's records and write counts included) and the streams end bit for bit
+ * where the stage loop leaves them; ex->step advances by N · world per step run, only on success; the network is only read.
+ * budget < 0 (StopAfterNSteps): exactly max_steps steps, nothing counted (*episodes_done = 0), allocated or synchronised; a sharded
+ * ctx is accepted.  budget >= 0 (StopAfterNEpisodes, budget = max(0, k - cur)): stops after s*, *steps_done and *episodes_done as
+ * b200rl_onpolicy_run_episodes.  Stretches of at most 1024 steps, one fused evaluation launch each for hidden = 64 on the tensor-core
+ * path (staged plan! / act! / count launches otherwise, no host sync per step), and one synchronisation per stretch; a stretch that
+ * could reach the budget first copies the env's step arrays and the streams to a shadow (about 100 B per env, allocated by the
+ * handle's first call with a budget), and stretches of 64 steps are used once fewer than 64 N episodes remain.  Refused before any
+ * side effect: the create checks again, max_steps < 1, an explorer outside mode 2, missing streams, a bad explorer or an explorer
+ * step overflow (B200RL_ERR_INVALID; with a budget: when not one more step fits, and a run stops early where the next would not),
+ * and a budget on a sharded ctx (B200RL_ERR_UNSUPPORTED). */
+int b200rl_eval_run_episodes(b200rl_eval* h, uint64_t* rng_dev, b200rl_explorer* ex, int64_t max_steps, int64_t budget,
+                             int64_t* steps_done, int64_t* episodes_done);
 
 /* ---------------------------------------------------------------- on-policy agent -- */
 /* PPO (clipped surrogate) / A2C hyper-parameters; defaults of the in-tree example

@@ -162,6 +162,9 @@ SIGNATURES = {
     "b200rl_net_act_greedy": (_i32, [_vp, _vp, _i64, _vp, _i32]),
     "b200rl_evaluate": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32]),
     "b200rl_evaluate_explore": (_i32, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32]),
+    "b200rl_eval_create": (_i32, [_vp, _vp, _i32, _vp]),
+    "b200rl_eval_destroy": (_i32, [_vp]),
+    "b200rl_eval_run_episodes": (_i32, [_vp, _vp, _vp, _i64, _i64, C.POINTER(_i64), C.POINTER(_i64)]),
     "b200rl_net_ac_step": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _f32, _f32, _i32, _vp]),
     "b200rl_onpolicy_create": (_i32, [_vp, _vp, _vp, _vp, _vp, _pp]),
     "b200rl_onpolicy_destroy": (_i32, [_vp]),

@@ -283,10 +283,10 @@ def _flush(logs):
 
 def _run_fused(policy, env, stop_condition, hook):
     """StopAfterNSteps or StopAfterNEpisodes on the fused paths: windows of at most the episode log's capacity, each one library call
-    (b200rl_*_run_episodes) followed by a flush.  The library cuts a window into stretches; a StopAfterNEpisodes window stops at the
+    (b200rl_*_run_episodes, b200rl_eval_run_episodes) followed by a flush.  The library cuts a window into stretches; a StopAfterNEpisodes window stops at the
     crossing of the remaining budget, a StopAfterNSteps one (no budget) may end early at the end of a rollout.  Returns False
     (nothing run) where the stage loop keeps the run: an episode count on a sharded ctx (the stop would count the episodes of every
-    rank), a replay agent the device loop does not take."""
+    rank), a replay agent the device loop does not take, an evaluation policy / env pair the fused evaluation does not take."""
     episodes = isinstance(stop_condition, StopAfterNEpisodes)
     if episodes and env.ctx.rank_world()[1] > 1:
         return False
@@ -294,6 +294,10 @@ def _run_fused(policy, env, stop_condition, hook):
         if not policy.replay_supported(env):
             return False
         step = lambda n, budget: policy.run_replay_episodes(env, n, budget)
+    elif hasattr(policy, "eval_handle"):       # EvaluationPolicy, a QBasedPolicy on its own
+        if policy.eval_handle(env) is None:
+            return False
+        step = lambda n, budget: policy.run_episodes(env, n, budget)
     else:
         step = policy.run_episodes
     logs, window = _episode_log_window(hook)

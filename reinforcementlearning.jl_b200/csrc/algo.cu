@@ -295,12 +295,12 @@ struct Shadow {
         return B200RL_OK;
     }
 };
-// Per-step counts of one stretch and its crossing: `counts` (s + 2 entries; the last two receive {s*, episodes}) is zeroed, `count`
-// launches the counting kernel, the crossing is read back through the pinned pair `host` (synchronises: once per stretch).
+// Per-step counts of one stretch and its crossing: `counts` (s + 2 entries; the last two receive {s*, episodes}; zeroed before the
+// stretch ran, which may have counted already), `count` launches the counting kernel, the crossing is read back through the pinned
+// pair `host` (synchronises: once per stretch).
 template <class Count>
 static int stop_crossing(b200rl_ctx* ctx, unsigned long long* counts, int64_t s, int64_t remaining, long long* host, Count&& count,
                          StopCrossing* out) {
-    CUDA_TRY(cudaMemsetAsync(counts, 0, (size_t)s * sizeof(unsigned long long), ctx->stream));
     TRY(count());
     long long* dev_out = (long long*)(counts + s);
     stop::crossing_kernel<<<1, 1, 0, ctx->stream>>>(counts, s, remaining, dev_out);
@@ -331,15 +331,15 @@ struct StopBuffers {
 };
 
 /* The one loop of a fused run: at most max_steps env steps of run(agent, env, StopAfterNSteps | StopAfterNEpisodes), cut into
- * stretches by the agent (`ops`: OnPolicyStretches, ReplayStretches).  budget >= 0: a stretch that could reach the budget
+ * stretches by the agent (`ops`: OnPolicyStretches, ReplayStretches, EvalStretches).  budget >= 0: a stretch that could reach the budget
  * (N · s >= budget - episodes so far) is marked first; the terminal flags it wrote are counted; if the budget is reached before its
  * last step, the mark and the host counters are restored and its first s* steps run instead.  budget < 0: nothing is marked or
  * counted — no allocation and no synchronisation per stretch, so a sharded ctx may run it — and the run returns at the agent's
  * last boundary (the end of a rollout) inside max_steps, if there is one: a window of the caller never splits a rollout that
  * would otherwise run as one graph launch.
  * Ops: Saved save() / restore(Saved) of the host counters; shadow_bytes() and longest() (stretch) of the buffers; mark() the
- * device state into the shadow; stretch(left, counting) -> s; run(s, may_stop); count(s, Saved) launches the counting kernel;
- * end_stretch() after the count; at_boundary(left). */
+ * device state into the shadow; stretch(left, counting, remaining) -> s; run(s, may_stop), which may add the per-step counts itself
+ * (the counts are zeroed before it); count(s, Saved) launches the counting kernel; end_stretch() after the count; at_boundary(left). */
 template <class Ops>
 static int run_stretches(b200rl_ctx* ctx, StopBuffers& sb, int64_t N, Ops& ops, int64_t max_steps, int64_t budget, int64_t* steps_done,
                          int64_t* episodes_done) {
@@ -347,8 +347,8 @@ static int run_stretches(b200rl_ctx* ctx, StopBuffers& sb, int64_t N, Ops& ops, 
     if (counting) TRY(sb.alloc(ctx, ops.shadow_bytes(), ops.longest()));
     int64_t done = 0, episodes = 0;
     while (done < max_steps) {
-        const int64_t s = ops.stretch(max_steps - done, counting);
         const int64_t remaining = budget - episodes;
+        const int64_t s = ops.stretch(max_steps - done, counting, remaining);
         const typename Ops::Saved saved = ops.save();
         const bool may_stop = counting && remaining <= N * s;   // (a lane ends at most one episode per step)
         if (may_stop) {
@@ -356,6 +356,7 @@ static int run_stretches(b200rl_ctx* ctx, StopBuffers& sb, int64_t N, Ops& ops, 
             TRY(ops.mark(sb.shadow));
             TRY(sb.shadow.copy(ctx, true));
         }
+        if (counting) CUDA_TRY(cudaMemsetAsync(sb.counts, 0, (size_t)s * sizeof(unsigned long long), ctx->stream));
         TRY(ops.run(s, may_stop));
         StopCrossing c{0, 0};
         if (counting) {
@@ -825,6 +826,174 @@ int b200rl_evaluate_explore(b200rl_net* n, b200rl_env* env, int32_t n_steps, int
     return B200RL_OK;
 }
 
+}  // extern "C"
+
+// ------------------------------------------------------------------ evaluation policies under run() ---------
+// run(EvaluationPolicy | QBasedPolicy, env, StopAfterNSteps | StopAfterNEpisodes, hook) on the fused evaluation kernel: the handle
+// holds the StopBuffers of run_stretches across the windows of a run (and the runs of a policy).  mode 0 greedy, 1 sampled
+// (kinds 0 / 1), 2 a Q-network planned by an explorer (kinds 2 / 3).
+struct b200rl_eval {
+    b200rl_ctx* ctx;
+    b200rl_net* net;
+    b200rl_env* env;
+    int mode;
+    StopBuffers stop;
+};
+
+// the net <-> env <-> mode checks of b200rl_evaluate / b200rl_evaluate_explore, with their statuses
+static int eval_check(b200rl_net* n, b200rl_env* env, int mode) {
+    REQUIRE(b200rl_env_internal_ctx(env) == n->ctx, B200RL_ERR_INVALID, "net/env belong to another ctx");
+    const float* obs;
+    TRY(learner_obs(env, &obs));
+    REQUIRE(b200rl_env_internal_kind(env) != B200RL_ENV_ACROBOT, B200RL_ERR_UNSUPPORTED, "AcrobotEnv has 6 observations (networks take at most 4)");
+    REQUIRE(mode >= 0 && mode <= 2, B200RL_ERR_INVALID, "mode must be 0 (greedy), 1 (sample) or 2 (QBasedPolicy)");
+    REQUIRE(!(mode == 1 && is_q_kind(n->kind)), B200RL_ERR_UNSUPPORTED, "mode 1 samples a policy head: evaluate a Q-network with mode 0 or QBasedPolicy");
+    const bool cont = b200rl_env_internal_continuous(env);
+    if (mode == 2) {
+        REQUIRE(!cont, B200RL_ERR_UNSUPPORTED, "QBasedPolicy needs a discrete action space");
+        REQUIRE(is_q_kind(n->kind), B200RL_ERR_INVALID, "needs a Q-network (kind 2 or 3)");
+    }
+    REQUIRE(b200rl_env_internal_nobs(env) == n->actor.in, B200RL_ERR_INVALID, "network input width != observation width");
+    REQUIRE(mode == 2 || cont == (n->kind == 1), B200RL_ERR_INVALID, "head kind != action-space kind (Gaussian head <-> continuous actions)");
+    REQUIRE(cont || n->actor.nout == b200rl_env_internal_n_actions(env), B200RL_ERR_INVALID, "head width != number of discrete actions");
+    return B200RL_OK;
+}
+
+// One stretch of s steps from the env's current state: the fused evaluation kernel (RUN instantiations) or, where it returns
+// B200RL_ERR_UNSUPPORTED, s x {plan!, act! (auto-reset, episode log), count} as staged launches without a host sync — plan! with the
+// launches of the stage loop's EvaluationPolicy / QBasedPolicy (b200rl_net_act_greedy | b200rl_net_act | b200rl_net_q_act |
+// b200rl_net_q_explore).  counts (may be null): counts[j] += lanes terminal after step j + 1.  ex->step is not advanced here.
+static int eval_run_stretch(b200rl_eval* h, unsigned long long* prng, const b200rl_explorer* ex, int64_t s, unsigned long long* counts) {
+    b200rl_ctx* ctx = h->ctx;
+    b200rl_net* n = h->net;
+    b200rl_env* env = h->env;
+    const int mode = h->mode;
+    int st = nn_tc_enabled() ? nn_tc_eval_run(ctx, env, n->actor, n->params, kSamplerHyper, mode, (int)s, prng, ex, counts)
+                             : B200RL_ERR_UNSUPPORTED;
+    if (st != B200RL_ERR_UNSUPPORTED) return st;
+    const int64_t N = b200rl_env_internal_n(env);
+    const int64_t NW = N * b200rl_comm_world(ctx);
+    const float* obs;
+    TRY(learner_obs(env, &obs));
+    const bool cont = b200rl_env_internal_continuous(env), f64 = b200rl_env_internal_dtype(env) == B200RL_F64;
+    const float bound = b200rl_env_internal_action_bound(env);
+    void* sc;
+    TRY(ctx_scratch(ctx, round256((size_t)N * 4) + round256((size_t)N * 8) + round256((size_t)N * n->actor.nout * 4), &sc));
+    uint32_t* act = (uint32_t*)sc;
+    void* act_clamped = (char*)sc + round256((size_t)N * 4);
+    float* heads = (float*)((char*)sc + round256((size_t)N * 4) + round256((size_t)N * 8));
+    const uint8_t* flags = (const uint8_t*)env_field(env, B200RL_FIELD_FLAGS);
+    for (int64_t k = 0; k < s; ++k) {
+        const void* a_env = act;
+        if (mode == 0) {
+            TRY(nn_mlp_forward(ctx, n->actor, n->params, obs, N, heads));
+            greedy_select_kernel<<<grid_for(N, 256), 256, 0, ctx->stream>>>(heads, n->actor, N, cont ? 1 : 0, -bound, bound, act);
+            LAUNCH_CHECK(ctx);
+            if (cont && f64) {   // Float64 of the clamped mu
+                TRY(env_action_clamped(env, (const float*)act, N, act_clamped));
+                a_env = act_clamped;
+            }
+        } else if (mode == 1) {
+            TRY(nn_policy_act(ctx, n->actor, n->critic, n->params, kSamplerHyper, obs, N, prng, act, nullptr, nullptr, nullptr, nullptr));
+            if (cont) {
+                TRY(env_action_clamped(env, (const float*)act, N, act_clamped));
+                a_env = act_clamped;
+            }
+        } else if (!ex) {   // GreedyExplorer
+            TRY(nn_q_act(ctx, n->actor, n->params, obs, N, nullptr, 0.0f, (int32_t*)act, heads));
+        } else {
+            b200rl_explorer e = *ex;
+            e.step = ex->step + k * NW;    // BatchExplorer: the inner explorer's step moved N · world times per plan!
+            TRY(nn_q_explore(ctx, n->actor, n->params, obs, N, prng, e, (int32_t*)act, heads));
+        }
+        TRY(b200rl_env_step(env, a_env, 1, 1));
+        if (counts) {
+            stop::count_columns_kernel<<<dim3(grid_for(N, stop::kCountBlock), 1), stop::kCountBlock, 0, ctx->stream>>>(flags, N, 0, 1, counts + k);
+            LAUNCH_CHECK(ctx);
+        }
+    }
+    return B200RL_OK;
+}
+
+/* The evaluation policy's part of run_stretches: stretches of stop::eval_stretch steps, each of which counts as it runs
+ * (eval_run_stretch).  The shadow is the env's step regions and the (4, N) policy or explorer streams; a rollback restores the env's step
+ * counter and the explorer step. */
+struct EvalStretches {
+    b200rl_eval* h;
+    unsigned long long* prng;      // (4, N) policy streams (mode 1), explorer streams (mode 2 with an explorer), or null
+    b200rl_explorer* ex;           // mode 2; null: GreedyExplorer
+    bool counting;
+    int64_t N, NW;
+    struct Saved { int64_t ex_step; uint64_t env_steps; };
+    Saved save() const { return {ex ? ex->step : 0, b200rl_env_internal_steps(h->env)}; }
+    void restore(const Saved& s0) const {
+        if (ex) ex->step = s0.ex_step;
+        b200rl_env_internal_add_steps(h->env, s0.env_steps - b200rl_env_internal_steps(h->env));
+    }
+    size_t shadow_bytes() const { return b200rl_env_internal_step_bytes_max(h->env) + round256((size_t)N * 32); }
+    int64_t longest() const { return stop::kEvalStretchMax; }
+    int mark(Shadow& sh) const {
+        DevRegion er[kEnvStepRegionsMax];
+        TRY(sh.add_regions(er, b200rl_env_internal_step_regions(h->env, er)));
+        return prng ? sh.add(prng, (size_t)N * 32) : B200RL_OK;
+    }
+    int64_t stretch(int64_t left, bool c, int64_t remaining) const { return stop::eval_stretch(left, remaining, N, c); }
+    int run(int64_t s, bool) {
+        TRY(eval_run_stretch(h, prng, ex, s, counting ? h->stop.counts : nullptr));
+        if (ex) ex->step += s * NW;
+        return B200RL_OK;
+    }
+    int count(int64_t, const Saved&, unsigned long long*) const { return B200RL_OK; }   // (counted by run)
+    int end_stretch() const { return B200RL_OK; }
+    bool at_boundary(int64_t) const { return false; }
+};
+
+extern "C" {
+
+int b200rl_eval_create(b200rl_net* net, b200rl_env* env, int32_t mode, b200rl_eval** out) {
+    REQUIRE(net && env && out, B200RL_ERR_INVALID, "null argument");
+    TRY(eval_check(net, env, mode));
+    b200rl_eval* h = new b200rl_eval();
+    h->ctx = net->ctx; h->net = net; h->env = env; h->mode = mode;
+    *out = h;
+    return B200RL_OK;
+}
+
+int b200rl_eval_destroy(b200rl_eval* h) {
+    if (!h) return B200RL_OK;
+    cudaSetDevice(h->ctx->device);
+    cudaStreamSynchronize(h->ctx->stream);
+    h->stop.release();
+    delete h;
+    return B200RL_OK;
+}
+
+/* run(policy, env, StopAfterNSteps | StopAfterNEpisodes(k)) for at most max_steps env steps (include/b200rl.h): run_stretches */
+int b200rl_eval_run_episodes(b200rl_eval* h, uint64_t* rng_dev, b200rl_explorer* ex, int64_t max_steps, int64_t budget, int64_t* steps_done,
+                             int64_t* episodes_done) {
+    REQUIRE(h && steps_done && episodes_done, B200RL_ERR_INVALID, "null argument");
+    REQUIRE(max_steps >= 1, B200RL_ERR_INVALID, "max_steps must be >= 1");
+    REQUIRE(budget < 0 || b200rl_comm_world(h->ctx) == 1, B200RL_ERR_UNSUPPORTED,
+            "StopAfterNEpisodes counts the episodes of every rank: a sharded ctx keeps the stage loop");
+    TRY(eval_check(h->net, h->env, h->mode));   // (the Float32 wrapper may have been removed since create)
+    REQUIRE(h->mode == 2 || !ex, B200RL_ERR_INVALID, "an explorer plans a Q-network: mode 2 only");
+    REQUIRE(h->mode != 1 || rng_dev, B200RL_ERR_INVALID, "mode 1 needs the (4, N) device policy streams");
+    const int64_t N = b200rl_env_internal_n(h->env);
+    const int64_t NW = N * b200rl_comm_world(h->ctx);   // columns of one plan! over the ranks' union (DESIGN.md §3)
+    int64_t run_steps = max_steps;
+    if (ex) {
+        REQUIRE(rng_dev, B200RL_ERR_INVALID, "an explorer other than GreedyExplorer needs the (4, N) device explorer streams");
+        TRY(check_explorer(ex));
+        const int64_t room = ((1ll << 62) - (ex->step > 0 ? ex->step : 0)) / NW;   // steps before the explorer step overflows
+        REQUIRE(budget < 0 ? max_steps <= room : room >= 1, B200RL_ERR_INVALID, "explorer step would overflow");
+        if (room < run_steps) run_steps = room;   // (with a budget the run stops there; the next call is refused)
+    }
+    TRY(ctx_bind(h->ctx));
+    unsigned long long* prng = (h->mode == 1 || ex) ? (unsigned long long*)rng_dev : nullptr;
+    EvalStretches ops{h, prng, ex, budget >= 0, N, NW};
+    return run_stretches(h->ctx, h->stop, N, ops, run_steps, budget, steps_done, episodes_done);
+}
+
 /* One optimiser step from explicit on-policy minibatch arrays (all HOST; test / generic entry):
  * loss + gradient (K7), global-norm clip + Adam (K8).  losses_out[6] = actor_loss, critic_loss,
  * entropy, loss, grad_norm (pre-clip), 0.  apply_update = 0 leaves the parameters untouched (gradient only). */
@@ -1227,7 +1396,7 @@ struct OnPolicyStretches {
         }
         return B200RL_OK;
     }
-    int64_t stretch(int64_t left, bool) const { return a->T - a->t < left ? a->T - a->t : left; }
+    int64_t stretch(int64_t left, bool, int64_t) const { return a->T - a->t < left ? a->T - a->t : left; }
     int run(int64_t s, bool may_stop) {
         whole = !may_stop && a->t == 0 && s == a->T;
         if (!whole) return b200rl_onpolicy_collect(a, (int)s);
@@ -1645,7 +1814,7 @@ struct ReplayStretches {
         TRY(sh.add(n->beta_t, 2 * 4)); TRY(sh.add(n->loss4, 4 * 4)); TRY(sh.add(n->gnorm, 4));
         return sh.add(r->td_keep, (size_t)r->B * 4);
     }
-    int64_t stretch(int64_t left, bool counting) const { return counting && r->stop_chunk < left ? r->stop_chunk : left; }
+    int64_t stretch(int64_t left, bool counting, int64_t) const { return counting && r->stop_chunk < left ? r->stop_chunk : left; }
     int run(int64_t s, bool) const { return b200rl_replay_run(r, rng, ex, ctl, s, nullptr); }
     int count(int64_t s, const Saved&, unsigned long long* counts) const {
         b200rl_ctx* ctx = r->ctx;

@@ -450,6 +450,11 @@ struct EvalExploreArgs : EvalArgs {
     long long col0, stride;             // rank · N and world · N (0 and N on one GPU)
 };
 template <int MODE> using EvalArgsOf = typename std::conditional<MODE == 2, EvalExploreArgs, EvalArgs>::type;
+// RUN: the arguments of MODE and the per-step terminal counts of a stretch of run() (b200rl_eval_run_episodes)
+template <int MODE> struct EvalRunArgs : EvalArgsOf<MODE> {
+    unsigned long long* step_counts;    // (nsteps): += lanes terminal after step j + 1 of the window; may be null
+};
+template <int MODE, bool RUN> using EvalKernelArgs = typename std::conditional<RUN, EvalRunArgs<MODE>, EvalArgsOf<MODE>>::type;
 // the window reads and writes back a (4, N) stream per env: the policy streams (MODE 1) or the explorer streams (MODE 2, not greedy)
 template <int MODE> __device__ __forceinline__ bool eval_streams(const EvalArgsOf<MODE>& g) {
     if constexpr (MODE == 2) return !g.greedy;
@@ -459,9 +464,13 @@ template <int MODE> __device__ __forceinline__ bool eval_streams(const EvalArgsO
 // MODE 0: greedy (greedy.cuh, no draw), 1: sample_head on the policy streams, 2: a Q-network planned by its explorer
 // (plan_q_column, b200rl_evaluate_explore).  DUEL (MODE 0 / 2): a dueling Q-network, its head rows combined into Q (duel.cuh) before
 // the selection; the instantiations without it are the code of the other kinds.  XEXT (MODE 2): the explorer kinds 2-4 compiled.
+// RUN: a stretch of run(policy, env, stop) rather than an evaluation of its own — no records (K = 0); each step's terminal lanes are
+// added to g.step_counts[step] (one __syncthreads_count per resident tile, one atomic per CTA and step), and with LOG the finished episodes
+// go to the env's episode log as the rollout and collect kernels write it.  The instantiations without RUN are the code of b200rl_evaluate.
 // (layer 1 and the head epilogue not unrolled: the relu variants would exceed 128 registers and spill)
-template <class Env, int ACT, int MODE, bool DUEL = false, bool XEXT = false>
-__global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgsOf<MODE> g, typename Env::P p, EnvArrays ea) {
+template <class Env, int ACT, int MODE, bool DUEL = false, bool XEXT = false, bool RUN = false, bool LOG = false>
+__global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalKernelArgs<MODE, RUN> g, typename Env::P p, EnvArgs<LOG> ea) {
+    static_assert(RUN || !LOG, "b200rl_evaluate writes no episode log");
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     SmemEval<Env>& sm = *reinterpret_cast<SmemEval<Env>*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -489,6 +498,7 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgsOf<MODE> g, 
         __syncthreads();
 #pragma unroll 1
         for (int step = 0; step < g.nsteps; ++step) {
+            int ended = 0;                  // RUN: lanes of the group terminal after this step (the same in every thread)
 #pragma unroll 1
             for (int k = 0; k < nslots; ++k) {
                 // (env index and slot are recomputed after the GEMM rather than held in registers across it)
@@ -501,6 +511,7 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgsOf<MODE> g, 
                 __syncthreads();
                 tile_forward<ACT, 1>(sm.net, g.actor.act, c, s, sm.T, sm.X, sm.Zp);
                 const int64_t i = (base + (int64_t)k * nctas) * TM + s;
+                bool done = false;
                 if (owner && i < N) {
                     EvalSlot<Env>& sl = sm.slot[k];
                     float z[kOutMax];
@@ -519,9 +530,12 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgsOf<MODE> g, 
                         a_bits = policy::sample_head(g.actor.heads2, g.actor.nout, g.hp, z, pr, lp);
                         put_stream(sl.prng, s, pr);
                     }
-                    // (no episode log: an evaluation is a run of its own, whose episodes the training hook does not see)
-                    const ActStep<float> r = slot_act(sl, s, p, ea.max_timeout, env_action<Env>(a_bits), sm.fin_cnt[s], sm.fin_ret[s], sm.fin_len[s]);
-                    if (r.done) {
+                    // (no episode log without RUN: an evaluation is a run of its own, whose episodes the training hook does not see)
+                    const ActStep<float> r = slot_act<Env, LOG>(sl, s, p, ea.max_timeout, env_action<Env>(a_bits), sm.fin_cnt[s], sm.fin_ret[s],
+                                                                sm.fin_len[s], episode_log_of(ea), i);
+                    if constexpr (RUN) {
+                        done = r.done;
+                    } else if (r.done) {
                         const int e = sl.cnt[s];   // record of the episode that ends: its return and env.t
                         if (e < g.K) {
                             if (g.returns) g.returns[(size_t)g.K * i + e] = r.ret;
@@ -530,6 +544,10 @@ __global__ void __launch_bounds__(NT, 2) evaluate_tc_kernel(EvalArgsOf<MODE> g, 
                         sl.cnt[s] = e + 1;
                     }
                 }
+                if constexpr (RUN) ended += __syncthreads_count(done);
+            }
+            if constexpr (RUN) {
+                if (tid == 0 && ended && g.step_counts) atomicAdd(g.step_counts + step, (unsigned long long)ended);
             }
         }
         // (each owner thread touches only its own entries: no barrier before the next group's loads)
@@ -746,17 +764,23 @@ template <class F> int with_learner_env(const EnvView& v, F&& f) {
 }
 
 // the evaluate_tc_kernel instantiation of the network's activation (and, MODE 0 / 2, of a dueling head)
-template <class Env, int MODE, bool XEXT = false>
-int launch_evaluate(b200rl_ctx* ctx, int64_t groups, const EvalArgsOf<MODE>& g, const typename Env::P& p, const EnvArrays& ea) {
+template <class Env, int MODE, bool XEXT = false, bool RUN = false, bool LOG = false>
+int launch_evaluate(b200rl_ctx* ctx, int64_t groups, const EvalKernelArgs<MODE, RUN>& g, const typename Env::P& p, const EnvArgs<LOG>& ea) {
     constexpr int RELU = B200RL_ACT_RELU, TANH = B200RL_ACT_TANH;
     const bool relu = g.actor.act == RELU;
     if constexpr (MODE != 1) {
         if (g.actor.duel)
-            return relu ? launch_fused<evaluate_tc_kernel<Env, RELU, MODE, true, XEXT>, SmemEval<Env>>(ctx, groups, g, p, ea)
-                        : launch_fused<evaluate_tc_kernel<Env, TANH, MODE, true, XEXT>, SmemEval<Env>>(ctx, groups, g, p, ea);
+            return relu ? launch_fused<evaluate_tc_kernel<Env, RELU, MODE, true, XEXT, RUN, LOG>, SmemEval<Env>>(ctx, groups, g, p, ea)
+                        : launch_fused<evaluate_tc_kernel<Env, TANH, MODE, true, XEXT, RUN, LOG>, SmemEval<Env>>(ctx, groups, g, p, ea);
     }
-    return relu ? launch_fused<evaluate_tc_kernel<Env, RELU, MODE, false, XEXT>, SmemEval<Env>>(ctx, groups, g, p, ea)
-                : launch_fused<evaluate_tc_kernel<Env, TANH, MODE, false, XEXT>, SmemEval<Env>>(ctx, groups, g, p, ea);
+    return relu ? launch_fused<evaluate_tc_kernel<Env, RELU, MODE, false, XEXT, RUN, LOG>, SmemEval<Env>>(ctx, groups, g, p, ea)
+                : launch_fused<evaluate_tc_kernel<Env, TANH, MODE, false, XEXT, RUN, LOG>, SmemEval<Env>>(ctx, groups, g, p, ea);
+}
+// a stretch of run(): the instantiation with the episode log when the env has one attached, the one without it otherwise
+template <class Env, int MODE, bool XEXT = false>
+int launch_eval_run(b200rl_ctx* ctx, int64_t groups, const EvalRunArgs<MODE>& g, const typename Env::P& p, const EnvView& v) {
+    if (v.log.count) return launch_evaluate<Env, MODE, XEXT, true, true>(ctx, groups, g, p, EnvArraysLog{v.a, v.log});
+    return launch_evaluate<Env, MODE, XEXT, true, false>(ctx, groups, g, p, v.a);
 }
 
 template <class Env, bool XEXT, bool LOG>
@@ -851,6 +875,35 @@ int nn_tc_evaluate(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const
         if constexpr (std::is_floating_point<typename Env::act_t>::value) return (int)B200RL_ERR_UNSUPPORTED;   // (rejected above)
         else if (ex && ex->kind >= 2) return launch_evaluate<Env, 2, true>(ctx, groups, gx, p, v.a);
         else return launch_evaluate<Env, 2>(ctx, groups, gx, p, v.a);
+    });
+    if (st == B200RL_OK) b200rl_env_internal_add_steps(env, (uint64_t)nsteps);
+    return st;
+}
+
+// A stretch of nsteps steps of run(policy, env, stop) on the fused evaluation kernel (RUN instantiations): the window of
+// nn_tc_evaluate from the env's current state, without records, with the episode log and the per-step counts.  The caller has
+// validated net <-> env <-> explorer; B200RL_ERR_UNSUPPORTED (no side effect, no error message) = outside the fused envelope.
+int nn_tc_eval_run(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const float* params, const AcHyper& hp, int mode, int nsteps,
+                   unsigned long long* policy_rng, const b200rl_explorer* ex, unsigned long long* step_counts) {
+    EnvView v;
+    TRY(b200rl_env_internal_view(env, &v));
+    if (!nn_tc_supported(actor) || !b200rl_env_internal_obs_f32(env) || (mode == 2 && v.continuous)) return B200RL_ERR_UNSUPPORTED;
+    const b200rl_explorer e = ex ? *ex : b200rl_explorer{};
+    const EvalArgs g{actor, params, hp, v.N, nsteps, 0, policy_rng, nullptr, nullptr, nullptr};
+    const EvalRunArgs<0> g0{g, step_counts};
+    const EvalRunArgs<2> gx{EvalExploreArgs{g, ex ? 0 : 1,
+                                            QExplorer{e.eps_stable, e.eps_init, e.warmup_steps, e.decay_steps, e.step, e.kind, e.is_break_tie},
+                                            e.beta, (long long)e.step, (long long)b200rl_comm_rank(ctx) * v.N,
+                                            (long long)b200rl_comm_world(ctx) * v.N},
+                            step_counts};
+    const int64_t groups = ((v.N + TM - 1) / TM + kSlots - 1) / kSlots;
+    const int st = with_learner_env(v, [&](auto env_type, const auto& p) {
+        using Env = typename decltype(env_type)::type;
+        if (mode == 0) return launch_eval_run<Env, 0>(ctx, groups, g0, p, v);
+        if (mode == 1) return launch_eval_run<Env, 1>(ctx, groups, EvalRunArgs<1>{g, step_counts}, p, v);
+        if constexpr (std::is_floating_point<typename Env::act_t>::value) return (int)B200RL_ERR_UNSUPPORTED;   // (rejected above)
+        else if (ex && ex->kind >= 2) return launch_eval_run<Env, 2, true>(ctx, groups, gx, p, v);
+        else return launch_eval_run<Env, 2>(ctx, groups, gx, p, v);
     });
     if (st == B200RL_OK) b200rl_env_internal_add_steps(env, (uint64_t)nsteps);
     return st;

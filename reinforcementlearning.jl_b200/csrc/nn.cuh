@@ -145,6 +145,11 @@ int nn_tc_rollout(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const 
 // staged launches instead
 int nn_tc_evaluate(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const float* params, const AcHyper& hp, int mode, int nsteps,
                    int K, unsigned long long* policy_rng, float* returns, int32_t* lengths, int32_t* counts, const b200rl_explorer* ex = nullptr);
+// the same window as a stretch of run(policy, env, stop) (b200rl_eval_run_episodes): from the env's current state, no records; the
+// finished episodes go to the env's episode log when one is attached, and step_counts (may be null) gets, per window step j, the
+// lanes terminal after step j + 1 added.  B200RL_ERR_UNSUPPORTED = outside the fused envelope
+int nn_tc_eval_run(b200rl_ctx* ctx, b200rl_env* env, const MlpDesc& actor, const float* params, const AcHyper& hp, int mode, int nsteps,
+                   unsigned long long* policy_rng, const b200rl_explorer* ex, unsigned long long* step_counts);
 // fused DQN collect window (fwd_tc.cu): nsteps x {Q -> explorer column | findmax, env step, ring push} for H = 64; the touched
 // sum-tree leaves of each lane go to keys / vals (stride, N) for one tree rebuild.  B200RL_ERR_UNSUPPORTED = outside the envelope
 struct Ring;

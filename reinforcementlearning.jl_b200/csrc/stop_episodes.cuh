@@ -29,6 +29,21 @@ __host__ __device__ inline StopCrossing crossing(const unsigned long long* count
     return StopCrossing{0, sum};
 }
 
+// The stretches of b200rl_eval_run_episodes (an evaluation policy under run(), one fused evaluation launch per stretch).
+// kEvalStretchMax bounds every stretch: the counts buffer holds kEvalStretchMax + 2 entries, and one launch stays short (about
+// 10 ms at 65 536 CartPole envs).  With an episode budget a stretch that cannot reach it (N · s < remaining) runs unmarked for as
+// long as possible; once fewer than N · kEvalStretchMarked episodes remain, stretches of kEvalStretchMarked steps are marked, so a
+// rollback re-runs at most that many steps.
+constexpr int64_t kEvalStretchMax = 1024;
+constexpr int64_t kEvalStretchMarked = 64;
+__host__ __device__ inline int64_t eval_stretch(int64_t left, int64_t remaining, int64_t N, bool counting) {
+    const int64_t s = left < kEvalStretchMax ? left : kEvalStretchMax;
+    if (!counting) return s;
+    const int64_t unmarked = remaining > 0 ? (remaining - 1) / N : 0;   // the longest stretch with N · s < remaining
+    if (unmarked >= kEvalStretchMarked) return s < unmarked ? s : unmarked;
+    return s < kEvalStretchMarked ? s : kEvalStretchMarked;
+}
+
 }  // namespace stop
 
 #ifdef __CUDACC__

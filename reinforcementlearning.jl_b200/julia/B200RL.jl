@@ -334,11 +334,13 @@ function RLCore._run(policy::AbstractPolicy, env::B200VecEnv, stop_condition::Ab
     # condition that counts steps or episodes let whole stretches of the loop run on the device, with the stage loop's results.
     # Windows of at most a B200EpisodeLog's capacity, each one library call (episodes!) followed by a flush of the log; the library
     # cuts a window into stretches.  A StopAfterNEpisodes window stops at the crossing of the remaining budget (an episode count on
-    # a sharded ctx keeps the stage loop), a StopAfterNSteps one (budget -1) may end early at the end of a rollout.
+    # a sharded ctx keeps the stage loop), a StopAfterNSteps one (budget -1) may end early at the end of a rollout.  A policy that
+    # does not train (B200GreedyPolicy, a B200QBasedPolicy on its own) runs on the fused evaluation kernel (b200rl_eval_run_episodes).
     window = hook isa B200EpisodeLog ? hook.capacity : typemax(Int)
     if hook isa Union{B200EpisodeStats,B200EpisodeLog,RLCore.EmptyHook} && reset_condition isa ResetIfEnvTerminated && env.auto_reset &&
        (stop_condition isa StopAfterNSteps || (stop_condition isa StopAfterNEpisodes && ctx_world(env) == 1)) &&
-       ((policy isa B200OnPolicyAgent && policy.fused) || (policy isa B200Agent && replay!(policy, env, 0)))
+       ((policy isa B200OnPolicyAgent && policy.fused) || (policy isa B200Agent && replay!(policy, env, 0)) ||
+        (policy isa Union{B200GreedyPolicy,B200QBasedPolicy} && eval_fusable(policy, env)))
         while true
             if stop_condition isa StopAfterNSteps                  # check! is true once cur >= step, then cur += 1
                 steps, _ = episodes!(policy, env, min(window, max(1, stop_condition.step - stop_condition.cur + 1)), -1)
@@ -905,6 +907,52 @@ function episodes!(a::B200OnPolicyAgent, ::B200VecEnv, max_steps::Integer, budge
     t, T = Ref{Cint}(0), Ref{Cint}(0)
     check(ccall((:b200rl_onpolicy_fill, LIB), Cint, (Ptr{Cvoid}, Ref{Cint}, Ref{Cint}), a.h, t, T))
     a.t = Int(t[])                                                  # a stop inside a rollout leaves it part-filled
+    steps[], eps[]
+end
+# The b200rl_eval handle of an evaluation policy for `env` (made on the policy's first fused run on it, destroyed with the policy or
+# when it runs on another env); C_NULL where the library refuses the pair (the stage loop then keeps the run).
+const EVAL_HANDLES = Dict{UInt,Tuple{Ptr{Cvoid},Ptr{Cvoid}}}()   # objectid(policy) => (env handle, b200rl_eval handle)
+function eval_handle!(p, net::B200Network, env::B200VecEnv, mode::Integer)
+    id = objectid(p)
+    e = get(EVAL_HANDLES, id, nothing)
+    e !== nothing && e[1] == env.h && return e[2]
+    e === nothing || ccall((:b200rl_eval_destroy, LIB), Cint, (Ptr{Cvoid},), e[2])
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    if ccall((:b200rl_eval_create, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Int32, Ref{Ptr{Cvoid}}), net.h, env.h, mode, h) != 0
+        delete!(EVAL_HANDLES, id)
+        return C_NULL
+    end
+    e === nothing && finalizer(p) do _
+        x = pop!(EVAL_HANDLES, id, nothing)
+        x === nothing || net.ctx.h == C_NULL || ccall((:b200rl_eval_destroy, LIB), Cint, (Ptr{Cvoid},), x[2])   # (a closed ctx took its buffers)
+    end
+    EVAL_HANDLES[id] = (env.h, h[])
+    h[]
+end
+eval_fusable(p::B200GreedyPolicy, env::B200VecEnv) = !env.continuous && eval_handle!(p, p.net, env, 0) != C_NULL
+eval_fusable(p::B200QBasedPolicy, env::B200VecEnv) =
+    (device_explorer(p.explorer) || p.explorer isa GreedyExplorer) && eval_handle!(p, p.learner.net, env, 2) != C_NULL
+
+# run(policy, env, stop) of a policy that does not train (b200rl_eval_run_episodes, `_run` made the handle): the stage loop's steps,
+# episode log, streams and explorer step.  budget < 0: exactly max_steps steps.
+function episodes!(p::B200GreedyPolicy, env::B200VecEnv, max_steps::Integer, budget::Integer)
+    steps, eps = Ref{Int64}(0), Ref{Int64}(0)
+    check(ccall((:b200rl_eval_run_episodes, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Int64, Int64, Ref{Int64}, Ref{Int64}),
+                eval_handle!(p, p.net, env, 0), C_NULL, C_NULL, max_steps, budget, steps, eps))
+    steps[], eps[]
+end
+function episodes!(p::B200QBasedPolicy, env::B200VecEnv, max_steps::Integer, budget::Integer)
+    h = eval_handle!(p, p.learner.net, env, 2)
+    steps, eps = Ref{Int64}(0), Ref{Int64}(0)
+    if device_explorer(p.explorer)
+        ex = Ref(ExplorerC(p.explorer))
+        check(ccall((:b200rl_eval_run_episodes, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ref{ExplorerC}, Int64, Int64, Ref{Int64}, Ref{Int64}),
+                    h, p.d_rng, ex, max_steps, budget, steps, eps))
+        set_step!(p.explorer, ex[].step)
+    else                                                            # GreedyExplorer: findmax, no draw
+        check(ccall((:b200rl_eval_run_episodes, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Int64, Int64, Ref{Int64}, Ref{Int64}),
+                    h, C_NULL, C_NULL, max_steps, budget, steps, eps))
+    end
     steps[], eps[]
 end
 function episodes!(a::B200Agent, ::B200VecEnv, max_steps::Integer, budget::Integer)   # (replay!(a, env, 0) made the handle)

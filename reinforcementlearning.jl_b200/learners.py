@@ -455,7 +455,53 @@ class InsertSampleRatioController:
         return False
 
 
-class QBasedPolicy(AbstractPolicy):
+class _FusedEvaluation:
+    """run(policy, env, StopAfterNSteps | StopAfterNEpisodes, hook) of a policy that does not train, on the fused evaluation kernel
+    (b200rl_eval_run_episodes): the steps, episode log, streams and explorer step of the stage loop.  The library handle is created
+    for the env on the first run and kept until the env or network changes or the policy is closed."""
+    _eval = _eval_key = None
+
+    def eval_handle(self, env):
+        """the handle for runs on env, or None where the library refuses the pair or the policy has no device plan (the stage loop
+        then keeps the run and raises its own errors)"""
+        net, mode = self._eval_net_mode()
+        if net is None:
+            return None
+        key = (env.h.value, net.h.value, mode)
+        if self._eval is not None and self._eval_key == key:
+            return self._eval
+        self._close_eval()
+        h = C.c_void_p()
+        st = self.lib.b200rl_eval_create(net.h, env.h, mode, C.byref(h))
+        if st in (L.ERR_UNSUPPORTED, L.ERR_INVALID):
+            return None
+        L.check(st)
+        self._eval, self._eval_key = h, key
+        return h
+
+    def _close_eval(self):
+        if self._eval is not None:
+            if self.ctx.h:         # (a closed ctx took the handle's device buffers with it)
+                self.lib.b200rl_eval_destroy(self._eval)
+            self._eval = None
+
+    def run_episodes(self, env, max_steps, budget):
+        """At most max_steps env steps of run(policy, env, stop) on the fused path.  budget = k - cur for StopAfterNEpisodes(k): stops
+        after the step at which the episodes counted reach it, as the stage loop does (a budget <= 0: one step); budget None for
+        StopAfterNSteps: runs max_steps steps.  Returns (steps run, episodes they ended; 0 without a budget)."""
+        h = self.eval_handle(env)
+        if h is None:
+            raise RuntimeError("the fused evaluation does not take this policy / env pair")
+        ex = self._eval_explorer()
+        steps, episodes = C.c_int64(), C.c_int64()
+        L.check(self.lib.b200rl_eval_run_episodes(h, None if self._d_rng is None else C.c_void_p(self._d_rng), None if ex is None else C.byref(ex),
+                                                  int(max_steps), _library_budget(budget), C.byref(steps), C.byref(episodes)))
+        if ex is not None and hasattr(self.explorer, "step"):
+            self.explorer.step = ex.step
+        return steps.value, episodes.value
+
+
+class QBasedPolicy(_FusedEvaluation, AbstractPolicy):
     """QBasedPolicy(learner = DQNLearner(...), explorer = EpsilonGreedyExplorer(...)) (q_based_policy.jl:13-49) on a batched
     env: ``plan`` = BatchExplorer over Q(state(env), .) — forward pass, schedule, draws and arg-max in one device call.
 
@@ -471,8 +517,18 @@ class QBasedPolicy(AbstractPolicy):
         self._d_rng = ctx.malloc(rng.nbytes)
         ctx.h2d(self._d_rng, rng)
         self._d_action = ctx.malloc(self.n * 4)
+        # run() on its own (not inside an Agent) may hand whole stretches of env steps to run_episodes() when the explorer plans on
+        # the device (eval_handle checks it per run)
+        self.fusable = True
+
+    def _eval_net_mode(self):
+        return (self.learner.net if type(self.explorer) in DEVICE_EXPLORERS + (GreedyExplorer,) else None), 2
+
+    def _eval_explorer(self):
+        return self.explorer.as_struct() if type(self.explorer) in DEVICE_EXPLORERS else None
 
     def close(self):
+        self._close_eval()
         for name in ("_d_rng", "_d_action"):
             p = getattr(self, name, None)
             if p:
@@ -522,7 +578,7 @@ class QBasedPolicy(AbstractPolicy):
 EVAL_MODES = {"greedy": 0, "sample": 1}
 
 
-class EvaluationPolicy(AbstractPolicy):
+class EvaluationPolicy(_FusedEvaluation, AbstractPolicy):
     """The network's policy without training: ``plan`` runs one forward pass on state(env) and leaves the actions on the
     device, ``act_fused`` hands them to ``env.act_``.  ``run(EvaluationPolicy(net, n), env, StopAfterNSteps(k), hook)`` is the
     stage protocol of :func:`evaluate`.
@@ -530,7 +586,11 @@ class EvaluationPolicy(AbstractPolicy):
     mode "greedy": findmax of the logits / Q-values, mu of a Gaussian head (b200rl_net_act_greedy; no RNG).
     mode "sample": b200rl_net_act's sampler on one policy stream per env; ``rng``: (N, 4) uint64 raw Xoshiro states.
     A continuous action goes to the env as clamp(a, lo, hi) of its action space (through the host, like OnPolicyAgent's
-    host-action path)."""
+    host-action path).
+
+    Under run() with a hook that does nothing per step (EmptyHook, DeviceEpisodeStats, DeviceEpisodeLog) and StopAfterNSteps or
+    StopAfterNEpisodes, the loop runs on the fused evaluation kernel instead (run_episodes, b200rl_eval_run_episodes) with the
+    stage loop's results; ``fusable = False`` keeps the stage loop."""
 
     def __init__(self, net, n, mode="greedy", rng=None):
         if mode not in EVAL_MODES:
@@ -545,8 +605,16 @@ class EvaluationPolicy(AbstractPolicy):
             self._d_rng = self.ctx.malloc(rng.nbytes)
             self.ctx.h2d(self._d_rng, rng)
         self._host_act = None
+        self.fusable = True     # run() may hand whole stretches of env steps to run_episodes()
+
+    def _eval_net_mode(self):
+        return self.net, EVAL_MODES[self.mode]
+
+    def _eval_explorer(self):
+        return None
 
     def close(self):
+        self._close_eval()
         for name in ("_d_action", "_d_rng"):
             p = getattr(self, name, None)
             if p:
