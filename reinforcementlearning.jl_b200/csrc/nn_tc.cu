@@ -60,16 +60,15 @@ struct SmemBwd {
     static_assert(FIMG % 128 == 0 && WIMG_BYTES % 128 == 0 && (2 * GS_T) % 16 == 0, "operand images must stay 128-byte aligned");
     alignas(128) uint8_t FP_full[FIMG];    // dP2^T hi (rows = feature j, K = sample), fp16
     alignas(128) uint8_t FP_lo[FIMG];
-    alignas(128) uint8_t FH_lo[FIMG];      // H1^T lo
-    alignas(128) uint8_t FH_full[FIMG];    // H1^T hi
+    // H1 hi | lo by CTA-local tile parity, written by layer1(): the A operand of GEMM1 read K-major, the B operand of GEMM3 read
+    // MN-major (the same bytes), and H1 for the tanh branch of the GEMM2 epilogue
+    alignas(128) uint8_t AH[2][2][FIMG];
     alignas(128) uint8_t FQ_full[FIMG];    // dP1^T hi | lo: A operand of GEMM4, written by the MMA warpgroup from GEMM2's accumulators
     alignas(128) uint8_t FQ_lo[FIMG];
     alignas(128) uint8_t B1[WIMG_BYTES];   // rows 0..63: hi, 64..127: lo of (n = out o, k = in i)  = 64 W2[o + 64 i]
     // B operand of GEMM4, double-buffered by tile parity (written at publish time, read by the GEMM3 / GEMM4 of the same tile):
     // features 0..3 = x_i hi, 4 = 1.0 (-> db1, and db2 in GEMM3), 8..11 = x_i lo, the rest 0;  K = sample
     alignas(128) uint8_t XT[2][2 * GS_T];
-    alignas(128) uint8_t AH_full[FIMG];    // H1 hi | lo of the tile GEMM1 runs on (same layout as FH)
-    alignas(128) uint8_t AH_lo[FIMG];
     alignas(16) float D[TM * H];           // FP32 result of GEMM1 for the workers (d_off layout)
     // relu trunks: bit f = (H1[s][f] > 0) of sample s, by tile parity (written by layer1(), read by the GEMM2 epilogue: act'(H1));
     // the sign is not recoverable from the fp16 image (hi > 0 and H1 > 0 differ for tiny positive H1)
@@ -82,7 +81,7 @@ struct SmemBwd {
     float Red[32];
     double RedD[16];
     float step_scale;
-    alignas(8) uint64_t bar1;
+    alignas(8) uint64_t bar1[2];           // per 64-sample half
     alignas(8) uint64_t bar3;
     alignas(8) uint64_t bar4;
     float AccW2[64 * 65 + 64];             // FP32 accumulators of GEMM3: dW2[j][i] at j * 65 + i, then db2[j] (all still operand-scaled)
@@ -149,9 +148,10 @@ __device__ __forceinline__ void worker_sync() { asm volatile("bar.sync 1, 512;" 
 // sample, i.e. inside such a group, so the per-tile barriers are group-local (ids 5..8, 128 threads) and the four groups — one
 // per warp scheduler — drift freely within a tile; the tensor-core hand-overs (bar.arrive) and the mbarrier waits bound the drift.
 __device__ __forceinline__ void group_sync(int q) { asm volatile("bar.sync %0, 128;" ::"r"(5 + q) : "memory"); }
-// operand hand-over to the MMA warpgroup: 512 worker threads arrive without waiting, its 128 threads wait
-__device__ __forceinline__ void ready_arrive(int id) { asm volatile("bar.arrive %0, 640;" ::"r"(id) : "memory"); }
-__device__ __forceinline__ void ready_wait(int id) { asm volatile("bar.sync %0, 640;" ::"r"(id) : "memory"); }
+// operand hand-over of one 64-sample half to the MMA warpgroup: the 256 worker threads of quadrants 2h, 2h+1 arrive without
+// waiting, its 128 threads wait
+__device__ __forceinline__ void ready_arrive(int id) { asm volatile("bar.arrive %0, 384;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void ready_wait(int id) { asm volatile("bar.sync %0, 384;" ::"r"(id) : "memory"); }
 #ifdef B200RL_K7_TIMING   // debug build only: per-phase cycle sums seen by one watched worker thread
 __device__ unsigned long long g_k7_phase[40];
 __device__ int g_k7_watch = 0;   // watched worker thread (low 16 bits) of CTA (high bits; CTAs below n_actor = actor) whose timeline is recorded
@@ -166,7 +166,9 @@ __device__ int g_k7_watch = 0;   // watched worker thread (low 16 bits) of CTA (
 constexpr int NT7_ALL = NT7 + 128;
 constexpr int kRegsMma = 64, kRegsWorker = 104;
 static_assert(128 * kRegsMma + NT7 * kRegsWorker <= NT7_ALL * 96, "setmaxnreg split must fit the CTA's register allocation");
-constexpr int kBarRdyA = 2, kBarRdyB = 3;   // named barriers: workers arrive (bar.arrive), the MMA warpgroup waits (bar.sync)
+// Named barriers (11 of the 16): 0 __syncthreads, 1 worker_sync, 2 + h RdyA[h], 4 mma_sync, 5..8 group_sync(q), 9 + h RdyB[h].
+// RdyA[h] / RdyB[h]: the workers of half h arrive (bar.arrive), the MMA warpgroup waits (bar.sync).
+constexpr int kBarRdyA = 2, kBarRdyB = 9;   // + h
 constexpr int kBarMma = 4;                  // named barrier of the MMA warpgroup's 128 threads alone
 __device__ __forceinline__ void mma_sync() { asm volatile("bar.sync %0, 128;" ::"n"(kBarMma) : "memory"); }
 
@@ -201,6 +203,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int q = warp & 3, c = (warp >> 2) & 3;
     const int s = 32 * q + lane;
+    const int half = q >> 1;   // 64-sample half of the tile (wgmma M block) this worker's sample is in
     {   // weights: small ones plain, W2 as two operand images
         const float* b1 = p + (int64_t)H * d.in;
         const float* W2 = b1 + H;
@@ -217,7 +220,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         tcfwd::fill_w2_image<NT7_ALL>(sm.B1, W2);
     }
     if (tid == 32) {   // every thread of the MMA warpgroup arrives once per phase
-        wg::mbar_init(&sm.bar1, 128); wg::mbar_init(&sm.bar3, 128); wg::mbar_init(&sm.bar4, 128);
+        wg::mbar_init(&sm.bar1[0], 128); wg::mbar_init(&sm.bar1[1], 128); wg::mbar_init(&sm.bar3, 128); wg::mbar_init(&sm.bar4, 128);
     }
     wg::fence_proxy_async();
     __syncthreads();
@@ -239,7 +242,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
                 for (int hh = 0; hh < 2; ++hh)
                     *reinterpret_cast<float2*>(sm.D + d_off(64 * h + row0 + 8 * hh, 8 * j + col0)) = make_float2(dacc[4 * j + 2 * hh], dacc[4 * j + 2 * hh + 1]);
         };
-        auto gemm1 = [&](int h) { gemm_ts3<0>(dacc, sm.AH_full, sm.AH_lo, h, dB1k, 2 * G_F); };
+        auto gemm1 = [&](int h, int buf) { gemm_ts3<0>(dacc, sm.AH[buf][0], sm.AH[buf][1], h, dB1k, 2 * G_F); };
         auto gemm2 = [&](int h) { gemm_ts3<1>(dacc, sm.FP_full, sm.FP_lo, h, dB1t, 2 * GW_S); };   // dH1 = dP2 x W2
         // GEMM2 epilogue, samples 64h .. 64h+63: dP1 = D2 .* act'(H1) -> the dP1^T image (A operand of GEMM4).  Each thread
         // writes its fragment's feature pairs as half2 words: a quad covers one 16-byte feature group of one sample and a warp
@@ -257,10 +260,10 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
                     if (relu) {   // act'(H1) = (H1 > 0): the signs layer1() kept
                         v0 = ((pos >> (8 * j)) & 1u) ? v0 : 0.f;
                         v1 = ((pos >> (8 * j + 1)) & 1u) ? v1 : 0.f;
-                    } else {      // this tile's H1 = (hi + lo) / scale (the H1^T image is rewritten only after GEMM3 of this tile)
+                    } else {      // this tile's H1 = (hi + lo) / scale
                         const float inv_h = 1.0f / kScaleH;
-                        const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(sm.FH_full + off));
-                        const float2 lf = __half22float2(*reinterpret_cast<const __half2*>(sm.FH_lo + off));
+                        const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(sm.AH[pbuf][0] + off));
+                        const float2 lf = __half22float2(*reinterpret_cast<const __half2*>(sm.AH[pbuf][1] + off));
                         v0 *= dact_f(act, (hf.x + lf.x) * inv_h);
                         v1 *= dact_f(act, (hf.y + lf.y) * inv_h);
                     }
@@ -276,7 +279,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         // N = 8 accumulator.  Added into AccW2 by the fragment's owner thread.
         auto gemm3 = [&](int buf) {
             const uint64_t dPh = wg::make_desc(wg::smem_u32(sm.FP_full), GF_T, GS_T), dPl = wg::make_desc(wg::smem_u32(sm.FP_lo), GF_T, GS_T);
-            const uint64_t dHh = wg::make_desc(wg::smem_u32(sm.FH_full), GF_T, GS_T), dHl = wg::make_desc(wg::smem_u32(sm.FH_lo), GF_T, GS_T);
+            const uint64_t dHh = wg::make_desc(wg::smem_u32(sm.AH[buf][0]), GF_T, GS_T), dHl = wg::make_desc(wg::smem_u32(sm.AH[buf][1]), GF_T, GS_T);
             wg::fence();
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
@@ -330,24 +333,44 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
                 for (int e = 0; e < 2; ++e)
                     if (col0 + e < 5) sm.AccD4[(row0 + 8 * hh) * 9 + col0 + e] += d4[2 * hh + e];
         };
-        // Per tile: G2(t) + epilogue (dP1^T image) | G1(t+1) | G3(t) | G4(t).  Only G2 -> G1 sits between the workers' hand-over
-        // of tile t (RdyA) and their P3 of tile t + 1 (bar1); G3(t) and G4(t) run under P3 / P45(t+1).  D holds D1 only: D1(t) is
-        // read in the workers' P3(t), before they hand over RdyA(t).
+        // Per tile, per 64-sample half h: G2(t, h) + epilogue (dP1^T image) | G1(t+1, h); then G3(t) | G4(t) over all 128 samples.
+        // Only G2 -> G1 of its own half sits between the hand-over of half h of tile t (RdyA[h]) and the P3 of tile t + 1 of
+        // quadrants 2h, 2h+1 (bar1[h]): half 0's GEMM chain runs under half 1's loss work and the reverse.  G3(t) and G4(t) run under
+        // P3 / P45(t+1).  D holds D1 only: rows 64h .. 64h+63 of D1(t) are read in P3(t) of half h, before it hands over RdyA[h](t).
+        //
+        // Phase accounting (W_h = the 256 worker threads of quadrants 2h, 2h+1; M = the 128 MMA threads; once per tile each):
+        //   RdyA[h]  named, 384: W_h arrive after their dP2 stores of tile t, M waits before G2(t, h).  W_h arrive for t + 1 only
+        //            behind bar1[h](t+1), which M completes after it has passed RdyA[h](t): no early arrival joins an open phase.
+        //   RdyB[h]  named, 384: W_h arrive after layer1(t+1), M waits before G1(t+1, h).  W_h arrive for t + 2 behind
+        //            bar1[h](t+1), which M completes after its RdyB[h](t+1) wait.
+        //   bar1[h]  mbarrier, count 128: M arrives after store_d(h) of G1(t+1), W_h wait before P3(t+1).  Phase t+2 needs
+        //            RdyB[h](t+2), which every thread of W_h arrives after its wait for phase t+1.
+        //   bar3     mbarrier, count 128: M arrives after G3(t), all 512 workers wait in P45(t+1) before their dP2 stores (FP is
+        //            G3(t)'s A operand) and so before layer1(t+2) overwrites AH[t&1] (G3(t)'s B operand; G1(t) and the tanh epilogue
+        //            of t read it earlier in M's order).  Phase t+1 needs G2(t+1, 0 and 1), i.e. RdyA[0, 1](t+1), which every
+        //            worker arrives after that wait.
+        //   bar4     mbarrier, count 128: M arrives after G4(t), all workers wait before RdyA(t+1) (publish(t+2) rewrites XT[t&1]);
+        //            phase t+1 needs RdyA[0, 1](t+1) as above.
         if (cta < ntiles) {
-            ready_wait(kBarRdyB);                      // H1 operand of the first tile
-            for (int h = 0; h < 2; ++h) { gemm1(h); store_d(h); }
-            wg::mbar_arrive(&sm.bar1);
+            for (int h = 0; h < 2; ++h) {
+                ready_wait(kBarRdyB + h);              // H1 operand of the first tile
+                gemm1(h, 0); store_d(h);
+                wg::mbar_arrive(&sm.bar1[h]);
+            }
         }
         int buf = 0;
         for (int64_t tile = cta; tile < ntiles; tile += nctas, buf ^= 1) {
-            ready_wait(kBarRdyA);                      // dP2 / H1^T images of this tile; the workers have read D1(t)
-            for (int h = 0; h < 2; ++h) { gemm2(h); store_dp1(h, buf); }
-            wg::fence_proxy_async();                   // this thread's share of the dP1^T image -> visible to GEMM4 (after mma_sync)
-            if (tile + nctas < ntiles) {
-                ready_wait(kBarRdyB);                  // H1 operand of the next tile
-                for (int h = 0; h < 2; ++h) { gemm1(h); store_d(h); }
-                wg::mbar_arrive(&sm.bar1);
+            const bool has_next = tile + nctas < ntiles;
+            for (int h = 0; h < 2; ++h) {
+                ready_wait(kBarRdyA + h);              // dP2 image of this half; its workers have read their D1(t)
+                gemm2(h); store_dp1(h, buf);
+                if (has_next) {
+                    ready_wait(kBarRdyB + h);          // H1 operand of this half of the next tile
+                    gemm1(h, buf ^ 1); store_d(h);
+                    wg::mbar_arrive(&sm.bar1[h]);
+                }
             }
+            wg::fence_proxy_async();                   // this thread's share of the dP1^T image -> visible to GEMM4 (after mma_sync)
             gemm3(buf);
             wg::mbar_arrive(&sm.bar3);
             mma_sync();                                // every thread's share of the dP1^T image is in place
@@ -415,10 +438,11 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
     for (int k = tid; k < 64 * 9; k += NT7) sm.AccD4[k] = 0.f;
     // ---- software pipeline (one tile = 128 samples; tensor core and CUDA cores work on different tiles / phases) ----
     //   workers        : ... P3(t) P45(t) | P0(t+1) P1(t+1) | P3(t+1) P45(t+1) ...
-    //   MMA warpgroup  :              G2(t) + dP1(t) ..... G1(t+1) | G3(t) G4(t) ...
+    //   MMA warpgroup  :              G2(t,0) + dP1 G1(t+1,0) | G2(t,1) + dP1 G1(t+1,1) | G3(t) G4(t) ...
     // G2(t) and its epilogue (dP1 = dH1 .* act'(H1) -> the GEMM4 operand) run under P0/P1(t+1), G3(t) / G4(t) under
     // P3 / P45(t+1); the MMA warpgroup starts each GEMM as soon as the workers have handed its operands over (ready_arrive), so
-    // no worker waits for a GEMM whose result it does not need.
+    // no worker waits for a GEMM whose result it does not need.  The hand-overs and the wait for GEMM1 are per 64-sample half
+    // (quadrants 2h, 2h+1): half 0's workers start P3(t+1) while the tensor core still runs half 1's G2(t) / G1(t+1).
     // P0: the next tile's records leave the prefetch registers (x -> layer 1 and the x^T operand of GEMM4, scalars -> aux),
     // the records of the tile after it are requested, the index of the one after that computed / requested
     float xo[kInMax];
@@ -467,9 +491,9 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             split2(h[2], h[3], hi8[2 * ch + 1], lo8[2 * ch + 1]);
         }
         if (relu) reinterpret_cast<uint16_t*>(&sm.H1pos[pbuf][s])[c] = (uint16_t)pos;   // bits 16c .. 16c+15 of the sample's word
+        store16_feat(sm.AH[pbuf][0], 16 * c, s, hi8);
+        store16_feat(sm.AH[pbuf][1], 16 * c, s, lo8);
         pbuf ^= 1;
-        store16_feat(sm.AH_full, 16 * c, s, hi8);
-        store16_feat(sm.AH_lo, 16 * c, s, lo8);
     };
     if (cta < ntiles) {   // prologue: P0 / P1 of the first tile (the MMA warpgroup runs its G1)
         request(index_of(cta), pfx, pfa);
@@ -477,7 +501,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         publish(cta);
         layer1();
         wg::fence_proxy_async();
-        ready_arrive(kBarRdyB);
+        ready_arrive(kBarRdyB + half);
     }
 #ifdef B200RL_K7_TIMING
     tprev_ = clock64();
@@ -485,7 +509,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
     for (int64_t tile = cta; tile < ntiles; tile += nctas) {
         const bool has_next = tile + nctas < ntiles;
         // ---- P3: H2 = act(D1 + b2) (registers) + head partials ---------------------------------------
-        wg::mbar_wait(&sm.bar1, ph1);
+        wg::mbar_wait(&sm.bar1[half], ph1);
         ph1 ^= 1u;
         K7_T(0);
         float h2[16];
@@ -507,8 +531,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         group_sync(q);
         K7_T(2);
         // ---- P4+P5: loss (evaluated by all four feature-block threads of a sample: no exchange, no idle warps),
-        //            dW3 / db2 partials, dP2 = (W3^T dz) .* act'(H2) -> dP2^T image (A operand of GEMM2 and GEMM3) and
-        //            the H1^T image for GEMM3 -------------------------------------------------------------------------
+        //            dW3 / db2 partials, dP2 = (W3^T dz) .* act'(H2) -> dP2^T image (A operand of GEMM2 and GEMM3) ----------
         {
             float z[kNo];
 #pragma unroll
@@ -545,14 +568,6 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             K7_T(4);
             store16_feat(sm.FP_full, 16 * c, s, hi8);
             store16_feat(sm.FP_lo, 16 * c, s, lo8);
-            // H1 of this tile (this thread's own entries of the GEMM1 operand, which layer1() of the next tile overwrites) -> H1^T image
-            {
-                const uint32_t off = fimg_off(16 * c, s);
-                const uint4 h0 = *reinterpret_cast<const uint4*>(sm.AH_full + off), h1 = *reinterpret_cast<const uint4*>(sm.AH_full + off + GS_T);
-                const uint4 l0 = *reinterpret_cast<const uint4*>(sm.AH_lo + off), l1 = *reinterpret_cast<const uint4*>(sm.AH_lo + off + GS_T);
-                *reinterpret_cast<uint4*>(sm.FH_full + off) = h0; *reinterpret_cast<uint4*>(sm.FH_full + off + GS_T) = h1;
-                *reinterpret_cast<uint4*>(sm.FH_lo + off) = l0; *reinterpret_cast<uint4*>(sm.FH_lo + off + GS_T) = l1;
-            }
         }
         K7_T(5);
         wg::fence_proxy_async();
@@ -564,7 +579,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             ph4 ^= 1u;
         }
         K7_T(6);
-        ready_arrive(kBarRdyA);     // this thread's share of the GEMM2 / GEMM3 operands is in place
+        ready_arrive(kBarRdyA + half);   // this thread's share of the GEMM2 / GEMM3 operands is in place
         gemm3_pending = true;       // (Zp is rewritten in P3 of the next tile, behind its wait for GEMM1, i.e. after every thread has passed
         gemm4_pending = true;       //  this point: no barrier needed here)
         K7_T(7);
@@ -573,7 +588,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
             layer1();
             wg::fence_proxy_async();
             K7_T(8);
-            ready_arrive(kBarRdyB);
+            ready_arrive(kBarRdyB + half);
             K7_T(9);
         }
 #ifdef B200RL_K7_TIMING
