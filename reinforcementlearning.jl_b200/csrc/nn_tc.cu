@@ -54,6 +54,9 @@ constexpr int GF_T = 128;                 // stride between 8-sample groups
 constexpr int GS_T = 16 * GF_T;           // stride between 8-feature blocks (128 samples)
 constexpr int FIMG = 8 * GS_T;            // [64 features x 128 samples] fp16 = 16 KB
 constexpr float kScaleH = 64.0f, kScaleX = 64.0f;   // power-of-two scales of the H1 / observation operands (weights: kScaleW)
+// Row stride of the GEMM3 accumulators in shared memory: 72 = 8 (mod 32), so the fragment's owner threads, reading and writing
+// 8-byte column pairs, hit 16 different bank pairs per half-warp (a stride of 65 put up to 4 lanes on one bank)
+constexpr int kAccW2S = 72;
 constexpr int kNo = 2;   // head outputs this kernel handles (nn_tc_bwd_supported: actor n_out <= 2, critic n_out = 1)
 
 struct SmemBwd {
@@ -84,7 +87,7 @@ struct SmemBwd {
     alignas(8) uint64_t bar1[2];           // per 64-sample half
     alignas(8) uint64_t bar3;
     alignas(8) uint64_t bar4;
-    float AccW2[64 * 65 + 64];             // FP32 accumulators of GEMM3: dW2[j][i] at j * 65 + i, then db2[j] (all still operand-scaled)
+    alignas(8) float AccW2[64 * kAccW2S + 64];        // FP32 accumulators of GEMM3: dW2[j][i] at j * kAccW2S + i, then db2[j] (all still operand-scaled)
     float AccD4[64 * 9];                   // ... of GEMM4: dW1[f][i] at f * 9 + i, db1[f] at f * 9 + 4
 };
 // D[s][col] (floats): 16-byte units XOR-swizzled by the sample, so that 8 consecutive samples read at the same column hit 8
@@ -276,10 +279,18 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
         };
         // GEMM3 (K = 128 samples, M = 64 features j): dP2^T hi x H1^T hi, lo x hi and hi x lo into one accumulator, then
         // [dP2^T hi | lo] x the x^T operand, whose feature 4 is 1.0 for every sample: sum_s dP2 = db2 lands in column 4 of an
-        // N = 8 accumulator.  Added into AccW2 by the fragment's owner thread.
-        auto gemm3 = [&](int buf) {
+        // N = 8 accumulator.  GEMM4 (K = 128 samples, M = 64 features f): dP1^T hi x [x hi, 1], hi x x lo, lo x [x hi, 1];
+        // columns 0..3 = dW1, 4 = db1.  GEMM3's two parts go to the tensor core back to back as two commit groups, and the N = 64
+        // result is added into AccW2 by the fragment's owner thread while the N = 8 part still runs (not between them); GEMM4
+        // follows.  Each accumulator sees the same wgmma sequence as before.  (GEMM4 cannot join the batch: with its accumulator
+        // live too, 64 registers are too few and ptxas serialises every wgmma of the kernel.)
+        // Every MMA thread's share of the dP1^T image (GEMM4's A operand) is in place before the call (mma_sync).
+        auto gemm34 = [&](int buf) {
             const uint64_t dPh = wg::make_desc(wg::smem_u32(sm.FP_full), GF_T, GS_T), dPl = wg::make_desc(wg::smem_u32(sm.FP_lo), GF_T, GS_T);
             const uint64_t dHh = wg::make_desc(wg::smem_u32(sm.AH[buf][0]), GF_T, GS_T), dHl = wg::make_desc(wg::smem_u32(sm.AH[buf][1]), GF_T, GS_T);
+            const uint64_t dQh = wg::make_desc(wg::smem_u32(sm.FQ_full), GF_T, GS_T), dQl = wg::make_desc(wg::smem_u32(sm.FQ_lo), GF_T, GS_T);
+            const uint64_t dX = wg::make_desc(wg::smem_u32(sm.XT[buf]), GF_T, GS_T);
+            float d8[4] = {0.f, 0.f, 0.f, 0.f}, d4[4] = {0.f, 0.f, 0.f, 0.f};
             wg::fence();
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
@@ -289,16 +300,6 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
                 wg::mma_m64n64k16<1, 1>(dacc, wg::desc_add(dPh, a), wg::desc_add(dHl, a), 1u);
             }
             wg::commit();
-            wg::wait_all();
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) sm.AccW2[(row0 + 8 * hh) * 65 + 8 * j + col0 + e] += dacc[4 * j + 2 * hh + e];
-            const uint64_t dX = wg::make_desc(wg::smem_u32(sm.XT[buf]), GF_T, GS_T);
-            float d8[4] = {0.f, 0.f, 0.f, 0.f};
-            wg::fence();
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
                 const uint32_t a = k * 2 * GF_T;
@@ -306,17 +307,23 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
                 wg::mma_m64n8k16<1, 1>(d8, wg::desc_add(dPl, a), wg::desc_add(dX, a), 1u);
             }
             wg::commit();
-            wg::wait_all();
+            wg::wait_groups<1>();                      // GEMM3's N = 64 part
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    float2* a = reinterpret_cast<float2*>(sm.AccW2 + (row0 + 8 * hh) * kAccW2S + 8 * j + col0);
+                    float2 v = *a;
+                    v.x += dacc[4 * j + 2 * hh];
+                    v.y += dacc[4 * j + 2 * hh + 1];
+                    *a = v;
+                }
+            wg::wait_all();                            // db2
             if (col0 == 4) {
-                sm.AccW2[64 * 65 + row0] += d8[0];
-                sm.AccW2[64 * 65 + row0 + 8] += d8[2];
+                sm.AccW2[64 * kAccW2S + row0] += d8[0];
+                sm.AccW2[64 * kAccW2S + row0 + 8] += d8[2];
             }
-        };
-        // GEMM4 (K = 128 samples, M = 64 features f): dP1^T hi x [x hi, 1], hi x x lo, lo x [x hi, 1]; columns 0..3 = dW1, 4 = db1
-        auto gemm4 = [&](int buf) {
-            const uint64_t dQh = wg::make_desc(wg::smem_u32(sm.FQ_full), GF_T, GS_T), dQl = wg::make_desc(wg::smem_u32(sm.FQ_lo), GF_T, GS_T);
-            const uint64_t dX = wg::make_desc(wg::smem_u32(sm.XT[buf]), GF_T, GS_T);
-            float d4[4] = {0.f, 0.f, 0.f, 0.f};
+            wg::mbar_arrive(&sm.bar3);                 // GEMM3 has read FP and AH[buf]
             wg::fence();
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
@@ -326,12 +333,13 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
                 wg::mma_m64n8k16<1, 1>(d4, wg::desc_add(dQl, a), wg::desc_add(dX, a), 1u);
             }
             wg::commit();
-            wg::wait_all();
+            wg::wait_all();                            // GEMM4
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
                 for (int e = 0; e < 2; ++e)
                     if (col0 + e < 5) sm.AccD4[(row0 + 8 * hh) * 9 + col0 + e] += d4[2 * hh + e];
+            wg::mbar_arrive(&sm.bar4);
         };
         // Per tile, per 64-sample half h: G2(t, h) + epilogue (dP1^T image) | G1(t+1, h); then G3(t) | G4(t) over all 128 samples.
         // Only G2 -> G1 of its own half sits between the hand-over of half h of tile t (RdyA[h]) and the P3 of tile t + 1 of
@@ -371,11 +379,8 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
                 }
             }
             wg::fence_proxy_async();                   // this thread's share of the dP1^T image -> visible to GEMM4 (after mma_sync)
-            gemm3(buf);
-            wg::mbar_arrive(&sm.bar3);
             mma_sync();                                // every thread's share of the dP1^T image is in place
-            gemm4(buf);                                // (its x^T | 1 operand was written at publish time)
-            wg::mbar_arrive(&sm.bar4);
+            gemm34(buf);                               // (GEMM4's x^T | 1 operand was written at publish time)
         }
     } else {
     // ================= 16 worker warps =======================================================================
@@ -434,7 +439,7 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
     float* const gb1 = out + (int64_t)H * d.in;
     float* const gW2 = gb1 + H;
     float* const gb2 = gW2 + (int64_t)H * H;
-    for (int k = tid; k < 64 * 65 + 64; k += NT7) sm.AccW2[k] = 0.f;
+    for (int k = tid; k < 64 * kAccW2S + 64; k += NT7) sm.AccW2[k] = 0.f;
     for (int k = tid; k < 64 * 9; k += NT7) sm.AccD4[k] = 0.f;
     // ---- software pipeline (one tile = 128 samples; tensor core and CUDA cores work on different tiles / phases) ----
     //   workers        : ... P3(t) P45(t) | P0(t+1) P1(t+1) | P3(t+1) P45(t+1) ...
@@ -506,59 +511,81 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
 #ifdef B200RL_K7_TIMING
     tprev_ = clock64();
 #endif
-    for (int64_t tile = cta; tile < ntiles; tile += nctas) {
-        const bool has_next = tile + nctas < ntiles;
+    // P3 and P4+P5 of one tile (below) for NO head outputs.  The critic (n_out = 1) runs NO = 1 and skips the second head: its W3
+    // column and b3 are zero and its dz is +0 there, and nothing reads its g3[1] / gb3a1 / l1.  Same bits as NO = 2: that head's term
+    // of dh is w.y * dzs1 = +0, which the fmaf against +0 keeps (a -0 product still comes out +0).
+    auto tile_loss = [&](auto no, int64_t tile, uint32_t(&hi8)[8], uint32_t(&lo8)[8]) {
+        constexpr int NO = decltype(no)::value;
         // ---- P3: H2 = act(D1 + b2) (registers) + head partials ---------------------------------------
-        wg::mbar_wait(&sm.bar1[half], ph1);
-        ph1 ^= 1u;
-        K7_T(0);
         float h2[16];
         {
             float v[16];
             d_ld16(sm.D, s, 16 * c, v);
-            float zp[kNo] = {0.f, 0.f};
+            float zp[NO];
+#pragma unroll
+            for (int o = 0; o < NO; ++o) zp[o] = 0.f;
 #pragma unroll
             for (int k = 0; k < 16; ++k) {
                 const int f = 16 * c + k;
                 h2[k] = act_f(act, fmaf(v[k], inv_s1, sm.b2[f]));   // operand scales undone (exact)
-                float2 w = *reinterpret_cast<const float2*>(sm.W3 + f * kNo);
-                zp[0] = fmaf(w.x, h2[k], zp[0]); zp[1] = fmaf(w.y, h2[k], zp[1]);
+                if constexpr (NO == 2) {
+                    float2 w = *reinterpret_cast<const float2*>(sm.W3 + f * kNo);
+                    zp[0] = fmaf(w.x, h2[k], zp[0]); zp[1] = fmaf(w.y, h2[k], zp[1]);
+                } else {
+                    zp[0] = fmaf(sm.W3[f * kNo], h2[k], zp[0]);
+                }
             }
 #pragma unroll
-            for (int o = 0; o < kNo; ++o) sm.Zp[(c * kNo + o) * TM + s] = zp[o];
+            for (int o = 0; o < NO; ++o) sm.Zp[(c * kNo + o) * TM + s] = zp[o];
         }
         K7_T(1);
         group_sync(q);
         K7_T(2);
         // ---- P4+P5: loss (evaluated by all four feature-block threads of a sample: no exchange, no idle warps),
         //            dW3 / db2 partials, dP2 = (W3^T dz) .* act'(H2) -> dP2^T image (A operand of GEMM2 and GEMM3) ----------
-        {
-            float z[kNo];
+        float z[kNo] = {0.f, 0.f};
 #pragma unroll
-            for (int o = 0; o < kNo; ++o)
-                z[o] = sm.b3[o] + ((sm.Zp[o * TM + s] + sm.Zp[(kNo + o) * TM + s]) + (sm.Zp[(2 * kNo + o) * TM + s] + sm.Zp[(3 * kNo + o) * TM + s]));
-            const bool valid = (tile * TM + s) < b.B;
-            // (evaluated by all four feature-block threads of a sample: identical arithmetic on each)
-            const policy::LossOut<kNo> lo_ = policy::sample_loss(actor.heads2, actor.nout, role, hp, b.inv_B, z, aux[0], aux[1], aux[2], aux[3]);
-            float dz[kNo];
+        for (int o = 0; o < NO; ++o)
+            z[o] = sm.b3[o] + ((sm.Zp[o * TM + s] + sm.Zp[(kNo + o) * TM + s]) + (sm.Zp[(2 * kNo + o) * TM + s] + sm.Zp[(3 * kNo + o) * TM + s]));
+        const bool valid = (tile * TM + s) < b.B;
+        // (evaluated by all four feature-block threads of a sample: identical arithmetic on each)
+        const policy::LossOut<kNo> lo_ = policy::sample_loss(actor.heads2, actor.nout, NO == 2 ? 0 : 1, hp, b.inv_B, z, aux[0], aux[1], aux[2], aux[3]);
+        float dz[kNo];
 #pragma unroll
-            for (int o = 0; o < kNo; ++o) dz[o] = valid ? lo_.dz[o] : 0.f;
-            if (c == 0 && valid) { l0 += lo_.l0; l1 += lo_.l1; gb3a0 += dz[0]; gb3a1 += dz[1]; }
-            // dP2 operand = scale_p * (W3^T dz) .* act'(H2): the power-of-two operand scale rides on dz (exact, bit-identical to scaling dP2)
-            const float dzs0 = dz[0] * scale_p, dzs1 = dz[1] * scale_p;
-            float dp[16];
+        for (int o = 0; o < kNo; ++o) dz[o] = valid ? lo_.dz[o] : 0.f;
+        if (c == 0 && valid) {
+            l0 += lo_.l0; gb3a0 += dz[0];
+            if constexpr (NO == 2) { l1 += lo_.l1; gb3a1 += dz[1]; }
+        }
+        // dP2 operand = scale_p * (W3^T dz) .* act'(H2): the power-of-two operand scale rides on dz (exact, bit-identical to scaling dP2)
+        const float dzs0 = dz[0] * scale_p, dzs1 = dz[1] * scale_p;
+        float dp[16];
 #pragma unroll
-            for (int k = 0; k < 16; ++k) {
-                const int f = 16 * c + k;
+        for (int k = 0; k < 16; ++k) {
+            const int f = 16 * c + k;
+            float dh;
+            if constexpr (NO == 2) {
                 float2 w = *reinterpret_cast<const float2*>(sm.W3 + f * kNo);
-                const float dh = fmaf(w.x, dzs0, w.y * dzs1);
-                dp[k] = relu ? (h2[k] > 0.f ? dh : 0.f) : dh * (1.f - h2[k] * h2[k]);
-                g3[0][k] = fmaf(dz[0], h2[k], g3[0][k]);
-                g3[1][k] = fmaf(dz[1], h2[k], g3[1][k]);
+                dh = fmaf(w.x, dzs0, w.y * dzs1);
+            } else {
+                dh = fmaf(sm.W3[f * kNo], dzs0, 0.f);
             }
-            uint32_t hi8[8], lo8[8];
+            dp[k] = relu ? (h2[k] > 0.f ? dh : 0.f) : dh * (1.f - h2[k] * h2[k]);
+            g3[0][k] = fmaf(dz[0], h2[k], g3[0][k]);
+            if constexpr (NO == 2) g3[1][k] = fmaf(dz[1], h2[k], g3[1][k]);
+        }
 #pragma unroll
-            for (int m = 0; m < 8; ++m) split2(dp[2 * m], dp[2 * m + 1], hi8[m], lo8[m]);
+        for (int m = 0; m < 8; ++m) split2(dp[2 * m], dp[2 * m + 1], hi8[m], lo8[m]);
+    };
+    for (int64_t tile = cta; tile < ntiles; tile += nctas) {
+        const bool has_next = tile + nctas < ntiles;
+        wg::mbar_wait(&sm.bar1[half], ph1);
+        ph1 ^= 1u;
+        K7_T(0);
+        {
+            uint32_t hi8[8], lo8[8];
+            if (role) tile_loss(std::integral_constant<int, 1>{}, tile, hi8, lo8);
+            else tile_loss(std::integral_constant<int, 2>{}, tile, hi8, lo8);
             K7_T(3);
             if (gemm3_pending) {   // the previous tile's GEMM2 / GEMM3 must have consumed the images before they are overwritten
                 wg::mbar_wait(&sm.bar3, ph3);
@@ -599,9 +626,9 @@ ac_loss_grad_tc_kernel(MlpDesc actor, MlpDesc critic, const float* params /* no 
     if (gemm3_pending) wg::mbar_wait(&sm.bar3, ph3);
     if (gemm4_pending) wg::mbar_wait(&sm.bar4, ph4);
     worker_sync();                                       // (a CTA without tiles writes the zeros the accumulators were initialised with)
-    for (int k = tid; k < H * H; k += NT7) gW2[k] = sm.AccW2[(k & 63) * 65 + (k >> 6)] * inv_s3;     // gW2[j + 64 i]
+    for (int k = tid; k < H * H; k += NT7) gW2[k] = sm.AccW2[(k & 63) * kAccW2S + (k >> 6)] * inv_s3;     // gW2[j + 64 i]
     if (tid < H) {
-        gb2[tid] = sm.AccW2[64 * 65 + tid] * inv_sp;
+        gb2[tid] = sm.AccW2[64 * kAccW2S + tid] * inv_sp;
         gb1[tid] = sm.AccD4[tid * 9 + 4] * inv_sp;
         for (int i = 0; i < d.in; ++i) gW1[tid + H * i] = sm.AccD4[tid * 9 + i] * inv_s4;
     }

@@ -36,6 +36,9 @@ __device__ __forceinline__ void fence() { asm volatile("wgmma.fence.sync.aligned
 __device__ __forceinline__ void commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 // every committed wgmma of this thread has completed: its accumulators are valid and its shared-memory reads are done
 __device__ __forceinline__ void wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// every commit group of this thread but the N most recent has completed
+template <int N>
+__device__ __forceinline__ void wait_groups() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // generic-proxy st.shared -> visible to the async proxy (tensor-core operand reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
